@@ -1,14 +1,20 @@
 #!/usr/bin/env python
 """bench.py — frames/s of the PoseCNN hot path on synthetic 640x480 batches (BASELINE.json).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload full|hough|rgbd|project] [--batch B]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload full|hough|rgbd|project|train] [--batch B]
+                    [--dump-outputs DIR]
     python bench.py --impl reference ...      # the same path restated on the host cores (oracle/cpu_pipeline.py)
 
 One JSON line on stdout (rank 0).  A "step" is one pass of the hot path over ONE GLOBAL batch of `--batch` synthetic
 frames: with N GPUs the batch is cut into contiguous image shards (strong scaling, SURVEY.md §8(e): index_size =
 128 / B_global, global batch indices, one NCCL all-gather of the pose-hypothesis records per step); the weak-scaling
 figure (a full batch per GPU) is reported beside it in `weak`.  Device time is measured with CUDA events on the
-launching stream; clocks are sampled with nvidia-smi during the timed region.
+launching stream; clocks are sampled with nvidia-smi during the timed region.  Every timed loop runs exactly --steps steps.
+
+--dump-outputs DIR writes what the timed path returned in its last timed step as DIR/<name>.npy (float32, or float64
+where the output is float64), at most 64 MB in all: an array larger than its share of the budget is replaced by a fixed
+sample of its flattened elements (indices sorted, drawn with numpy's default_rng(0), so two runs with the same arguments
+sample the same elements).  Inputs depend only on the arguments, so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -41,11 +47,12 @@ def measured_peaks():
         d = json.load(open(p))
         return dict(hbm_gbs=d["hbm_gbs"], bf16_tflops=d["bf16_tflops"], bf16_tflops_sustained=d.get("bf16_tflops_sustained"),
                     source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_tflops_sustained=1400.0, source="fallback (B200_PROFILING.md)")
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_tflops_sustained=None,
+                source="H100 SXM data sheet (dense BF16, 700 W card), not a measured peak")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -148,11 +155,28 @@ def count_own_launches(fn):
         return None
 
 
-def profile_json(name):
-    try:
-        return json.load(open(os.path.join(ROOT, "profiles", name)))
-    except Exception:
-        return None
+DUMP_BYTES = 64 * 1024 * 1024
+
+
+def dump_outputs(out_dir, arrays):
+    """Write name -> tensor / array as out_dir/<name>.npy in float32 (float64 stays float64), DUMP_BYTES in all: the smallest
+    arrays first, each within an equal share of what is left; a larger one is replaced by a fixed sample of its flattened
+    elements (sorted indices from numpy's default_rng(0), the same for every run with the same shapes)."""
+    os.makedirs(out_dir, exist_ok=True)
+    items = []
+    for name, a in arrays.items():
+        a = a.detach().cpu().numpy() if hasattr(a, "detach") else np.asarray(a)
+        items.append((name, a.astype(np.float64 if a.dtype == np.float64 else np.float32)))
+    items.sort(key=lambda kv: kv[1].nbytes)
+    left = DUMP_BYTES
+    for i, (name, a) in enumerate(items):
+        share = left // (len(items) - i)
+        if a.nbytes > share:
+            n = share // a.itemsize
+            idx = np.sort(np.random.default_rng(0).choice(a.size, size=n, replace=False))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+        left -= a.nbytes
 
 
 # ------------------------------------------------------------------------------------------
@@ -189,7 +213,7 @@ def measure_hough(B, rank, world, local, steps, warmup, use_graph=True, e2e_batc
     vertex = torch.from_numpy(inp["vertex"]).to(dev)
     meta = torch.from_numpy(inp["meta"]).to(dev)
     ext = torch.from_numpy(inp["extents"]).to(dev)
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)  # > 50 MB L2
 
     def step():
         return hop.hough_voting_gpu_capacity(label, vertex, ext, meta, None, 0, -1.0, 0.02, 10)
@@ -260,7 +284,7 @@ def measure_hough(B, rank, world, local, steps, warmup, use_graph=True, e2e_batc
 
         e2e_step()
         torch.cuda.synchronize()
-        k = max(2, min(steps, 5))
+        k = steps
         t0 = time.perf_counter()
         for _ in range(k):
             e2e_step()
@@ -270,6 +294,7 @@ def measure_hough(B, rank, world, local, steps, warmup, use_graph=True, e2e_batc
                           d2h_bytes_per_step=int(h_box.numel() * 4 + h_pose.numel() * 4 + 4),
                           note="the op's registered inputs are the dense fp32 label / vertex_pred maps (82 MB/frame): e2e is the PCIe "
                                "upload of those maps")
+    res["outputs"] = dict(rois=out[0], poses=out[1], num_rois=out[5])
     return res
 
 
@@ -289,7 +314,6 @@ def run_hough(args, rank, world, local):
     rec = measure_hough(B, rank, world, local, args.steps, args.warmup, not args.no_graph, args.e2e_batch, not args.no_e2e)
     clocks = sampler.stop()
     peaks = measured_peaks()
-    traffic = profile_json("r02_hough_traffic.json")
     res = dict(
         metric="frames/sec on 640x480, 21 classes (Hough voting op)", value=rec["frames_per_s"], unit="frames/s",
         n_gpus=world, steps=args.steps, warmup=max(args.warmup, 3), ms_per_step=rec["device_ms"], higher_is_better=True,
@@ -299,14 +323,13 @@ def run_hough(args, rank, world, local):
                     cuda_graph=rec["cuda_graph"]),
         clocks=clocks, gpu_launches=7 * args.steps,
         roofline=dict(bound="hbm", achieved=rec["footprint_gbs"], peak=peaks["hbm_gbs"], unit="GB/s",
-                      frac=rec["footprint_gbs"] / peaks["hbm_gbs"], traffic=(traffic or {}).get("dram_bytes_per_step_b%d" % B),
-                      peak_source=peaks["source"],
+                      frac=rec["footprint_gbs"] / peaks["hbm_gbs"], peak_source=peaks["source"],
                       note="achieved = op-boundary footprint 82.33 MB/frame (label + full vertex_pred) / whole-op device "
                            "time; the kernels read only the sampled pixels' 12 B, so >1.0 is possible (SURVEY §8(d))"),
     )
     if "e2e" in rec:
         res["e2e"] = rec["e2e"]
-    return res
+    return res, rec["outputs"]
 
 
 # ------------------------------------------------------------------------------------------
@@ -320,7 +343,7 @@ def make_network(dev, input_format="COLOR"):
 
 
 def rotating_inputs(h_img_np, dev, min_bytes=140 * 1024 * 1024, max_bufs=48):
-    """Device-resident input batches that together exceed the 126 MB L2 (the timing rule's "inputs larger than L2"):
+    """Device-resident input batches that together exceed the 50 MB L2 (inputs larger than L2):
     the same frames rolled along the batch axis, so every buffer is a distinct tensor with identical statistics."""
     import torch
     nb = int(min(max_bufs, max(2, -(-min_bytes // h_img_np.nbytes))))
@@ -372,8 +395,10 @@ def measure_pipeline(net, imgs_np, meta, ext, rank, world, dev, steps, warmup, b
     in_step_gather_ms = float(np.mean([pipe.last_gather_ms(last), pipe.last_gather_ms(last - 1)])) if steps >= 2 else None
     gathered = pipe.results(last)
     ndet = int((gathered[:, -1] > 0).sum().item())
+    outputs = dict(records=gathered, label_2d=L["label_2d"], detections_rois=L["detections_rois"], detections_poses=L["detections_poses"],
+                   num_detections=L["num_detections"])
     out = dict(ms_step=ms_step, layers=L, detections=ndet, nbufs=len(bufs), pipe=pipe, in_step_gather_ms=in_step_gather_ms, step=step,
-               bufs=bufs)
+               bufs=bufs, outputs={k: v.clone() for k, v in outputs.items()})
 
     if want_e2e:
         # end to end through the public API with HOST buffers: every step uploads its own pinned uint8 batch (H2D) and
@@ -410,7 +435,7 @@ def measure_pipeline(net, imgs_np, meta, ext, rank, world, dev, steps, warmup, b
 
         run_e2e(2)
         barrier(world)
-        k = max(steps, 30)       # the first upload cannot overlap anything: amortised over >= 30 steps like a serving loop's steady state
+        k = steps                # the first upload cannot overlap anything: more steps amortise it as a serving loop's steady state does
         t0 = time.perf_counter()
         run_e2e(k)
         dt = max_over_ranks((time.perf_counter() - t0) / k, world)
@@ -491,7 +516,7 @@ def run_full(args, rank, world, local, input_format="COLOR"):
     flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)
     d_img = m["bufs"][0]
     tr = []
-    for _ in range(max(3, min(args.steps, 10))):
+    for _ in range(args.steps):
         flush.zero_()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record(); net._trunk(d_img); e1.record()
@@ -502,7 +527,7 @@ def run_full(args, rank, world, local, input_format="COLOR"):
     # Houghvotinggpu alone as the pipeline runs it (vertex head sampled from `lowres`) on the network's own label maps
     from posecnn_b200.hough_voting_gpu_layer import hough_voting_gpu_op as hop
     hs = []
-    for _ in range(5):
+    for _ in range(args.steps):
         flush.zero_()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
@@ -531,7 +556,6 @@ def run_full(args, rank, world, local, input_format="COLOR"):
     peaks = measured_peaks()
     tf = VGG_FLOP_PER_FRAME * Bl / (trunk_ms * 1e-3) / 1e12
     burst, sust = peaks["bf16_tflops"], peaks["bf16_tflops_sustained"] or peaks["bf16_tflops"]
-    traffic = profile_json("r02_full_b32_trunk_traffic.json") or profile_json("r01_full_b32_trunk_traffic.json")
     res = dict(
         metric=METRIC_FULL if input_format == "COLOR" else "frames/sec on 640x480 RGB-D, 21 classes, batch 32 (two-trunk VGG16 + Hough + ROI pose head)",
         value=Bg / (ms_step * 1e-3),
@@ -545,7 +569,7 @@ def run_full(args, rank, world, local, input_format="COLOR"):
                     global_batch=Bg, per_gpu_batch=Bl,
                     parallelism="contiguous image shards x%d of the global batch (index_size = 128 // %d, global batch indices), NCCL "
                                 "all-gather of post-NMS pose records on a side stream" % (world, Bg),
-                    l2="no flush: %d rotating device-resident input batches (%.0f MB > 126 MB L2) and %.1f GB of activations per step"
+                    l2="no flush: %d rotating device-resident input batches (%.0f MB > 50 MB L2) and %.1f GB of activations per step"
                        % (m_nbufs(Bl), m_nbufs(Bl) * Bl * H * W * 3 / 1e6, 0.172 * Bl * ntrunks),
                     detections_last_step=int(L["num_detections"].item()), cuda_graph=not args.no_graph,
                     dense_vertex_pred=False,
@@ -554,11 +578,10 @@ def run_full(args, rank, world, local, input_format="COLOR"):
                                            "un-calibrated random init labels ~100%% of pixels foreground" % bg_shift),
         clocks=clocks, gpu_launches=(LAUNCHES_FULL + (14 if input_format == "RGBD" else 0)) * args.steps,
         roofline=dict(bound="tensor", achieved=tf, peak=burst, unit="TFLOP/s", frac=tf / burst, frac_sustained=tf / sust,
-                      peak_sustained=sust, traffic=(traffic or {}).get("trunk_dram_bytes_per_launch_group") if (traffic or {}).get("batch") == Bl else None,
-                      peak_source=peaks["source"] + ": burst cuBLAS bf16 (kernel group timed alone); frac_sustained = vs the sustained figure",
+                      peak_sustained=sust, peak_source=peaks["source"],
                       kernel="conv trunk: k_conv1_tc, k_conv_row2 x3, k_conv_tc<256> x9, 1 max-pool (3 pools fused)",
                       ms_per_launch_group=trunk_ms * ntrunks, frames_per_launch_group=Bl,
-                      note="achieved = 187.918 GFLOP/frame x this rank's frames / device time of the conv trunk (13 tcgen05 launches, im2col "
+                      note="achieved = 187.918 GFLOP/frame x this rank's frames / device time of the conv trunk (13 wgmma launches, im2col "
                            "and three of the four max-pools fused into them), CUDA events, L2 flushed; BF16 operands, FP32 accumulation"),
         breakdown_ms=dict(step=ms_step, conv_trunk=trunk_ms * ntrunks, hough_on_network_maps=hough_net_ms),
         hough_on_network_maps=dict(ms=hough_net_ms, frames=Bl, footprint_gbs=HOUGH_BYTES_PER_FRAME * Bl / (hough_net_ms * 1e-3) / 1e9,
@@ -574,7 +597,7 @@ def run_full(args, rank, world, local, input_format="COLOR"):
         res["comm"] = comm
     if weak:
         res["weak"] = weak
-    return res, net
+    return res, net, m["outputs"]
 
 
 def m_nbufs(Bl):
@@ -623,12 +646,14 @@ def run_project(args, rank, world, local):
     clocks = sampler.stop()
     ms_step = max_over_ranks(e0.elapsed_time(e1) / args.steps, world)
     # the dominant kernel alone
+    outputs = dict(projected=out)
+    del out
     tb0.record()
-    for _ in range(3):
-        td = bop.backproject(data, lab, depth, meta, l3, G, ks, thr)
+    for _ in range(args.steps):
+        bop.backproject(data, lab, depth, meta, l3, G, ks, thr)     # result dropped at once: one grid of outputs alive at a time
     tb1.record()
     torch.cuda.synchronize()
-    bp_ms = tb0.elapsed_time(tb1) / 3
+    bp_ms = tb0.elapsed_time(tb1) / args.steps
     peaks = measured_peaks()
     bp_bytes = Bl * G ** 3 * (2 * Cf + C) * 4 + Bl * H * W * (Cf + C + 1) * 4
     pj_bytes = Bl * H * W * (4 + 8 * Cf)
@@ -648,9 +673,9 @@ def run_project(args, rank, world, local):
 
         e2e_step()
         t0 = time.perf_counter()
-        for _ in range(3):
+        for _ in range(args.steps):
             e2e_step()
-        dt = max_over_ranks((time.perf_counter() - t0) / 3, world)
+        dt = max_over_ranks((time.perf_counter() - t0) / args.steps, world)
         e2e = dict(value=eb * world / dt, unit="frames/s", batch_per_gpu=eb, h2d_bytes_per_step=int((h_data.numel() + h_lab.numel() + h_depth.numel()) * 4),
                    d2h_bytes_per_step=int(h_out.numel() * 4), note="pinned host feature / label / depth maps in, projected features out")
     res = dict(
@@ -660,7 +685,7 @@ def run_project(args, rank, world, local):
         config=dict(workload="configs[3]: backprojecting_layer + projecting_layer, ONE global batch of %d frames image-sharded x%d "
                              "(per-image ops: no collective), G = %d, Cf = 64, C = 22, kernel_size 3, threshold 0.02" % (Bg, world, G),
                     global_batch=Bg, per_gpu_batch=Bl,
-                    l2="no flush: %.1f GB written and %.1f GB read per step on this rank (>> 126 MB L2)" % (bp_bytes / 1e9, (bp_bytes + pj_bytes) / 1e9)),
+                    l2="no flush: %.1f GB written and %.1f GB read per step on this rank (>> 50 MB L2)" % (bp_bytes / 1e9, (bp_bytes + pj_bytes) / 1e9)),
         clocks=clocks, gpu_launches=2 * args.steps,
         roofline=dict(bound="hbm", achieved=gbs, peak=peaks["hbm_gbs"], unit="GB/s", frac=gbs / peaks["hbm_gbs"], traffic=None,
                       peak_source=peaks["source"], kernel="k_backproject (dominant: %.2f of %.2f ms per step)" % (bp_ms, ms_step),
@@ -669,7 +694,7 @@ def run_project(args, rank, world, local):
     )
     if e2e:
         res["e2e"] = e2e
-    return res
+    return res, outputs
 
 
 # ------------------------------------------------------------------------------------------
@@ -757,10 +782,11 @@ def run_train(args, rank, world, local):
 
     run_e2e(2)                                    # first touch of the staging buffers, allocator growth
     barrier(world)
-    k = max(6, args.steps)
+    k = args.steps
     t0 = time.perf_counter()
     run_e2e(k)
     dt = max_over_ranks((time.perf_counter() - t0) / k, world)
+    outputs = {k_: v for k_, v in out.items() if hasattr(v, "detach")}
     launches = count_own_launches(lambda: step(data, gtl))
     peaks = measured_peaks()
     flop = 3.0 * VGG_FLOP_PER_FRAME * Bl                      # forward + input-gradient + weight-gradient GEMMs of the trunk
@@ -774,16 +800,16 @@ def run_train(args, rank, world, local):
         config=dict(workload="configs[4]: training step, ONE global batch of %d 640x480 frames, synthetic YCB-shaped labels / poses, 22 classes, "
                              "keep_prob 1.0" % Bg, global_batch=Bg, per_gpu_batch=Bl,
                     parallelism="image shards x%d, global loss normalisers, per-tensor NCCL all-reduce (SUM) of the gradients on a side stream" % world,
-                    l2="no flush: %.1f GB of saved activations per step (>> 126 MB L2)" % (0.31 * Bl), rois_rows=int(out["num_rois"].item()),
+                    l2="no flush: %.1f GB of saved activations per step (>> 50 MB L2)" % (0.31 * Bl), rois_rows=int(out["num_rois"].item()),
                     losses=dict(cls=float(out["loss_cls"].item()), vertex=float(out["loss_vertex"].item()), pose=float(out["loss_pose"].item()))),
         clocks=clocks, gpu_launches=(launches["own"] if launches else TRAIN_OWN_LAUNCHES_PER_STEP) * args.steps,
-        launches_per_step=launches or dict(own=TRAIN_OWN_LAUNCHES_PER_STEP, source="ncu launch list profiles/r02_train_b16_launches.csv"),
+        launches_per_step=launches or dict(own=TRAIN_OWN_LAUNCHES_PER_STEP, source="launch list of the training step, counted by hand"),
         roofline=dict(bound="tensor", achieved=tf, peak=sust, unit="TFLOP/s", frac=tf / sust, traffic=None, peak_source=peaks["source"] + " (sustained: a kernel "
                       "group inside a long step)", kernel="trunk GEMMs: 13 forward convolutions + 12 dgrad (k_conv_tc / k_conv_row2) + 12 wgrad (k_wgrad_tc)",
                       note="achieved = 3 x 187.918 GFLOP/frame x this rank's frames / WHOLE step time (heads, losses, pose head, update included)"),
         e2e=dict(value=Bg / dt, unit="frames/s", h2d_bytes_per_step=int(h_img.numel() + h_lab.numel() * 4), d2h_bytes_per_step=4,
                  note="pinned host uint8 images + int32 label maps in (upload of step i + 1 overlapped with step i on a copy stream), loss scalar out; "
-                      "wall clock over %d steps" % k))
+                      "wall clock over %d steps" % k)), outputs
 
 
 # ------------------------------------------------------------------------------------------
@@ -883,6 +909,7 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-weak", action="store_true", help="skip the weak-scaling record of multi-GPU runs")
     ap.add_argument("--no-hough-record", action="store_true", help="skip the Hough-op sub-records of the default line")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the outputs of the last timed step as DIR/<name>.npy")
     args = ap.parse_args()
 
     if args.impl == "reference":
@@ -894,15 +921,15 @@ def main():
 
     rank, world, local = dist_setup(args.gpus)
     if args.workload == "hough":
-        res = run_hough(args, rank, world, local)
+        res, outputs = run_hough(args, rank, world, local)
     elif args.workload == "project":
-        res = run_project(args, rank, world, local)
+        res, outputs = run_project(args, rank, world, local)
     elif args.workload == "train":
         if args.batch == 32:
             args.batch = 64                                   # configs[4] names batch 64
-        res = run_train(args, rank, world, local)
+        res, outputs = run_train(args, rank, world, local)
     else:
-        res, net = run_full(args, rank, world, local, "RGBD" if args.workload == "rgbd" else "COLOR")
+        res, net, outputs = run_full(args, rank, world, local, "RGBD" if args.workload == "rgbd" else "COLOR")
         if rank == 0 and world == 1 and args.workload == "full" and not args.no_hough_record:
             del net
             import torch
@@ -910,12 +937,10 @@ def main():
             peaks = measured_peaks()
             hb = {}
             for B in (32, 1):
-                r = measure_hough(B, 0, 1, 0, max(args.steps, 10), args.warmup, True, 32, True)
+                r = measure_hough(B, 0, 1, 0, args.steps, args.warmup, True, 32, True)
+                del r["outputs"]
                 r["frac"] = r["footprint_gbs"] / peaks["hbm_gbs"]
                 hb["b%d" % B] = r
-            traffic = profile_json("r02_hough_traffic.json")
-            if traffic:
-                hb["physical_dram_bytes_per_step"] = traffic
             if not args.no_cpu_baseline:
                 cpu = cpu_hough_same_frames()
                 hb["cpu_same_frames"] = cpu
@@ -924,11 +949,13 @@ def main():
                                               device_b1=hb["b1"]["frames_per_s"] / cpu["value"])
             hb["note"] = ("Houghvotinggpu op alone on the SURVEY 8(d) synthetic scenes (8 distinct frames tiled to the batch; the CPU op runs "
                           "the same 8 frames): footprint = 82.33 MB/frame (label + dense vertex_pred) / device time of the whole op "
-                          "(CUDA-graph replay, L2 flushed); peak = measured HBM copy bandwidth; the kernels read only ~2 MB/frame "
+                          "(CUDA-graph replay, L2 flushed); peak = %s; the kernels read only ~2 MB/frame " % peaks["source"] +
                           "(compulsory_bytes_per_frame), so the footprint fraction is a throughput-per-input-byte figure, not DRAM traffic")
             res["hough"] = hb
             res["roofline_hough"] = dict(bound="hbm", achieved=hb["b32"]["footprint_gbs"], peak=peaks["hbm_gbs"], unit="GB/s",
                                          frac=hb["b32"]["frac"], ms=hb["b32"]["device_ms"], scenes="SURVEY 8(d) synthetic scenes, batch 32")
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, outputs)
     if rank == 0:
         if not args.no_cpu_baseline and world == 1 and args.workload in ("full",):
             try:

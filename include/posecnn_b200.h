@@ -1,5 +1,5 @@
 /*
- * posecnn_b200.h — C ABI of libposecnn_b200.so (hand-written sm_100a CUDA).
+ * posecnn_b200.h — C ABI of libposecnn_b200.so (hand-written sm_90a CUDA).
  *
  * One entry point per native launcher of the reference (yuxng/PoseCNN @ 9f3dd7b).  The
  * reference's launchers take raw device pointers + ints + an Eigen::GpuDevice; these take
@@ -163,7 +163,7 @@ int pcnn_average_distance_bwd(const float* top_diff, const float* bottom_diff, i
  * VGG16 convolution stack on the tensor cores — replaces Network.conv / Network.max_pool
  * (networks/network.py:159-188, 303-310: tf.nn.conv2d NHWC x HWIO, SAME, stride 1, bias, ReLU;
  * 2x2/2 max pool) as wired by networks/vgg16_convs.py:80-97, 128-163.
- * Implicit GEMM on tcgen05 (BF16 operands, FP32 accumulation in TMEM, TMA-fed, im2col folded
+ * Implicit GEMM on wgmma (BF16 operands, FP32 accumulation in registers, TMA-fed, im2col folded
  * into the TMA box coordinates).  Activations are NHWC bf16; weights are [Cout][k*k*Cin] bf16
  * (tap-major, channel-minor; converted once from the TF HWIO layout).  block_n = 0 picks the
  * N tile (64 / 128 / 256) from Cout.
@@ -195,7 +195,7 @@ int pcnn_maxpool2x2_bf16(const void* in_bf16, void* out_bf16, int B, int H, int 
  * TensorFlow's gradients of Network.conv / Network.fc / Network.max_pool, networks/network.py:159-188, 303-310, 392-422):
  *   dz = dy * [y > 0];  dW[r,s,ci,co] = sum_{n,h,w} x[n,h+r-1,w+s-1,ci] * dz[n,h,w,co];  db = sum dz;
  *   dx = conv(dz, W flipped and transposed) = pcnn_conv_bf16_tc on conv.hwio_to_tc_dgrad weights.
- *  pcnn_conv_wgrad_bf16_tc   weight gradient on tcgen05 with BOTH operands MN-major (the reduction index = pixel is the row of
+ *  pcnn_conv_wgrad_bf16_tc   weight gradient on wgmma with BOTH operands MN-major (the reduction index = pixel is the row of
  *      the NHWC activation tiles as TMA delivers them: no transposed copies), split-K over pixel ranges with a fixed-order
  *      reduction; x [B,H,W,Cin], dz [B,H,W,Cout] bf16 -> dW [Cout][ksize*ksize*Cin] f32 (the tensor-core weight layout) =
  *      scale * gradient (+ decay * w when w != NULL: the l2_regularizer term, network.py:171-172).  A fully connected layer is
@@ -269,7 +269,7 @@ int pcnn_conv1_wgrad(const void* img_u8, const float* mean3_host, const void* dz
  *      [num_rois, pooled_h*pooled_w*C] in (h, w, c) order.  f5 [B,H5,W5,C], f4 [B,H4,W4,C] bf16 NHWC; rois
  *      [num_rois, roi_stride] f32 rows [batch, cls, x1,y1,x2,y2,...]; the image index is rois[:,0] - batch_offset
  *      (image shards carry global batch indices); an index outside [0, B) pools nothing (zeros).
- *  pcnn_fc_f16_tc          out = act(A[M,K] @ W[N,K]^T + bias): tcgen05 GEMM, FP16 operands (11-bit mantissa: the 1e-3 quaternion tolerance), FP32 accumulation, split-K
+ *  pcnn_fc_f16_tc          out = act(A[M,K] @ W[N,K]^T + bias): wgmma GEMM, FP16 operands (11-bit mantissa: the 1e-3 quaternion tolerance), FP32 accumulation, split-K
  *      over the grid with a fixed-order reduction (deterministic); A, W fp16 row-major with K contiguous, N % 128 == 0,
  *      K % 64 == 0; rows n_valid..N of W are zero padding; act 0 none / 1 ReLU / 2 tanh; outputs: out_f16 [M, ld_out]
  *      (optional) and / or out_f32 [M, n_valid] (optional).  workspace: pcnn_fc_workspace_bytes(M, N, K).

@@ -22,9 +22,9 @@
  *
  * Parity pinning: the reference ships no golden vectors (SURVEY.md §4).  This
  * oracle is pinned against the reference's own CUDA kernels, compiled unmodified
- * from /root/reference for sm_100a behind a header shim (oracle/ref_shim,
- * oracle/ref_driver.cu -> oracle/_ref/libposecnn_ref.so) and run on the B200 box;
- * tests/golden/ holds vectors produced that way (tests/golden/README.md).
+ * from a checkout of the reference behind a header shim (oracle/ref_shim,
+ * oracle/ref_driver.cu -> oracle/_ref/libposecnn_ref.so) and run on the GPU;
+ * tests/golden/ holds vectors produced that way (tests/golden/make_golden.py).
  */
 #include <float.h>
 #include <math.h>

@@ -1,9 +1,9 @@
 """ctypes front-end of oracle/_ref/libposecnn_ref.so — the reference's OWN CUDA kernels
-(compiled unmodified from /root/reference behind oracle/ref_shim; see oracle/ref_driver.cu).
+(compiled unmodified from a checkout of the reference behind oracle/ref_shim; see oracle/ref_driver.cu).
 
 TEST INFRASTRUCTURE ONLY (second oracle, SURVEY.md §8(c)).  Needs a GPU.  The library is
-built in the build container (`make -C oracle ref`), where /root/reference exists, and
-travels to the GPU box as a built artefact; nothing here reads /root/reference at run time.
+built by `make -C oracle ref` where a checkout of the reference exists; it is used to regenerate
+tests/golden/ (tests/golden/make_golden.py), which the tests compare against.
 """
 from __future__ import annotations
 

@@ -2,7 +2,7 @@
 //
 // TEST INFRASTRUCTURE ONLY.  Each section #includes one of the reference's *_gpu.cu.cc files
 // from where it lies under /root/reference (never copied into this repo) and compiles it
-// unmodified for sm_100a behind oracle/ref_shim.  The result (oracle/_ref/libposecnn_ref.so)
+// unmodified for sm_90a behind oracle/ref_shim.  The result (oracle/_ref/libposecnn_ref.so)
 // is the "second oracle" of SURVEY.md §8(c): it pins the CPU restatement
 // (oracle/posecnn_oracle.c) and produces the golden vectors under tests/golden/.
 // One section per translation unit: compile with -DREF_SECTION=<n> (see oracle/Makefile).

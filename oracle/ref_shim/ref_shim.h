@@ -1,6 +1,6 @@
 // ref_shim.h — minimal stand-ins for the TensorFlow / Eigen declarations that the
 // reference's *_gpu.cu.cc files mention, so that those files compile UNMODIFIED with nvcc
-// for sm_100a (oracle/Makefile `ref` target).  TEST INFRASTRUCTURE ONLY; written from
+// for sm_90a (oracle/Makefile `ref` target).  TEST INFRASTRUCTURE ONLY; written from
 // scratch (the kernels need nothing from TF beyond a stream handle and temp allocations).
 #pragma once
 #include <cuda_runtime.h>

@@ -1,4 +1,4 @@
-"""posecnn_b200 — B200-native (sm_100a) implementation of the PoseCNN hot path.
+"""posecnn_b200 — H100-native (sm_90a) implementation of the PoseCNN hot path.
 
 Sub-packages mirror the reference's op modules one to one (lib/<layer>/<layer>_op.py of
 yuxng/PoseCNN): put this directory on sys.path and `import hough_voting_gpu_layer.

@@ -1,7 +1,7 @@
-"""Build libposecnn_b200.so (hand-written sm_100a CUDA + C ABI) in-tree with nvcc.
+"""Build libposecnn_b200.so (hand-written sm_90a CUDA + C ABI) in-tree with nvcc.
 
-The shared object lands in posecnn_b200/_build/ so that it travels with the source tree
-(it is git-ignored, not gpurun-ignored).  nvcc cross-compiles without a GPU.
+The shared object lands in posecnn_b200/_build/ (git-ignored) next to the sources, so the
+package is importable from the repository tree.  nvcc cross-compiles without a GPU.
 """
 from __future__ import annotations
 
@@ -15,7 +15,7 @@ OUT_DIR = os.path.join(HERE, "_build")
 LIB = os.path.join(OUT_DIR, "libposecnn_b200.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC", "-shared", "--expt-relaxed-constexpr",
 ]
 
@@ -35,7 +35,8 @@ def needs_build() -> bool:
     if not os.path.exists(LIB):
         return True
     t = os.path.getmtime(LIB)
-    deps = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(HERE, "..", "include", "posecnn_b200.h")]
+    deps = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(HERE, "..", "include", "posecnn_b200.h"),
+                                                                  os.path.abspath(__file__)]  # the flags live here
     return any(os.path.getmtime(d) > t for d in deps)
 
 
@@ -58,7 +59,7 @@ def build_native(force: bool = False, verbose: bool = False) -> str:
             raise RuntimeError(f"nvcc failed for {src}:\n{out}")
         if verbose and out:
             print(out)
-    cmd = [_nvcc(), "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB] + objs
+    cmd = [_nvcc(), "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", LIB] + objs
     subprocess.check_call(cmd)
     return LIB
 

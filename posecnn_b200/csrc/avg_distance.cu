@@ -1,4 +1,4 @@
-// avg_distance.cu — Averagedistance (ADD / ADD-S pose loss) for sm_100a.
+// avg_distance.cu — Averagedistance (ADD / ADD-S pose loss) for sm_90a.
 //
 // Behavioural spec: lib/average_distance_loss/average_distance_loss_op_gpu.cu.cc:34-252
 // (per (roi, point) thread, 54-float rotation scratch + [N,P,4C] diff scratch in global

@@ -1,4 +1,4 @@
-// common.cuh — shared helpers for the sm_100a kernels behind include/posecnn_b200.h
+// common.cuh — shared helpers for the sm_90a kernels behind include/posecnn_b200.h
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -35,7 +35,7 @@ inline int check_launch(const char* what)
         }                                  \
     } while (0)
 
-constexpr int kNumSMs = 148;  // B200: 2 dies x 74 SMs
+constexpr int kNumSMs = 132;  // H100 SXM
 
 __host__ __device__ inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 

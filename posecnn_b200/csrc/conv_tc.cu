@@ -1,4 +1,4 @@
-// conv_tc.cu — the VGG16 convolution stack on the sm_100a tensor cores (tcgen05 + TMEM + TMA).
+// conv_tc.cu — the VGG16 convolution stack on the sm_90a tensor cores (wgmma + TMA + mbarrier).
 //
 // Behavioural spec: Network.conv, lib/networks/network.py:159-188 (NHWC x HWIO, SAME padding,
 // stride 1, bias add, optional ReLU) as wired by lib/networks/vgg16_convs.py:80-97, 128-163.
@@ -11,11 +11,11 @@
 //     box {64 ch, 16 w, 8 h, 1 n} of the NHWC activation tensor at the tap's (dy, dx) offset;
 //     out-of-image coordinates are zero-filled by the TMA unit = SAME padding;
 //   * the box lands in shared memory as 128 rows x 128 B with the 128-byte swizzle, which is
-//     exactly the canonical K-major UMMA operand layout, so tcgen05.mma reads it in place;
-//   * accumulators live in TMEM (two stages of BN fp32 columns), the epilogue (bias, ReLU,
-//     bf16 pack) runs out of TMEM while the next tile's MMAs are already being issued;
-//   * warp roles: warps 0-3 epilogue (TMEM lanes 32w..32w+31), warp 4 TMA producer, warp 5
-//     MMA issuer; persistent CTAs, one per SM, static round-robin tile schedule.
+//     exactly the canonical K-major wgmma operand layout, so wgmma reads it in place;
+//   * warp roles: warps 0-7 = two consumer warpgroups (pixel rows 0-63 / 64-127 of the tile): wgmma with the
+//     accumulators in registers, then the epilogue (bias, ReLU, bf16 pack, TMA store) from registers; warp 8 is the
+//     TMA producer, which keeps filling the stage ring during the epilogue.  Persistent CTAs, one per SM, static
+//     round-robin tile schedule.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <stdlib.h>
@@ -29,9 +29,11 @@ namespace pcnn {
 namespace convtc {
 
 constexpr int kTileH = 8, kTileW = 16;                            // 128 output pixels per tile (kTileM, tc_common.cuh)
-static_assert(kTileH * kTileW == kTileM, "pixel tile = UMMA M");
+static_assert(kTileH * kTileW == kTileM, "pixel tile = two wgmma M blocks");
 constexpr int kABytes = kTileM * kKC * 2;                         // 16 KB
-constexpr int kThreadsConv = 192;
+constexpr int kConsumers = 256;                                   // two consumer warpgroups
+constexpr int kProducerWarp = kConsumers / 32;                    // warp 8
+constexpr int kThreadsConv = kConsumers + 32;                     // wgmma kernels get registers per warpgroup: 3 x 128 x 168 fit
 constexpr int kStageBytes = 16 * 1024;                            // epilogue staging: one 64-channel group
 
 struct ConvParams {
@@ -43,6 +45,54 @@ struct ConvParams {
     int pool;                 // 1: the epilogue applies the 2x2 / stride-2 max pool and stores ONLY the pooled tensor
     const float* bias;
 };
+
+__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+
+// a warp of a consumer warpgroup is done with a stage (its wgmma reads of it have completed)
+__device__ __forceinline__ void release(uint64_t* bar, int lane)
+{
+    __syncwarp();
+    if (lane == 0) mbar_arrive(bar);
+}
+
+// 64 channels of the fragment rows (row, row + 8) — the 32 accumulator registers of one 64-column group — plus bias,
+// optional ReLU, bf16 -> the swizzled 128-byte staging rows that the TMA store reads (q = lane % 4)
+__device__ __forceinline__ void stage_rows(uint8_t* ob, const float* a, const float* bias, int relu, int row, int q)
+{
+#pragma unroll
+    for (int i = 0; i < 2; i++) {
+        const int r = row + 8 * i;
+#pragma unroll
+        for (int jj = 0; jj < 8; jj++) {
+            const int c = 8 * jj + 2 * q;
+            float v0 = a[4 * jj + 2 * i] + __ldg(bias + c), v1 = a[4 * jj + 2 * i + 1] + __ldg(bias + c + 1);
+            if (relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+            *reinterpret_cast<uint32_t*>(ob + r * 128 + ((jj ^ (r & 7)) << 4) + 4 * q) = pack_bf16(v0, v1);
+        }
+    }
+}
+
+// fused max_pool 2x2/2 (network.py:303-310) of a staged 8 x 16 tile (row m = 16 h + w), in place: pooled row
+// p = 8 ph + pw is the max of rows 32 ph + 2 pw + {0, 1, 16, 17}.  One 16-byte piece per consumer thread.  max on the
+// bf16 values = bf16 of the fp32 max (rounding is monotone).
+__device__ __forceinline__ void pool_staged(uint8_t* ob, int t)
+{
+    const int p = t >> 3, piece = t & 7;
+    const int m = 32 * (p >> 3) + 2 * (p & 7);
+    const int rows[4] = {m, m + 1, m + 16, m + 17};
+    __nv_bfloat162 v[4];
+    uint4 x = *reinterpret_cast<const uint4*>(ob + rows[0] * 128 + ((piece ^ (rows[0] & 7)) << 4));
+    *reinterpret_cast<uint4*>(v) = x;
+#pragma unroll
+    for (int k = 1; k < 4; k++) {
+        uint4 y = *reinterpret_cast<const uint4*>(ob + rows[k] * 128 + ((piece ^ (rows[k] & 7)) << 4));
+        const __nv_bfloat162* yv = reinterpret_cast<const __nv_bfloat162*>(&y);
+#pragma unroll
+        for (int q = 0; q < 4; q++) v[q] = __hmax2(v[q], yv[q]);
+    }
+    consumer_sync();   // every source row has been read before any pooled row overwrites one
+    *reinterpret_cast<uint4*>(ob + p * 128 + ((piece ^ (p & 7)) << 4)) = *reinterpret_cast<const uint4*>(v);
+}
 
 template <int BN>
 struct SmemPlan {
@@ -65,32 +115,21 @@ k_conv_tc(const __grid_constant__ CUtensorMap map_in, const __grid_constant__ CU
     uint8_t* out_stage = smem + Plan::kStages * Plan::kStage;
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + Plan::kBarOff);
     uint64_t* empty = full + Plan::kStages;
-    uint64_t* tfull = empty + Plan::kStages;
-    uint64_t* tempty = tfull + 2;
-    uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(tempty + 2);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int kchunks = p.Cin / kKC;
     const int ksteps = p.taps * kchunks;
-    constexpr uint32_t kTmemCols = 2 * BN >= 32 ? 2 * BN : 32;
 
-    if (warp == 4 && lane == 0) {
+    if (warp == kProducerWarp && lane == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_in) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_out) : "memory");
-    }
-    if (warp == 5 && lane == 0) {
-        for (int s = 0; s < Plan::kStages; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        for (int a = 0; a < 2; a++) { mbar_init(&tfull[a], 1); mbar_init(&tempty[a], 4); }
+        for (int s = 0; s < Plan::kStages; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], kConsumers / 32); }
         fence_barrier_init();
     }
-    if (warp == 4) tmem_alloc(tmem_holder, kTmemCols);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_holder;
 
-    if (warp == 4) {
+    if (warp == kProducerWarp) {
         // ===================== TMA producer =====================
         if (elect_one()) {
             int stage = 0;
@@ -115,101 +154,54 @@ k_conv_tc(const __grid_constant__ CUtensorMap map_in, const __grid_constant__ CU
                 }
             }
         }
-    } else if (warp == 5) {
-        // ===================== MMA issuer =====================
-        if (elect_one()) {
-            constexpr uint32_t idesc = make_idesc(BN);
-            int stage = 0;
-            uint32_t phase = 0;
-            int it = 0;
-            for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, it++) {
-                const int acc = it & 1;
-                const uint32_t acc_phase = (it >> 1) & 1;
-                mbar_wait(&tempty[acc], acc_phase ^ 1);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + acc * BN;
-                for (int ks = 0; ks < ksteps; ks++) {
-                    mbar_wait(&full[stage], phase);
-                    tc_fence_after();
-                    const uint32_t sa = smem_u32(smem + stage * Plan::kStage);
-                    const uint64_t da = make_desc(sa), db = make_desc(sa + kABytes);
-#pragma unroll
-                    for (int k = 0; k < kKC / 16; k++)
-                        umma_bf16(d_tmem, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), idesc, (ks | k) != 0);
-                    umma_commit(&empty[stage]);  // smem slot free once these MMAs have read it
-                    if (++stage == Plan::kStages) { stage = 0; phase ^= 1; }
-                }
-                umma_commit(&tfull[acc]);  // accumulator complete
-            }
-        }
     } else {
-        // ===================== epilogue warps 0..3 =====================
-        int it = 0;
-        int obuf = 0;
-        const int row = warp * 32 + lane;  // pixel of the tile = TMEM lane
-        for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, it++) {
+        // ===================== consumer warpgroups: MMA + epilogue =====================
+        const int wg = warp >> 2, wq = warp & 3;
+        const int row = wg * 64 + wq * 16 + (lane >> 2);   // first of the two tile rows (pixels) this thread holds
+        float acc[BN / 2];
+        int stage = 0, obuf = 0;
+        uint32_t phase = 0;
+        for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
             const int nt = tile % p.n_tiles_n;
             int rest = tile / p.n_tiles_n;
             const int tw = rest % p.tiles_w; rest /= p.tiles_w;
             const int th = rest % p.tiles_h;
             const int img = rest / p.tiles_h;
             const int h0 = th * p.tile_h, w0 = tw * p.tile_w, n0 = nt * BN;
-            const int acc = it & 1;
-            const uint32_t acc_phase = (it >> 1) & 1;
-            mbar_wait(&tfull[acc], acc_phase);
-            tc_fence_after();
-            const uint32_t t_addr = tmem_base + ((uint32_t)(warp * 32) << 16) + acc * BN;
-#pragma unroll 1
+            int prev = -1;
+            for (int ks = 0; ks < ksteps; ks++) {
+                mbar_wait(&full[stage], phase);
+                const uint32_t sa = smem_u32(smem + stage * Plan::kStage);
+                const uint64_t da = make_desc(sa + wg * 64 * 128), db = make_desc(sa + kABytes);
+                acc_fence<BN / 2>(acc);
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < kKC / 16; k++) wgmma<BN, 0, 0, 0>(acc, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (ks | k) != 0);
+                wgmma_commit();
+                acc_fence<BN / 2>(acc);
+                if (prev >= 0) {   // the previous stage's MMAs are complete: its slot may be refilled
+                    wgmma_wait<1>();
+                    release(&empty[prev], lane);
+                }
+                prev = stage;
+                if (++stage == Plan::kStages) { stage = 0; phase ^= 1; }
+            }
+            wgmma_wait<0>();
+            acc_fence<BN / 2>(acc);
+            release(&empty[prev], lane);
+#pragma unroll
             for (int g = 0; g < BN / 64; g++) {
                 // staging buffer obuf must have been read out by the TMA store issued two groups ago
                 if (threadIdx.x == 0) tma_store_wait_read<1>();
-                asm volatile("bar.sync 1, 128;" ::: "memory");
+                consumer_sync();
                 uint8_t* ob = out_stage + obuf * kStageBytes;
-#pragma unroll
-                for (int half = 0; half < 2; half++) {
-                    uint32_t r[32];
-                    tmem_ld_32x32(t_addr + g * 64 + half * 32, r);
-                    tmem_ld_wait();
-                    const float* bias = p.bias + n0 + g * 64 + half * 32;
-#pragma unroll
-                    for (int j = 0; j < 4; j++) {  // four 16-byte pieces = 8 channels each
-                        uint32_t packed[4];
-#pragma unroll
-                        for (int q = 0; q < 4; q++) {
-                            float v0 = __uint_as_float(r[j * 8 + q * 2]) + __ldg(bias + j * 8 + q * 2);
-                            float v1 = __uint_as_float(r[j * 8 + q * 2 + 1]) + __ldg(bias + j * 8 + q * 2 + 1);
-                            if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-                            __nv_bfloat162 b2 = __floats2bfloat162_rn(v0, v1);
-                            packed[q] = *reinterpret_cast<uint32_t*>(&b2);
-                        }
-                        const int piece = half * 4 + j;  // 16-byte piece index within the 128-byte row
-                        if (!p.pool) {
-                            uint4* dst = reinterpret_cast<uint4*>(ob + row * 128 + ((piece ^ (row & 7)) << 4));
-                            *dst = make_uint4(packed[0], packed[1], packed[2], packed[3]);
-                        } else {
-                            // fused max_pool 2x2/2 (network.py:303-310): tile row m = 16 h + w, a warp holds two image
-                            // rows; the 2x2 window of (h even, w even) lives in lanes l, l^1, l^16, l^17.  max on the
-                            // bf16 values = bf16 of the fp32 max (rounding is monotone).
-#pragma unroll
-                            for (int q = 0; q < 4; q++) {
-                                __nv_bfloat162 v = *reinterpret_cast<__nv_bfloat162*>(&packed[q]);
-                                uint32_t o1 = __shfl_xor_sync(0xffffffffu, packed[q], 1);
-                                v = __hmax2(v, *reinterpret_cast<__nv_bfloat162*>(&o1));
-                                uint32_t vv = *reinterpret_cast<uint32_t*>(&v);
-                                uint32_t o2 = __shfl_xor_sync(0xffffffffu, vv, 16);
-                                v = __hmax2(v, *reinterpret_cast<__nv_bfloat162*>(&o2));
-                                packed[q] = *reinterpret_cast<uint32_t*>(&v);
-                            }
-                            if ((lane & 17) == 0) {
-                                const int prow = warp * 8 + (lane >> 1);  // pooled tile: 4 rows x 8 cols, row = ph * 8 + pw
-                                uint4* dst = reinterpret_cast<uint4*>(ob + prow * 128 + ((piece ^ (prow & 7)) << 4));
-                                *dst = make_uint4(packed[0], packed[1], packed[2], packed[3]);
-                            }
-                        }
-                    }
+                stage_rows(ob, acc + g * 32, p.bias + n0 + g * 64, p.relu, row, lane & 3);
+                if (p.pool) {
+                    consumer_sync();
+                    pool_staged(ob, threadIdx.x);
                 }
                 fence_proxy_async();
-                asm volatile("bar.sync 1, 128;" ::: "memory");
+                consumer_sync();
                 if (threadIdx.x == 0) {
                     if (!p.pool) tma_store_4d(&map_out, ob, n0 + g * 64, w0, h0, img);
                     else tma_store_4d(&map_out, ob, n0 + g * 64, w0 >> 1, h0 >> 1, img);
@@ -217,43 +209,35 @@ k_conv_tc(const __grid_constant__ CUtensorMap map_in, const __grid_constant__ CU
                 }
                 obuf ^= 1;
             }
-            // all TMEM reads of this accumulator stage are done
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tempty[acc]);
         }
         if (threadIdx.x == 0) tma_store_wait_all();
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 4) tmem_dealloc(tmem_base, kTmemCols);
 }
 
 // ---------------------------------------------------------------------------------------------
 // Row mode for the K-small layers (conv1_2, conv2_x: Cin, Cout <= 128), which are bound by L2 -> SM operand
-// traffic in the tile kernel (every tap re-fetches its A tile; profiles/r01_conv_tile_kernel_ncu_full_early.txt).
+// traffic in the tile kernel (every tap re-fetches its A tile).
 // A work item is TWO output rows x 128 pixels of one image:
 //   * per 64-channel chunk ONE TMA box {64 ch, 130 px, 4 rows} (halo included) is loaded; the A operand of
 //     tap (r, s) for output row j is the 128 consecutive patch rows starting at ((r + j) * 130 + s): a
-//     row-shifted view of the same shared-memory patch (the UMMA swizzle is a function of the shared-memory
-//     address, so a start address that is 128-B but not 1024-B aligned needs no descriptor change — checked on
-//     hardware with tools/probe/umma_probe.cu);
-//   * every weight stage feeds both output rows (two accumulators), halving the weight traffic as well;
+//     row-shifted view of the same shared-memory patch (the swizzle is a function of the shared-memory address, so
+//     a start address that is 128-B but not 1024-B aligned needs no descriptor change);
+//   * every weight stage feeds both output rows (two register accumulators), halving the weight traffic as well;
 //   * the two rows of a pair are exactly the rows a 2x2 max pool combines, so the pool stays fused: vertical
-//     max in registers (both rows live in the same TMEM lane), horizontal max by shuffle.
+//     max in registers (the same thread holds the same pixel of both rows), horizontal max by shuffle.
 // Operand bytes per 128 output pixels drop from 9 * (16 + BN/8) KB to (32.5 + 4.5 * BN/8) KB per chunk.
 // ---------------------------------------------------------------------------------------------
 constexpr int kRowPx = 128, kPatchW = 130, kPatchH = 4;
 constexpr int kPatchBytes = kPatchW * kPatchH * 128;  // 66,560 = 65 * 1024
 constexpr int kRowAStages = 2;
 
-// RESB (Cin = 64, BN = 64 only): the nine 8-KB weight slices of the CTA's N tile stay resident in shared memory for
-// the whole kernel (a 48-KB ring cannot keep enough weight bytes in flight to hide the L2 latency); every CTA keeps
-// one N tile (nt = blockIdx.x % n_tiles_n).  The epilogue staging shrinks to 16 KB to make room.
+// BN = 64.  RESB (Cin = 64 only): the nine 8-KB weight slices of the CTA's N tile stay resident in shared memory for
+// the whole kernel; every CTA keeps one N tile (nt = blockIdx.x % n_tiles_n).  The epilogue staging shrinks to 16 KB
+// to make room.
 template <int BN, bool RESB>
 struct RowPlan {
     static constexpr int kBBytes = BN * 128;
-    static constexpr int kBStages = RESB ? 9 : (BN == 64 ? 6 : 3);
+    static constexpr int kBStages = RESB ? 9 : 6;
     static constexpr int kBOff = kRowAStages * kPatchBytes;
     static constexpr int kOutOff = kBOff + kBStages * kBBytes;
     static constexpr int kOutBytes = RESB ? kStageBytes : 2 * kStageBytes;
@@ -268,7 +252,7 @@ k_conv_row2(const __grid_constant__ CUtensorMap map_in /*box {64,130,4,1}*/, con
             const ConvParams p)
 {
     using Plan = RowPlan<BN, RESB>;
-    static_assert(!RESB || BN == 64, "resident weights: BN = 64 only");
+    static_assert(BN == 64, "row mode: 64-channel N tiles");
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     uint8_t* sB = smem + Plan::kBOff;
@@ -277,48 +261,35 @@ k_conv_row2(const __grid_constant__ CUtensorMap map_in /*box {64,130,4,1}*/, con
     uint64_t* emptyA = fullA + kRowAStages;
     uint64_t* fullB = emptyA + kRowAStages;
     uint64_t* emptyB = fullB + Plan::kBStages;
-    uint64_t* tfull = emptyB + Plan::kBStages;
-    uint64_t* tempty = tfull + 2;
-    uint64_t* wbar = tempty + 2;
-    uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(wbar + 1);
+    uint64_t* wbar = emptyB + Plan::kBStages;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int kchunks = p.Cin / kKC;
-    constexpr uint32_t kTmemCols = 4 * BN;
     // work items of this CTA: RESB -> fixed N tile, spatial tiles strided; otherwise all (spatial, N) tiles strided
     const int tile0 = RESB ? blockIdx.x / p.n_tiles_n : blockIdx.x;
     const int tstep = RESB ? gridDim.x / p.n_tiles_n : gridDim.x;
     const int tcount = RESB ? p.total_tiles / p.n_tiles_n : p.total_tiles;
-    const int nt_fixed = blockIdx.x % p.n_tiles_n;  // 2 accumulator stages x 2 output rows
+    const int nt_fixed = blockIdx.x % p.n_tiles_n;
     // tiles_h = row pairs, tiles_w = 128-pixel segments
-    if (warp == 4 && lane == 0) {
+    if (warp == kProducerWarp && lane == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_in) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_out) : "memory");
-    }
-    if (warp == 5 && lane == 0) {
-        for (int s = 0; s < kRowAStages; s++) { mbar_init(&fullA[s], 1); mbar_init(&emptyA[s], 1); }
-        for (int s = 0; s < Plan::kBStages; s++) { mbar_init(&fullB[s], 1); mbar_init(&emptyB[s], 1); }
-        for (int a = 0; a < 2; a++) { mbar_init(&tfull[a], 1); mbar_init(&tempty[a], 4); }
+        for (int s = 0; s < kRowAStages; s++) { mbar_init(&fullA[s], 1); mbar_init(&emptyA[s], kConsumers / 32); }
+        for (int s = 0; s < Plan::kBStages; s++) { mbar_init(&fullB[s], 1); mbar_init(&emptyB[s], kConsumers / 32); }
         mbar_init(wbar, 1);
         fence_barrier_init();
     }
-    if (warp == 4) tmem_alloc(tmem_holder, kTmemCols);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_holder;
 
-    if (warp == 4) {
+    if (warp == kProducerWarp) {
         // ===================== TMA producer =====================
         if (elect_one()) {
             int sa = 0, sb = 0;
             uint32_t pa = 0, pb = 0;
             if (RESB) {
                 mbar_arrive_expect_tx(wbar, 9 * Plan::kBBytes);
-                // resident slices in (s, r) order: the slices of taps (r - 1, s) and (r, s) are adjacent and form ONE
-                // 128-row B tile for the merged two-row MMA below
-                for (int tap = 0; tap < 9; tap++)
-                    tma_load_2d(sB + ((tap % 3) * 3 + tap / 3) * Plan::kBBytes, &map_w, wbar, tap * p.Cin, nt_fixed * BN);
+                for (int tap = 0; tap < 9; tap++)      // resident slices in tap order
+                    tma_load_2d(sB + tap * Plan::kBBytes, &map_w, wbar, tap * p.Cin, nt_fixed * BN);
             }
             for (int tile = tile0; tile < tcount; tile += tstep) {
                 const int nt = RESB ? nt_fixed : tile % p.n_tiles_n;
@@ -343,167 +314,130 @@ k_conv_row2(const __grid_constant__ CUtensorMap map_in /*box {64,130,4,1}*/, con
                 }
             }
         }
-    } else if (warp == 5) {
-        // ===================== MMA issuer =====================
-        if (elect_one()) {
-            constexpr uint32_t idesc = make_idesc(BN);
-            int sa = 0, sb = 0;
-            uint32_t pa = 0, pb = 0;
-            int it = 0;
-            if (RESB) mbar_wait(wbar, 0);
-            for (int tile = tile0; tile < tcount; tile += tstep, it++) {
-                const int acc = it & 1;
-                const uint32_t acc_phase = (it >> 1) & 1;
-                mbar_wait(&tempty[acc], acc_phase ^ 1);
-                tc_fence_after();
-                for (int c = 0; c < kchunks; c++) {
-                    mbar_wait(&fullA[sa], pa);
-                    const uint32_t a_base = smem_u32(smem + sa * kPatchBytes);
-                    if (RESB) {
-                        // The A operand of tap (r, s) for output row j is patch row rho = r + j: rows 0 and 1 of the pair
-                        // read the SAME A tile for rho = 1, 2 (taps r = rho and r = rho - 1).  One N = 2 BN MMA against
-                        // the two adjacent weight slices [W(rho-1, s) | W(rho, s)] writes [acc(row 1) | acc(row 0)]:
-                        // A is fetched once instead of twice (with N = 64 the MMA is bound by the 128 B/clk shared-memory
-                        // operand fetch, ncu: 65 clk per MMA for 33 clk of math).  rho = 1 goes first so that the first
-                        // MMA initialises both accumulators.
-                        tc_fence_after();
-                        constexpr uint32_t idesc2 = make_idesc(2 * BN);
-                        const uint32_t d_pair = tmem_base + (acc * 2) * BN;      // [row 1 | row 0]
-#pragma unroll
-                        for (int o = 0; o < 4; o++) {
-                            const int rho = o == 0 ? 1 : (o == 1 ? 2 : (o == 2 ? 0 : 3));
-#pragma unroll
-                            for (int s3 = 0; s3 < 3; s3++) {
-                                const uint64_t da = make_desc(a_base + (uint32_t)((rho * kPatchW + s3) * 128));
-                                if (rho == 1 || rho == 2) {
-                                    const uint64_t db = make_desc(smem_u32(sB + (s3 * 3 + rho - 1) * Plan::kBBytes));
-#pragma unroll
-                                    for (int k = 0; k < kKC / 16; k++)
-                                        umma_bf16(d_pair, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), idesc2, (c | o | s3 | k) != 0);
-                                } else {
-                                    // rho = 0: row 0 only, tap r = 0;  rho = 3: row 1 only, tap r = 2
-                                    const uint64_t db = make_desc(smem_u32(sB + (s3 * 3 + (rho == 0 ? 0 : 2)) * Plan::kBBytes));
-                                    const uint32_t d1 = d_pair + (rho == 0 ? BN : 0);
-#pragma unroll
-                                    for (int k = 0; k < kKC / 16; k++) umma_bf16(d1, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), idesc, 1);
-                                }
-                            }
-                        }
-                    }
-                    for (int tap = 0; tap < (RESB ? 0 : 9); tap++) {
-                        if (!RESB) mbar_wait(&fullB[sb], pb);
-                        tc_fence_after();
-                        const int r = tap / 3, s = tap - 3 * r;
-                        const uint64_t db = make_desc(smem_u32(sB + (RESB ? tap : sb) * Plan::kBBytes));
-#pragma unroll
-                        for (int j = 0; j < 2; j++) {
-                            const uint64_t da = make_desc(a_base + (uint32_t)(((r + j) * kPatchW + s) * 128));
-                            const uint32_t d_tmem = tmem_base + (acc * 2 + j) * BN;
-#pragma unroll
-                            for (int k = 0; k < kKC / 16; k++)
-                                umma_bf16(d_tmem, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), idesc, (c | tap | k) != 0);
-                        }
-                        if (!RESB) {
-                            umma_commit(&emptyB[sb]);
-                            if (++sb == Plan::kBStages) { sb = 0; pb ^= 1; }
-                        }
-                    }
-                    umma_commit(&emptyA[sa]);
-                    if (++sa == kRowAStages) { sa = 0; pa ^= 1; }
-                }
-                umma_commit(&tfull[acc]);
-            }
-        }
     } else {
-        // ===================== epilogue warps 0..3: thread = pixel x0 + row of both output rows =====================
-        int it = 0, obuf = 0;
-        const int row = warp * 32 + lane;
-        for (int tile = tile0; tile < tcount; tile += tstep, it++) {
+        // ===================== consumer warpgroups: thread = pixels (row, row + 8) of both output rows =====================
+        constexpr int kH = BN / 2;                  // accumulator registers of one output row (m64nBN): row j at acc[j * kH]
+        const int wg = warp >> 2, wq = warp & 3;
+        const int row = wg * 64 + wq * 16 + (lane >> 2);
+        float acc[2 * kH];
+        int sa = 0, sb = 0, obuf = 0;
+        uint32_t pa = 0, pb = 0;
+        if (RESB) mbar_wait(wbar, 0);
+        for (int tile = tile0; tile < tcount; tile += tstep) {
             const int nt = RESB ? nt_fixed : tile % p.n_tiles_n;
             int rest = RESB ? tile : tile / p.n_tiles_n;
             const int tw = rest % p.tiles_w; rest /= p.tiles_w;
             const int yp = rest % p.tiles_h;
             const int img = rest / p.tiles_h;
             const int y0 = 2 * yp, x0 = tw * kRowPx, n0 = nt * BN;
-            const int acc = it & 1;
-            const uint32_t acc_phase = (it >> 1) & 1;
-            mbar_wait(&tfull[acc], acc_phase);
-            tc_fence_after();
-            const uint32_t t_lane = tmem_base + ((uint32_t)(warp * 32) << 16);
-            if (!p.pool) {
-#pragma unroll 1
-                for (int jg = 0; jg < 2 * (BN / 64); jg++) {
-                    const int j = jg / (BN / 64), g = jg % (BN / 64);
-                    if (threadIdx.x == 0) { if (RESB) tma_store_wait_read<0>(); else tma_store_wait_read<1>(); }
-                    asm volatile("bar.sync 1, 128;" ::: "memory");
-                    uint8_t* ob = out_stage + (RESB ? 0 : obuf * kStageBytes);
+            for (int c = 0; c < kchunks; c++) {
+                mbar_wait(&fullA[sa], pa);
+                const uint32_t a_base = smem_u32(smem + sa * kPatchBytes) + wg * 64 * 128;
+                if constexpr (RESB) {
+                    // weights resident: all nine taps x two rows in one commit group, same MMA shape throughout.  The A operand
+                    // of tap (r, s) for output row j is patch row rho = r + j; taps are issued by patch row in the order
+                    // rho = 1, 2, 0, 3 (both rows read rows 1 and 2), which fixes the accumulation order of every output.
+                    acc_fence<2 * kH>(acc);
+                    wgmma_fence();
 #pragma unroll
-                    for (int half = 0; half < 2; half++) {
-                        uint32_t rr[32];
-                        tmem_ld_32x32(t_lane + (acc * 2 + (RESB ? 1 - j : j)) * BN + g * 64 + half * 32, rr);   // RESB: [row 1 | row 0]
-                        tmem_ld_wait();
-                        const float* bias = p.bias + n0 + g * 64 + half * 32;
+                    for (int o = 0; o < 4; o++) {
+                        const int rho = o == 0 ? 1 : (o == 1 ? 2 : (o == 2 ? 0 : 3));
 #pragma unroll
-                        for (int q4 = 0; q4 < 4; q4++) {
-                            uint32_t packed[4];
+                        for (int s3 = 0; s3 < 3; s3++) {
+                            const uint64_t da = make_desc(a_base + (uint32_t)((rho * kPatchW + s3) * 128));
 #pragma unroll
-                            for (int q = 0; q < 4; q++) {
-                                float v0 = __uint_as_float(rr[q4 * 8 + q * 2]) + __ldg(bias + q4 * 8 + q * 2);
-                                float v1 = __uint_as_float(rr[q4 * 8 + q * 2 + 1]) + __ldg(bias + q4 * 8 + q * 2 + 1);
-                                if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-                                __nv_bfloat162 b2 = __floats2bfloat162_rn(v0, v1);
-                                packed[q] = *reinterpret_cast<uint32_t*>(&b2);
+                            for (int j = 0; j < 2; j++) {
+                                const int r = rho - j;
+                                if (r < 0 || r > 2) continue;
+                                const uint64_t db = make_desc(smem_u32(sB + (r * 3 + s3) * Plan::kBBytes));
+#pragma unroll
+                                for (int k = 0; k < kKC / 16; k++)
+                                    wgmma<BN, 0, 0, 0>(acc + j * kH, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (c | o | s3 | k) != 0);
                             }
-                            const int piece = half * 4 + q4;
-                            *reinterpret_cast<uint4*>(ob + row * 128 + ((piece ^ (row & 7)) << 4)) = make_uint4(packed[0], packed[1], packed[2], packed[3]);
                         }
                     }
-                    fence_proxy_async();
-                    asm volatile("bar.sync 1, 128;" ::: "memory");
-                    if (threadIdx.x == 0) {
-                        tma_store_4d(&map_out, ob, n0 + g * 64, x0, y0 + j, img);
-                        tma_store_commit();
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    acc_fence<2 * kH>(acc);
+                } else {
+                    int prevb = -1;
+                    for (int tap = 0; tap < 9; tap++) {
+                        mbar_wait(&fullB[sb], pb);
+                        const int r = tap / 3, s = tap - 3 * r;
+                        const uint64_t db = make_desc(smem_u32(sB + sb * Plan::kBBytes));
+                        acc_fence<2 * kH>(acc);
+                        wgmma_fence();
+#pragma unroll
+                        for (int j = 0; j < 2; j++) {
+                            const uint64_t da = make_desc(a_base + (uint32_t)(((r + j) * kPatchW + s) * 128));
+#pragma unroll
+                            for (int k = 0; k < kKC / 16; k++)
+                                wgmma<BN, 0, 0, 0>(acc + j * kH, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (c | tap | k) != 0);
+                        }
+                        wgmma_commit();
+                        acc_fence<2 * kH>(acc);
+                        if (prevb >= 0) {
+                            wgmma_wait<1>();
+                            release(&emptyB[prevb], lane);
+                        }
+                        prevb = sb;
+                        if (++sb == Plan::kBStages) { sb = 0; pb ^= 1; }
                     }
-                    obuf ^= 1;
+                    wgmma_wait<0>();
+                    acc_fence<2 * kH>(acc);
+                    release(&emptyB[prevb], lane);
+                }
+                release(&emptyA[sa], lane);
+                if (++sa == kRowAStages) { sa = 0; pa ^= 1; }
+            }
+            if (!p.pool) {
+#pragma unroll
+                for (int j = 0; j < 2; j++) {
+#pragma unroll
+                    for (int g = 0; g < BN / 64; g++) {
+                        if (threadIdx.x == 0) { if (RESB) tma_store_wait_read<0>(); else tma_store_wait_read<1>(); }
+                        consumer_sync();
+                        uint8_t* ob = out_stage + (RESB ? 0 : obuf * kStageBytes);
+                        stage_rows(ob, acc + j * kH + g * 32, p.bias + n0 + g * 64, p.relu, row, lane & 3);
+                        fence_proxy_async();
+                        consumer_sync();
+                        if (threadIdx.x == 0) {
+                            tma_store_4d(&map_out, ob, n0 + g * 64, x0, y0 + j, img);
+                            tma_store_commit();
+                        }
+                        obuf ^= 1;
+                    }
                 }
             } else {
-#pragma unroll 1
+#pragma unroll
                 for (int g = 0; g < BN / 64; g++) {
                     if (threadIdx.x == 0) tma_store_wait_read<1>();
-                    asm volatile("bar.sync 1, 128;" ::: "memory");
+                    consumer_sync();
                     uint8_t* ob = out_stage + obuf * (RESB ? kStageBytes / 2 : kStageBytes);  // pooled tile: 64 rows = 8 KB
+                    const float* a0 = acc + g * 32;
+                    const float* a1 = acc + kH + g * 32;
+                    const float* bias = p.bias + n0 + g * 64;
+                    const int q = lane & 3;
 #pragma unroll
-                    for (int half = 0; half < 2; half++) {
-                        uint32_t r0[32], r1[32];
-                        tmem_ld_32x32(t_lane + (acc * 2 + 0) * BN + g * 64 + half * 32, r0);
-                        tmem_ld_32x32(t_lane + (acc * 2 + 1) * BN + g * 64 + half * 32, r1);
-                        tmem_ld_wait();
-                        const float* bias = p.bias + n0 + g * 64 + half * 32;
+                    for (int i = 0; i < 2; i++) {
+                        const int r = row + 8 * i;
+                        const int prow = r >> 1;  // pooled pixel within the 64-wide pooled segment
 #pragma unroll
-                        for (int q4 = 0; q4 < 4; q4++) {
-                            uint32_t packed[4];
-#pragma unroll
-                            for (int q = 0; q < 4; q++) {
-                                const float b0 = __ldg(bias + q4 * 8 + q * 2), b1 = __ldg(bias + q4 * 8 + q * 2 + 1);
-                                // vertical max of the pair (same bias, monotone ReLU / rounding: order is irrelevant)
-                                float v0 = fmaxf(__uint_as_float(r0[q4 * 8 + q * 2]), __uint_as_float(r1[q4 * 8 + q * 2])) + b0;
-                                float v1 = fmaxf(__uint_as_float(r0[q4 * 8 + q * 2 + 1]), __uint_as_float(r1[q4 * 8 + q * 2 + 1])) + b1;
-                                if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-                                __nv_bfloat162 b2 = __floats2bfloat162_rn(v0, v1);
-                                uint32_t pk = *reinterpret_cast<uint32_t*>(&b2);
-                                uint32_t o1 = __shfl_xor_sync(0xffffffffu, pk, 1);  // horizontal neighbour x ^ 1
-                                b2 = __hmax2(b2, *reinterpret_cast<__nv_bfloat162*>(&o1));
-                                packed[q] = *reinterpret_cast<uint32_t*>(&b2);
-                            }
-                            if ((lane & 1) == 0) {
-                                const int prow = row >> 1;  // pooled pixel within the 64-wide pooled segment
-                                const int piece = half * 4 + q4;
-                                *reinterpret_cast<uint4*>(ob + prow * 128 + ((piece ^ (prow & 7)) << 4)) = make_uint4(packed[0], packed[1], packed[2], packed[3]);
-                            }
+                        for (int jj = 0; jj < 8; jj++) {
+                            const int c = 8 * jj + 2 * q;
+                            // vertical max of the pair (same bias, monotone ReLU / rounding: order is irrelevant)
+                            float v0 = fmaxf(a0[4 * jj + 2 * i], a1[4 * jj + 2 * i]) + __ldg(bias + c);
+                            float v1 = fmaxf(a0[4 * jj + 2 * i + 1], a1[4 * jj + 2 * i + 1]) + __ldg(bias + c + 1);
+                            if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+                            uint32_t pk = pack_bf16(v0, v1);
+                            uint32_t o1 = __shfl_xor_sync(0xffffffffu, pk, 4);  // horizontal neighbour: pixel r ^ 1
+                            __nv_bfloat162 m2 = __hmax2(*reinterpret_cast<__nv_bfloat162*>(&pk), *reinterpret_cast<__nv_bfloat162*>(&o1));
+                            if ((lane & 4) == 0)
+                                *reinterpret_cast<__nv_bfloat162*>(ob + prow * 128 + ((jj ^ (prow & 7)) << 4) + 4 * q) = m2;
                         }
                     }
                     fence_proxy_async();
-                    asm volatile("bar.sync 1, 128;" ::: "memory");
+                    consumer_sync();
                     if (threadIdx.x == 0) {
                         tma_store_4d(&map_out, ob, n0 + g * 64, x0 >> 1, y0 >> 1, img);
                         tma_store_commit();
@@ -511,31 +445,24 @@ k_conv_row2(const __grid_constant__ CUtensorMap map_in /*box {64,130,4,1}*/, con
                     obuf ^= 1;
                 }
             }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tempty[acc]);
         }
         if (threadIdx.x == 0) tma_store_wait_all();
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 4) tmem_dealloc(tmem_base, kTmemCols);
 }
 
 // ---------------------------------------------------------------------------------------------
 // First layer (conv1_1, Cin = 3, K = 27 -> 32) on the tensor cores with the im2col done in shared memory:
 // warps 8-23 (four groups, round-robin over tiles) build the A tile of an 8x16 pixel tile straight from the uint8 / f32
 // image (pre-processing `BGR - PIXEL_MEANS` fused, zero outside the image = SAME padding) in the swizzled K-major
-// layout, warp 24 issues two K = 16 UMMAs per tile against the resident 64 x 64 weight tile, warps 0-7 are two
-// epilogue groups, one per TMEM accumulator.  No im2col tensor ever exists in HBM.
-// The layer is a 1.26 GB write with almost no math: per tile the builder (27 dependent-free byte loads, ~1 us) and
-// the epilogue (TMEM load -> pack -> TMA store) are latency chains, so the kernel keeps four builds and two
-// epilogues in flight per SM (ncu on the 2-builder / 1-epilogue version: issue slots 44 % busy, 0.9 us per tile).
+// layout; warps 0-7 are two consumer warpgroups that take the tiles alternately: per tile two halves of 64 pixels,
+// each two K = 16 wgmmas against the resident 64 x 64 weight tile, then bf16 pack and TMA store.  No im2col tensor
+// ever exists in HBM.
+// The layer is a large write with almost no math: per tile the builder (27 dependent-free byte loads) and the
+// epilogue are latency chains, so the kernel keeps four builds and two epilogues in flight per SM.
 // ---------------------------------------------------------------------------------------------
 constexpr int kC1Stages = 6;
-constexpr int kC1EpiGroups = 2, kC1BuildGroups = 4, kC1Accs = 4;
-constexpr int kC1Threads = 128 * (kC1EpiGroups + kC1BuildGroups) + 32;  // 8 epilogue warps, 16 A-builder warps, 1 MMA warp
-constexpr int kC1MmaWarp = 4 * (kC1EpiGroups + kC1BuildGroups);
+constexpr int kC1EpiGroups = 2, kC1BuildGroups = 4;
+constexpr int kC1Threads = 128 * (kC1EpiGroups + kC1BuildGroups);  // 8 consumer warps, 16 A-builder warps
 constexpr int kC1PatchWords = 10 * 16;   // raw uint8 input patch of a tile: 10 rows x 14 words (+2 pad), per builder group x 2 buffers
 constexpr int kC1PatchOff = kC1Stages * kABytes + 64 * 128 + kC1EpiGroups * 2 * kStageBytes;
 constexpr int kC1BarOff = kC1PatchOff + kC1BuildGroups * 2 * kC1PatchWords * 4;
@@ -558,28 +485,19 @@ k_conv1_tc(const TIn* __restrict__ in, const __grid_constant__ CUtensorMap map_w
     uint8_t* out_stage = sb + 64 * 128;
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + kC1BarOff);
     uint64_t* empty = full + kC1Stages;
-    uint64_t* tfull = empty + kC1Stages;
-    uint64_t* tempty = tfull + kC1Accs;
-    uint64_t* wbar = tempty + kC1Accs;
-    uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(wbar + 1);
+    uint64_t* wbar = empty + kC1Stages;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    constexpr uint32_t kTmemCols = kC1Accs * BN;
 
-    if (warp == kC1MmaWarp && lane == 0) {
+    if (threadIdx.x == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_out) : "memory");
-        for (int s = 0; s < kC1Stages; s++) { mbar_init(&full[s], 4); mbar_init(&empty[s], 1); }
-        for (int a = 0; a < kC1Accs; a++) { mbar_init(&tfull[a], 1); mbar_init(&tempty[a], 4); }
+        for (int s = 0; s < kC1Stages; s++) { mbar_init(&full[s], 4); mbar_init(&empty[s], 4); }
         mbar_init(wbar, 1);
         fence_barrier_init();
     }
-    if (warp == kC1MmaWarp) tmem_alloc(tmem_holder, kTmemCols);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_holder;
 
-    if (warp >= 4 * kC1EpiGroups && warp < kC1MmaWarp) {
+    if (warp >= 4 * kC1EpiGroups) {
         // ===================== A builders: one tile row (pixel) per thread; the groups take tiles round-robin =====================
         const int group = (threadIdx.x - 128 * kC1EpiGroups) >> 7;
         const int r = (threadIdx.x - 128 * kC1EpiGroups) & 127;
@@ -698,93 +616,69 @@ k_conv1_tc(const TIn* __restrict__ in, const __grid_constant__ CUtensorMap map_w
             __syncwarp();
             if (lane == 0) mbar_arrive(&full[stage]);
         }
-    } else if (warp == kC1MmaWarp) {
-        // ===================== MMA issuer (+ one-time weight load) =====================
-        if (elect_one()) {
-            mbar_arrive_expect_tx(wbar, 64 * 128);
-            tma_load_2d(sb, &map_w, wbar, 0, 0);
-        }
-        __syncwarp();
-        mbar_wait(wbar, 0);   // every lane observes the completed TMA before it patches the tile
-        // bias -> weight rows K = 27 (bf16 of the bias) and K = 28 (bf16 of the remainder), swizzled K-major layout:
-        // element k of output channel n sits at n * 128 + ((k / 8) ^ (n & 7)) * 16 + (k % 8) * 2
-        __syncwarp();
-        for (int n = lane; n < BN; n += 32) {
-            const float bv = p.bias[n];
-            const __nv_bfloat16 hi = __float2bfloat16_rn(bv);
-            const __nv_bfloat16 lo = __float2bfloat16_rn(bv - __bfloat162float(hi));
-            uint8_t* rowp = sb + n * 128 + ((3 ^ (n & 7)) << 4);
-            *reinterpret_cast<__nv_bfloat16*>(rowp + 6) = hi;    // k = 27
-            *reinterpret_cast<__nv_bfloat16*>(rowp + 8) = lo;    // k = 28
-        }
-        fence_proxy_async();
-        __syncwarp();
-        if (elect_one()) {
-            constexpr uint32_t idesc = make_idesc(BN);
-            const uint64_t db = make_desc(smem_u32(sb));
-            int stage = 0;
-            uint32_t phase = 0;
-            int it = 0;
-            for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, it++) {
-                const int acc = it % kC1Accs;
-                const uint32_t acc_phase = (it / kC1Accs) & 1;
-                mbar_wait(&tempty[acc], acc_phase ^ 1);
-                mbar_wait(&full[stage], phase);
-                tc_fence_after();
-                const uint64_t da = make_desc(smem_u32(smem + stage * kABytes));
-                umma_bf16(tmem_base + acc * BN, da, db, idesc, 0);            // K 0..15
-                umma_bf16(tmem_base + acc * BN, da + 2, db + 2, idesc, 1);    // K 16..31 (27..31 are zero)
-                // ONE commit per tile: the epilogue that observes tfull also releases the A stage (software arrive on
-                // empty[stage]) -- a second tcgen05.commit per 2-MMA tile costs more than the tile's math
-                umma_commit(&tfull[acc]);
-                if (++stage == kC1Stages) { stage = 0; phase ^= 1; }
-            }
-        }
     } else {
-        // ===================== epilogue: group g = warps 4g..4g+3 owns TMEM accumulator g (tiles with it & 1 == g) =====================
-        int it = 0, obuf = 0;
+        // ===================== consumer warpgroup eg = warps 4 eg .. 4 eg + 3: the tiles with it & 1 == eg =====================
         const int eg = warp >> 2, wq = warp & 3;
-        const int row = wq * 32 + lane;
         const bool issuer = (threadIdx.x & 127) == 0;
+        // one-time weight load; bias -> weight rows K = 27 (bf16 of the bias) and K = 28 (bf16 of the remainder), swizzled
+        // K-major layout: element k of output channel n sits at n * 128 + ((k / 8) ^ (n & 7)) * 16 + (k % 8) * 2
+        if (warp == 0) {
+            if (elect_one()) {
+                mbar_arrive_expect_tx(wbar, 64 * 128);
+                tma_load_2d(sb, &map_w, wbar, 0, 0);
+            }
+            __syncwarp();
+            mbar_wait(wbar, 0);   // every lane observes the completed TMA before it patches the tile
+            for (int n = lane; n < BN; n += 32) {
+                const float bv = p.bias[n];
+                const __nv_bfloat16 hi = __float2bfloat16_rn(bv);
+                const __nv_bfloat16 lo = __float2bfloat16_rn(bv - __bfloat162float(hi));
+                uint8_t* rowp = sb + n * 128 + ((3 ^ (n & 7)) << 4);
+                *reinterpret_cast<__nv_bfloat16*>(rowp + 6) = hi;    // k = 27
+                *reinterpret_cast<__nv_bfloat16*>(rowp + 8) = lo;    // k = 28
+            }
+            fence_proxy_async();  // generic-proxy writes -> visible to the wgmma (async proxy) reads
+        }
+        asm volatile("bar.sync 7, 256;" ::: "memory");
+        const uint64_t db = make_desc(smem_u32(sb));
         uint8_t* my_stage = out_stage + eg * 2 * kStageBytes;
+        const __nv_bfloat162 floor2 = __floats2bfloat162_rn(p.relu ? 0.f : -INFINITY, p.relu ? 0.f : -INFINITY);
+        int it = 0, obuf = 0;
         for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, it++) {
             if ((it & 1) != eg) continue;
             const int tw = tile % p.tiles_w;
             const int rest = tile / p.tiles_w;
             const int th = rest % p.tiles_h, img = rest / p.tiles_h;
-            const int acc = it % kC1Accs;                 // four TMEM accumulators: the MMA warp runs up to four tiles ahead
-            const uint32_t acc_phase = (it / kC1Accs) & 1;
-            mbar_wait(&tfull[acc], acc_phase);
-            tc_fence_after();
-            if (wq == 0 && lane == 0) mbar_arrive(&empty[it % kC1Stages]);   // the tile's MMAs are done reading its A stage
-            const uint32_t t_addr = tmem_base + ((uint32_t)(wq * 32) << 16) + acc * BN;
-            // both halves of the accumulator into registers, then hand the TMEM stage back before any math
-            uint32_t rr[2][32];
-            tmem_ld_32x32(t_addr, rr[0]);
-            tmem_ld_32x32(t_addr + 32, rr[1]);
-            if (issuer) tma_store_wait_read<1>();         // overlaps the TMEM read latency
-            tmem_ld_wait();
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tempty[acc]);
+            const int stage = it % kC1Stages;
+            mbar_wait(&full[stage], (it / kC1Stages) & 1);
+            if (issuer) tma_store_wait_read<1>();         // staging buffer obuf: the store of two tiles ago has read it
             if (eg == 0) asm volatile("bar.sync 1, 128;" ::: "memory");
             else asm volatile("bar.sync 2, 128;" ::: "memory");
             uint8_t* ob = my_stage + obuf * kStageBytes;
-            const __nv_bfloat162 floor2 = __floats2bfloat162_rn(p.relu ? 0.f : -INFINITY, p.relu ? 0.f : -INFINITY);
+            const uint32_t sa = smem_u32(smem + stage * kABytes);
 #pragma unroll
-            for (int half = 0; half < 2; half++) {
+            for (int half = 0; half < 2; half++) {       // pixels 64 half .. 64 half + 63 of the tile
+                float acc[BN / 2];
+                acc_fence<BN / 2>(acc);
+                wgmma_fence();
+                const uint64_t da = make_desc(sa + half * 64 * 128);
+                wgmma<BN, 0, 0, 0>(acc, da, db, 0);          // K 0..15
+                wgmma<BN, 0, 0, 0>(acc, da + 2, db + 2, 1);  // K 16..31 (27, 28 = bias; 29..31 are zero)
+                wgmma_commit();
+                wgmma_wait<0>();
+                acc_fence<BN / 2>(acc);
+                if (half == 1) release(&empty[stage], lane);   // the tile's MMAs are done reading its A stage
+                const int q = lane & 3;
 #pragma unroll
-                for (int j = 0; j < 4; j++) {
-                    uint32_t packed[4];
+                for (int i = 0; i < 2; i++) {
+                    const int r = half * 64 + wq * 16 + (lane >> 2) + 8 * i;
 #pragma unroll
-                    for (int q = 0; q < 4; q++) {
+                    for (int jj = 0; jj < 8; jj++) {
                         // bias already inside the accumulator; ReLU on the packed pair (rounding is monotone, 0 is exact)
-                        __nv_bfloat162 b2 = __floats2bfloat162_rn(__uint_as_float(rr[half][j * 8 + q * 2]), __uint_as_float(rr[half][j * 8 + q * 2 + 1]));
-                        b2 = __hmax2(b2, floor2);
-                        packed[q] = *reinterpret_cast<uint32_t*>(&b2);
+                        uint32_t pk = pack_bf16(acc[4 * jj + 2 * i], acc[4 * jj + 2 * i + 1]);
+                        __nv_bfloat162 b2 = __hmax2(*reinterpret_cast<__nv_bfloat162*>(&pk), floor2);
+                        *reinterpret_cast<__nv_bfloat162*>(ob + r * 128 + ((jj ^ (r & 7)) << 4) + 4 * q) = b2;
                     }
-                    const int piece = half * 4 + j;
-                    *reinterpret_cast<uint4*>(ob + row * 128 + ((piece ^ (row & 7)) << 4)) = make_uint4(packed[0], packed[1], packed[2], packed[3]);
                 }
             }
             fence_proxy_async();
@@ -798,9 +692,6 @@ k_conv1_tc(const TIn* __restrict__ in, const __grid_constant__ CUtensorMap map_w
         }
         if (issuer) tma_store_wait_all();
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == kC1MmaWarp) tmem_dealloc(tmem_base, kTmemCols);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -854,7 +745,7 @@ k_conv_small_cin(const float* __restrict__ in, const float* __restrict__ w /*[3]
     }
 }
 
-// im2col for the first layer only (Cin = 3, K = 27 < one UMMA K step): [B,H,W,3] -> [B,H,W,64] bf16 with
+// im2col for the first layer only (Cin = 3, K = 27 < one wgmma K chunk of 64): [B,H,W,3] -> [B,H,W,64] bf16 with
 // K index = tap * 3 + c (zero beyond 27), so conv1_1 runs on the tensor cores as a 1x1 convolution.
 // The input pre-processing of the caller (lib/fcn/test.py:37-110: BGR - PIXEL_MEANS) is fused for uint8
 // input: value = (float)u8 - mean[c].
@@ -1002,7 +893,9 @@ static int conv_bf16_tc_impl(const void* in, const void* weights, const float* b
     PCNN_REQUIRE(Cout % 64 == 0 && Cout >= 64, "conv: Cout must be a multiple of 64 (got %d)", Cout);
     PCNN_REQUIRE(B >= 1 && H >= 1 && W >= 1, "conv: bad shape");
     int bn = block_n;
-    if (bn == 0) bn = Cout % 256 == 0 ? 256 : (Cout % 128 == 0 ? 128 : 64);
+    // default N tile: 256 for the deep layers (K = taps * Cin >= 2304), where it is faster on the H100 although its two m64n256
+    // accumulators spill a few registers at the 168-register cap (tools/bench_conv.py: conv4_2 1.08 vs 1.37 ms at batch 32); 128 below
+    if (bn == 0) bn = Cout % 256 == 0 && ksize * ksize * Cin >= 2304 ? 256 : (Cout % 128 == 0 ? 128 : 64);
     PCNN_REQUIRE((bn == 64 || bn == 128 || bn == 256) && Cout % bn == 0, "conv: block_n %d does not divide Cout %d", bn, Cout);
     int dev = 0, sms = kNumSMs;
     cudaGetDevice(&dev);
@@ -1013,10 +906,12 @@ static int conv_bf16_tc_impl(const void* in, const void* weights, const float* b
     // row mode (two output rows x 128 px per work item, A patch reused by all nine taps) for the K-small layers
     static const bool row_mode_on = getenv("PCNN_CONV_ROWMODE") == nullptr || atoi(getenv("PCNN_CONV_ROWMODE")) != 0;
     if (row_mode_on && block_n == 0 && ksize == 3 && Cin <= 128 && Cout <= 128 && H % 2 == 0 && W >= kRowPx) {
-        // conv1_2 shape (Cin = Cout = 64): the nine 8-KB weight slices stay resident in shared memory (measured:
-        // 0.70 -> 0.65 ms); with two N tiles (conv2_1) the doubled A traffic costs more than the weight ring saves
+        // conv1_2 shape (Cin = Cout = 64): the nine 8-KB weight slices stay resident in shared memory.  The N tile is 64
+        // channels (two N tiles for conv2_x) so that both rows' accumulators fit the 168 registers of a thread.  Measured on
+        // the H100 at batch 32 (tools/bench_conv.py): conv1_2 1.19 ms here vs 1.94 on the tile kernel, but conv2_1 / conv2_2
+        // 0.75 / 1.33 ms vs 0.65 / 1.16 on the tile kernel with BN = 128
         const bool resb = Cin == 64 && Cout == 64;
-        bn = Cout;  // 64 or 128
+        bn = 64;
         rc = make_map_nhwc(&mi, in, B, H, W, Cin, kKC, kPatchW, kPatchH);
         if (rc) return rc;
         rc = make_map_weights(&mw, weights, 9 * Cin, Cout, bn);
@@ -1032,7 +927,7 @@ static int conv_bf16_tc_impl(const void* in, const void* weights, const float* b
         p.total_tiles = B * p.tiles_h * p.tiles_w * p.n_tiles_n;
         p.relu = relu; p.pool = pool; p.bias = bias;
         if (resb && p.total_tiles >= p.n_tiles_n) return launch_conv_row2<64, true>(mi, mw, mo, p, sms, st);
-        return bn == 128 ? launch_conv_row2<128, false>(mi, mw, mo, p, sms, st) : launch_conv_row2<64, false>(mi, mw, mo, p, sms, st);
+        return launch_conv_row2<64, false>(mi, mw, mo, p, sms, st);
     }
     // pixel tile: 8 x 16, or 16 x 8 when that covers the map with fewer tiles (conv5: 30 x 40 -> 10 tiles instead of 12).
     // The tile's pixel order is whatever the TMA box says (row = h * tile_w + w for load and store alike), so only

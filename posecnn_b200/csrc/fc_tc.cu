@@ -10,7 +10,7 @@
 //   k_roi_pool_pair   ONE kernel pools conv5_3 (scale 1/16) and conv4_3 (scale 1/8) with the RoiPool rule of
 //                     roi_pooling_op_gpu.cu.cc:19-101, adds them in fp32 (`pool_score`, vgg16_convs.py:183) and writes the
 //                     fp16 A operand [N, 25088] of fc6 directly (no fp32 pooled tensors, no argmax: inference only).
-//   k_fc_tc           D[128 rows, BN] partial = A[128, Kslice] * W[BN, Kslice]^T on tcgen05 (FP16 x FP16 -> FP32 in TMEM),
+//   k_fc_tc           D[128 rows, BN] partial = A[128, Kslice] * W[BN, Kslice]^T on wgmma (FP16 x FP16 -> FP32 in registers),
 //                     both operands K-major, TMA-fed through a 6-stage mbarrier ring; split-K over the grid so that
 //                     128 CTAs stream disjoint slices of the weight matrix; partials land in a small fp32 workspace.
 //   k_fc_finish       fixed-order sum of the split-K partials + bias + ReLU / tanh -> fp16 activation of the next layer
@@ -33,43 +33,33 @@ constexpr int kFcBBytes = kFcBN * kKC * 2;        // 16 KB
 constexpr int kFcStage = kFcABytes + kFcBBytes;
 constexpr int kFcBarOff = kFcStages * kFcStage;
 constexpr int kFcSmem = kFcBarOff + 256 + 1024;
-constexpr int kFcThreads = 192;                   // warps 0-3 epilogue, warp 4 TMA producer, warp 5 MMA issuer
+constexpr int kFcThreads = 288;                   // warps 0-7: two consumer warpgroups (rows 0-63 / 64-127), warp 8 TMA producer
 
 // grid = (N / 128, splits, M tiles).  partial: [splits][M][N] f32.
 __global__ void __launch_bounds__(kFcThreads, 1)
-k_fc_tc(const __grid_constant__ CUtensorMap map_a /*[M][K] bf16, box {64, 128}*/,
-        const __grid_constant__ CUtensorMap map_w /*[N][K] bf16, box {64, 128}*/, float* __restrict__ partial, int M, int N,
+k_fc_tc(const __grid_constant__ CUtensorMap map_a /*[M][K] f16, box {64, 128}*/,
+        const __grid_constant__ CUtensorMap map_w /*[N][K] f16, box {64, 128}*/, float* __restrict__ partial, int M, int N,
         int kchunks_total, int chunks_per_split)
 {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + kFcBarOff);
     uint64_t* empty = full + kFcStages;
-    uint64_t* tfull = empty + kFcStages;
-    uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(tfull + 1);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int n0 = blockIdx.x * kFcBN, split = blockIdx.y, m0 = blockIdx.z * kTileM;
     const int c_lo = split * chunks_per_split;
     const int c_hi = min(c_lo + chunks_per_split, kchunks_total);
     const int nchunks = c_hi - c_lo;               // >= 1 by construction of the grid
-    constexpr uint32_t kTmemCols = kFcBN;
 
-    if (warp == 4 && lane == 0) {
+    if (warp == 8 && lane == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w) : "memory");
-    }
-    if (warp == 5 && lane == 0) {
-        for (int s = 0; s < kFcStages; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        mbar_init(tfull, 1);
+        for (int s = 0; s < kFcStages; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
         fence_barrier_init();
     }
-    if (warp == 4) tmem_alloc(tmem_holder, kTmemCols);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_holder;
 
-    if (warp == 4) {
+    if (warp == 8) {
         if (elect_one()) {
             int stage = 0;
             uint32_t phase = 0;
@@ -82,49 +72,42 @@ k_fc_tc(const __grid_constant__ CUtensorMap map_a /*[M][K] bf16, box {64, 128}*/
                 if (++stage == kFcStages) { stage = 0; phase ^= 1; }
             }
         }
-    } else if (warp == 5) {
-        if (elect_one()) {
-            constexpr uint32_t idesc = make_idesc_f16(kFcBN);
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int c = 0; c < nchunks; c++) {
-                mbar_wait(&full[stage], phase);
-                tc_fence_after();
-                const uint32_t sa = smem_u32(smem + stage * kFcStage);
-                const uint64_t da = make_desc(sa), db = make_desc(sa + kFcABytes);
-#pragma unroll
-                for (int k = 0; k < kKC / 16; k++)
-                    umma_bf16(tmem_base, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), idesc, (c | k) != 0);
-                umma_commit(&empty[stage]);
-                if (++stage == kFcStages) { stage = 0; phase ^= 1; }
-            }
-            umma_commit(tfull);
-        }
     } else {
-        // epilogue: TMEM lane = row of the M tile
-        mbar_wait(tfull, 0);
-        tc_fence_after();
-        const int row = m0 + warp * 32 + lane;
-        const uint32_t t_addr = tmem_base + ((uint32_t)(warp * 32) << 16);
-        float* dst = partial + ((size_t)split * M + row) * N + n0;
-#pragma unroll 1
-        for (int g = 0; g < kFcBN / 32; g++) {
-            uint32_t r[32];
-            tmem_ld_32x32(t_addr + g * 32, r);
-            tmem_ld_wait();
-            if (row < M) {
+        const int wg = warp >> 2, wq = warp & 3;
+        float acc[kFcBN / 2];
+        int stage = 0, prev = -1;
+        uint32_t phase = 0;
+        for (int c = 0; c < nchunks; c++) {
+            mbar_wait(&full[stage], phase);
+            const uint32_t sa = smem_u32(smem + stage * kFcStage);
+            const uint64_t da = make_desc(sa + wg * 64 * 128), db = make_desc(sa + kFcABytes);
+            acc_fence<kFcBN / 2>(acc);
+            wgmma_fence();
 #pragma unroll
-                for (int j = 0; j < 8; j++)
-                    *reinterpret_cast<float4*>(dst + g * 32 + j * 4) =
-                        make_float4(__uint_as_float(r[4 * j]), __uint_as_float(r[4 * j + 1]), __uint_as_float(r[4 * j + 2]),
-                                    __uint_as_float(r[4 * j + 3]));
+            for (int k = 0; k < kKC / 16; k++) wgmma<kFcBN, 1, 0, 0>(acc, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (c | k) != 0);
+            wgmma_commit();
+            acc_fence<kFcBN / 2>(acc);
+            if (prev >= 0) {
+                wgmma_wait<1>();
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty[prev]);
+            }
+            prev = stage;
+            if (++stage == kFcStages) { stage = 0; phase ^= 1; }
+        }
+        wgmma_wait<0>();
+        acc_fence<kFcBN / 2>(acc);
+        // epilogue straight from the accumulator fragment: rows (r, r + 8), columns 8 j + 2 (lane % 4) (+ 1)
+#pragma unroll
+        for (int i = 0; i < 2; i++) {
+            const int row = m0 + wg * 64 + wq * 16 + (lane >> 2) + 8 * i;
+            if (row < M) {
+                float* dst = partial + ((size_t)split * M + row) * N + n0 + 2 * (lane & 3);
+#pragma unroll
+                for (int j = 0; j < kFcBN / 8; j++) *reinterpret_cast<float2*>(dst + 8 * j) = make_float2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
             }
         }
-        tc_fence_before();
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 4) tmem_dealloc(tmem_base, kTmemCols);
 }
 
 // fp16 activations saturate instead of overflowing to inf (|x| <= 65504)

@@ -1,4 +1,4 @@
-// hough_vote.cu — Houghvotinggpu for sm_100a, whole batch per call, no host round trips.
+// hough_vote.cu — Houghvotinggpu for sm_90a, whole batch per call, no host round trips.
 //
 // Behavioural spec: lib/hough_voting_gpu_layer/hough_voting_gpu_op.cu.cc:253-333 (vote
 // predicate: cosine cone > inlier, clipped to a depth-dependent square), :335-383 (maxima),

@@ -1,9 +1,9 @@
-// pixel_ops.cu — RoiPool, Hardlabel, Project / Backproject and their gradients for sm_100a.
+// pixel_ops.cu — RoiPool, Hardlabel, Project / Backproject and their gradients for sm_90a.
 //
 // All of these are HBM-bound gathers / streams (SURVEY.md §8(d)); the kernels keep the
 // channel dimension (NHWC innermost) on adjacent lanes with 128-bit accesses, compute each
 // geometric quantity once per (pixel|voxel|bin) group of lanes, and size grids from the
-// element count (grid-stride loops, 148 SMs x resident CTAs).
+// element count (grid-stride loops, kNumSMs x resident CTAs).
 //
 // Behavioural specs (paths relative to /root/reference/lib):
 //   RoiPool fwd/bwd  roi_pooling_layer/roi_pooling_op_gpu.cu.cc:19-101, 134-229

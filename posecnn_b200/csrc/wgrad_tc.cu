@@ -1,4 +1,4 @@
-// wgrad_tc.cu — weight gradients of the convolution / fully connected layers on the sm_100a tensor cores, and the
+// wgrad_tc.cu — weight gradients of the convolution / fully connected layers on the sm_90a tensor cores, and the
 // element-wise halves of the backward pass (ReLU mask, max-pool routing, bias gradients).
 //
 // Behavioural spec: the gradients TensorFlow derives for Network.conv / Network.fc / Network.max_pool
@@ -9,14 +9,14 @@
 // Weight gradient as a GEMM whose REDUCTION dimension is the pixel index:
 //      dW_tap[co, ci] = sum_p  dZ[p, co] * X[p + tap offset, ci]
 // Both operands are NHWC activation tiles exactly as TMA delivers them — 64 pixels x 64 channels, rows of 128 B,
-// SWIZZLE_128B — i.e. "MN-major" UMMA operands (the M / N index is the contiguous one, the K index = pixel is the row):
+// SWIZZLE_128B — i.e. "MN-major" wgmma operands (the M / N index is the contiguous one, the K index = pixel is the row):
 // no transposed copy of any activation is ever made.  One box {64 ch, bw, bh, 1} of dZ at the tile origin and one box
 // of X at the origin shifted by the tap (out-of-image = zero = SAME padding) have the same pixel order, so row p of one
-// pairs with row p of the other.  tcgen05.mma M = 128 (two 64-channel blocks, LBO apart), N <= 256, K = 16 pixels per
-// instruction, FP32 accumulation in TMEM.
+// pairs with row p of the other.  Two consumer warpgroups take one 64-channel dZ block each (wgmma M = 64), N <= 256
+// (B blocks LBO apart), K = 16 pixels per instruction, FP32 accumulation in registers.
 //
 //   work item  = (pixel range s, tap group, Cin tile, Cout tile) — for Cin <= 128 up to four taps share one MMA as extra N blocks
-//                (N = 256 instead of 64: conv1_2's weight gradient 2.27 -> ms at batch 16); items of one pixel range are adjacent in launch order so
+//                (N = 256 instead of 64); items of one pixel range are adjacent in launch order so
 //                that the 9 taps x tiles that re-read the same activations run together and hit in L2
 //   split-K    = the pixel ranges; partial [split][tap][Cout][Cin] fp32 in a workspace, fixed-order reduction
 //                (k_wgrad_finish) -> dW in the tensor-core weight layout [Cout][tap * Cin + ci] fp32
@@ -37,7 +37,7 @@ constexpr int kWgStage = (2 + kWgMaxNB) * kWgBlk;  // 48 KB
 constexpr int kWgStages = 4;
 constexpr int kWgBarOff = kWgStages * kWgStage;
 constexpr int kWgSmem = kWgBarOff + 256 + 1024;
-constexpr int kWgThreads = 192;
+constexpr int kWgThreads = 288;                  // warps 0-7: two consumer warpgroups (dZ channel blocks), warp 8 TMA producer
 
 struct WgParams {
     int B, H, W, Cin, Cout, ksize, taps;
@@ -61,81 +61,110 @@ struct WgParams {
     float* dW;
 };
 
-// MN-major, 128-byte-swizzled operand: K rows of 128 B (64 channels), 8-row groups 1024 B apart (SBO), 64-channel
-// blocks `lbo` bytes apart (cute::UMMA make_umma_desc<Major::MN>, SWIZZLE_128B canonical layout)
-__device__ __forceinline__ uint64_t make_desc_mn(uint32_t smem_addr, uint32_t lbo_bytes)
+// Consumer warpgroup wg: D[64 channels of dZ block wg, N] over the item's pixel tiles, then the epilogue from registers.
+// Both operands are MN-major (wgmma transpose flags): K rows of 128 B (64 channels), 8-row groups 1024 B apart (SBO),
+// 64-channel blocks kWgBlk bytes apart (LBO).
+template <int N, int F16>
+__device__ __forceinline__ void wgrad_consume(uint8_t* smem, uint64_t* full, uint64_t* empty, int nk, const WgParams& p,
+                                              float* __restrict__ partial, int split, int m0, int n0, int tap0, int cb, bool upper,
+                                              int wg, int wq, int lane)
 {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-    d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-    d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
+    float acc[N / 2];
+    int stage = 0, prev = -1;
+    uint32_t phase = 0;
+    for (int k = 0; k < nk; k++) {
+        mbar_wait(&full[stage], phase);
+        const uint32_t sa = smem_u32(smem + stage * kWgStage) + wg * kWgBlk;
+        const uint32_t sb = smem_u32(smem + stage * kWgStage) + 2 * kWgBlk;
+        acc_fence<N / 2>(acc);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < kWgPx / 16; kk++) {      // 16 pixel rows = 2048 B per K step
+            const uint64_t da = make_desc_lbo(sa + kk * 2048, kWgBlk), db = make_desc_lbo(sb + kk * 2048, kWgBlk);
+            wgmma<N, F16, 1, 1>(acc, da, db, (k | kk) != 0);
+        }
+        wgmma_commit();
+        acc_fence<N / 2>(acc);
+        if (prev >= 0) {
+            wgmma_wait<1>();
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty[prev]);
+        }
+        prev = stage;
+        if (++stage == kWgStages) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+    acc_fence<N / 2>(acc);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[prev]);
+    // accumulator row = output channel of the tile, column = B column (block j / 8 = tap and input-channel block)
+#pragma unroll
+    for (int i = 0; i < 2; i++) {
+        const int co = m0 + wg * 64 + wq * 16 + (lane >> 2) + 8 * i - (upper ? 64 : 0);   // upper: the same channels, tap - 3
+        if (co >= p.Cout) continue;
+#pragma unroll
+        for (int j = 0; j < N / 8; j++) {
+            const int jb = j / 8;
+            const int tap = tap0 + jb / cb - (upper ? 3 : 0), ci = n0 + 64 * (jb % cb) + 8 * (j % 8) + 2 * (lane & 3);
+            float2 v = make_float2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
+            if (p.direct) {
+                const size_t o = ((size_t)co * p.taps + tap) * p.Cin + ci;
+                v.x *= p.scale; v.y *= p.scale;
+                if (p.w) {
+                    const float2 wv = __ldg(reinterpret_cast<const float2*>(p.w + o));
+                    v.x = fmaf(p.decay, wv.x, v.x); v.y = fmaf(p.decay, wv.y, v.y);
+                }
+                *reinterpret_cast<float2*>(p.dW + o) = v;
+            } else {
+                *reinterpret_cast<float2*>(partial + (((size_t)split * p.taps + tap) * p.Cout + co) * p.Cin + ci) = v;
+            }
+        }
+    }
 }
 
-__host__ __device__ constexpr uint32_t make_idesc_mn(int n, int f16)
-{
-    // c F32, a = b = BF16 (format 1) or F16 (format 0), a_major = b_major = MN (bits 15, 16), N >> 3 @17, M = 128 >> 4 @24
-    return (1u << 4) | (f16 ? 0u : ((1u << 7) | (1u << 10))) | (1u << 15) | (1u << 16) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-}
-
+// NB = B blocks per stage (wgmma N = 64 NB), the same for every item of a launch: the launch covers the tap groups
+// tg_lo .. tg_lo + tg_count - 1 (wgrad_impl launches the full groups and a shorter last group separately)
+template <int NB, int F16>
 __global__ void __launch_bounds__(kWgThreads, 1)
 k_wgrad_tc(const __grid_constant__ CUtensorMap map_x /*[B,H,W,Cin] box {64,bw,bh,1}*/,
-           const __grid_constant__ CUtensorMap map_dz /*[B,H,W,Cout] box {64,bw,bh,1}*/, float* __restrict__ partial, const WgParams p)
+           const __grid_constant__ CUtensorMap map_dz /*[B,H,W,Cout] box {64,bw,bh,1}*/, float* __restrict__ partial, const WgParams p,
+           int tg_lo, int tg_count)
 {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + kWgBarOff);
     uint64_t* empty = full + kWgStages;
-    uint64_t* tfull = empty + kWgStages;
-    uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(tfull + 1);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     // item -> (split, tap group, n tile, m tile); m fastest
     int item = blockIdx.x;
     const int mt = item % p.m_tiles; item /= p.m_tiles;
     const int nt = item % p.n_tiles; item /= p.n_tiles;
-    const int tgi = item % p.tap_groups;
-    const int split = item / p.tap_groups;
+    const int tgi = tg_lo + item % tg_count;
+    const int split = item / tg_count;
     const int k_lo = split * p.ktiles_per_split, k_hi = min(k_lo + p.ktiles_per_split, p.ktiles);
     const int nk = k_hi - k_lo;
     const int m0 = mt * 128, n0 = nt * p.n_tile;
-    const int tap0 = p.pair64 ? (tgi == 0 ? 6 : 0) : tgi * p.tg, ntaps = min(p.tg, p.taps - tap0);
+    const int tap0 = p.pair64 ? (tgi == 0 ? 6 : 0) : tgi * p.tg;
     const bool up_shift = p.pair64 && tgi == 0;         // upper A block = dZ one row down (see WgParams::pair64)
     const int cb = p.n_tile / 64;                       // 64-channel B blocks per tap
-    const int nb = ntaps * cb;                          // B blocks per stage (<= 4): block j = (tap0 + j / cb, channels n0 + 64 (j % cb))
-    const int n_item = nb * 64;                         // UMMA N of this item
+    constexpr int nb = NB;                              // block j = (tap0 + j / cb, channels n0 + 64 (j % cb))
     const bool a2 = m0 + 64 < p.Cout;                   // second 64-channel block of dZ exists
-    const uint32_t tmem_cols = 256;
+    const bool wg1 = a2 || up_shift;                    // the second consumer warpgroup has a dZ block (else it exits at once)
     const int pad = p.ksize / 2;
 
-    if (warp == 4 && lane == 0) {
+    if (warp == 8 && lane == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_x) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_dz) : "memory");
-    }
-    if (warp == 5 && lane == 0) {
-        for (int s = 0; s < kWgStages; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        mbar_init(tfull, 1);
+        for (int s = 0; s < kWgStages; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], wg1 ? 8 : 4); }
         fence_barrier_init();
     }
-    if (!a2 && !up_shift) {
-        // Cout tile of 64 channels only: the upper half of the M = 128 operand stays zero for the whole kernel
-        for (int s = 0; s < kWgStages; s++)
-            for (int i = threadIdx.x; i < kWgBlk / 16; i += kWgThreads)
-                reinterpret_cast<uint4*>(smem + s * kWgStage + kWgBlk)[i] = make_uint4(0u, 0u, 0u, 0u);
-        fence_proxy_async();
-    }
-    if (warp == 4) tmem_alloc(tmem_holder, tmem_cols);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_holder;
 
-    if (warp == 4) {
+    if (warp == 8) {
         if (elect_one()) {
             int stage = 0;
             uint32_t phase = 0;
-            const uint32_t tx = (uint32_t)((a2 || up_shift ? 2 : 1) + nb) * kWgBlk;
+            const uint32_t tx = (uint32_t)((wg1 ? 2 : 1) + nb) * kWgBlk;
             int bdx[kWgMaxNB], bdy[kWgMaxNB], bch[kWgMaxNB];       // per B block: tap offset and channel origin (loop invariant)
 #pragma unroll
             for (int j = 0; j < kWgMaxNB; j++) {
@@ -160,65 +189,11 @@ k_wgrad_tc(const __grid_constant__ CUtensorMap map_x /*[B,H,W,Cin] box {64,bw,bh
                 if (++stage == kWgStages) { stage = 0; phase ^= 1; }
             }
         }
-    } else if (warp == 5) {
-        if (elect_one()) {
-            const uint32_t idesc = make_idesc_mn(n_item, p.f16);
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int k = 0; k < nk; k++) {
-                mbar_wait(&full[stage], phase);
-                tc_fence_after();
-                const uint32_t sa = smem_u32(smem + stage * kWgStage);
-                const uint32_t sb = sa + 2 * kWgBlk;
-#pragma unroll
-                for (int kk = 0; kk < kWgPx / 16; kk++)      // 16 pixel rows = 2048 B per K step
-                    umma_bf16(tmem_base, make_desc_mn(sa + kk * 2048, kWgBlk), make_desc_mn(sb + kk * 2048, kWgBlk), idesc, (k | kk) != 0);
-                umma_commit(&empty[stage]);
-                if (++stage == kWgStages) { stage = 0; phase ^= 1; }
-            }
-            umma_commit(tfull);
-        }
     } else {
-        // epilogue: TMEM lane = output channel of the tile, columns = input channels of the tile
-        mbar_wait(tfull, 0);
-        tc_fence_after();
-        const bool upper = up_shift && warp >= 2;           // lanes 64..127 of the paired item: the same channels, tap - 3
-        const int co = m0 + warp * 32 + lane - (upper ? 64 : 0);
-        const uint32_t t_addr = tmem_base + ((uint32_t)(warp * 32) << 16);
-        for (int g = 0; g < n_item / 32; g++) {
-            uint32_t r[32];
-            tmem_ld_32x32(t_addr + g * 32, r);
-            tmem_ld_wait();
-            if (co < p.Cout) {
-                const int j = g >> 1;                                   // B block of these 32 columns
-                const int tap = tap0 + j / cb - (upper ? 3 : 0), ci = n0 + 64 * (j % cb) + 32 * (g & 1);
-                if (p.direct) {
-                    const size_t o = ((size_t)co * p.taps + tap) * p.Cin + ci;
-#pragma unroll
-                    for (int q = 0; q < 8; q++) {
-                        float4 v = make_float4(__uint_as_float(r[4 * q]) * p.scale, __uint_as_float(r[4 * q + 1]) * p.scale,
-                                               __uint_as_float(r[4 * q + 2]) * p.scale, __uint_as_float(r[4 * q + 3]) * p.scale);
-                        if (p.w) {
-                            const float4 wv = __ldg(reinterpret_cast<const float4*>(p.w + o) + q);
-                            v.x = fmaf(p.decay, wv.x, v.x); v.y = fmaf(p.decay, wv.y, v.y); v.z = fmaf(p.decay, wv.z, v.z); v.w = fmaf(p.decay, wv.w, v.w);
-                        }
-                        *reinterpret_cast<float4*>(p.dW + o + q * 4) = v;
-                    }
-                } else {
-                    float* dst = partial + (((size_t)split * p.taps + tap) * p.Cout + co) * p.Cin + ci;
-#pragma unroll
-                    for (int q = 0; q < 8; q++)
-                        *reinterpret_cast<float4*>(dst + q * 4) =
-                            make_float4(__uint_as_float(r[4 * q]), __uint_as_float(r[4 * q + 1]), __uint_as_float(r[4 * q + 2]),
-                                        __uint_as_float(r[4 * q + 3]));
-                }
-            }
-        }
-        tc_fence_before();
+        const int wg = warp >> 2, wq = warp & 3;
+        if (wg == 1 && !wg1) return;
+        wgrad_consume<64 * NB, F16>(smem, full, empty, nk, p, partial, split, m0, n0, tap0, cb, up_shift && wg == 1, wg, wq, lane);
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 4) tmem_dealloc(tmem_base, tmem_cols);
 }
 
 // dW[co][tap * Cin + ci] = scale * sum_s partial[s][tap][co][ci] (+ decay * w[co][tap * Cin + ci]: l2_regularizer, network.py:171-172)
@@ -500,6 +475,34 @@ extern "C" int pcnn_fc_wgrad_f16_tc(const void* x_f16, const void* dy_f16, int r
     return wgrad_impl(x_f16, dy_f16, 1, 1, rows, Cin, Cout, 1, scale, w_f32, decay, dW, workspace, workspace_bytes, stream, 1);
 }
 
+template <int NB, int F16>
+static int launch_wgrad_nb(const CUtensorMap& mx, const CUtensorMap& mz, float* partial, const WgParams& p, int tg_lo, int tg_count,
+                           cudaStream_t st)
+{
+    PCNN_SMEM_OPTIN((k_wgrad_tc<NB, F16>), kWgSmem, "wgrad_tc");
+    const unsigned items = (unsigned)((long long)p.splits * tg_count * p.n_tiles * p.m_tiles);
+    k_wgrad_tc<NB, F16><<<items, kWgThreads, kWgSmem, st>>>(mx, mz, partial, p, tg_lo, tg_count);
+    return check_launch("wgrad_tc");
+}
+
+// one launch over tap groups tg_lo .. tg_lo + tg_count - 1, all with nb B blocks per stage (nb = 0 or tg_count = 0: nothing to do)
+static int launch_wgrad(int nb, int f16, const CUtensorMap& mx, const CUtensorMap& mz, float* partial, const WgParams& p, int tg_lo,
+                        int tg_count, cudaStream_t st)
+{
+    if (nb == 0 || tg_count == 0) return PCNN_OK;
+    PCNN_REQUIRE(nb >= 1 && nb <= kWgMaxNB, "conv_wgrad: %d B blocks per stage", nb);
+    switch (nb * 2 + (f16 ? 1 : 0)) {
+        case 2: return launch_wgrad_nb<1, 0>(mx, mz, partial, p, tg_lo, tg_count, st);
+        case 3: return launch_wgrad_nb<1, 1>(mx, mz, partial, p, tg_lo, tg_count, st);
+        case 4: return launch_wgrad_nb<2, 0>(mx, mz, partial, p, tg_lo, tg_count, st);
+        case 5: return launch_wgrad_nb<2, 1>(mx, mz, partial, p, tg_lo, tg_count, st);
+        case 6: return launch_wgrad_nb<3, 0>(mx, mz, partial, p, tg_lo, tg_count, st);
+        case 7: return launch_wgrad_nb<3, 1>(mx, mz, partial, p, tg_lo, tg_count, st);
+        case 8: return launch_wgrad_nb<4, 0>(mx, mz, partial, p, tg_lo, tg_count, st);
+        default: return launch_wgrad_nb<4, 1>(mx, mz, partial, p, tg_lo, tg_count, st);
+    }
+}
+
 static int wgrad_impl(const void* x_bf16, const void* dz_bf16, int B, int H, int W, int Cin, int Cout, int ksize, float scale,
                       const float* w_f32, float decay, float* dW, void* workspace, size_t workspace_bytes, void* stream, int f16)
 {
@@ -516,13 +519,17 @@ static int wgrad_impl(const void* x_bf16, const void* dz_bf16, int B, int H, int
     if (rc) return rc;
     rc = make_map_nhwc_box(&mz, dz_bf16, B, H, W, Cout, p.bw, p.bh);
     if (rc) return rc;
-    PCNN_SMEM_OPTIN(k_wgrad_tc, kWgSmem, "wgrad_tc");
     cudaStream_t st = (cudaStream_t)stream;
     const long long items = (long long)p.splits * p.tap_groups * p.n_tiles * p.m_tiles;
     PCNN_REQUIRE(items < 0x7fffffffLL, "conv_wgrad: too many work items");
     if (p.splits == 1) { p.direct = 1; p.scale = scale; p.decay = decay; p.w = w_f32; p.dW = dW; }
-    k_wgrad_tc<<<(unsigned)items, kWgThreads, kWgSmem, st>>>(mx, mz, (float*)workspace, p);
-    rc = check_launch("wgrad_tc");
+    // tap groups of tg taps, then (when tg does not divide the taps) one shorter last group; the paired 64-channel case has
+    // two groups of three taps
+    const int cb = p.n_tile / 64;
+    const int full_groups = p.pair64 ? p.tap_groups : p.taps / p.tg;
+    rc = launch_wgrad(full_groups ? p.tg * cb : 0, f16, mx, mz, (float*)workspace, p, 0, full_groups, st);
+    if (rc) return rc;
+    if (full_groups < p.tap_groups) rc = launch_wgrad((p.taps - full_groups * p.tg) * cb, f16, mx, mz, (float*)workspace, p, full_groups, 1, st);
     if (rc || p.direct) return rc;
     const size_t n4 = (size_t)p.taps * Cout * Cin / 4;
     int blocks = (int)std::min<size_t>((n4 + 255) / 256, (size_t)kNumSMs * 8);

@@ -1,14 +1,14 @@
-"""vgg16_convs — the PoseCNN network of lib/networks/vgg16_convs.py on the B200-native kernels.
+"""vgg16_convs — the PoseCNN network of lib/networks/vgg16_convs.py on the H100-native kernels.
 
 Mirrors the reference class (constructor arguments, layer names, parameter names `<layer>/weights`,
 `<layer>/biases` in TF layouts: conv HWIO, fc [in, out]) so that a TF1 checkpoint / VGG16 .npy
 dictionary (lib/networks/network.py:71-107) maps one to one.  The graph of
 vgg16_convs.setup() (vgg16_convs.py:79-212) is executed eagerly on one CUDA stream:
 
-    conv1_1 .. conv5_3 (+ _p trunk for RGBD)   tcgen05 implicit GEMM, bf16 x bf16 -> fp32   csrc/conv_tc.cu
-    score / vertex heads                         1x1 on tcgen05 + fused bilinear/softmax     csrc/heads.cu
+    conv1_1 .. conv5_3 (+ _p trunk for RGBD)   wgmma implicit GEMM, bf16 x bf16 -> fp32   csrc/conv_tc.cu
+    score / vertex heads                         1x1 on wgmma + fused bilinear/softmax     csrc/heads.cu
     hough_voting_gpu                             csrc/hough_vote.cu
-    roi_pool x2 + add, fc6-fc8, tanh             csrc/fc_tc.cu (fused pooling, split-K tcgen05 GEMMs, fused epilogues)
+    roi_pool x2 + add, fc6-fc8, tanh             csrc/fc_tc.cu (fused pooling, split-K wgmma GEMMs, fused epilogues)
 
 PyTorch supplies device memory and streams only.
 """

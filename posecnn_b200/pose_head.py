@@ -1,5 +1,5 @@
 """Host-side bindings of the pose-regression head kernels (include/posecnn_b200.h, csrc/fc_tc.cu):
-RoiPool x2 + add (-> fp16 fc6 operand), and the fully connected layers as split-K tcgen05 GEMMs with fused
+RoiPool x2 + add (-> fp16 fc6 operand), and the fully connected layers as split-K wgmma GEMMs with fused
 bias / ReLU / tanh (lib/networks/vgg16_convs.py:177-197, lib/networks/network.py:392-422)."""
 from __future__ import annotations
 

@@ -1,4 +1,4 @@
-"""One SGD training step of the vgg16_convs network (BASELINE configs[4]) on the B200-native kernels.
+"""One SGD training step of the vgg16_convs network (BASELINE configs[4]) on the H100-native kernels.
 
 Reference: the training graph lib/networks/vgg16_convs.py:79-212 driven by lib/fcn/train.py:206-260 —
     loss = loss_cls + VERTEX_W * loss_vertex + loss_pose + l2 regularisation (train.py:486-500),
@@ -9,11 +9,11 @@ Reference: the training graph lib/networks/vgg16_convs.py:79-212 driven by lib/f
 This is the keep_prob = 1.0 graph (the reference trains with dropout 0.5; random masks cannot be compared, SURVEY App. A.7).
 
 Everything heavy runs on this package's own kernels:
-    forward   tcgen05 convolutions (bf16), un-fused heads (add + up2, 1x1 on the tensor cores, fused up8 / softmax / arg-max),
+    forward   wgmma convolutions (bf16), un-fused heads (add + up2, 1x1 on the tensor cores, fused up8 / softmax / arg-max),
               Houghvotinggpu in train mode, RoiPool with arg-max, fp16 tensor-core fc6-fc8, fused losses
-    backward  wgrad on tcgen05 with MN-major operands (csrc/wgrad_tc.cu), dgrad = the forward kernel on flipped weights,
+    backward  wgrad on wgmma with MN-major operands (csrc/wgrad_tc.cu), dgrad = the forward kernel on flipped weights,
               ReLU / max-pool routing with bias gradients, fused loss-gradient up-sampling adjoint (csrc/train_bwd.cu),
-              RoiPoolGrad, fc input / weight gradients on tcgen05
+              RoiPoolGrad, fc input / weight gradients on wgmma
     update    fused SGD-with-momentum + weight decay + refresh of the 16-bit tensor-core weight copies
     multi-GPU images shard across ranks; loss normalisers use GLOBAL counts (one small all-reduce), gradients are summed with
               bucketed NCCL all-reduces issued on a communication stream while the backward pass continues (SURVEY.md §8(e))

@@ -1,9 +1,9 @@
 """Generate tests/golden/*.npz by running the REFERENCE'S OWN CUDA kernels
-(oracle/_ref/libposecnn_ref.so = /root/reference/lib/*/*_gpu.cu.cc compiled unmodified for
-sm_100a behind oracle/ref_shim) on the GPU box.
+(oracle/_ref/libposecnn_ref.so = the reference project's lib/*/*_gpu.cu.cc compiled unmodified for
+sm_90a behind oracle/ref_shim, `make -C oracle ref`) on an H100.
 
-    gpurun -- 'python tests/golden/make_golden.py gpurun_out/golden'
-    cp gpurun_out/golden/*.npz tests/golden/
+    python tests/golden/make_golden.py /tmp/golden
+    cp /tmp/golden/*.npz tests/golden/
 
 The Hough vectors use the canonical list order (oracle/ref_driver.cu: ref_hough_canonical);
 vote planes are stored as int16 (full planes for the small cases, row/column marginals +
@@ -39,6 +39,11 @@ def main(out_dir):
             d["votes"] = v.astype(np.int16)
         np.savez_compressed(os.path.join(out_dir, name + ".npz"), **d)
         print(name, "rows", nr, "max votes", v.max())
+    # the reference launcher exactly as shipped (atomicAdd list order); with skip_pixels = 1 its rows are order independent as a set
+    sc, is_train, vt, pt, _ = cases.hough_inputs("h_skip1_d")
+    outs, nr = ref.hough_full(T(sc["label"]), T(sc["vertex"]), T(sc["extents"]), T(sc["meta"]), T(sc["gt"]), 0, vt, pt, 1)
+    np.savez_compressed(os.path.join(out_dir, "h_skip1_d_shipped.npz"), box=N(outs[0]), pose=N(outs[1]), target=N(outs[2]),
+                        weight=N(outs[3]), domain=N(outs[4]), num_rois=np.int32(nr))
     data, rois, grad = cases.roi_inputs()
     top, arg = ref.roi_pool(T(data), T(rois), 7, 7, 1.0 / 16.0, 0)
     gin = ref.roi_pool_grad(T(data), T(rois), arg, T(grad), 7, 7, 1.0 / 16.0, 0)
@@ -62,4 +67,4 @@ def main(out_dir):
 
 
 if __name__ == "__main__":
-    main(sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "gpurun_out", "golden"))
+    main(sys.argv[1])

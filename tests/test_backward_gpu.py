@@ -1,5 +1,5 @@
 """Backward-pass kernels (csrc/wgrad_tc.cu) against torch autograd of the same layer in fp32 on the SAME bf16-rounded
-operands: weight gradients on tcgen05 (MN-major operands, split-K), ReLU-mask / max-pool routing, bias gradients, and the
+operands: weight gradients on wgmma (MN-major operands, split-K), ReLU-mask / max-pool routing, bias gradients, and the
 input gradient through the forward kernel on flipped weights.  Reference semantics: TensorFlow's gradients of
 Network.conv / max_pool (lib/networks/network.py:159-188, 303-310) as driven by lib/fcn/train.py:206-260."""
 import pytest
@@ -75,7 +75,7 @@ def test_relu_and_maxpool_backward(cuda):
 
 @pytest.mark.parametrize("Cin,Cout,k", [(64, 128, 3), (512, 512, 3), (512, 64, 1)])
 def test_conv_dgrad_through_forward_kernel(cuda, Cin, Cout, k):
-    """dx = conv(dz, W flipped / transposed): the forward tcgen05 kernel on conv.hwio_to_tc_dgrad weights, zero bias, no ReLU."""
+    """dx = conv(dz, W flipped / transposed): the forward wgmma kernel on conv.hwio_to_tc_dgrad weights, zero bias, no ReLU."""
     from posecnn_b200 import conv
     g = torch.Generator().manual_seed(Cin + Cout + k)
     B, H, W = 2, 16, 24
@@ -104,7 +104,7 @@ def test_conv1_wgrad_cuda_cores(cuda):
     F.conv2d(x, w, padding=1).backward(dz.float().permute(0, 3, 1, 2))
     want = w.grad.permute(0, 2, 3, 1).reshape(64, 27)                       # [co][tap * 3 + c]
     got = torch.empty((64, 27), device=cuda)
-    ws = workspace("conv1_wgrad", 4 * 148 * 4 * 64 * 27, cuda)
+    ws = workspace("conv1_wgrad", 4 * 132 * 4 * 64 * 27, cuda)
     m = (ctypes.c_float * 3)(*mean)
     check(lib().pcnn_conv1_wgrad(ptr(img), m, ptr(dz), B, H, W, f32(1.0), ptr(None), f32(0.0), ptr(got), ptr(ws), ctypes.c_size_t(ws.numel()), stream()))
     assert rel_l2(got, want) < 1e-5

@@ -1,4 +1,4 @@
-"""tcgen05 implicit-GEMM convolution vs a plain PyTorch fp32 reference of the same op
+"""wgmma implicit-GEMM convolution vs a plain PyTorch fp32 reference of the same op
 (tf.nn.conv2d semantics of lib/networks/network.py:159-188: NHWC x HWIO, SAME, stride 1, bias, ReLU).
 Inputs and weights are rounded to bf16 first, so only the fp32 accumulation order and the final
 bf16 rounding of the output differ: tolerance = 2 bf16 ulps of the output magnitude."""
@@ -106,7 +106,7 @@ def test_conv1_fused_matches_im2col_path(cuda, dtype, H, W):
 
 @pytest.mark.parametrize("B,H,W,Cin,Cout", [(2, 24, 256, 64, 64), (1, 30, 320, 64, 128), (1, 16, 130, 128, 128), (2, 8, 640, 64, 64)])
 def test_conv_row_mode(cuda, B, H, W, Cin, Cout):
-    """Row mode (two output rows x 128 px per work item, one halo patch shared by the nine taps through row-shifted UMMA
+    """Row mode (two output rows x 128 px per work item, one halo patch shared by the nine taps through row-shifted wgmma
     views; picked automatically for Cin, Cout <= 128 and W >= 128) must agree bit for bit with the 8x16-tile kernel
     (explicit block_n), with and without the fused max pool, and with the fp32 reference."""
     from posecnn_b200 import conv

@@ -1,4 +1,4 @@
-"""GPU parity of Houghvotinggpu (hand-written sm_100a kernels, through the C ABI) against the
+"""GPU parity of Houghvotinggpu (hand-written sm_90a kernels, through the C ABI) against the
 CPU oracle.  Tolerances: integer outputs exact; box / pose 1e-4 (SURVEY.md §8(c))."""
 import numpy as np
 import pytest

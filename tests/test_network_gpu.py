@@ -1,4 +1,4 @@
-"""Network-level parity: the B200 pipeline (posecnn_b200.networks.vgg16_convs) against a plain PyTorch fp32
+"""Network-level parity: the H100 pipeline (posecnn_b200.networks.vgg16_convs) against a plain PyTorch fp32
 restatement of the reference graph (tests/ref_network.py), stage by stage, on a small synthetic image.
 Precision: the trunk computes in BF16 x BF16 -> FP32; stated tolerance rel-L2 <= 2e-2 per tensor (SURVEY §8(c))."""
 import numpy as np

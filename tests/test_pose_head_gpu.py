@@ -1,4 +1,4 @@
-"""Pose-regression head on own kernels (csrc/fc_tc.cu): fused RoiPool pair, split-K tcgen05 fully connected layers,
+"""Pose-regression head on own kernels (csrc/fc_tc.cu): fused RoiPool pair, split-K wgmma fully connected layers,
 and the two pipeline extensions of Houghvotinggpu (vertex values sampled from the low-resolution head tensor; image
 shards of a larger batch).  Reference: lib/networks/vgg16_convs.py:177-197, lib/networks/network.py:392-422,
 lib/roi_pooling_layer/roi_pooling_op_gpu.cu.cc:19-101, lib/hough_voting_gpu_layer/hough_voting_gpu_op.cu.cc:733."""
@@ -48,7 +48,7 @@ def test_roi_pool_pair_equals_two_roi_pools(cuda):
 @pytest.mark.parametrize("M,K,N,act", [(128, 25088, 4096, "relu"), (128, 4096, 4096, "relu"), (128, 4096, 88, "tanh"),
                                         (37, 1024, 256, "none"), (300, 512, 128, "relu")])
 def test_fc_tc_against_fp32_matmul(cuda, M, K, N, act):
-    """Split-K tcgen05 GEMM + fused epilogue against an fp64 product of the SAME fp16-rounded operands (isolates the
+    """Split-K wgmma GEMM + fused epilogue against an fp64 product of the SAME fp16-rounded operands (isolates the
     kernel from the operand rounding): |err| <= 1e-3 * (1 + |ref|) before the fp16 output rounding, fp16-exact after."""
     from posecnn_b200 import pose_head
     g = torch.Generator().manual_seed(K + N)

@@ -70,7 +70,7 @@ for nm, K, N in (("fc6", 25088, 4096), ("fc7", 4096, 4096), ("fc8", 4096, 88)):
     wt = pose_head.fc_weights_to_tc(torch.randn((K, N), device=dev) * 0.01); bs = torch.zeros(N, device=dev)
     a = xa if K == 25088 else torch.randn((128, K), device=dev).to(torch.float16)
     ms = timeit(lambda: pose_head.fc(a, wt, bs, "relu" if N > 88 else "tanh", torch.float16 if N > 88 else torch.float32))
-    report(f"{nm} 128 x {K} x {N} fp16 (split-K tcgen05 + finish)", ms, wt.numel() * 2 + 128 * K * 2 + 128 * N * 4, "weights + A + out; 2*M*K*N = %.1f GFLOP" % (2 * 128 * K * N / 1e9))
+    report(f"{nm} 128 x {K} x {N} fp16 (split-K wgmma + finish)", ms, wt.numel() * 2 + 128 * K * 2 + 128 * N * 4, "weights + A + out; 2*M*K*N = %.1f GFLOP" % (2 * 128 * K * N / 1e9))
     del wt
 del f5, f4, xa
 # Project / Backproject, G = 128, Cf = 64, batch 4 (8.6 GB of voxel grids at batch 4)
@@ -92,7 +92,7 @@ nsym = int(sum(1 for n in range(576) if wt[n].any() and sym[int(torch.argmax(wt[
 report("average_distance fwd N576 P2620", ms, 576 * 4 * C * 12 + C * 2620 * 12, f"{nsym} symmetric rois (O(P^2) closest-point search, compute bound)")
 nact = int(sum(1 for n in range(576) if wt[n].any()))
 flop = (nact - nsym) * 2620 * 60.0 + nsym * 2620.0 * 2620.0 * 20.0      # SURVEY 8(d): non-sym N*P*~60, sym N*P^2*~20
-fp32_peak = 148 * 128 * 2 * 1.965e9 / 1e12                               # CUDA-core fp32 FMA peak at the max SM clock, TFLOP/s
+fp32_peak = 132 * 128 * 2 * 1.98e9 / 1e12                                # H100 SXM CUDA-core fp32 FMA peak at the max SM clock, TFLOP/s
 rows[-1].update(flop=flop, tflops=flop / ms / 1e9, frac_of_fp32_peak=flop / ms / 1e9 / fp32_peak)
 print(f"  average_distance FLOP view: {flop/1e9:.2f} GFLOP ({nsym} symmetric of {nact} active rois) -> {flop/ms/1e9:.2f} TFLOP/s = {flop/ms/1e9/fp32_peak*100:.1f}% of the {fp32_peak:.1f} TFLOP/s fp32 CUDA-core peak")
 json.dump(rows, open(os.path.join(os.path.dirname(__file__), "..", "gpurun_out", "bench_ops.json"), "w"), indent=1)

@@ -1,6 +1,6 @@
-"""Device time of the reference's OWN CUDA kernels (oracle/_ref, compiled unmodified for sm_100a) next to this repo's,
+"""Device time of the reference's OWN CUDA kernels (oracle/_ref, compiled unmodified for sm_90a) next to this repo's,
 on the same inputs: Houghvotinggpu (one 640x480x22 frame and batch 4), RoiPool, Hardlabel.  Context for BASELINE.md:
-the reference publishes no numbers; this is what its code does on a B200."""
+the reference publishes no numbers; this is what its code does on the GPU it runs on."""
 import json, os, sys, time
 import numpy as np
 import torch
