@@ -228,39 +228,41 @@ k_wgrad_finish(const float* __restrict__ partial, int splits, int taps, int Cout
 //   k_relu_bwd           dz = g * [y > 0]                                  (+ per-CTA bias-gradient partials)
 //   k_maxpool_relu_bwd   dz[n, 2h+i, 2w+j, c] = g[n,h,w,c] at the window's first maximum (raster order) if that y > 0
 // Bias gradient: every CTA owns a fixed set of pixels, accumulates its per-channel sums in fp32 and writes them to
-// bias_partial[cta][C]; k_bias_finish adds the CTAs in index order (run-to-run deterministic).
+// bias_partial[cta][C]; k_bias_finish adds the CTAs in index order.  Every sum has a fixed order (run-to-run deterministic).
 // ---------------------------------------------------------------------------------------------
 constexpr int kEwThreads = 256;
 
-// Bias-gradient accumulation: the grid-stride step (gridDim.x * blockDim.x = 592 * 256) is a multiple of the channel-group
-// count for every C <= 4096 that is a multiple of 8 * 2^k, so a thread always meets the SAME 8 channels: it sums them in
-// registers and touches shared memory once at the end.
-__device__ __forceinline__ void bias_flush(float* s_acc /*[C]*/, int c0, const float v[8])
+// The grid-stride step (grid * kEwThreads, ew_grid) is a multiple of the channel-group count C / 8, so a thread always meets the
+// SAME 8 channels, group (blockIdx.x * kEwThreads + threadIdx.x) % cg: it sums them in registers.  The CTA partial of a channel
+// is then the sum of its threads' registers in thread order (no shared-memory atomics, whose order varies from run to run).
+__device__ __forceinline__ void bias_cta_partial(const float racc[8], int C, float* __restrict__ out /*[C]*/)
 {
+    __shared__ float s_part[kEwThreads * 8];
 #pragma unroll
-    for (int j = 0; j < 8; j++)
-        if (v[j] != 0.f) atomicAdd(&s_acc[c0 + j], v[j]);
+    for (int j = 0; j < 8; j++) s_part[threadIdx.x * 8 + j] = racc[j];
+    __syncthreads();
+    const int cg = C / 8;
+    const int first = (int)(((size_t)blockIdx.x * kEwThreads) % cg);    // channel group of thread 0
+    for (int c = threadIdx.x; c < C; c += kEwThreads) {
+        int t = (c >> 3) - first;
+        if (t < 0) t += cg;
+        float s = 0.f;
+        for (; t < kEwThreads; t += cg) s += s_part[t * 8 + (c & 7)];
+        out[c] = s;
+    }
 }
 
 __global__ void __launch_bounds__(kEwThreads)
 k_relu_bwd(const __nv_bfloat16* __restrict__ g, const __nv_bfloat16* __restrict__ y, size_t npix, int C, int has_relu,
            __nv_bfloat16* __restrict__ dz, float* __restrict__ bias_partial /*[grid][C] or null*/)
 {
-    extern __shared__ float s_acc[];
-    if (bias_partial)
-        for (int c = threadIdx.x; c < C; c += kEwThreads) s_acc[c] = 0.f;
-    __syncthreads();
     const int cg = C / 8;
     const size_t total = npix * cg;
     const size_t step = (size_t)gridDim.x * blockDim.x;
-    const bool fixed = step % cg == 0;              // this thread's channel group never changes
     float racc[8];
 #pragma unroll
     for (int j = 0; j < 8; j++) racc[j] = 0.f;
-    int c_fixed = 0;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += step) {
-        const int c0 = (int)(i % cg) * 8;
-        c_fixed = c0;
         const uint4 gv = __ldg(reinterpret_cast<const uint4*>(g) + i);
         uint4 ov = gv;
         if (has_relu) {
@@ -274,34 +276,22 @@ k_relu_bwd(const __nv_bfloat16* __restrict__ g, const __nv_bfloat16* __restrict_
         if (dz) reinterpret_cast<uint4*>(dz)[i] = ov;
         if (bias_partial) {
             const __nv_bfloat16* op = reinterpret_cast<const __nv_bfloat16*>(&ov);
-            if (fixed) {
 #pragma unroll
-                for (int j = 0; j < 8; j++) racc[j] += __bfloat162float(op[j]);
-            } else {
-                float v[8];
-#pragma unroll
-                for (int j = 0; j < 8; j++) v[j] = __bfloat162float(op[j]);
-                bias_flush(s_acc, c0, v);
-            }
+            for (int j = 0; j < 8; j++) racc[j] += __bfloat162float(op[j]);
         }
     }
-    if (bias_partial) {
-        if (fixed) bias_flush(s_acc, c_fixed, racc);
-        __syncthreads();
-        for (int c = threadIdx.x; c < C; c += kEwThreads) bias_partial[(size_t)blockIdx.x * C + c] = s_acc[c];
-    }
+    if (bias_partial) bias_cta_partial(racc, C, bias_partial + (size_t)blockIdx.x * C);
 }
 
 __global__ void __launch_bounds__(kEwThreads)
 k_maxpool_relu_bwd(const __nv_bfloat16* __restrict__ g /*[B,H/2,W/2,C]*/, const __nv_bfloat16* __restrict__ y /*[B,H,W,C]*/, int B, int H,
                    int W, int C, __nv_bfloat16* __restrict__ dz /*[B,H,W,C]*/, float* __restrict__ bias_partial)
 {
-    extern __shared__ float s_acc[];
-    if (bias_partial)
-        for (int c = threadIdx.x; c < C; c += kEwThreads) s_acc[c] = 0.f;
-    __syncthreads();
     const int Ho = H / 2, Wo = W / 2, cg = C / 8;
     const size_t total = (size_t)B * Ho * Wo * cg;
+    float racc[8];
+#pragma unroll
+    for (int j = 0; j < 8; j++) racc[j] = 0.f;
     for (size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
         const int gch = (int)(idx % cg);
         size_t r = idx / cg;
@@ -316,7 +306,6 @@ k_maxpool_relu_bwd(const __nv_bfloat16* __restrict__ g /*[B,H/2,W/2,C]*/, const 
         const uint4 gv = __ldg(reinterpret_cast<const uint4*>(g + ((n * Ho + yo) * Wo + xo) * C + gch * 8));
         const __nv_bfloat16* gp = reinterpret_cast<const __nv_bfloat16*>(&gv);
         uint4 ov[4];
-        float bsum[8];
 #pragma unroll
         for (int j = 0; j < 8; j++) {
             float best = __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(&yv[0])[j]);
@@ -330,16 +319,12 @@ k_maxpool_relu_bwd(const __nv_bfloat16* __restrict__ g /*[B,H/2,W/2,C]*/, const 
 #pragma unroll
             for (int k = 0; k < 4; k++)
                 reinterpret_cast<__nv_bfloat16*>(&ov[k])[j] = (pass && k == bi) ? gp[j] : __float2bfloat16_rn(0.f);
-            bsum[j] = pass ? __bfloat162float(gp[j]) : 0.f;
+            if (pass) racc[j] += __bfloat162float(gp[j]);
         }
 #pragma unroll
         for (int k = 0; k < 4; k++) *reinterpret_cast<uint4*>(dz + offs[k]) = ov[k];
-        if (bias_partial) bias_flush(s_acc, gch * 8, bsum);
     }
-    if (bias_partial) {
-        __syncthreads();
-        for (int c = threadIdx.x; c < C; c += kEwThreads) bias_partial[(size_t)blockIdx.x * C + c] = s_acc[c];
-    }
+    if (bias_partial) bias_cta_partial(racc, C, bias_partial + (size_t)blockIdx.x * C);
 }
 
 // db[c] = scale * sum_k partial[k][c] (+ decay * b[c]); block = 32 channels x 8 row groups, groups combined in fixed order
@@ -537,16 +522,28 @@ static int wgrad_impl(const void* x_bf16, const void* dz_bf16, int B, int H, int
     return check_launch("wgrad_finish");
 }
 
+// grid of the element-wise backward kernels: about four CTAs per SM, rounded down to a multiple of cg / gcd(cg, kEwThreads) (cg = C / 8
+// channel groups) so that the grid-stride step is a multiple of cg and every thread keeps its channel group (bias_cta_partial)
+static int ew_grid(int C)
+{
+    const int cg = C / 8;
+    if (cg < 1) return kNumSMs * 4;
+    int a = cg, b = kEwThreads;
+    while (b) { const int t = a % b; a = b; b = t; }
+    const int q = cg / a;
+    return kNumSMs * 4 >= q ? kNumSMs * 4 / q * q : q;
+}
+
 // dz = g * [y > 0] (has_relu) or g; optional db [C] = scale * sum_pixels dz (+ decay * b).  bias_ws: >= grid * C floats.
 extern "C" int pcnn_relu_bwd_bf16(const void* g_bf16, const void* y_bf16, size_t npix, int C, int has_relu, void* dz_bf16, float scale,
                                   const float* b, float decay, float* db, void* bias_ws, size_t bias_ws_bytes, void* stream)
 {
     PCNN_REQUIRE(g_bf16 && (y_bf16 || !has_relu) && (dz_bf16 || db), "relu_bwd: NULL tensor pointer");
     PCNN_REQUIRE(C % 8 == 0 && C >= 8 && C <= 8192, "relu_bwd: C must be a multiple of 8 (got %d)", C);
-    const int grid = kNumSMs * 4;
+    const int grid = ew_grid(C);
     PCNN_REQUIRE(!db || (bias_ws && bias_ws_bytes >= sizeof(float) * (size_t)grid * C), "relu_bwd: bias workspace too small");
     cudaStream_t st = (cudaStream_t)stream;
-    k_relu_bwd<<<grid, kEwThreads, db ? sizeof(float) * C : 0, st>>>((const __nv_bfloat16*)g_bf16, (const __nv_bfloat16*)y_bf16, npix, C, has_relu,
+    k_relu_bwd<<<grid, kEwThreads, 0, st>>>((const __nv_bfloat16*)g_bf16, (const __nv_bfloat16*)y_bf16, npix, C, has_relu,
                                                                      (__nv_bfloat16*)dz_bf16, db ? (float*)bias_ws : nullptr);
     if (db) k_bias_finish<<<(C + 31) / 32, 256, 0, st>>>((const float*)bias_ws, grid, C, scale, b, decay, db);
     return check_launch("relu_bwd");
@@ -558,10 +555,10 @@ extern "C" int pcnn_maxpool_relu_bwd_bf16(const void* g_bf16, const void* y_bf16
 {
     PCNN_REQUIRE(g_bf16 && y_bf16 && dz_bf16, "maxpool_relu_bwd: NULL tensor pointer");
     PCNN_REQUIRE(C % 8 == 0 && H % 2 == 0 && W % 2 == 0, "maxpool_relu_bwd: needs even H, W and C %% 8 == 0");
-    const int grid = kNumSMs * 4;
+    const int grid = ew_grid(C);
     PCNN_REQUIRE(!db || (bias_ws && bias_ws_bytes >= sizeof(float) * (size_t)grid * C), "maxpool_relu_bwd: bias workspace too small");
     cudaStream_t st = (cudaStream_t)stream;
-    k_maxpool_relu_bwd<<<grid, kEwThreads, db ? sizeof(float) * C : 0, st>>>((const __nv_bfloat16*)g_bf16, (const __nv_bfloat16*)y_bf16, B, H, W, C,
+    k_maxpool_relu_bwd<<<grid, kEwThreads, 0, st>>>((const __nv_bfloat16*)g_bf16, (const __nv_bfloat16*)y_bf16, B, H, W, C,
                                                                              (__nv_bfloat16*)dz_bf16, db ? (float*)bias_ws : nullptr);
     if (db) k_bias_finish<<<(C + 31) / 32, 256, 0, st>>>((const float*)bias_ws, grid, C, scale, b, decay, db);
     return check_launch("maxpool_relu_bwd");
@@ -570,7 +567,7 @@ extern "C" int pcnn_maxpool_relu_bwd_bf16(const void* g_bf16, const void* y_bf16
 extern "C" int pcnn_bias_ws_bytes(int C, size_t* bytes)
 {
     PCNN_REQUIRE(bytes && C >= 1, "bias_ws_bytes: bad arguments");
-    *bytes = sizeof(float) * (size_t)kNumSMs * 4 * C;
+    *bytes = sizeof(float) * (size_t)ew_grid(C) * C;
     return PCNN_OK;
 }
 

@@ -38,6 +38,17 @@ def test_conv_wgrad_against_autograd(cuda, B, H, W, Cin, Cout, k):
     assert torch.allclose(both, 0.5 * got + 1e-2 * wm, rtol=1e-5, atol=1e-6)
 
 
+def first_max_route(g, y):
+    """Max-pool 2x2/2 backward fused with the ReLU mask, plainly: the window [..., 4] in raster order, its FIRST maximum
+    (torch.argmax) takes g when that maximum is > 0; every other element gets 0.  g [B,H/2,W/2,C], y [B,H,W,C] -> [B,H,W,C]."""
+    B, H, W, C = y.shape
+    win = y.float().view(B, H // 2, 2, W // 2, 2, C).permute(0, 1, 3, 5, 2, 4).reshape(B, H // 2, W // 2, C, 4)
+    first = win.argmax(-1, keepdim=True)
+    take = (torch.arange(4, device=y.device) == first) & (win.amax(-1, keepdim=True) > 0)
+    dz = torch.where(take, g.float()[..., None], torch.zeros((), device=y.device))
+    return dz.view(B, H // 2, W // 2, C, 2, 2).permute(0, 1, 4, 2, 5, 3).reshape(B, H, W, C).to(torch.bfloat16)
+
+
 def test_relu_and_maxpool_backward(cuda):
     from posecnn_b200 import backward
     g = torch.Generator().manual_seed(3)
@@ -63,7 +74,7 @@ def test_relu_and_maxpool_backward(cuda):
     unique = F.avg_pool2d(ties, 2) * 4 <= 1.0                                # windows with a unique maximum (zeros tie after ReLU)
     mask = unique.repeat_interleave(2, 2).repeat_interleave(2, 3).permute(0, 2, 3, 1)
     assert torch.equal(got.float()[mask], z.grad.permute(0, 2, 3, 1)[mask])
-    assert (got.float()[~mask] == 0).all() or True
+    assert torch.equal(got, first_max_route(gp.permute(0, 2, 3, 1).contiguous().to(torch.bfloat16), ynhwc))   # every window, ties included
     assert torch.allclose(dbp, got.float().sum((0, 1, 2)), rtol=1e-5, atol=1e-4)
     tie = torch.zeros(1, 2, 2, 8, dtype=torch.bfloat16, device=cuda); tie[0, :, :, :] = 1.5
     gt = torch.ones(1, 1, 1, 8, dtype=torch.bfloat16, device=cuda)
@@ -262,3 +273,113 @@ def test_add_up2_and_adjoint(cuda):
     assert rel_l2(d5.float(), want) < 3e-3
     check(lib().pcnn_up2_bwd_bf16(ptr(dadd), ptr(None), B, h, w, C, ptr(d5), stream()))
     assert rel_l2(d5.float(), F.conv2d(dadd.float().permute(0, 3, 1, 2), filt, stride=2, padding=1, groups=C).permute(0, 2, 3, 1)) < 3e-3
+
+
+def test_relu_and_maxpool_backward_at_conv1_2(cuda):
+    """ReLU-mask / max-pool routing and the bias gradients at conv1_2's pre-pool shape (2 x 480 x 640 x 64).  Small integer
+    activations make ReLU zeros and equal window values common, so the first-maximum rule is checked on many ties; integer
+    gradients make the bias sums exact (every fp32 partial is an integer < 2^24), so they must equal the fp64 sum.  With
+    random gradients two runs must give bit-identical bias gradients (fixed-order per-CTA and cross-CTA reductions)."""
+    from posecnn_b200 import backward
+    from tests.util import int_operands
+    g = torch.Generator().manual_seed(12)
+    B, H, W, C = 2, 480, 640, 64
+    y = torch.relu(int_operands((B, H, W, C), -3, 3, g)).to(torch.bfloat16).to(cuda)
+    gp = int_operands((B, H // 2, W // 2, C), -2, 2, g).to(torch.bfloat16).to(cuda)
+    gf = int_operands((B, H, W, C), -2, 2, g).to(torch.bfloat16).to(cuda)
+    dz, db = backward.maxpool_relu_bwd(gp, y, want_bias=True)
+    want = first_max_route(gp, y)
+    assert torch.equal(dz, want)
+    assert torch.equal(db, want.double().sum((0, 1, 2)).float())
+    dz2, db2 = backward.relu_bwd(gf, y, True, want_bias=True)
+    want2 = gf.float() * (y.float() > 0)
+    assert torch.equal(dz2.float(), want2)
+    assert torch.equal(db2, want2.double().sum((0, 1, 2)).float())
+    gr = torch.randn((B, H // 2, W // 2, C), generator=g).to(torch.bfloat16).to(cuda)
+    grf = torch.randn((B, H, W, C), generator=g).to(torch.bfloat16).to(cuda)
+    a = backward.maxpool_relu_bwd(gr, y, want_bias=True)[1].clone()
+    b = backward.maxpool_relu_bwd(gr, y, want_bias=True)[1]
+    assert torch.equal(a, b)
+    a = backward.relu_bwd(grf, y, True, want_bias=True)[1].clone()
+    b = backward.relu_bwd(grf, y, True, want_bias=True)[1]
+    assert torch.equal(a, b)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Weight gradients at training shapes with exact integer operands ({-1, 0, 1}: every sum is an integer <= the pixel count,
+# far below 2^24), so the fp32 gradient must equal the float64 reference exactly.  The batch of every case is the smallest
+# whose every work item runs at least eight K tiles (twice k_wgrad_tc's four-stage ring): stages are reused, the
+# release-previous-stage path runs, and direct mode (splits == 1) reduces over many tiles.
+# ---------------------------------------------------------------------------------------------------------------------
+def _wgrad_cases(H=480, W=640):
+    """(id, H, W, Cin, Cout, k) of every convolution weight gradient of the training step (train.py: backward)."""
+    from posecnn_b200.networks.vgg16_convs import VGG_CFG
+    cases, h, w = [], H, W
+    for item in VGG_CFG:
+        if isinstance(item, str):
+            h, w = h // 2, w // 2
+            continue
+        name, ci, co = item
+        # conv1_1: the 1x1 weight gradient on the im2col view of the image (K = tap * 3 + c in 64 columns)
+        cases.append((name, h, w, 64, co, 1) if name == "conv1_1" else (name, h, w, ci, co, 3))
+    h4, w4 = H // 8, W // 8
+    cases += [("score_conv4", h4, w4, 512, 64, 1), ("score_conv5", h4 // 2, w4 // 2, 512, 64, 1),
+              ("score_conv4_vertex", h4, w4, 512, 128, 1), ("score_conv5_vertex", h4 // 2, w4 // 2, 512, 128, 1),
+              ("score", h4, w4, 64, 64, 1), ("vertex_pred", h4, w4, 128, 128, 1)]
+    return cases
+
+
+_WG = _wgrad_cases()
+
+
+@pytest.mark.parametrize("name,H,W,Cin,Cout,k", _WG, ids=[c[0] for c in _WG])
+def test_conv_wgrad_exact_at_training_shapes(cuda, name, H, W, Cin, Cout, k):
+    from posecnn_b200 import backward, conv
+    from tests.util import int_operands, ref_wgrad_exact, wgrad_batch_for_coverage
+    B, plan = wgrad_batch_for_coverage(H, W, Cin, Cout, k)
+    print(f"{name}: B={B} splits={plan['splits']} ktiles={plan['ktiles']} -> {plan['min_ktiles']}..{plan['ktiles_per_split']} "
+          f"K tiles per item")
+    assert plan["min_ktiles"] >= 8
+    g = torch.Generator().manual_seed(H + Cin + 5 * Cout + k)
+    if name == "conv1_1":
+        mean = (103.0, 116.0, 123.0)                  # integer means: the im2col values are the bytes' offsets {-1, 0, 1}
+        img = (int_operands((B, H, W, 3), -1, 1, g) + torch.tensor(mean)).to(torch.uint8).to(cuda)
+        x = conv.im2col_c3(img, mean)
+    else:
+        x = int_operands((B, H, W, Cin), -1, 1, g).to(torch.bfloat16).to(cuda)
+    dz = int_operands((B, H, W, Cout), -1, 1, g).to(torch.bfloat16).to(cuda)
+    want = ref_wgrad_exact(x, dz, k).float()
+    got = backward.conv_wgrad(x, dz, k, scale=0.5)
+    torch.cuda.synchronize()
+    bad = got != 0.5 * want
+    assert not bool(bad.any()), f"{int(bad.sum())} of {bad.numel()} gradients differ; first at {bad.nonzero()[0].tolist()}"
+
+
+@pytest.mark.parametrize("name,Cin,Cout,rows", [("fc6", 25088, 4096, 600), ("fc7", 4096, 4096, 600),
+                                                ("cin192", 192, 4096, 0), ("cin384", 384, 4096, 0)])
+def test_fc_wgrad_exact(cuda, name, Cin, Cout, rows):
+    """pcnn_fc_wgrad_f16_tc at the fc6 / fc7 shapes with 600 ROI rows (direct mode, ten 64-row K tiles, the last ragged) and
+    at Cin = 192 / 384 (one / two 64-channel B blocks), with a power-of-two scale: exact against the float64 product."""
+    import ctypes
+    from posecnn_b200._lib import check, f32, lib, ptr, stream, workspace
+    from tests.util import int_operands, wgrad_batch_for_coverage, wgrad_plan
+    if rows == 0:
+        rows, plan = wgrad_batch_for_coverage(1, 1, Cin, Cout, 1)
+    else:
+        plan = wgrad_plan(1, 1, rows, Cin, Cout, 1)
+    print(f"{name}: rows={rows} splits={plan['splits']} direct={plan['direct']} -> {plan['min_ktiles']}..{plan['ktiles_per_split']} "
+          f"K tiles per item")
+    assert plan["min_ktiles"] >= 8
+    g = torch.Generator().manual_seed(Cin + rows)
+    x = int_operands((rows, Cin), -1, 1, g).to(torch.float16).to(cuda)
+    dy = int_operands((rows, Cout), -1, 1, g).to(torch.float16).to(cuda)
+    dw = torch.empty((Cout, Cin), dtype=torch.float32, device=cuda)
+    nbytes = ctypes.c_size_t(0)
+    check(lib().pcnn_conv_wgrad_workspace_bytes(1, 1, rows, Cin, Cout, 1, ctypes.byref(nbytes)))
+    ws = workspace("wgrad", nbytes.value, cuda)
+    check(lib().pcnn_fc_wgrad_f16_tc(ptr(x), ptr(dy), rows, Cin, Cout, f32(0.25), ptr(None), f32(0.0), ptr(dw), ptr(ws),
+                                     ctypes.c_size_t(ws.numel()), stream()))
+    want = (dy.double().t() @ x.double()).float() * 0.25
+    torch.cuda.synchronize()
+    bad = dw != want
+    assert not bool(bad.any()), f"{int(bad.sum())} of {bad.numel()} gradients differ; first at {bad.nonzero()[0].tolist()}"

@@ -130,3 +130,105 @@ def test_conv_row_mode(cuda, B, H, W, Cin, Cout):
     assert torch.equal(rowp, conv.maxpool2x2(row))
     if Cin == 64 and Cout == 128:
         assert torch.equal(rowp, tilep)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Exact tests at network shapes (tests/util.py: integer operands make every fp32 sum exact in any order, so the bf16 output
+# must equal the float64 reference rounded to bf16, bit for bit).  The batch of every case is the smallest that gives each
+# persistent CTA at least three work items: the tile loop, the producer running ahead into the next tile, the reuse of the
+# epilogue staging buffers and the row mode's resident weights all run.  Shapes are those of a 480 x 640 input.
+# ---------------------------------------------------------------------------------------------------------------------
+def _network_conv_cases(H=480, W=640):
+    """(id, H, W, Cin, Cout, k, pool, dgrad) of every tensor-core convolution of the network and of its training step."""
+    from posecnn_b200.networks.vgg16_convs import VGG_CFG
+    cases, h, w = [], H, W
+    for i, item in enumerate(VGG_CFG):
+        if isinstance(item, str):
+            h, w = h // 2, w // 2
+            continue
+        name, ci, co = item
+        if name == "conv1_1":                                 # Cin = 3: conv1_fused, below
+            continue
+        cases.append((name, h, w, ci, co, 3, False, False))   # conv_bf16, as the training step runs every layer
+        pooled = i + 1 < len(VGG_CFG) and isinstance(VGG_CFG[i + 1], str) and name not in ("conv4_3", "conv5_3")
+        if pooled:                                            # conv_pool_bf16, as inference runs conv1_2, conv2_2, conv3_3
+            cases.append((name + "+pool", h, w, ci, co, 3, True, False))
+        if ci != co:                                          # input gradient: channels swapped, flipped weights
+            cases.append((name + "_dgrad", h, w, co, ci, 3, False, True))
+    h4, w4 = H // 8, W // 8
+    cases += [("score_conv4", h4, w4, 512, 64, 1, False, False), ("score_conv5", h4 // 2, w4 // 2, 512, 64, 1, False, False),
+              ("vertex_folded", h4, w4, 512, 128, 1, False, False),
+              ("score_conv4_dgrad", h4, w4, 64, 512, 1, False, True), ("score_conv4_vertex_dgrad", h4, w4, 128, 512, 1, False, True)]
+    return cases
+
+
+def _assert_bits(got, want, what):
+    bad = got.view(torch.int16) != want.view(torch.int16)
+    if bool(bad.any()):
+        idx = bad.nonzero()[0].tolist()
+        raise AssertionError(f"{what}: {int(bad.sum())} of {bad.numel()} outputs differ; first at {idx}: "
+                             f"got {got[tuple(idx)].item()} want {want[tuple(idx)].item()}")
+
+
+_CASES = _network_conv_cases()
+
+
+@pytest.mark.parametrize("name,H,W,Cin,Cout,k,pool,dgrad", _CASES, ids=[c[0] for c in _CASES])
+def test_conv_exact_at_network_shapes(cuda, name, H, W, Cin, Cout, k, pool, dgrad):
+    from posecnn_b200 import conv
+    from tests.util import conv_batch_for_coverage, int_operands, ref_conv_dgrad_exact, ref_conv_exact
+    B, plan = conv_batch_for_coverage(H, W, Cin, Cout, k, pool=pool)
+    print(f"{name}: B={B} {plan['kernel']} BN={plan['bn']} tile={plan['tile']} items={plan['items']} grid={plan['grid']} "
+          f"-> {plan['per_cta']} items per CTA")
+    assert plan["per_cta"] >= 3
+    g = torch.Generator().manual_seed(H * 7 + Cin + 3 * Cout + k)
+    x = int_operands((B, H, W, Cin), -2, 2, g)
+    # forward: HWIO [k, k, Cin, Cout]; input gradient: the forward layer's HWIO [k, k, Cout, Cin] (it maps Cout -> Cin channels)
+    w = int_operands((k, k, Cout, Cin) if dgrad else (k, k, Cin, Cout), -2, 2, g)
+    bias = int_operands((Cout,), -8, 8, g)
+    xd, wd, bd = x.to(cuda), w.to(cuda), bias.to(cuda)
+    w_tc = conv.hwio_to_tc_dgrad(wd) if dgrad else conv.hwio_to_tc(wd)
+    lin = (ref_conv_dgrad_exact(xd, wd) + bd.double()) if dgrad else ref_conv_exact(xd, wd, bd, False)
+    xb = xd.to(torch.bfloat16)
+    for relu in (True, False):
+        want = lin.clamp(min=0) if relu else lin
+        if pool:
+            want = torch.nn.functional.max_pool2d(want.permute(0, 3, 1, 2), 2).permute(0, 2, 3, 1)
+            got = conv.conv_pool_bf16(xb, w_tc, bd, k, relu)
+        else:
+            got = conv.conv_bf16(xb, w_tc, bd, k, relu)
+        torch.cuda.synchronize()
+        _assert_bits(got, want.float().to(torch.bfloat16).contiguous(), f"{name} relu={relu}")
+    del lin, want, got
+
+
+@pytest.mark.parametrize("dtype", [torch.uint8, torch.float32])
+def test_conv1_fused_exact_480x640(cuda, dtype):
+    """conv1_1 at 480 x 640, batch 2 (4,800 tiles, 36 per CTA): every builder group, both patch buffers of each group and
+    both consumer warpgroups run.  uint8 input with integer means (the staged fast path: W % 4 == 0) makes byte - mean an
+    integer of magnitude <= 255, exact in bf16, and an integer bias splits into hi + lo with lo = 0: bit-exact output."""
+    from posecnn_b200 import conv
+    from tests.util import int_operands, num_sms, ref_conv_exact
+    B, H, W = 2, 480, 640
+    tiles = B * (H // 8) * (W // 16)
+    per_cta = tiles // min(tiles, num_sms())
+    print(f"conv1_1 {dtype}: {tiles} tiles, {per_cta} per CTA")
+    assert per_cta >= 2 * 4                      # four builder groups x two patch buffers
+    g = torch.Generator().manual_seed(17)
+    if dtype == torch.uint8:
+        mean = (103.0, 116.0, 123.0)
+        x = torch.randint(0, 256, (B, H, W, 3), generator=g, dtype=torch.uint8)
+        xf = x.float() - torch.tensor(mean)
+    else:
+        mean = None
+        x = int_operands((B, H, W, 3), -255, 255, g)
+        xf = x
+    w = int_operands((3, 3, 3, 64), -2, 2, g)
+    bias = int_operands((64,), -8, 8, g)
+    wt = conv.conv1_1_weights_to_tc(w.to(cuda))
+    lin = ref_conv_exact(xf.to(cuda), w.to(cuda), bias.to(cuda), False)
+    for relu in (True, False):
+        got = conv.conv1_fused(x.to(cuda), wt, bias.to(cuda), mean, relu)
+        torch.cuda.synchronize()
+        want = (lin.clamp(min=0) if relu else lin).float().to(torch.bfloat16)
+        _assert_bits(got, want, f"conv1_1 {dtype} relu={relu}")

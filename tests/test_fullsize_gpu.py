@@ -114,13 +114,10 @@ def test_pose_head_480x640_against_fp32_head(full):
     assert e_pre < 1.5e-3 and err < 1e-3, (e_pre, err)
 
 
-def test_depth_blob_fused_into_conv1(cuda):
-    """f2: conv1_1_p on the RAW depth image (blob clip(d / 2000, 0, 1) * 255 x3 - PIXEL_MEANS formed in the loader,
-    lib/fcn/test.py:70-76) == the same kernel fed the host-side blob of posecnn_b200/utils/blob.py: bit-identical."""
+def _depth_blob_case(cuda, B, H, W):
     from posecnn_b200 import conv
     from posecnn_b200.utils import blob
     g = np.random.default_rng(5)
-    B, H, W = 2, 48, 80
     depth = g.uniform(-100.0, 2600.0, (B, H, W)).astype(np.float32)      # mm; values below 0 and above 2000 exercise the clip
     depth[0, :3] = 0.0
     w = torch.randn((3, 3, 3, 64), generator=torch.Generator().manual_seed(1)) * 0.1
@@ -130,6 +127,17 @@ def test_depth_blob_fused_into_conv1(cuda):
     want = conv.conv1_fused(host_blob, w_tc, bias.to(cuda), None, True)
     got = conv.conv1_depth_fused(torch.from_numpy(depth).to(cuda), w_tc, bias.to(cuda), MEANS, True)
     assert torch.equal(got, want)
+
+
+def test_depth_blob_fused_into_conv1(cuda):
+    """f2: conv1_1_p on the RAW depth image (blob clip(d / 2000, 0, 1) * 255 x3 - PIXEL_MEANS formed in the loader,
+    lib/fcn/test.py:70-76) == the same kernel fed the host-side blob of posecnn_b200/utils/blob.py: bit-identical."""
+    _depth_blob_case(cuda, 2, 48, 80)
+
+
+def test_depth_blob_fused_into_conv1_480x640(cuda):
+    """The same at 480 x 640: every CTA runs 36 tiles, so all four builder groups and both consumer warpgroups take part."""
+    _depth_blob_case(cuda, 2, 480, 640)
 
 
 def test_rgbd_network_with_raw_depth_input(cuda):

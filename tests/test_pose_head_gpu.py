@@ -163,3 +163,57 @@ def test_sharded_network_equals_whole_batch(cuda):
             parts.append(parallel.pack_detections(L))
         got = parallel.compact_records(torch.cat(parts))
         assert torch.equal(got, whole), world
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Exact tests of the fully connected kernels at the head's shapes (tests/util.py): operands in {-1, 0, 1} and integer biases,
+# so every sum is an integer <= 25,096 (below fp16's 65,504) and the fp32 output must equal the float64 reference exactly,
+# the fp16 output that value rounded once.  M = 600 ROI rows = five M tiles.
+# ---------------------------------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("M", [128, 600])
+@pytest.mark.parametrize("layer,K,N", [("fc6", 25088, 4096), ("fc7", 4096, 4096), ("fc8", 4096, 88)])
+def test_fc_exact_at_head_shapes(cuda, layer, K, N, M):
+    from posecnn_b200 import pose_head
+    from tests.util import fc_plan, int_operands
+    g = torch.Generator().manual_seed(K + N + M)
+    a = int_operands((M, K), -1, 1, g).to(torch.float16).to(cuda)
+    w = int_operands((K, N), -1, 1, g).to(cuda)
+    bias = int_operands((N,), -8, 8, g).to(cuda)
+    w_tc = pose_head.fc_weights_to_tc(w)
+    plan = fc_plan(M, w_tc.shape[0], K)
+    print(f"{layer} M={M}: {plan['m_tiles']} M tiles, {plan['splits']} splits x {plan['chunks_per_split']} K chunks "
+          f"(fewest {plan['min_chunks']})")
+    assert plan["min_chunks"] > 6 or plan["splits"] > 1      # the 6-stage ring is reused, or the split-K finish reduces
+    lin = a.double() @ w.double() + bias.double()
+    for act in ("none", "relu"):
+        want = (lin.clamp(min=0) if act == "relu" else lin).float()
+        out32 = pose_head.fc(a, w_tc, bias, act, torch.float32)
+        out16 = pose_head.fc(a, w_tc, bias, act, torch.float16)
+        torch.cuda.synchronize()
+        assert torch.equal(out32, want), (act, int((out32 != want).sum()))
+        assert torch.equal(out16[:, :N], want.to(torch.float16)), act
+        assert not bool(out16[:, N:].any())
+
+
+@pytest.mark.parametrize("M", [128, 600])
+def test_fc_dgrad_exact_at_fc6(cuda, M):
+    """pcnn_fc_dgrad_f16_tc at fc6 (N = 25,088 input features, K = 4096) with the ReLU mask of the stored pooled features:
+    out = (dy @ W^T) * [mask > 0], exact against the float64 product."""
+    import ctypes
+    from posecnn_b200._lib import check, lib, ptr, stream, workspace
+    from tests.util import fc_plan, int_operands
+    N, K = 25088, 4096
+    g = torch.Generator().manual_seed(M + 1)
+    dy = int_operands((M, K), -1, 1, g).to(torch.float16).to(cuda)
+    wt = int_operands((N, K), -1, 1, g).to(torch.float16).to(cuda)          # [in][out]: the transposed fc6 weights
+    mask = int_operands((M, N), -1, 1, g).to(torch.float16).to(cuda)
+    plan = fc_plan(M, N, K)
+    print(f"fc6 dgrad M={M}: {plan['splits']} splits x {plan['chunks_per_split']} K chunks")
+    out = torch.empty((M, N), dtype=torch.float16, device=cuda)
+    nbytes = ctypes.c_size_t(0)
+    check(lib().pcnn_fc_workspace_bytes(M, N, K, ctypes.byref(nbytes)))
+    ws = workspace("fc", nbytes.value, cuda)
+    check(lib().pcnn_fc_dgrad_f16_tc(ptr(dy), ptr(wt), M, N, K, ptr(mask), ptr(out), N, ptr(ws), ctypes.c_size_t(ws.numel()), stream()))
+    want = ((dy.double() @ wt.double().t()) * (mask > 0)).float().to(torch.float16)
+    torch.cuda.synchronize()
+    assert torch.equal(out, want), int((out != want).sum())
