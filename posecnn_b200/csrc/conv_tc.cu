@@ -13,9 +13,10 @@
 //   * the box lands in shared memory as 128 rows x 128 B with the 128-byte swizzle, which is
 //     exactly the canonical K-major wgmma operand layout, so wgmma reads it in place;
 //   * warp roles: warps 0-7 = two consumer warpgroups (pixel rows 0-63 / 64-127 of the tile): wgmma with the
-//     accumulators in registers, then the epilogue (bias, ReLU, bf16 pack, TMA store) from registers; warp 8 is the
-//     TMA producer, which keeps filling the stage ring during the epilogue.  Persistent CTAs, one per SM, static
-//     round-robin tile schedule.
+//     accumulators in registers, then the epilogue (bias, ReLU, bf16 pack, TMA store) from registers; warpgroup 2
+//     (warps 8-11) gives its registers to the consumers (setmaxnreg: 2 x 128 x 232 + 128 x 40 <= 64 K) and one thread of
+//     it is the TMA producer, which keeps filling the stage ring during the epilogue.  Persistent CTAs, one per SM,
+//     static round-robin tile schedule.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <stdlib.h>
@@ -33,7 +34,9 @@ static_assert(kTileH * kTileW == kTileM, "pixel tile = two wgmma M blocks");
 constexpr int kABytes = kTileM * kKC * 2;                         // 16 KB
 constexpr int kConsumers = 256;                                   // two consumer warpgroups
 constexpr int kProducerWarp = kConsumers / 32;                    // warp 8
-constexpr int kThreadsConv = kConsumers + 32;                     // wgmma kernels get registers per warpgroup: 3 x 128 x 168 fit
+constexpr int kThreadsConv = kConsumers + 128;                    // k_conv_tc: consumer warpgroups + a producer warpgroup
+constexpr int kConsumerRegs = 232, kProducerRegs = 40;            // k_conv_tc after setmaxnreg: 256 x 232 + 128 x 40 <= 64 K
+constexpr int kThreadsRow = kConsumers + 32;                      // k_conv_row2: consumer warpgroups + one producer warp (168 regs)
 constexpr int kStageBytes = 16 * 1024;                            // epilogue staging: one 64-channel group
 
 struct ConvParams {
@@ -129,9 +132,10 @@ k_conv_tc(const __grid_constant__ CUtensorMap map_in, const __grid_constant__ CU
     }
     __syncthreads();
 
-    if (warp == kProducerWarp) {
-        // ===================== TMA producer =====================
-        if (elect_one()) {
+    if (warp >= kProducerWarp) {
+        // ===================== TMA producer: one thread of warpgroup 2 =====================
+        setmaxnreg_dec<kProducerRegs>();
+        if (warp == kProducerWarp && elect_one()) {
             int stage = 0;
             uint32_t phase = 0;
             for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
@@ -142,6 +146,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap map_in, const __grid_constant__ CU
                 const int img = rest / p.tiles_h;
                 const int h0 = th * p.tile_h, w0 = tw * p.tile_w, n0 = nt * BN;
                 const int pad = p.ksize / 2;
+#pragma unroll 1   // the producer runs on 40 registers
                 for (int ks = 0; ks < ksteps; ks++) {
                     const int tap = ks / kchunks, c0 = (ks % kchunks) * kKC;
                     const int dy = tap / p.ksize - pad, dx = tap % p.ksize - pad;
@@ -156,6 +161,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap map_in, const __grid_constant__ CU
         }
     } else {
         // ===================== consumer warpgroups: MMA + epilogue =====================
+        setmaxnreg_inc<kConsumerRegs>();
         const int wg = warp >> 2, wq = warp & 3;
         const int row = wg * 64 + wq * 16 + (lane >> 2);   // first of the two tile rows (pixels) this thread holds
         float acc[BN / 2];
@@ -246,7 +252,7 @@ struct RowPlan {
 };
 
 template <int BN, bool RESB>
-__global__ void __launch_bounds__(kThreadsConv, 1)
+__global__ void __launch_bounds__(kThreadsRow, 1)
 k_conv_row2(const __grid_constant__ CUtensorMap map_in /*box {64,130,4,1}*/, const __grid_constant__ CUtensorMap map_w,
             const __grid_constant__ CUtensorMap map_out /*box {64,128,1,1}, or {64,64,1,1} of the pooled tensor*/,
             const ConvParams p)
@@ -855,7 +861,7 @@ static int launch_conv_row2(const CUtensorMap& mi, const CUtensorMap& mw, const 
     PCNN_SMEM_OPTIN((k_conv_row2<BN, RESB>), Plan::kTotal, "conv_row2");
     int grid = p.total_tiles < num_sms ? p.total_tiles : num_sms;
     if (RESB) grid = grid / p.n_tiles_n * p.n_tiles_n;  // every CTA owns one N tile
-    k_conv_row2<BN, RESB><<<grid, kThreadsConv, Plan::kTotal, st>>>(mi, mw, mo, p);
+    k_conv_row2<BN, RESB><<<grid, kThreadsRow, Plan::kTotal, st>>>(mi, mw, mo, p);
     return check_launch("conv_row2");
 }
 
@@ -893,8 +899,8 @@ static int conv_bf16_tc_impl(const void* in, const void* weights, const float* b
     PCNN_REQUIRE(Cout % 64 == 0 && Cout >= 64, "conv: Cout must be a multiple of 64 (got %d)", Cout);
     PCNN_REQUIRE(B >= 1 && H >= 1 && W >= 1, "conv: bad shape");
     int bn = block_n;
-    // default N tile: 256 for the deep layers (K = taps * Cin >= 2304), where it is faster on the H100 although its two m64n256
-    // accumulators spill a few registers at the 168-register cap (tools/bench_conv.py: conv4_2 1.08 vs 1.37 ms at batch 32); 128 below
+    // default N tile: 256 for the deep layers (K = taps * Cin >= 2304), where it is faster on the H100 (tools/bench_trunk.py prints
+    // every such layer at both N tiles); 128 below
     if (bn == 0) bn = Cout % 256 == 0 && ksize * ksize * Cin >= 2304 ? 256 : (Cout % 128 == 0 ? 128 : 64);
     PCNN_REQUIRE((bn == 64 || bn == 128 || bn == 256) && Cout % bn == 0, "conv: block_n %d does not divide Cout %d", bn, Cout);
     int dev = 0, sms = kNumSMs;

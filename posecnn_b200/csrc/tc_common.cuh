@@ -74,6 +74,12 @@ __device__ __forceinline__ void tma_load_2d(void* smem, const CUtensorMap* map, 
         "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
         : "memory");
 }
+// warpgroup register reallocation (the whole warpgroup executes it)
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+
 __device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, const void* smem, int c0, int c1, int c2, int c3)
 {
     asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(map),
