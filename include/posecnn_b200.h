@@ -180,6 +180,10 @@ int pcnn_conv3x3_small_cin(const float* in, const float* weights_hwio, const flo
  * pre-processing of lib/fcn/test.py:37-110 fused) -> [B,H,W,64] bf16 with K = tap*3 + c, then a 1x1 pcnn_conv_bf16_tc */
 int pcnn_im2col_c3(const void* in, int in_is_u8, const float* mean3_host, void* out_bf16, int B, int H, int W,
                    void* stream);
+/* the same im2col view of the RGB-D network's depth blob, formed from a RAW depth image [B,H,W] f32 (sensor units) with
+ * the operation sequence of pcnn_conv1_depth_fused_tc (clip(d / 2000, 0, 1) * 255 tiled x3 - mean, float32 like numpy):
+ * the input of the conv1_1_p weight gradient */
+int pcnn_im2col_depth(const float* depth, const float* mean3_host, void* out_bf16, int B, int H, int W, void* stream);
 /* conv1_1 with the im2col built in shared memory (no HBM round trip): in [B,H,W,3] u8 (minus mean) or f32,
  * weights [64][64] bf16 in the K order tap*3 + c (zero padded), bias [64] -> out [B,H,W,64] bf16 */
 int pcnn_conv1_fused_tc(const void* in, int in_is_u8, const float* mean3_host, const void* weights_bf16,

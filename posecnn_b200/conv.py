@@ -79,6 +79,18 @@ def im2col_c3(x: torch.Tensor, mean=None) -> torch.Tensor:
     return out
 
 
+def im2col_depth(depth: torch.Tensor, mean) -> torch.Tensor:
+    """First layer of the depth trunk: depth [B,H,W] f32 (raw, sensor units) -> [B,H,W,64] bf16, the im2col view (K = tap*3 + c)
+    of the blob clip(d / 2000, 0, 1) * 255 tiled x3 - mean, formed as conv1_depth_fused forms it (the conv1_1_p weight-gradient input)."""
+    import ctypes
+    assert depth.is_cuda and depth.is_contiguous() and depth.dtype == torch.float32 and depth.dim() == 3
+    B, H, W = depth.shape
+    out = torch.empty((B, H, W, 64), dtype=torch.bfloat16, device=depth.device)
+    m = (ctypes.c_float * 3)(*mean)
+    check(lib().pcnn_im2col_depth(ptr(depth), m, ptr(out), B, H, W, stream()))
+    return out
+
+
 def conv1_1_weights_to_tc(w_hwio: torch.Tensor) -> torch.Tensor:
     """[3,3,3,Cout] f32 -> [Cout, 64] bf16 matching im2col_c3's K order (tap*3 + c)."""
     co = w_hwio.shape[3]

@@ -479,6 +479,14 @@ constexpr int kC1Smem = kC1BarOff + 256 + 1024;
 // (lib/fcn/test.py:70-76) is formed on the fly in float32 exactly as numpy forms it.
 struct DepthIn { float d; };
 
+// The grey value clip(d / 2000, 0, 1) * 255 of the depth blob, one rounding per numpy operation (the caller subtracts the
+// channel mean with __fsub_rn).  k_conv1_tc and k_im2col_c3 both form the blob here, so the conv1_1_p weight gradient sees
+// exactly the values the forward MMA consumed.
+__device__ __forceinline__ float depth_gray(float d)
+{
+    return __fmul_rn(fminf(fmaxf(__fdiv_rn(d, 2000.f), 0.f), 1.f), 255.f);
+}
+
 template <typename TIn>
 __global__ void __launch_bounds__(kC1Threads, 1)
 k_conv1_tc(const TIn* __restrict__ in, const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_out,
@@ -593,7 +601,7 @@ k_conv1_tc(const TIn* __restrict__ in, const __grid_constant__ CUtensorMap map_w
                         const bool ok = rowok && xx >= 0 && xx < p.W;
                         if constexpr (std::is_same<TIn, DepthIn>::value) {
                             float g = 0.f;
-                            if (ok) g = __fmul_rn(fminf(fmaxf(__fdiv_rn(base[(size_t)yy * p.W + xx].d, 2000.f), 0.f), 1.f), 255.f);
+                            if (ok) g = depth_gray(base[(size_t)yy * p.W + xx].d);
                             v[(dy * 3 + dx) * 3 + 0] = ok ? __fsub_rn(g, m0) : 0.f;
                             v[(dy * 3 + dx) * 3 + 1] = ok ? __fsub_rn(g, m1) : 0.f;
                             v[(dy * 3 + dx) * 3 + 2] = ok ? __fsub_rn(g, m2) : 0.f;
@@ -754,7 +762,8 @@ k_conv_small_cin(const float* __restrict__ in, const float* __restrict__ w /*[3]
 // im2col for the first layer only (Cin = 3, K = 27 < one wgmma K chunk of 64): [B,H,W,3] -> [B,H,W,64] bf16 with
 // K index = tap * 3 + c (zero beyond 27), so conv1_1 runs on the tensor cores as a 1x1 convolution.
 // The input pre-processing of the caller (lib/fcn/test.py:37-110: BGR - PIXEL_MEANS) is fused for uint8
-// input: value = (float)u8 - mean[c].
+// input: value = (float)u8 - mean[c].  DepthIn: the depth blob depth_gray(d) - mean[c] of a raw [B,H,W] depth image, the
+// values k_conv1_tc<DepthIn> feeds its MMA (the im2col view the conv1_1_p weight gradient reads).
 template <typename TIn>
 __global__ void __launch_bounds__(256)
 k_im2col_c3(const TIn* __restrict__ in, __nv_bfloat16* __restrict__ out, int H, int W, float m0, float m1, float m2)
@@ -763,15 +772,21 @@ k_im2col_c3(const TIn* __restrict__ in, __nv_bfloat16* __restrict__ out, int H, 
     // CTAs at batch 64 were launch-bound).  The 3 x 130 x 3 input patch (mean subtracted, zero outside the image = SAME padding)
     // is staged in shared memory once; thread (x, j) then packs the 8 K-values k = 8j .. 8j+7 (K order tap*3 + c) into one 16-byte store.
     constexpr int kSeg = 128;
+    constexpr int kInCh = std::is_same<TIn, DepthIn>::value ? 1 : 3;
     __shared__ float patch[3][(kSeg + 2) * 3];
     const int y = blockIdx.y, n = blockIdx.z, x0 = blockIdx.x * kSeg, t = threadIdx.x;
-    const TIn* img = in + (size_t)n * H * W * 3;
+    const TIn* img = in + (size_t)n * H * W * kInCh;
     constexpr int kRow = (kSeg + 2) * 3;
     for (int i = t; i < 3 * kRow; i += 256) {
         const int r = i / kRow, rem = i - r * kRow, px = rem / 3, c = rem - px * 3;
         const int yy = y + r - 1, xx = x0 + px - 1;
         float v = 0.f;
-        if (yy >= 0 && yy < H && xx >= 0 && xx < W) v = (float)img[(yy * W + xx) * 3 + c] - (c == 0 ? m0 : (c == 1 ? m1 : m2));
+        if (yy >= 0 && yy < H && xx >= 0 && xx < W) {
+            if constexpr (std::is_same<TIn, DepthIn>::value)
+                v = __fsub_rn(depth_gray(img[yy * W + xx].d), c == 0 ? m0 : (c == 1 ? m1 : m2));
+            else
+                v = (float)img[(yy * W + xx) * 3 + c] - (c == 0 ? m0 : (c == 1 ? m1 : m2));
+        }
         patch[r][rem] = v;
     }
     __syncthreads();
@@ -1002,6 +1017,20 @@ extern "C" int pcnn_im2col_c3(const void* in, int in_is_u8, const float* mean3_h
     else
         k_im2col_c3<float><<<grid, 256, 0, st>>>((const float*)in, (__nv_bfloat16*)out_bf16, H, W, m0, m1, m2);
     return check_launch("im2col_c3");
+}
+
+// first-layer im2col of the depth trunk: a raw depth image [B,H,W] f32 (sensor units) -> [B,H,W,64] bf16 of its blob
+// clip(d / 2000, 0, 1) * 255 tiled x3 - mean (lib/fcn/test.py:70-76), the view the conv1_1_p weight gradient reads
+extern "C" int pcnn_im2col_depth(const float* depth, const float* mean3_host, void* out_bf16, int B, int H, int W, void* stream)
+{
+    PCNN_REQUIRE(depth && out_bf16, "im2col_depth: NULL tensor pointer");
+    PCNN_REQUIRE(B >= 1 && H >= 1 && W >= 1, "im2col_depth: bad shape (%d,%d,%d)", B, H, W);
+    PCNN_REQUIRE(H <= 65535 && B <= 65535, "im2col_depth: image too tall for the launch grid");
+    float m0 = 0.f, m1 = 0.f, m2 = 0.f;
+    if (mean3_host) { m0 = mean3_host[0]; m1 = mean3_host[1]; m2 = mean3_host[2]; }
+    dim3 grid((W + 127) / 128, H, B);
+    k_im2col_c3<DepthIn><<<grid, 256, 0, (cudaStream_t)stream>>>((const DepthIn*)depth, (__nv_bfloat16*)out_bf16, H, W, m0, m1, m2);
+    return check_launch("im2col_depth");
 }
 
 // conv1_1 fused: in [B,H,W,3] (u8 minus mean, or f32), weights [64][64] bf16 in im2col K order (tap*3 + c, zero padded),

@@ -7,6 +7,8 @@ Reference: the training graph lib/networks/vgg16_convs.py:79-212 driven by lib/f
     loss_pose   = Averagedistance(l2_normalize(poses_tanh * poses_weight), poses_target, poses_weight, points, symmetry)
     optimizer   = tf.train.MomentumOptimizer(lr, 0.9) (train.py:633), l2_regularizer(WEIGHT_REG) on every conv / fc weight AND bias.
 This is the keep_prob = 1.0 graph (the reference trains with dropout 0.5; random masks cannot be compared, SURVEY App. A.7).
+input_format='RGBD' adds the depth trunk conv1_1_p .. conv5_3_p (vgg16_convs.py:99-126): score_conv4 / score_conv5 read the channel
+concat [colour | depth] of conv4_3 / conv5_3 (c_i = 1024), the vertex heads, Hough voting and RoiPool read the colour trunk only.
 
 Everything heavy runs on this package's own kernels:
     forward   wgmma convolutions (bf16), un-fused heads (add + up2, 1x1 on the tensor cores, fused up8 / softmax / arg-max),
@@ -48,8 +50,10 @@ def _tc_dgrad(w_tc: torch.Tensor, k: int) -> torch.Tensor:
 
 class Trainer:
     def __init__(self, net, lr=0.001, momentum=0.9, weight_decay=1e-4, vertex_w=1.0, vertex_w_inside=10.0, margin=0.01, world=1):
-        assert net.is_train and not net.fold_vertex_head and net.input_format == "COLOR", \
-            "Trainer needs vgg16_convs(is_train=True, fold_vertex_head=False, input_format='COLOR')"
+        assert net.is_train and not net.fold_vertex_head and net.input_format in ("COLOR", "RGBD"), \
+            "Trainer needs vgg16_convs(is_train=True, fold_vertex_head=False, input_format='COLOR' or 'RGBD')"
+        self.rgbd = net.input_format == "RGBD"
+        self.trunks = ("", "_p") if self.rgbd else ("",)           # conv*_p: the depth trunk (vgg16_convs.py:99-117)
         self.net, self.lr, self.mu, self.wd = net, float(lr), float(momentum), float(weight_decay)
         self.vertex_w, self.w_inside, self.margin, self.world = float(vertex_w), float(vertex_w_inside), float(margin), int(world)
         self.C = net.num_classes
@@ -65,16 +69,19 @@ class Trainer:
             self.tc[name] = copy16
             self.kind[name] = kind
 
-        for name in CONV_NAMES:
-            w = P[f"{name}/weights"]
-            if name == "conv1_1":
-                add(name + "/w", w.reshape(27, 64).t().contiguous(), None, 0)                     # [64][27], refreshed into the padded [64][64] copy
-            else:
-                wt = w.permute(3, 0, 1, 2).reshape(w.shape[3], -1)
-                add(name + "/w", wt, wt.to(torch.bfloat16).contiguous(), 0)
-            add(name + "/b", P[f"{name}/biases"].clone(), None, 0)
+        for sfx in self.trunks:
+            for layer in CONV_NAMES:
+                name = layer + sfx
+                w = P[f"{name}/weights"]
+                if layer == "conv1_1":
+                    add(name + "/w", w.reshape(27, 64).t().contiguous(), None, 0)                 # [64][27], refreshed into the padded [64][64] copy
+                else:
+                    wt = w.permute(3, 0, 1, 2).reshape(w.shape[3], -1)
+                    add(name + "/w", wt, wt.to(torch.bfloat16).contiguous(), 0)
+                add(name + "/b", P[f"{name}/biases"].clone(), None, 0)
         for name in ("score_conv4", "score_conv5", "score_conv4_vertex", "score_conv5_vertex"):
-            wt = P[f"{name}/weights"].reshape(512, -1).t().contiguous()                           # [Cout][512]
+            w = P[f"{name}/weights"]
+            wt = w.reshape(w.shape[2], w.shape[3]).t().contiguous()                               # [Cout][512], RGBD score: [Cout][1024] (colour first)
             add(name + "/w", wt, wt.to(torch.bfloat16).contiguous(), 0)
             add(name + "/b", P[f"{name}/biases"].clone(), None, 0)
         ws = torch.zeros((64, net.num_units), device=dev)                                         # `score` 1x1: [C -> 64 rows][64]
@@ -93,18 +100,26 @@ class Trainer:
             add(name + "/w", wt, wt.to(torch.float16).contiguous(), 1)
             add(name + "/b", P[f"{name}/biases"].clone(), None, 0)
         self.conv1_tc = conv.conv1_1_weights_to_tc(P["conv1_1/weights"])
+        self.conv1_tc_p = conv.conv1_1_weights_to_tc(P["conv1_1_p/weights"]) if self.rgbd else None
         self._refresh_derived()
         self.zero_bias = {n: torch.zeros(n, device=dev) for n in (64, 128, 256, 512)}
 
     # ------------------------------------------------------------------ derived weight copies
     def _refresh_derived(self):
         """Copies the backward GEMMs read: input-gradient (flipped / transposed) weights of every convolution, [in][out] fp16 copies of
-        the fully connected weights, the padded conv1_1 tile."""
+        the fully connected weights, the padded conv1_1 tile (and conv1_1_p's)."""
         self.dg = {}
-        for name in CONV_NAMES[1:]:
-            self.dg[name] = _tc_dgrad(self.tc[name + "/w"], 3)
+        for sfx in self.trunks:
+            for name in CONV_NAMES[1:]:
+                self.dg[name + sfx] = _tc_dgrad(self.tc[name + sfx + "/w"], 3)
         for name in ("score_conv4", "score_conv5", "score_conv4_vertex", "score_conv5_vertex", "score", "vertex_pred"):
             self.dg[name] = _tc_dgrad(self.tc[name + "/w"], 1)
+        if self.rgbd:
+            # score_conv4/5 read the concat [colour 512 | depth 512]: their input-gradient weights [1024][U] split into two
+            # contiguous [512][U] halves, one input-gradient convolution per trunk
+            for name in ("score_conv4", "score_conv5"):
+                d = self.dg[name]
+                self.dg[name], self.dg[name + "_p"] = d[:512], d[512:]
         self.fc_t = {}
         for name in ("fc6", "fc7", "fc8"):
             w = self.tc[name + "/w"]
@@ -113,17 +128,22 @@ class Trainer:
             self.fc_t[name] = t
         self.conv1_tc.zero_()
         self.conv1_tc[:, :27] = self.master["conv1_1/w"].to(torch.bfloat16)
+        if self.rgbd:
+            self.conv1_tc_p.zero_()
+            self.conv1_tc_p[:, :27] = self.master["conv1_1_p/w"].to(torch.bfloat16)
 
     def export_params(self):
         """Write the fp32 master weights back into net.params (TF layouts) and re-derive the inference copies."""
         P, C = self.net.params, self.C
-        for name in CONV_NAMES:
-            shp = P[f"{name}/weights"].shape
-            if name == "conv1_1":
-                P[f"{name}/weights"] = self.master[name + "/w"].t().reshape(shp).contiguous()
-            else:
-                P[f"{name}/weights"] = self.master[name + "/w"].view(shp[3], shp[0], shp[1], shp[2]).permute(1, 2, 3, 0).contiguous()
-            P[f"{name}/biases"] = self.master[name + "/b"].clone()
+        for sfx in self.trunks:
+            for layer in CONV_NAMES:
+                name = layer + sfx
+                shp = P[f"{name}/weights"].shape
+                if layer == "conv1_1":
+                    P[f"{name}/weights"] = self.master[name + "/w"].t().reshape(shp).contiguous()
+                else:
+                    P[f"{name}/weights"] = self.master[name + "/w"].view(shp[3], shp[0], shp[1], shp[2]).permute(1, 2, 3, 0).contiguous()
+                P[f"{name}/biases"] = self.master[name + "/b"].clone()
         for name in ("score_conv4", "score_conv5", "score_conv4_vertex", "score_conv5_vertex"):
             P[f"{name}/weights"] = self.master[name + "/w"].t().reshape(P[f"{name}/weights"].shape).contiguous()
             P[f"{name}/biases"] = self.master[name + "/b"].clone()
@@ -138,21 +158,40 @@ class Trainer:
         self.net.prepare()
 
     # ------------------------------------------------------------------ forward (training graph, activations kept)
-    def forward(self, data, gt_label_2d, centers, meta_data, extents, gt_poses, points, symmetry, batch_global=None, batch_offset=0):
+    def _trunk_fwd(self, A, x, sfx=""):
+        """conv1_2 .. conv5_3 of one trunk on its conv1_1 output x; every activation is kept in A (the backward pass reads them)."""
+        M, T = self.master, self.tc
+        A["conv1_1" + sfx] = x
+        for layer in CONV_NAMES[1:]:
+            name = layer + sfx
+            x = conv.conv_bf16(x, T[name + "/w"], M[name + "/b"], 3, True)
+            A[name] = x
+            if layer in POOL_AFTER and layer != "conv5_3":
+                x = conv.maxpool2x2(x)
+                A[name + "/pool"] = x
+
+    def forward(self, data, gt_label_2d, centers, meta_data, extents, gt_poses, points, symmetry, batch_global=None, batch_offset=0,
+                depth=None, data_p=None):
+        """RGBD: the depth trunk reads depth= (a raw [B,H,W] f32 depth image, sensor units; its blob is formed in conv1_1_p's loader)
+        or data_p= (the pre-processed blob [B,H,W,3] f32), as vgg16_convs.forward does."""
         net, C, M, T = self.net, self.C, self.master, self.tc
         B, H, W, _ = data.shape
         A = {}                                    # activations by layer name (bf16 NHWC), "<pool>" = pooled tensors
-        x = conv.conv1_fused(data, self.conv1_tc, M["conv1_1/b"], PIXEL_MEANS, True)
-        A["conv1_1"] = x
-        for name in CONV_NAMES[1:]:
-            x = conv.conv_bf16(x, T[name + "/w"], M[name + "/b"], 3, True)
-            A[name] = x
-            if name in POOL_AFTER and name != "conv5_3":
-                x = conv.maxpool2x2(x)
-                A[name + "/pool"] = x
+        self._trunk_fwd(A, conv.conv1_fused(data, self.conv1_tc, M["conv1_1/b"], PIXEL_MEANS, True))
         c4, c5 = A["conv4_3"], A["conv5_3"]
-        s4 = conv.conv_bf16(c4, T["score_conv4/w"], M["score_conv4/b"], 1, True)
-        s5 = conv.conv_bf16(c5, T["score_conv5/w"], M["score_conv5/b"], 1, True)
+        h4, h5 = c4, c5
+        if self.rgbd:
+            assert (depth is None) != (data_p is None), "the RGB-D training step needs exactly one of depth= and data_p="
+            if depth is not None:
+                x = conv.conv1_depth_fused(depth, self.conv1_tc_p, M["conv1_1_p/b"], PIXEL_MEANS, True)
+            else:
+                x = conv.conv1_fused(data_p, self.conv1_tc_p, M["conv1_1_p/b"], None, True)
+            self._trunk_fwd(A, x, "_p")
+            # concat_conv4 / concat_conv5 (vgg16_convs.py:119-126): colour channels first; kept as score_conv4/5's wgrad input
+            h4, h5 = torch.cat([c4, A["conv4_3_p"]], 3), torch.cat([c5, A["conv5_3_p"]], 3)
+            A.update(concat_conv4=h4, concat_conv5=h5, depth_in=depth if depth is not None else data_p)
+        s4 = conv.conv_bf16(h4, T["score_conv4/w"], M["score_conv4/b"], 1, True)
+        s5 = conv.conv_bf16(h5, T["score_conv5/w"], M["score_conv5/b"], 1, True)
         v4 = conv.conv_bf16(c4, T["score_conv4_vertex/w"], M["score_conv4_vertex/b"], 1, False)
         v5 = conv.conv_bf16(c5, T["score_conv5_vertex/w"], M["score_conv5_vertex/b"], 1, False)
         h, w = H // 8, W // 8
@@ -325,8 +364,9 @@ class Trainer:
         check(lib().pcnn_up2_bwd_bf16(ptr(d_add_v), ptr(None), B, h, w, 128, ptr(d_v5), stream()))
         self._emit(grads, "score_conv5_vertex/b", bw.relu_bwd(d_v5, None, False, want_bias=True, want_dz=False)[1])
         c4, c5 = A["conv4_3"], A["conv5_3"]
-        self._emit(grads, "score_conv4/w", bw.conv_wgrad(c4, d_s4, 1))
-        self._emit(grads, "score_conv5/w", bw.conv_wgrad(c5, d_s5, 1))
+        # RGB-D: score_conv4/5 read the 1024-channel concat, so their weight gradient is one wgrad on it
+        self._emit(grads, "score_conv4/w", bw.conv_wgrad(A["concat_conv4"] if self.rgbd else c4, d_s4, 1))
+        self._emit(grads, "score_conv5/w", bw.conv_wgrad(A["concat_conv5"] if self.rgbd else c5, d_s5, 1))
         self._emit(grads, "score_conv4_vertex/w", bw.conv_wgrad(c4, d_add_v, 1))
         self._emit(grads, "score_conv5_vertex/w", bw.conv_wgrad(c5, d_v5, 1))
         z512 = self.zero_bias[512]
@@ -334,30 +374,44 @@ class Trainer:
                             conv.conv_bf16(d_add_v, self.dg["score_conv4_vertex"], z512, 1, False), g4_roi)
         g5 = bw.add_to_bf16(conv.conv_bf16(d_s5, self.dg["score_conv5"], z512, 1, False),
                             conv.conv_bf16(d_v5, self.dg["score_conv5_vertex"], z512, 1, False), g5_roi)
-        # ---- trunk, top down.  g = gradient w.r.t. the (post-ReLU) output of the current layer
-        g = g5
-        for name in reversed(CONV_NAMES):
+        # ---- trunk, top down
+        self._trunk_bwd(grads, A, g5, g4, "", lambda: conv.im2col_c3(data, PIXEL_MEANS))
+        if self.rgbd:
+            # the depth trunk's gradient enters through the depth half of the concat only (the vertex heads and RoiPool read
+            # the colour trunk, vgg16_convs.py:151-182)
+            g4_p = conv.conv_bf16(d_s4, self.dg["score_conv4_p"], z512, 1, False)
+            g5_p = conv.conv_bf16(d_s5, self.dg["score_conv5_p"], z512, 1, False)
+            x_p = A["depth_in"]
+            cols_p = (lambda: conv.im2col_depth(x_p, PIXEL_MEANS)) if x_p.dim() == 3 else (lambda: conv.im2col_c3(x_p, None))
+            self._trunk_bwd(grads, A, g5_p, g4_p, "_p", cols_p)
+        return grads
+
+    def _trunk_bwd(self, grads, A, g5, g4, sfx, im2col):
+        """conv5_3 .. conv1_1 of one trunk, top down.  g5 / g4: the gradients entering conv5_3 / conv4_3 from the heads (and
+        RoiPool); im2col() builds the [B,H,W,64] view of the trunk's input that conv1_1's weight gradient reads."""
+        g = g5                                    # gradient w.r.t. the (post-ReLU) output of the current layer
+        for layer in reversed(CONV_NAMES):
+            name = layer + sfx
             y = A[name]
-            if name == "conv4_3":
+            if layer == "conv4_3":
                 # conv4_3 feeds pool4 (gradient routed to the window maxima) AND the heads / RoiPool (g4)
                 dz = bw.add_to_bf16(bw.maxpool_relu_bwd(g, y), bw.relu_bwd(g4, y, True))
                 db = bw.relu_bwd(dz, None, False, want_bias=True, want_dz=False)[1]
-            elif name in POOL_AFTER and name != "conv5_3":
+            elif layer in POOL_AFTER and layer != "conv5_3":
                 dz, db = bw.maxpool_relu_bwd(g, y, want_bias=True)
             else:
                 dz, db = bw.relu_bwd(g, y, True, want_bias=True)
             self._emit(grads, name + "/b", db)
-            if name == "conv1_1":
-                # Cin = 3: the weight gradient is the 1x1 tensor-core wgrad on the im2col view of the image (K = tap * 3 + c, the same
+            if layer == "conv1_1":
+                # Cin = 3: the weight gradient is the 1x1 tensor-core wgrad on the im2col view of the input (K = tap * 3 + c, the same
                 # bf16 (pixel - mean) values the forward MMA consumed); a CUDA-core kernel (pcnn_conv1_wgrad) took 2.6 ms at batch 16
-                cols = conv.im2col_c3(data, PIXEL_MEANS)                                       # [B,H,W,64] bf16, 27 columns used
+                cols = im2col()                                                                 # [B,H,W,64] bf16, 27 columns used
                 self._emit(grads, name + "/w", bw.conv_wgrad(cols, dz, 1)[:, :27].contiguous())
                 break
-            prev = CONV_NAMES[CONV_NAMES.index(name) - 1]
+            prev = CONV_NAMES[CONV_NAMES.index(layer) - 1] + sfx
             x_in = A.get(prev + "/pool", A[prev])
             self._emit(grads, name + "/w", bw.conv_wgrad(x_in, dz, 3))
             g = conv.conv_bf16(dz, self.dg[name], self.zero_bias[x_in.shape[3]], 3, False)      # gradient w.r.t. this layer's input
-        return grads
 
     def update(self, grads):
         """accum = mu * accum + (grad + wd * w); w -= lr * accum, on the fp32 masters; 16-bit tensor-core copies refreshed in the same
@@ -372,8 +426,10 @@ class Trainer:
                                           f32(1.0), ptr(c16), int(self.kind[name]), stream()))
         self._refresh_derived()
 
-    def step(self, data, gt_label_2d, centers, meta_data, extents, gt_poses, points, symmetry, batch_global=None, batch_offset=0):
-        A = self.forward(data, gt_label_2d, centers, meta_data, extents, gt_poses, points, symmetry, batch_global, batch_offset)
+    def step(self, data, gt_label_2d, centers, meta_data, extents, gt_poses, points, symmetry, batch_global=None, batch_offset=0,
+             depth=None, data_p=None):
+        A = self.forward(data, gt_label_2d, centers, meta_data, extents, gt_poses, points, symmetry, batch_global, batch_offset,
+                         depth=depth, data_p=data_p)
         grads = self.backward(A, gt_label_2d, centers)
         self.update(grads)
         loss_cls, loss_vertex, loss_pose = A["cls_out"][0:1], self.vertex_w * A["vtx_out"][0:1], A["loss_pose"]
