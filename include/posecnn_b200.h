@@ -286,6 +286,30 @@ int pcnn_fc_f16_tc(const void* a_f16, const void* w_f16, const float* bias, int 
                    void* out_f16, int ld_out, float* out_f32, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------
+ * Domain-adaptation branch (networks/vgg16_convs.py:202-212, loss fcn/train.py:508-513), csrc/domain.cu:
+ *   pool_score -> gradient_reversal(lambda) -> fc9 (25088 -> 256, ReLU) -> domain_score = fc(2) WITH ReLU (Network.fc's
+ *   default, network.py:393,420) -> softmax -> argmax.  fc9 itself runs on pcnn_fc_f16_tc / pcnn_fc_dgrad_f16_tc /
+ *   pcnn_fc_wgrad_f16_tc.
+ *  pcnn_domain_tail   one launch over rows <= PCNN_HOUGH_MAX_ROWS: fc9_f16 [rows, ld] (fc9's fp16 output, 256 units, ld % 8 == 0,
+ *      16-byte aligned), w10 [2][256] f32 (the domain_score weights, output-major), b10 [2] -> domain_score, domain_prob [rows, 2]
+ *      f32 (score after its ReLU), domain_label [rows] int32 (first maximum on ties).  label_domain [rows] int32 (Hough's
+ *      top_domain) may be NULL (inference: the gradient outputs are not touched).  With labels:
+ *        loss[0] = loss_scale * sum_rows (logsumexp(z) - z[label]);  loss_scale = ADAPT_WEIGHT / (global row count);
+ *        g = loss_scale * (softmax(z) - onehot(label)) * [z > 0];  dw10 [2][256] = g^T fc9;  db10 [2] = sum_rows g;
+ *        d = (g @ w10) * [fc9 > 0];  db9 [256] = sum_rows d;  amax[0] = max |d|;
+ *        dpre9_f16 [rows, ld] = grad_scale * d in fp16 (saturating at +-65504; columns >= 256 zero): the operand of fc9's
+ *        backward GEMMs, loss-scaled by the caller's power of two grad_scale (the gradients sit below fp16's normal range).
+ *      Every sum over rows runs in a fixed order: two launches give bit-identical outputs.
+ *  pcnn_domain_grad_merge   dst[i] = scale_a * a[i] + scale_b * b[i] (fp32 products rounded, then added; n % 8 == 0, 16-byte
+ *      aligned): the gradient of pool_score from the pose head (a = fc6's fp16 input gradient, scale_a = 1 / S) and the domain
+ *      branch (b = fc9's, scale_b = -lambda / S_d: the gradient reversal).  With b = 0 it equals pcnn_half_to_float(a, scale_a).
+ */
+int pcnn_domain_tail(const void* fc9_f16, int rows, int ld, const float* w10, const float* b10, const int32_t* label_domain,
+                     float loss_scale, float grad_scale, float* domain_score, float* domain_prob, int32_t* domain_label,
+                     float* loss, float* amax, float* dw10, float* db10, float* db9, void* dpre9_f16, void* stream);
+int pcnn_domain_grad_merge(const void* a_f16, float scale_a, const void* b_f16, float scale_b, size_t n, float* dst, void* stream);
+
+/* ---------------------------------------------------------------------------------------
  * FCN heads after the 1x1 convolutions on conv4_3 / conv5_3 (networks/vgg16_convs.py:128-163):
  * add + fixed-bilinear conv2d_transpose (networks/network.py:141-157, 207-222) + `score` /
  * `vertex_pred` 1x1 + softmax / arg-max.  The bilinear up-sampling commutes with the 1x1

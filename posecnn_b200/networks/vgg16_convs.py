@@ -9,6 +9,7 @@ vgg16_convs.setup() (vgg16_convs.py:79-212) is executed eagerly on one CUDA stre
     score / vertex heads                         1x1 on wgmma + fused bilinear/softmax     csrc/heads.cu
     hough_voting_gpu                             csrc/hough_vote.cu
     roi_pool x2 + add, fc6-fc8, tanh             csrc/fc_tc.cu (fused pooling, split-K wgmma GEMMs, fused epilogues)
+    adaptation: fc9, domain_score / prob / label  fc9 on csrc/fc_tc.cu, the 256 -> 2 tail in one launch (csrc/domain.cu)
 
 PyTorch supplies device memory and streams only.
 """
@@ -48,6 +49,9 @@ class vgg16_convs:
         self.vertex_reg = vertex_reg_2d or vertex_reg_3d
         self.vertex_reg_2d = vertex_reg_2d
         self.pose_reg = pose_reg
+        # domain classifier on pool_score (vgg16_convs.py:202-212); built only where the reference builds it
+        self.adaptation = bool(adaptation)
+        self.domain_branch = self.adaptation and bool(vertex_reg_2d) and bool(pose_reg)
         # vgg16_convs.py:18-29
         self.is_train = 1 if is_train else 0
         self.skip_pixels = 10
@@ -79,6 +83,9 @@ class vgg16_convs:
         shapes["fc6/weights"] = (7 * 7 * 512, 4096); shapes["fc6/biases"] = (4096,)
         shapes["fc7/weights"] = (4096, 4096); shapes["fc7/biases"] = (4096,)
         shapes["fc8/weights"] = (4096, 4 * C); shapes["fc8/biases"] = (4 * C,)
+        if self.domain_branch:   # after fc8: the seeded init of every other parameter is unchanged
+            shapes["fc9/weights"] = (7 * 7 * 512, 256); shapes["fc9/biases"] = (256,)
+            shapes["domain_score/weights"] = (256, 2); shapes["domain_score/biases"] = (2,)
         return shapes
 
     def init_random(self, seed=0, bias_std=0.0):
@@ -144,7 +151,7 @@ class vgg16_convs:
         P, T = self.params, self._tc
         T.clear()
         for name, shp in self.param_shapes().items():
-            if not name.endswith("weights") or name.startswith("fc") or name in ("score/weights", "vertex_pred/weights"):
+            if not name.endswith("weights") or name.startswith("fc") or name in ("score/weights", "vertex_pred/weights", "domain_score/weights"):
                 continue
             w = P[name]
             if w.shape[2] == 3:  # conv1_1: im2col K order
@@ -153,6 +160,9 @@ class vgg16_convs:
                 T[name] = conv.hwio_to_tc(w)
         for name in ("fc6", "fc7", "fc8"):
             T[f"{name}/weights"] = pose_head.fc_weights_to_tc(P[f"{name}/weights"])   # [out (padded to x128), in] fp16
+        if self.domain_branch:
+            T["fc9/weights"] = pose_head.fc_weights_to_tc(P["fc9/weights"])                # [256][25088] fp16
+            T["domain_score/w"] = P["domain_score/weights"].t().contiguous()               # [2][256] f32
         T["score/w"] = P["score/weights"].reshape(self.num_units, self.num_classes).contiguous()
         T["vertex_pred/w"] = P["vertex_pred/weights"].reshape(128, 3 * self.num_classes).contiguous()
         if self.fold_vertex_head:
@@ -281,6 +291,13 @@ class vgg16_convs:
             x = pose_head.fc(x, T["fc7/weights"], P["fc7/biases"], "relu")
             L["fc7"] = x
             L["poses_tanh"] = pose_head.fc(x, T["fc8/weights"], P["fc8/biases"], "tanh", torch.float32)   # fc8 + tanh
+            if self.domain_branch:
+                # gradient_reversal is the identity forward; fc9 + ReLU (drop9 keep_prob = 1), domain_score + ReLU, softmax, argmax
+                if self.is_train:
+                    L["label_domain"] = domain[:cap_rows]
+                h9 = pose_head.fc(L["pool_score"], T["fc9/weights"], P["fc9/biases"], "relu")
+                L["fc9"] = h9
+                L.update(pose_head.domain_tail(h9, T["domain_score/w"], P["domain_score/biases"]))
         if not self.is_train:
             # test-time post-processing on the device: per-class NMS + pose assembly (lib/utils/nms.py, test.py:197-211)
             keep, d_rois, d_poses, d_n = dev_nms.nms_pose_capacity(rois, L["poses_init"], L.get("poses_tanh"), num_rois,
@@ -295,17 +312,23 @@ class vgg16_convs:
                 L[k] = L[k][:n]
             if self.pose_reg:
                 L["poses_tanh"] = L["poses_tanh"][:n]
+            for k in ("label_domain", "fc9", "domain_score", "domain_prob", "domain_label"):
+                if k in L:
+                    L[k] = L[k][:n]
         return L
 
 
 def training_losses(net: vgg16_convs, layers: dict, gt_label_2d, vertex_targets, vertex_weights, points, symmetry,
-                    vertex_w: float = 1.0, margin: float = 0.01, centers=None, vertex_w_inside: float = 10.0) -> dict:
+                    vertex_w: float = 1.0, margin: float = 0.01, centers=None, vertex_w_inside: float = 10.0,
+                    adapt_weight: float = 0.1) -> dict:
     """The loss heads of the reference's training graph on the outputs of `forward(..., want_prob=True, want_score=True)`
     of an `is_train` network (lib/fcn/train.py:486-500, vgg16_convs.py:141-147,195-200):
       loss_cls    = cross entropy of log_softmax(score) over the Hardlabel selection (fused, mask not materialised)
       loss_vertex = VERTEX_W * smooth_l1_loss_vertex(vertex_pred, vertex_targets, vertex_weights)
                     (vertex_targets=None + centers [B,C,3]: the fused kernel that derives targets from gt_label_2d / centers)
       loss_pose   = Averagedistance(l2_normalize(poses_tanh * poses_weight), poses_target, poses_weight, points, symmetry)
+      loss_domain = adapt_weight * mean over the ROI rows of sparse_softmax_cross_entropy(domain_score, label_domain)
+                    (net.adaptation only; train.py:508-513, ADAPT_WEIGHT, config.py:95)
     This is the keep_prob = 1.0 graph: the reference TRAINS with dropout 0.5 after add_score / add_score_vertex / fc6 / fc7
     (lib/fcn/train.py:404-434); the folded vertex head and the commuted bilinear heads are algebraically exact only
     without that dropout, so the losses equal the reference's at keep_prob = 1 (SURVEY.md App. A.7 makes the same
@@ -336,6 +359,17 @@ def training_losses(net: vgg16_convs, layers: dict, gt_label_2d, vertex_targets,
             loss_pose, pose_diff = loss_pose * fix, pose_diff * fix
         out.update(loss_pose=loss_pose, poses_pred=pred, poses_pred_diff=pose_diff)
         total = total + loss_pose
+    if net.adaptation and "domain_score" in layers:
+        z, lab = layers["domain_score"], layers["label_domain"].long()
+        ce = torch.logsumexp(z, 1) - z.gather(1, lab[:, None])[:, 0]
+        if "num_rois" in layers and "rois" not in layers:      # capacity rows: the mean runs over max(num_rois, 1) real rows
+            n = layers["num_rois"].clamp(min=1)
+            ce = ce * (torch.arange(ce.shape[0], device=ce.device) < n).float()
+            loss_domain = adapt_weight * ce.sum(0, keepdim=True) / n.to(torch.float32)
+        else:
+            loss_domain = adapt_weight * ce.mean(0, keepdim=True)
+        out["loss_domain"] = loss_domain
+        total = total + loss_domain
     out["loss"] = total
     return out
 

@@ -56,3 +56,39 @@ def fc(a: torch.Tensor, w_tc: torch.Tensor, bias: torch.Tensor, act: str = "relu
         check(lib().pcnn_fc_f16_tc(ptr(a), ptr(w_tc), ptr(bias), M, N, K, nv, code, ptr(None), 0, ptr(out), ptr(ws),
                                     ctypes.c_size_t(ws.numel()), stream()))
     return out
+
+
+def domain_tail(h9: torch.Tensor, w10: torch.Tensor, b10: torch.Tensor, label_domain: torch.Tensor | None = None,
+                loss_scale: float = 1.0, grad_scale: float = 1.0) -> dict:
+    """The domain classifier after fc9 (vgg16_convs.py:209-212) in one launch (pcnn_domain_tail).  h9 [rows, ld] fp16 = fc9's
+    output, w10 [2][256] f32 (domain_score weights, output-major), b10 [2] f32.  Returns domain_score (after its ReLU) /
+    domain_prob [rows, 2] f32 and domain_label [rows] int32; with label_domain [rows] int32 also loss [1] (loss_scale *
+    sum of the rows' cross entropies), amax [1] (max |d fc9 pre-activation|), dw10 [2][256], db10 [2], db9 [256] and dpre9
+    [rows, ld] fp16 = grad_scale * d fc9 pre-activation.  No host synchronisation."""
+    assert h9.is_cuda and h9.dtype == torch.float16 and h9.is_contiguous() and h9.dim() == 2
+    assert w10.dtype == torch.float32 and w10.is_contiguous() and w10.shape == (2, 256) and b10.dtype == torch.float32
+    rows, ld = h9.shape
+    dev = h9.device
+    out = dict(domain_score=torch.empty((rows, 2), dtype=torch.float32, device=dev),
+               domain_prob=torch.empty((rows, 2), dtype=torch.float32, device=dev),
+               domain_label=torch.empty((rows,), dtype=torch.int32, device=dev))
+    if label_domain is not None:
+        assert label_domain.dtype == torch.int32 and label_domain.is_contiguous() and label_domain.numel() == rows
+        out.update(loss=torch.empty((1,), dtype=torch.float32, device=dev), amax=torch.empty((1,), dtype=torch.float32, device=dev),
+                   dw10=torch.empty((2, 256), dtype=torch.float32, device=dev), db10=torch.empty((2,), dtype=torch.float32, device=dev),
+                   db9=torch.empty((256,), dtype=torch.float32, device=dev), dpre9=torch.empty((rows, ld), dtype=torch.float16, device=dev))
+    g = lambda k: ptr(out.get(k))
+    check(lib().pcnn_domain_tail(ptr(h9), rows, ld, ptr(w10), ptr(b10), ptr(label_domain), f32(loss_scale), f32(grad_scale),
+                                 g("domain_score"), g("domain_prob"), g("domain_label"), g("loss"), g("amax"), g("dw10"), g("db10"),
+                                 g("db9"), g("dpre9"), stream()))
+    return out
+
+
+def domain_grad_merge(a: torch.Tensor, scale_a: float, b: torch.Tensor, scale_b: float, shape) -> torch.Tensor:
+    """f32 tensor of `shape` = scale_a * a + scale_b * b (pcnn_domain_grad_merge): the pool_score gradient of the pose head
+    (a, scale_a = 1 / S) and of the domain branch (b, scale_b = -lambda / S_d, the gradient reversal), a and b fp16."""
+    assert a.dtype == b.dtype == torch.float16 and a.is_contiguous() and b.is_contiguous() and a.numel() == b.numel()
+    out = torch.empty(shape, dtype=torch.float32, device=a.device)
+    assert out.numel() == a.numel()
+    check(lib().pcnn_domain_grad_merge(ptr(a), f32(scale_a), ptr(b), f32(scale_b), ctypes.c_size_t(a.numel()), ptr(out), stream()))
+    return out

@@ -9,6 +9,12 @@ Reference: the training graph lib/networks/vgg16_convs.py:79-212 driven by lib/f
 This is the keep_prob = 1.0 graph (the reference trains with dropout 0.5; random masks cannot be compared, SURVEY App. A.7).
 input_format='RGBD' adds the depth trunk conv1_1_p .. conv5_3_p (vgg16_convs.py:99-126): score_conv4 / score_conv5 read the channel
 concat [colour | depth] of conv4_3 / conv5_3 (c_i = 1024), the vertex heads, Hough voting and RoiPool read the colour trunk only.
+A network built with adaptation=True adds the domain classifier (vgg16_convs.py:202-212) and
+    loss_domain = adapt_weight * mean_rows sparse_softmax_cross_entropy(domain_score, label_domain)   (train.py:508-513)
+on pool_score behind gradient_reversal(0.01): fc9's and domain_score's own gradients are the plain ones, and the gradient that
+reaches pool_score (and through RoiPool the colour trunk) is multiplied by -0.01.  An "adapt" batch (real images without
+annotation, lib/gt_synthesize_layer/minibatch.py:510-511) is given as gt_label_2d = -1 everywhere and gt_poses with 0 rows: Hough
+then labels its rows domain 1, and the other losses and their gradients are exactly 0.
 
 Everything heavy runs on this package's own kernels:
     forward   wgmma convolutions (bf16), un-fused heads (add + up2, 1x1 on the tensor cores, fused up8 / softmax / arg-max),
@@ -38,6 +44,7 @@ from .roi_pooling_layer import roi_pooling_op
 
 CONV_NAMES = [item[0] for item in VGG_CFG if isinstance(item, tuple)]
 POOL_AFTER = {"conv1_2", "conv2_2", "conv3_3", "conv4_3"}          # pool1..pool4 (vgg16_convs.py:80-97)
+GRL_LAMBDA = 0.01                                                  # gradient_reversal(0.01, name='greversal'), vgg16_convs.py:207
 
 
 def _tc_dgrad(w_tc: torch.Tensor, k: int) -> torch.Tensor:
@@ -49,7 +56,8 @@ def _tc_dgrad(w_tc: torch.Tensor, k: int) -> torch.Tensor:
 
 
 class Trainer:
-    def __init__(self, net, lr=0.001, momentum=0.9, weight_decay=1e-4, vertex_w=1.0, vertex_w_inside=10.0, margin=0.01, world=1):
+    def __init__(self, net, lr=0.001, momentum=0.9, weight_decay=1e-4, vertex_w=1.0, vertex_w_inside=10.0, margin=0.01, world=1,
+                 adapt_weight=0.1):
         assert net.is_train and not net.fold_vertex_head and net.input_format in ("COLOR", "RGBD"), \
             "Trainer needs vgg16_convs(is_train=True, fold_vertex_head=False, input_format='COLOR' or 'RGBD')"
         self.rgbd = net.input_format == "RGBD"
@@ -58,6 +66,10 @@ class Trainer:
         self.vertex_w, self.w_inside, self.margin, self.world = float(vertex_w), float(vertex_w_inside), float(margin), int(world)
         self.C = net.num_classes
         self.pose_loss_scale = 1.0               # last dynamic loss scale of the fp16 pose-head backward (see backward())
+        self.adapt = net.domain_branch           # the domain classifier and loss_domain (ADAPT_WEIGHT, lib/fcn/config.py:95)
+        self.adapt_weight = float(adapt_weight)
+        self.domain_loss_scale = 1.0             # the same for the domain branch's fp16 backward
+        self.fc_names = ("fc6", "fc7", "fc8") + (("fc9",) if self.adapt else ())
         self.comm = torch.cuda.Stream(device=net.device) if world > 1 else None
         P, dev = net.params, net.device
         C = self.C
@@ -92,13 +104,16 @@ class Trainer:
         wv[:3 * C] = P["vertex_pred/weights"].reshape(128, 3 * C).t()
         add("vertex_pred/w", wv, wv.to(torch.bfloat16).contiguous(), 0)
         add("vertex_pred/b", P["vertex_pred/biases"].clone(), None, 0)
-        for name in ("fc6", "fc7", "fc8"):
+        for name in self.fc_names:
             w = P[f"{name}/weights"]                                                              # [in, out]
             npad = (w.shape[1] + 127) // 128 * 128
             wt = torch.zeros((npad, w.shape[0]), device=dev)
             wt[:w.shape[1]] = w.t()
             add(name + "/w", wt, wt.to(torch.float16).contiguous(), 1)
             add(name + "/b", P[f"{name}/biases"].clone(), None, 0)
+        if self.adapt:
+            add("domain_score/w", P["domain_score/weights"].t().contiguous(), None, 0)           # [2][256] f32, read by the tail kernel
+            add("domain_score/b", P["domain_score/biases"].clone(), None, 0)
         self.conv1_tc = conv.conv1_1_weights_to_tc(P["conv1_1/weights"])
         self.conv1_tc_p = conv.conv1_1_weights_to_tc(P["conv1_1_p/weights"]) if self.rgbd else None
         self._refresh_derived()
@@ -121,7 +136,7 @@ class Trainer:
                 d = self.dg[name]
                 self.dg[name], self.dg[name + "_p"] = d[:512], d[512:]
         self.fc_t = {}
-        for name in ("fc6", "fc7", "fc8"):
+        for name in self.fc_names:
             w = self.tc[name + "/w"]
             t = torch.empty((w.shape[1], w.shape[0]), dtype=torch.float16, device=w.device)
             check(lib().pcnn_transpose16(ptr(w), w.shape[0], w.shape[1], ptr(t), stream()))
@@ -151,10 +166,13 @@ class Trainer:
         P["score/biases"] = self.master["score/b"].clone()
         P["vertex_pred/weights"] = self.master["vertex_pred/w"][:3 * C].t().reshape(P["vertex_pred/weights"].shape).contiguous()
         P["vertex_pred/biases"] = self.master["vertex_pred/b"].clone()
-        for name in ("fc6", "fc7", "fc8"):
+        for name in self.fc_names:
             n_out = P[f"{name}/weights"].shape[1]
             P[f"{name}/weights"] = self.master[name + "/w"][:n_out].t().contiguous()
             P[f"{name}/biases"] = self.master[name + "/b"].clone()
+        if self.adapt:
+            P["domain_score/weights"] = self.master["domain_score/w"].t().contiguous()
+            P["domain_score/biases"] = self.master["domain_score/b"].clone()
         self.net.prepare()
 
     # ------------------------------------------------------------------ forward (training graph, activations kept)
@@ -244,6 +262,12 @@ class Trainer:
         loss_pose, pose_diff = average_distance_loss_op.average_distance_loss(pred, tw, wt, points, symmetry, self.margin)
         A.update(rois=rl, num_rois=num_rois, a5=a5, a4=a4, pool=pool, fc6=f6, fc7=f7, poses_tanh=tanh, poses_weight=wt, poses_target=tw,
                  pose_diff=pose_diff, loss_pose_raw=loss_pose, rows=rows, data=data)
+        if self.adapt:
+            # the domain classifier on the same fp16 pool_score (gradient_reversal is the identity forward); label_domain = Hough's
+            # top_domain, decided by the whole batch's gt count (every rank is given the whole gt array)
+            f9 = pose_head.fc(pool, T["fc9/w"], M["fc9/b"], "relu")
+            A.update(fc9=f9, label_domain=domain[:rows].contiguous())
+            A.update(pose_head.domain_tail(f9, M["domain_score/w"], M["domain_score/b"]))
         return A
 
     def dense_vertex_pred(self, A):
@@ -307,8 +331,17 @@ class Trainer:
             A["vtx_out"] = torch.stack([A["vtx_out"][0] * local[1] / norm[1].clamp(min=1e-10), norm[1]])
         rows_global = norm[2]
         # Averagedistance divides by the rows IT sees (capacity rows of this rank); the reference batch sees all of them
-        pose_scale = (float(rows) / rows_global).item() if self.world > 1 else 1.0
+        rows_g = float(rows)
+        if self.world == 1:
+            pose_scale = 1.0
+        elif self.adapt:
+            pose_scale, rows_g = torch.stack([float(rows) / rows_global, rows_global]).tolist()
+        else:
+            pose_scale = (float(rows) / rows_global).item()
         A["loss_pose"] = A["loss_pose_raw"] * pose_scale
+        if self.adapt:
+            # domain branch, un-scaled pass: its gradient maximum is read with the pose chain's below
+            dom = pose_head.domain_tail(A["fc9"], M["domain_score/w"], M["domain_score/b"], A["label_domain"], self.adapt_weight / rows_g, 1.0)
         # ---- pose head
         # The head's backward GEMMs run on FP16 operands like its forward.  The pose-loss gradients are tiny (a mean over rows x points:
         # 1e-6 .. 1e-4 per element, below fp16's normal range), so the chain is LOSS-SCALED by a dynamic power of two S where it enters fp16 and un-scaled
@@ -319,11 +352,26 @@ class Trainer:
                                         stream()))
         # dynamic loss scale: a power of two that puts the largest element of the chain's entry point at ~2^11 (one host read; the
         # un-scaled pass above is only used for its maximum, which fp16 represents well enough even when the small elements underflow)
-        amax = float(dpre.float().abs().max().item())
+        if self.adapt:
+            amax, amax_d = torch.stack([dpre.float().abs().max(), dom["amax"][0]]).tolist()
+        else:
+            amax = float(dpre.float().abs().max().item())
         if self.world > 1:
-            t = torch.tensor([amax], device=dev); dist.all_reduce(t, op=dist.ReduceOp.MAX); amax = float(t.item())
-        S = 2.0 ** max(0, min(24, int(torch.floor(torch.log2(torch.tensor(2048.0 / max(amax, 1e-30)))).item()))) if amax > 0 else 1.0
+            t = torch.tensor([amax, amax_d] if self.adapt else [amax], device=dev); dist.all_reduce(t, op=dist.ReduceOp.MAX)
+            amax, amax_d = t.tolist() if self.adapt else (float(t.item()), None)
+        S = self._loss_scale(amax)
         self.pose_loss_scale = S
+        if self.adapt:
+            # the same dynamic power of two for fc9's backward GEMMs (d fc9 is ~1e-5: below fp16's normal range)
+            S_d = self._loss_scale(amax_d)
+            self.domain_loss_scale = S_d
+            dom = pose_head.domain_tail(A["fc9"], M["domain_score/w"], M["domain_score/b"], A["label_domain"], self.adapt_weight / rows_g, S_d)
+            A["loss_domain"] = dom["loss"]
+            self._emit(grads, "domain_score/w", dom["dw10"])
+            self._emit(grads, "domain_score/b", dom["db10"])
+            self._emit(grads, "fc9/w", self._fc_wgrad(A["pool"], dom["dpre9"], 1.0 / S_d))
+            self._emit(grads, "fc9/b", dom["db9"])
+            d9 = self._fc_dgrad(dom["dpre9"], "fc9", None)                                    # [rows, 25088], scaled by S_d
         check(lib().pcnn_pose_chain_bwd(ptr(A["pose_diff"]), ptr(A["poses_tanh"]), ptr(A["poses_weight"]), rows, D, f32(pose_scale * S), ptr(dpre), 128,
                                         stream()))
         self._emit(grads, "fc8/w", self._fc_wgrad(A["fc7"], dpre, 1.0 / S))
@@ -335,8 +383,13 @@ class Trainer:
         self._emit(grads, "fc6/w", self._fc_wgrad(A["pool"], d6, 1.0 / S))
         self._emit(grads, "fc6/b", d6.float().sum(0) / S)
         dpool16 = self._fc_dgrad(d6, "fc6", None)                                              # [rows, 25088]
-        dpool = torch.empty((rows, 7, 7, 512), dtype=torch.float32, device=dev)
-        check(lib().pcnn_half_to_float(ptr(dpool16), ctypes.c_size_t(dpool16.numel()), f32(1.0 / S), ptr(dpool), stream()))
+        if self.adapt:
+            # pool_score's gradient from both branches in one pass; gradient_reversal is the factor -lambda of the domain term
+            dpool = pose_head.domain_grad_merge(dpool16, 1.0 / S, d9, -GRL_LAMBDA / S_d, (rows, 7, 7, 512))
+        else:
+            dpool = torch.empty((rows, 7, 7, 512), dtype=torch.float32, device=dev)
+            check(lib().pcnn_half_to_float(ptr(dpool16), ctypes.c_size_t(dpool16.numel()), f32(1.0 / S), ptr(dpool), stream()))
+        A["dpool"] = dpool                                                                      # d loss / d pool_score (kept for inspection)
         g5_roi = roi_pooling_op.roi_pool_grad(A["conv5_3"], A["rois"], A["a5"], dpool, 7, 7, 1.0 / 16.0, 0)       # fp32 dense
         g4_roi = roi_pooling_op.roi_pool_grad(A["conv4_3"], A["rois"], A["a4"], dpool, 7, 7, 1.0 / 8.0, 0)
         # ---- FCN heads
@@ -386,6 +439,11 @@ class Trainer:
             self._trunk_bwd(grads, A, g5_p, g4_p, "_p", cols_p)
         return grads
 
+    @staticmethod
+    def _loss_scale(amax):
+        """The power of two (1 .. 2^24) that puts a backward chain's largest fp16 entry at ~2^11."""
+        return 2.0 ** max(0, min(24, int(torch.floor(torch.log2(torch.tensor(2048.0 / max(amax, 1e-30)))).item()))) if amax > 0 else 1.0
+
     def _trunk_bwd(self, grads, A, g5, g4, sfx, im2col):
         """conv5_3 .. conv1_1 of one trunk, top down.  g5 / g4: the gradients entering conv5_3 / conv4_3 from the heads (and
         RoiPool); im2col() builds the [B,H,W,64] view of the trunk's input that conv1_1's weight gradient reads."""
@@ -433,5 +491,9 @@ class Trainer:
         grads = self.backward(A, gt_label_2d, centers)
         self.update(grads)
         loss_cls, loss_vertex, loss_pose = A["cls_out"][0:1], self.vertex_w * A["vtx_out"][0:1], A["loss_pose"]
-        return dict(loss_cls=loss_cls, loss_vertex=loss_vertex, loss_pose=loss_pose, loss=loss_cls + loss_vertex + loss_pose, num_rois=A["num_rois"],
-                    grads=grads)
+        out = dict(loss_cls=loss_cls, loss_vertex=loss_vertex, loss_pose=loss_pose, loss=loss_cls + loss_vertex + loss_pose, num_rois=A["num_rois"],
+                   grads=grads)
+        if self.adapt:
+            out.update(loss_domain=A["loss_domain"], loss=out["loss"] + A["loss_domain"], label_domain=A["label_domain"],
+                       domain_label=A["domain_label"])
+        return out
