@@ -227,23 +227,18 @@ int pcnn_add_to_bf16(const void* a_bf16, const void* b_bf16, const float* b_f32,
  * losses lib/fcn/train.py:455-465, 564-573, optimizer tf.train.MomentumOptimizer (train.py:633):
  *  pcnn_add_up2_bf16 / pcnn_up2_bwd_bf16   add = a4 + up2(a5) (fixed bilinear conv2d_transpose 4x4 / 2) and its adjoint (+ ReLU mask of a5)
  *  pcnn_pack_lowres       [score C | vertex 3C] f32 head tensor from the two bf16 1x1-convolution outputs (row strides Cs, Cv)
- *  pcnn_up8_heads_bwd     gradient of loss_cls (Hardlabel-selected cross entropy through log-softmax and the ReLU of `score`) and of
+ *  pcnn_up8_heads_bwd_ex  gradient of loss_cls (Hardlabel-selected cross entropy through log-softmax and the ReLU of `score`) and of
  *                         loss_vertex (smooth L1 on the labelled pixels' own class) w.r.t. the low-resolution head tensor, formed from
  *                         the loss structure on the fly: d_sc [B,h,w,Cs], d_vt [B,h,w,Cv] bf16 (padding channels zero), dbias [4C]
+ *                         (C even, 6..50); the labelled pixels' vertex values come from vertex_pred [B,H,W,3C], or with
+ *                         vertex_pred == NULL from the low-resolution head tensor `lowres` [B,h,w,4C] + bias_vertex [3C]
  *  pcnn_pose_chain_bwd    Averagedistance's bottom_diff through l2_normalize, * poses_weight and tanh -> d fc8 pre-activation (fp16)
  *  pcnn_sgd_momentum      accum = mu * accum + (gscale * grad + wd * w); w -= lr * accum; refreshed 16-bit tensor-core copy (kind 0 bf16, 1 fp16)
  *  pcnn_transpose16 / pcnn_half_to_float   layout / precision glue of the fully connected backward GEMMs
- *  pcnn_conv1_wgrad       conv1_1 weight gradient (Cin = 3) on the CUDA cores, input = uint8 image - mean
  */
 int pcnn_add_up2_bf16(const void* a4_bf16, const void* a5_bf16, int B, int h, int w, int C, void* out_bf16, void* stream);
 int pcnn_up2_bwd_bf16(const void* dadd_bf16, const void* y5_bf16, int B, int h, int w, int C, void* d5_bf16, void* stream);
 int pcnn_pack_lowres(const void* sc_bf16, int Cs, const void* vt_bf16, int Cv, int B, int h, int w, int C, float* lowres, void* stream);
-int pcnn_up8_heads_bwd(const float* prob, const float* score, const int32_t* gt, const float* cls_loss_out, float upstream_cls,
-                       float threshold, const float* vertex_pred, const float* centers, const float* vertex_loss_out,
-                       float upstream_vertex, float w_inside, float sigma, int B, int h, int w, int C, int Cs, int Cv,
-                       void* d_sc_bf16, void* d_vt_bf16, float* dbias, void* workspace, size_t workspace_bytes, void* stream);
-/* the same with vertex_pred == NULL: the labelled pixels' vertex values are formed from the low-resolution head tensor
- * `lowres` [B,h,w,4C] + bias_vertex [3C] (no dense vertex_pred in the training step; C = 22) */
 int pcnn_up8_heads_bwd_ex(const float* prob, const float* score, const int32_t* gt, const float* cls_loss_out, float upstream_cls,
                           float threshold, const float* vertex_pred, const float* lowres, const float* bias_vertex, const float* centers,
                           const float* vertex_loss_out, float upstream_vertex, float w_inside, float sigma, int B, int h, int w, int C,
@@ -262,8 +257,6 @@ int pcnn_fc_dgrad_f16_tc(const void* dy_f16, const void* w_in_out_f16, int M, in
                          int ld_out, void* workspace, size_t workspace_bytes, void* stream);
 int pcnn_transpose16(const void* in, int rows, int cols, void* out, void* stream);
 int pcnn_half_to_float(const void* src_f16, size_t n, float scale, float* dst, void* stream);
-int pcnn_conv1_wgrad(const void* img_u8, const float* mean3_host, const void* dz_bf16, int B, int H, int W, float scale,
-                     const float* w, float decay, float* dW, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * Pose-regression head (networks/vgg16_convs.py:177-197, Network.fc networks/network.py:392-422, tanh :436-438) on own

@@ -7,10 +7,10 @@ import torch
 from ._lib import check, lib, ptr, stream
 
 
-def hwio_to_tc(weights_hwio: torch.Tensor) -> torch.Tensor:
-    """TF filter layout [kh, kw, Cin, Cout] f32 (network.py:166-170) -> [Cout][kh*kw*Cin] bf16."""
+def hwio_to_tc(weights_hwio: torch.Tensor, dtype=torch.bfloat16) -> torch.Tensor:
+    """TF filter layout [kh, kw, Cin, Cout] f32 (network.py:166-170) -> [Cout][kh*kw*Cin] bf16 (or `dtype`)."""
     kh, kw, ci, co = weights_hwio.shape
-    return weights_hwio.permute(3, 0, 1, 2).reshape(co, kh * kw * ci).to(torch.bfloat16).contiguous()
+    return weights_hwio.permute(3, 0, 1, 2).reshape(co, kh * kw * ci).to(dtype).contiguous()
 
 
 def hwio_to_tc_dgrad(weights_hwio: torch.Tensor) -> torch.Tensor:

@@ -7,7 +7,7 @@
 //   loss_cls         = -sum_{selected p} log_softmax(score)[p, gt_p] / count     (Hardlabel selection, train.py:455-465)
 //   vertex_pred likewise from add_score_vertex; loss_vertex = smooth-L1 on the labelled pixels' own class (train.py:564-573)
 // Backward pieces here:
-//   k_up8_bwd       d lowres[b, my, mx, ch] = sum_{y, x} Wy Wx d up[b, y, x, ch]  with d up formed on the fly from the loss
+//   k_up8_bwd_strip d lowres[b, my, mx, ch] = sum_{y, x} Wy Wx d up[b, y, x, ch]  with d up formed on the fly from the loss
 //                   structure (one-hot cross-entropy through log-softmax and ReLU; sparse smooth-L1), never materialised
 //   k_add_up2 / k_up2_bwd   add = a4 + up2(a5) and its adjoint (+ ReLU mask)
 //   k_pose_chain_bwd        d fc8 pre-activation from Averagedistance's bottom_diff through l2_normalize, * weight, tanh
@@ -16,7 +16,6 @@
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <float.h>
-#include <stdlib.h>
 
 #include "common.cuh"
 #include "heads_common.cuh"
@@ -127,146 +126,21 @@ k_pack_lowres(const __nv_bfloat16* __restrict__ sc, int Cs, const __nv_bfloat16*
 }
 
 // ---------------------------------------------------------------------------------------------
-// k_up8_bwd: gradient of both losses w.r.t. the low-resolution head tensor.
+// k_up8_bwd_strip: gradient of both losses w.r.t. the low-resolution head tensor.
 //   score channel c:  d up[p, c] = up_cls * sel_p * (prob[p, c] - [c == gt_p]) / (count + 1e-10) * [score[p, c] > 0]
 //                     sel_p = gt_p != -1 and (gt_p > 0 or prob[p, gt_p] < threshold)          (Hardlabel, constant mask)
 //   vertex channel 3c+k: pixels labelled c with a listed centre: up_vtx * w_inside * smoothL1'(w_inside (pred - target)) / (sum w + 1e-10)
-// One CTA per (low-resolution row, image); thread = (cell, channel), channel fastest (coalesced prob / score reads).
 // Outputs d lowres as TWO bf16 tensors in the layouts the 1x1 backward GEMMs read: d_sc [B,h,w,Cs] (first C channels,
 // rest zero) and d_vt [B,h,w,Cv] (first 3C channels), plus per-CTA partial sums of d bias (the up-sampling weights of a
 // pixel sum to the same value for bias: d b[ch] = sum_p d up[p, ch]).
-// ---------------------------------------------------------------------------------------------
-// Separable form.  CTA = (low-resolution row my, image, chunk of kUbCells cells).  Pass 1, thread = output COLUMN x of the chunk
-// (+ 4-pixel halo): walks the 16 contributing output rows, forms d up[p, :] once per pixel (gt / prob / score read once), and
-// accumulates the vertical blend v[x][ch] = sum_ky Wy[ky] d up[(8 my - 4 + ky, x), ch] — score channels in registers, the three
-// vertex channels of the pixel's label straight into the thread's own shared-memory column.  Pass 2, thread = (cell, channel):
-// d lowres = sum_kx Wx[kx] v[8 mx - 4 + kx][ch].  Every (pixel, channel) gradient is computed once per CTA instead of once per
-// (cell, channel) it contributes to (the direct gather form cost 7.9 ms at batch 16; this one ~1 ms).
-constexpr int kUbCells = 16;
-constexpr int kUbCols = 8 * kUbCells + 8;          // 136 output columns incl. the halo
-
-template <int CT>
-__global__ void __launch_bounds__(kUbCols)
-k_up8_bwd(const float* __restrict__ prob, const float* __restrict__ score, const int* __restrict__ gt, const float* __restrict__ cls_out /*[2]*/,
-          float up_cls, float threshold, const float* __restrict__ vpred /*[B,H,W,3C]*/, const float* __restrict__ centers /*[B,C,3]*/,
-          const float* __restrict__ vtx_out /*[2]*/, float up_vtx, float w_inside, float sigma2, int h, int w, int C_rt, int Cs, int Cv,
-          __nv_bfloat16* __restrict__ d_sc, __nv_bfloat16* __restrict__ d_vt, float* __restrict__ dbias_partial /*[ctas][4C]*/)
-{
-    const int C = CT ? CT : C_rt;
-    const int H = 8 * h, W = 8 * w, No = 4 * C;
-    const int my = blockIdx.x, n = blockIdx.y, c_lo = blockIdx.z * kUbCells, c_hi = min(c_lo + kUbCells, w);
-    const float s_cls = up_cls / (cls_out[1] + 1e-10f), s_vtx = up_vtx / (vtx_out[1] + 1e-10f);
-    const size_t img = (size_t)n * H * W;
-    extern __shared__ float sm[];
-    float* v = sm;                                  // [kUbCols][No]: vertical blends, column-major by pixel column
-    float* s_db = sm + (size_t)kUbCols * No;        // [No] bias-gradient sums of the pixels this CTA owns
-    const int t = threadIdx.x;
-    for (int i = t; i < kUbCols * No; i += blockDim.x) v[i] = 0.f;
-    for (int i = t; i < No; i += blockDim.x) s_db[i] = 0.f;
-    __syncthreads();
-    {
-        const int x = 8 * c_lo - 4 + t;             // this thread's output column
-        if (t < kUbCols && x >= 0 && x < W && x < 8 * c_hi + 4) {
-            float* vcol = v + (size_t)t * No;
-            float acc[CT ? CT : 1];
-#pragma unroll
-            for (int c = 0; c < (CT ? CT : 1); c++) acc[c] = 0.f;
-            const bool own_x = x >= 8 * c_lo && x < 8 * c_hi;
-            for (int ky = 0; ky < 16; ky++) {
-                const int y = 8 * my - 4 + ky;
-                if (y < 0 || y >= H) continue;
-                const float wy = deconv_w(ky, 16);
-                const bool own = own_x && ky >= 4 && ky < 12;
-                const size_t p = img + (size_t)y * W + x;
-                const int g = __ldg(gt + p);
-                if (g >= 0 && g < C) {
-                    const float pg = __ldg(prob + p * C + g);
-                    if (g > 0 || pg < threshold) {
-                        const float* pp = prob + p * C;
-                        const float* sp = score + p * C;
-                        if (CT) {
-                            // C even: a pixel's C floats are 8-byte aligned -> 64-bit loads
-                            const float2* pp2 = reinterpret_cast<const float2*>(pp);
-                            const float2* sp2 = reinterpret_cast<const float2*>(sp);
-#pragma unroll
-                            for (int c2 = 0; c2 < (CT ? CT / 2 : 1); c2++) {
-                                const float2 sv = __ldg(sp2 + c2), pv = __ldg(pp2 + c2);
-                                const float d0 = sv.x > 0.f ? s_cls * (pv.x - (2 * c2 == g ? 1.f : 0.f)) : 0.f;
-                                const float d1 = sv.y > 0.f ? s_cls * (pv.y - (2 * c2 + 1 == g ? 1.f : 0.f)) : 0.f;
-                                acc[2 * c2] = fmaf(wy, d0, acc[2 * c2]);
-                                acc[2 * c2 + 1] = fmaf(wy, d1, acc[2 * c2 + 1]);
-                                if (own && d0 != 0.f) atomicAdd(&s_db[2 * c2], d0);
-                                if (own && d1 != 0.f) atomicAdd(&s_db[2 * c2 + 1], d1);
-                            }
-                        } else {
-                            for (int c = 0; c < C; c++) {
-                                float d = 0.f;
-                                if (__ldg(sp + c) > 0.f) d = s_cls * (__ldg(pp + c) - (c == g ? 1.f : 0.f));
-                                vcol[c] = fmaf(wy, d, vcol[c]);
-                                if (own && d != 0.f) atomicAdd(&s_db[c], d);
-                            }
-                        }
-                    }
-                    if (g > 0) {
-                        const float* cen = centers + ((size_t)n * C + g) * 3;
-                        const float z = cen[2];
-                        if (z > 0.f) {
-                            const double dx = (double)cen[0] - (double)x, dy = (double)cen[1] - (double)y;
-                            const double nrm = sqrt(dx * dx + dy * dy) + 1e-10;
-                            const float tg[3] = {(float)(dx / nrm), (float)(dy / nrm), (float)log((double)z)};
-#pragma unroll
-                            for (int k = 0; k < 3; k++) {
-                                const float diff = w_inside * (__ldg(vpred + p * 3 * C + 3 * g + k) - tg[k]);
-                                const float ad = fabsf(diff);
-                                const float dt = ad < 1.f / sigma2 ? diff * sigma2 : (diff > 0.f ? 1.f : (diff < 0.f ? -1.f : 0.f));
-                                const float d = s_vtx * w_inside * dt;
-                                vcol[C + 3 * g + k] = fmaf(wy, d, vcol[C + 3 * g + k]);
-                                if (own && d != 0.f) atomicAdd(&s_db[C + 3 * g + k], d);
-                            }
-                        }
-                    }
-                }
-            }
-            if (CT) {
-#pragma unroll
-                for (int c = 0; c < (CT ? CT : 1); c++) vcol[c] = acc[c];
-            }
-        }
-    }
-    __syncthreads();
-    for (int item = t; item < (c_hi - c_lo) * No; item += blockDim.x) {
-        const int ml = item / No, ch = item - ml * No, mx = c_lo + ml;
-        float acc = 0.f;
-#pragma unroll
-        for (int kx = 0; kx < 16; kx++) acc = fmaf(deconv_w(kx, 16), v[(size_t)(8 * ml + kx) * No + ch], acc);   // column 8 mx - 4 + kx
-        const size_t cell = ((size_t)n * h + my) * w + mx;
-        if (ch < C) d_sc[cell * Cs + ch] = __float2bfloat16_rn(acc);
-        else d_vt[cell * Cv + ch - C] = __float2bfloat16_rn(acc);
-    }
-    // zero the padding channels of the two GEMM operands
-    for (int item = t; item < (c_hi - c_lo) * (Cs - C); item += blockDim.x) {
-        const int mx = c_lo + item / (Cs - C), ch = C + item % (Cs - C);
-        d_sc[(((size_t)n * h + my) * w + mx) * Cs + ch] = __float2bfloat16_rn(0.f);
-    }
-    for (int item = t; item < (c_hi - c_lo) * (Cv - 3 * C); item += blockDim.x) {
-        const int mx = c_lo + item / (Cv - 3 * C), ch = 3 * C + item % (Cv - 3 * C);
-        d_vt[(((size_t)n * h + my) * w + mx) * Cv + ch] = __float2bfloat16_rn(0.f);
-    }
-    const size_t cta = ((size_t)blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
-    for (int i = t; i < No; i += blockDim.x) dbias_partial[cta * No + i] = s_db[i];
-}
-
-// ---------------------------------------------------------------------------------------------
-// k_up8_bwd_strip: the same gradient, organised so that every byte of prob / score is read (nearly) once and every load is
-// coalesced.  CTA = (image, strip of kSC low-resolution columns = 8 kSC + 8 output columns incl. the halo, band of `rb`
+// Organised so that every byte of prob / score is read (nearly) once and every load is coalesced.  CTA = (image, strip of kSC low-resolution columns = 8 kSC + 8 output columns incl. the halo, band of `rb`
 // low-resolution rows).  Thread = (output column, channel PAIR): the CTA's threads read one contiguous run of
 // kCols * C floats per output row of prob and of score (64-bit loads).  The thread walks DOWN the band's 8 rb + 8 output
 // rows; a pixel row contributes to exactly two low-resolution rows (taps ky and ky + 8), so two running vertical sums per
-// channel live in registers and the finished one is handed to the horizontal pass every 8 rows (same fmaf order as
-// k_up8_bwd: the two kernels agree bit for bit on d_sc / d_vt).  The three vertex channels of a labelled pixel go to a
+// channel live in registers and the finished one is handed to the horizontal pass every 8 rows.  The three vertex channels of a labelled pixel go to a
 // per-column shared-memory accumulator owned by thread (column, k).  Bias gradients: per-thread registers (fixed channel
 // pair) / per-column shared-memory cells, reduced over the columns in a fixed order (no atomics: run-to-run deterministic).
-// Redundant reads: (8 kSC + 8) / (8 kSC) x (8 rb + 8) / (8 rb) = 1.25 x 1.07 at kSC = 4, rb = 16 (k_up8_bwd: 2 x 1.06, stride-88-B loads).
+// Redundant reads: (8 kSC + 8) / (8 kSC) x (8 rb + 8) / (8 rb) = 1.25 x 1.07 at kSC = 4, rb = 16.
 // ---------------------------------------------------------------------------------------------
 constexpr int kSC = 4;
 constexpr int kSCols = 8 * kSC + 8;                 // 40 output columns
@@ -556,51 +430,6 @@ k_half_to_float(const __half* __restrict__ src, size_t n, float scale, float* __
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) dst[i] = scale * __half2float(src[i]);
 }
 
-// conv1_1 weight gradient (Cin = 3: below any tensor-core tile): dW[co][tap * 3 + c] = sum_pix x[pix + tap][c] * dz[pix][co],
-// x = uint8 BGR - mean (zero outside the image).  Fixed grid; every CTA loops over 256-pixel chunks, thread = (co, tap group).
-__global__ void __launch_bounds__(256)
-k_conv1_wgrad(const unsigned char* __restrict__ img /*[B,H,W,3]*/, const __nv_bfloat16* __restrict__ dz /*[B,H,W,64]*/, int B, int H, int W,
-              float m0, float m1, float m2, float* __restrict__ partial /*[grid][64][27]*/)
-{
-    __shared__ float s_patch[256][28];
-    const int co = threadIdx.x & 63, tg = threadIdx.x >> 6;       // 4 tap groups: k in [7 tg, min(7 tg + 7, 27))
-    const int k_lo = 7 * tg, k_hi = min(k_lo + 7, 27);
-    float acc[7];
-#pragma unroll
-    for (int j = 0; j < 7; j++) acc[j] = 0.f;
-    const size_t npix = (size_t)B * H * W;
-    for (size_t base = (size_t)blockIdx.x * 256; base < npix; base += (size_t)gridDim.x * 256) {
-        __syncthreads();
-        {   // stage the 27 input values of 256 pixels (thread = pixel)
-            const size_t p = base + threadIdx.x;
-            if (p < npix) {
-                const int x = (int)(p % W), y = (int)((p / W) % H);
-                const size_t n = p / ((size_t)W * H);
-#pragma unroll
-                for (int tap = 0; tap < 9; tap++) {
-                    const int yy = y + tap / 3 - 1, xx = x + tap % 3 - 1;
-                    const bool ok = yy >= 0 && yy < H && xx >= 0 && xx < W;
-                    const unsigned char* q = img + ((n * H + yy) * W + xx) * 3;
-                    s_patch[threadIdx.x][tap * 3 + 0] = ok ? (float)q[0] - m0 : 0.f;
-                    s_patch[threadIdx.x][tap * 3 + 1] = ok ? (float)q[1] - m1 : 0.f;
-                    s_patch[threadIdx.x][tap * 3 + 2] = ok ? (float)q[2] - m2 : 0.f;
-                }
-            }
-        }
-        __syncthreads();
-        const int cnt = (int)min((size_t)256, npix - base);
-        for (int i = 0; i < cnt; i++) {
-            const float d = __bfloat162float(dz[(base + i) * 64 + co]);
-            if (d == 0.f) continue;
-#pragma unroll
-            for (int j = 0; j < 7; j++)
-                if (k_lo + j < k_hi) acc[j] = fmaf(s_patch[i][k_lo + j], d, acc[j]);
-        }
-    }
-    for (int j = 0; j < 7; j++)
-        if (k_lo + j < k_hi) partial[((size_t)blockIdx.x * 64 + co) * 27 + k_lo + j] = acc[j];
-}
-
 }  // namespace pcnn
 
 using namespace pcnn;
@@ -631,24 +460,6 @@ extern "C" int pcnn_pack_lowres(const void* sc, int Cs, const void* vt, int Cv, 
     return check_launch("pack_lowres");
 }
 
-// d bias_score [C] and d bias_vertex [3C] come back in dbias [4C]; workspace: B * h * ceil(w / 16) * 4C floats
-// vertex_pred == NULL: the labelled pixels' vertex values come from `lowres` [B,h,w,4C] + bias_vertex [3C] (C = 22 strip kernel only)
-extern "C" int pcnn_up8_heads_bwd_ex(const float* prob, const float* score, const int32_t* gt, const float* cls_loss_out, float upstream_cls,
-                                     float threshold, const float* vertex_pred, const float* lowres, const float* bias_vertex, const float* centers,
-                                     const float* vertex_loss_out, float upstream_vertex, float w_inside, float sigma, int B, int h, int w, int C,
-                                     int Cs, int Cv, void* d_sc_bf16, void* d_vt_bf16, float* dbias, void* workspace, size_t workspace_bytes,
-                                     void* stream);
-
-extern "C" int pcnn_up8_heads_bwd(const float* prob, const float* score, const int32_t* gt, const float* cls_loss_out, float upstream_cls,
-                                  float threshold, const float* vertex_pred, const float* centers, const float* vertex_loss_out,
-                                  float upstream_vertex, float w_inside, float sigma, int B, int h, int w, int C, int Cs, int Cv,
-                                  void* d_sc_bf16, void* d_vt_bf16, float* dbias, void* workspace, size_t workspace_bytes, void* stream)
-{
-    PCNN_REQUIRE(vertex_pred, "up8_heads_bwd: NULL tensor pointer");
-    return pcnn_up8_heads_bwd_ex(prob, score, gt, cls_loss_out, upstream_cls, threshold, vertex_pred, nullptr, nullptr, centers, vertex_loss_out,
-                                 upstream_vertex, w_inside, sigma, B, h, w, C, Cs, Cv, d_sc_bf16, d_vt_bf16, dbias, workspace, workspace_bytes, stream);
-}
-
 extern "C" int pcnn_up8_heads_bwd_ex(const float* prob, const float* score, const int32_t* gt, const float* cls_loss_out, float upstream_cls,
                                      float threshold, const float* vertex_pred, const float* lowres, const float* bias_vertex, const float* centers,
                                      const float* vertex_loss_out, float upstream_vertex, float w_inside, float sigma, int B, int h, int w, int C,
@@ -659,48 +470,26 @@ extern "C" int pcnn_up8_heads_bwd_ex(const float* prob, const float* score, cons
                      d_vt_bf16 && dbias && workspace,
                  "up8_heads_bwd: NULL tensor pointer");
     PCNN_REQUIRE(Cs >= C && Cv >= 3 * C && h <= 65535 && B <= 65535, "up8_heads_bwd: bad shape");
-    const int chunks = (w + kUbCells - 1) / kUbCells;
-    const size_t need = sizeof(float) * (size_t)B * h * chunks * 4 * C;
+    PCNN_REQUIRE(C % 2 == 0 && C >= 6 && C <= 50, "up8_heads_bwd: C must be even and in 6..50 (C = %d)", C);
+    // coalesced strip kernel (see k_up8_bwd_strip); partial bias sums: one row of 4C floats per CTA
+    const int rb = 16, bands = (h + rb - 1) / rb, strips = (w + kSC - 1) / kSC;
+    const size_t need = sizeof(float) * (size_t)B * strips * bands * 4 * C;
+    PCNN_REQUIRE(workspace_bytes >= need, "up8_heads_bwd: workspace too small (%zu < %zu)", workspace_bytes, need);
+    PCNN_REQUIRE(bands <= 65535, "up8_heads_bwd: bad shape");
     cudaStream_t st = (cudaStream_t)stream;
-    static const bool strip_on = getenv("PCNN_UP8_BWD_STRIP") == nullptr || atoi(getenv("PCNN_UP8_BWD_STRIP")) != 0;
-    if (C % 2 == 0 && C >= 6 && C <= 50 && strip_on) {
-        // coalesced strip kernel (see k_up8_bwd_strip); partial bias sums: one row of 4C floats per CTA
-        const int rb = 16, bands = (h + rb - 1) / rb, strips = (w + kSC - 1) / kSC;
-        const size_t need2 = sizeof(float) * (size_t)B * strips * bands * 4 * C;
-        PCNN_REQUIRE(workspace_bytes >= need2, "up8_heads_bwd: workspace too small (%zu < %zu)", workspace_bytes, need2);
-        PCNN_REQUIRE(bands <= 65535, "up8_heads_bwd: bad shape");
-        const size_t smem2 = sizeof(float) * ((size_t)kSCols * 11 * C + C);
-        const dim3 grid2(strips, bands, B);
-        if (C == 22)
-            k_up8_bwd_strip<22><<<grid2, kSCols * 11, smem2, st>>>(prob, score, gt, cls_loss_out, upstream_cls, threshold, vertex_pred, lowres, bias_vertex,
-                                                                  centers, vertex_loss_out, upstream_vertex, w_inside, sigma * sigma, h, w, rb, C, Cs, Cv,
-                                                                  (__nv_bfloat16*)d_sc_bf16, (__nv_bfloat16*)d_vt_bf16, (float*)workspace);
-        else {
-            PCNN_SMEM_OPTIN(k_up8_bwd_strip<0>, 100 * 1024, "up8_bwd_strip<0>");
-            k_up8_bwd_strip<0><<<grid2, kSCols * (C / 2), smem2, st>>>(prob, score, gt, cls_loss_out, upstream_cls, threshold, vertex_pred, lowres,
-                                                                      bias_vertex, centers, vertex_loss_out, upstream_vertex, w_inside, sigma * sigma, h, w,
-                                                                      rb, C, Cs, Cv, (__nv_bfloat16*)d_sc_bf16, (__nv_bfloat16*)d_vt_bf16,
-                                                                      (float*)workspace);
-        }
-        k_sum_partials<<<(4 * C + 31) / 32, 256, 0, st>>>((const float*)workspace, B * strips * bands, 4 * C, 1.f, nullptr, 0.f, dbias);
-        return check_launch("up8_heads_bwd");
+    const size_t smem = sizeof(float) * ((size_t)kSCols * 11 * C + C);
+    const dim3 grid(strips, bands, B);
+    if (C == 22)
+        k_up8_bwd_strip<22><<<grid, kSCols * 11, smem, st>>>(prob, score, gt, cls_loss_out, upstream_cls, threshold, vertex_pred, lowres, bias_vertex,
+                                                            centers, vertex_loss_out, upstream_vertex, w_inside, sigma * sigma, h, w, rb, C, Cs, Cv,
+                                                            (__nv_bfloat16*)d_sc_bf16, (__nv_bfloat16*)d_vt_bf16, (float*)workspace);
+    else {
+        PCNN_SMEM_OPTIN(k_up8_bwd_strip<0>, 100 * 1024, "up8_bwd_strip<0>");
+        k_up8_bwd_strip<0><<<grid, kSCols * (C / 2), smem, st>>>(prob, score, gt, cls_loss_out, upstream_cls, threshold, vertex_pred, lowres,
+                                                                bias_vertex, centers, vertex_loss_out, upstream_vertex, w_inside, sigma * sigma, h, w,
+                                                                rb, C, Cs, Cv, (__nv_bfloat16*)d_sc_bf16, (__nv_bfloat16*)d_vt_bf16, (float*)workspace);
     }
-    PCNN_REQUIRE(vertex_pred, "up8_heads_bwd: the low-resolution vertex source needs the strip kernel (C even, 6..50)");
-    dim3 grid(h, B, chunks);
-    const size_t smem = sizeof(float) * ((size_t)kUbCols * 4 * C + 4 * C);
-    PCNN_REQUIRE(smem <= 200 * 1024, "up8_heads_bwd: too many classes for the shared-memory column buffer (C = %d)", C);
-    if (C == 22) {
-        PCNN_SMEM_OPTIN(k_up8_bwd<22>, 200 * 1024, "up8_bwd<22>");
-        k_up8_bwd<22><<<grid, kUbCols, smem, st>>>(prob, score, gt, cls_loss_out, upstream_cls, threshold, vertex_pred, centers, vertex_loss_out,
-                                                  upstream_vertex, w_inside, sigma * sigma, h, w, C, Cs, Cv, (__nv_bfloat16*)d_sc_bf16,
-                                                  (__nv_bfloat16*)d_vt_bf16, (float*)workspace);
-    } else {
-        PCNN_SMEM_OPTIN(k_up8_bwd<0>, 200 * 1024, "up8_bwd<0>");
-        k_up8_bwd<0><<<grid, kUbCols, smem, st>>>(prob, score, gt, cls_loss_out, upstream_cls, threshold, vertex_pred, centers, vertex_loss_out,
-                                                 upstream_vertex, w_inside, sigma * sigma, h, w, C, Cs, Cv, (__nv_bfloat16*)d_sc_bf16,
-                                                 (__nv_bfloat16*)d_vt_bf16, (float*)workspace);
-    }
-    k_sum_partials<<<(4 * C + 31) / 32, 256, 0, st>>>((const float*)workspace, B * h * chunks, 4 * C, 1.f, nullptr, 0.f, dbias);
+    k_sum_partials<<<(4 * C + 31) / 32, 256, 0, st>>>((const float*)workspace, B * strips * bands, 4 * C, 1.f, nullptr, 0.f, dbias);
     return check_launch("up8_heads_bwd");
 }
 
@@ -736,19 +525,4 @@ extern "C" int pcnn_half_to_float(const void* src_f16, size_t n, float scale, fl
     PCNN_REQUIRE(src_f16 && dst, "half_to_float: NULL tensor pointer");
     k_half_to_float<<<ew_blocks(n), 256, 0, (cudaStream_t)stream>>>((const __half*)src_f16, n, scale, dst);
     return check_launch("half_to_float");
-}
-
-// conv1_1 weight gradient: img [B,H,W,3] u8, dz [B,H,W,64] bf16 -> dW [64][27] f32 = scale * gradient (+ decay * w); workspace 592*64*27 floats
-extern "C" int pcnn_conv1_wgrad(const void* img_u8, const float* mean3_host, const void* dz_bf16, int B, int H, int W, float scale,
-                                const float* w, float decay, float* dW, void* workspace, size_t workspace_bytes, void* stream)
-{
-    PCNN_REQUIRE(img_u8 && dz_bf16 && dW && workspace, "conv1_wgrad: NULL tensor pointer");
-    const int grid = kNumSMs * 4;
-    PCNN_REQUIRE(workspace_bytes >= sizeof(float) * (size_t)grid * 64 * 27, "conv1_wgrad: workspace too small");
-    float m0 = 0.f, m1 = 0.f, m2 = 0.f;
-    if (mean3_host) { m0 = mean3_host[0]; m1 = mean3_host[1]; m2 = mean3_host[2]; }
-    cudaStream_t st = (cudaStream_t)stream;
-    k_conv1_wgrad<<<grid, 256, 0, st>>>((const unsigned char*)img_u8, (const __nv_bfloat16*)dz_bf16, B, H, W, m0, m1, m2, (float*)workspace);
-    k_sum_partials<<<(64 * 27 + 31) / 32, 256, 0, st>>>((const float*)workspace, grid, 64 * 27, scale, w, decay, dW);
-    return check_launch("conv1_wgrad");
 }

@@ -10,12 +10,12 @@ import torch
 from ._lib import check, f32, lib, ptr, stream, workspace
 
 
-def fc_weights_to_tc(w_in_out: torch.Tensor) -> torch.Tensor:
-    """TF fc weights [in, out] f32 (network.py:404-406) -> [out padded to a multiple of 128][in] fp16 (K contiguous)."""
+def fc_weights_to_tc(w_in_out: torch.Tensor, dtype=torch.float16) -> torch.Tensor:
+    """TF fc weights [in, out] f32 (network.py:404-406) -> [out padded to a multiple of 128][in] fp16 (or `dtype`; K contiguous)."""
     k, n = w_in_out.shape
     npad = (n + 127) // 128 * 128
-    w = torch.zeros((npad, k), dtype=torch.float16, device=w_in_out.device)
-    w[:n] = w_in_out.t().to(torch.float16)
+    w = torch.zeros((npad, k), dtype=dtype, device=w_in_out.device)
+    w[:n] = w_in_out.t().to(dtype)
     return w.contiguous()
 
 

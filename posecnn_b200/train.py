@@ -30,6 +30,7 @@ PyTorch supplies device memory, streams, NCCL plumbing and a few tiny glue ops o
 from __future__ import annotations
 
 import ctypes
+from typing import Callable, NamedTuple
 
 import torch
 import torch.distributed as dist
@@ -45,6 +46,60 @@ from .roi_pooling_layer import roi_pooling_op
 CONV_NAMES = [item[0] for item in VGG_CFG if isinstance(item, tuple)]
 POOL_AFTER = {"conv1_2", "conv2_2", "conv3_3", "conv4_3"}          # pool1..pool4 (vgg16_convs.py:80-97)
 GRL_LAMBDA = 0.01                                                  # gradient_reversal(0.01, name='greversal'), vgg16_convs.py:207
+SCORE_HEADS = ("score_conv4", "score_conv5", "score_conv4_vertex", "score_conv5_vertex")
+
+
+class Kind(NamedTuple):
+    to_master: Callable            # (TF-layout tensor, master rows or None) -> fp32 master
+    to_tf: Callable                # (master-layout tensor, TF shape) -> TF-layout tensor
+    copy16: torch.dtype | None     # the 16-bit tensor-core copy kept beside the master, refreshed by every update
+
+
+def _conv_master(w, rows=None):
+    """conv.hwio_to_tc's [Cout][kh*kw*Cin] layout in fp32, the Cout rows zero-padded to `rows`."""
+    t = conv.hwio_to_tc(w, torch.float32)
+    if rows is None:
+        return t
+    out = t.new_zeros((rows, t.shape[1]))
+    out[:t.shape[0]] = t
+    return out
+
+
+def _conv_to_tf(t, shape):
+    kh, kw, ci, co = shape
+    return t[:co].reshape(co, kh, kw, ci).permute(1, 2, 3, 0).contiguous()
+
+
+# How the step keeps each kind of parameter: the fp32 master is the layout the kernels read, so the 16-bit copy is the master rounded.
+KINDS = {
+    # 3x3 trunk [Cout][9 Cin]; 1x1 score heads [Cout][Cin] (RGB-D score_conv4 / 5: Cin = 1024); score / vertex_pred padded
+    "conv": Kind(_conv_master, _conv_to_tf, torch.bfloat16),
+    # [64][27] (K = tap * 3 + c); its bf16 copy is the padded [64][64] tile Trainer.conv1_tc, refreshed in _refresh_derived
+    "conv1_1": Kind(_conv_master, _conv_to_tf, None),
+    # [out padded to a multiple of 128][in]
+    "fc": Kind(lambda w, rows=None: pose_head.fc_weights_to_tc(w, torch.float32), lambda t, shape: t[:shape[1]].t().contiguous(),
+               torch.float16),
+    # [2][256], read in fp32 by the domain tail kernel
+    "domain_score": Kind(lambda w, rows=None: w.t().contiguous(), lambda t, shape: t.t().contiguous(), None),
+    "bias": Kind(lambda w, rows=None: w.clone(), lambda t, shape: t.clone(), None),
+}
+
+
+def param_layout(net) -> dict:
+    """{master name: (TF parameter name, kind, master rows)} for every parameter the training step updates.  score / vertex_pred
+    keep C / 3C rows zero-padded to 64 / 128: the channel counts of their 1x1 GEMMs, which pcnn_pack_lowres and the up8
+    backward read."""
+    trunks = ("", "_p") if net.input_format == "RGBD" else ("",)
+    weights = [(layer + sfx, "conv1_1" if layer == "conv1_1" else "conv", None) for sfx in trunks for layer in CONV_NAMES]
+    weights += [(name, "conv", None) for name in SCORE_HEADS] + [("score", "conv", 64), ("vertex_pred", "conv", 128)]
+    weights += [(name, "fc", None) for name in ("fc6", "fc7", "fc8") + (("fc9",) if net.domain_branch else ())]
+    if net.domain_branch:
+        weights.append(("domain_score", "domain_score", None))
+    layout = {}
+    for name, kind, rows in weights:
+        layout[name + "/w"] = (name + "/weights", kind, rows)
+        layout[name + "/b"] = (name + "/biases", "bias", None)
+    return layout
 
 
 def _tc_dgrad(w_tc: torch.Tensor, k: int) -> torch.Tensor:
@@ -72,48 +127,14 @@ class Trainer:
         self.fc_names = ("fc6", "fc7", "fc8") + (("fc9",) if self.adapt else ())
         self.comm = torch.cuda.Stream(device=net.device) if world > 1 else None
         P, dev = net.params, net.device
-        C = self.C
-        self.master, self.accum, self.tc, self.kind = {}, {}, {}, {}
-
-        def add(name, w32, copy16, kind):
-            self.master[name] = w32.contiguous()
-            self.accum[name] = torch.zeros_like(self.master[name])
-            self.tc[name] = copy16
-            self.kind[name] = kind
-
-        for sfx in self.trunks:
-            for layer in CONV_NAMES:
-                name = layer + sfx
-                w = P[f"{name}/weights"]
-                if layer == "conv1_1":
-                    add(name + "/w", w.reshape(27, 64).t().contiguous(), None, 0)                 # [64][27], refreshed into the padded [64][64] copy
-                else:
-                    wt = w.permute(3, 0, 1, 2).reshape(w.shape[3], -1)
-                    add(name + "/w", wt, wt.to(torch.bfloat16).contiguous(), 0)
-                add(name + "/b", P[f"{name}/biases"].clone(), None, 0)
-        for name in ("score_conv4", "score_conv5", "score_conv4_vertex", "score_conv5_vertex"):
-            w = P[f"{name}/weights"]
-            wt = w.reshape(w.shape[2], w.shape[3]).t().contiguous()                               # [Cout][512], RGBD score: [Cout][1024] (colour first)
-            add(name + "/w", wt, wt.to(torch.bfloat16).contiguous(), 0)
-            add(name + "/b", P[f"{name}/biases"].clone(), None, 0)
-        ws = torch.zeros((64, net.num_units), device=dev)                                         # `score` 1x1: [C -> 64 rows][64]
-        ws[:C] = P["score/weights"].reshape(net.num_units, C).t()
-        add("score/w", ws, ws.to(torch.bfloat16).contiguous(), 0)
-        add("score/b", P["score/biases"].clone(), None, 0)
-        wv = torch.zeros((128, 128), device=dev)                                                  # `vertex_pred` 1x1: [3C -> 128 rows][128]
-        wv[:3 * C] = P["vertex_pred/weights"].reshape(128, 3 * C).t()
-        add("vertex_pred/w", wv, wv.to(torch.bfloat16).contiguous(), 0)
-        add("vertex_pred/b", P["vertex_pred/biases"].clone(), None, 0)
-        for name in self.fc_names:
-            w = P[f"{name}/weights"]                                                              # [in, out]
-            npad = (w.shape[1] + 127) // 128 * 128
-            wt = torch.zeros((npad, w.shape[0]), device=dev)
-            wt[:w.shape[1]] = w.t()
-            add(name + "/w", wt, wt.to(torch.float16).contiguous(), 1)
-            add(name + "/b", P[f"{name}/biases"].clone(), None, 0)
-        if self.adapt:
-            add("domain_score/w", P["domain_score/weights"].t().contiguous(), None, 0)           # [2][256] f32, read by the tail kernel
-            add("domain_score/b", P["domain_score/biases"].clone(), None, 0)
+        self.layout = param_layout(net)
+        self.master, self.accum, self.tc = {}, {}, {}
+        for name, (tf, kind, rows) in self.layout.items():
+            k = KINDS[kind]
+            w = k.to_master(P[tf], rows)
+            self.master[name] = w
+            self.accum[name] = torch.zeros_like(w)
+            self.tc[name] = w.to(k.copy16).contiguous() if k.copy16 else None
         self.conv1_tc = conv.conv1_1_weights_to_tc(P["conv1_1/weights"])
         self.conv1_tc_p = conv.conv1_1_weights_to_tc(P["conv1_1_p/weights"]) if self.rgbd else None
         self._refresh_derived()
@@ -127,7 +148,7 @@ class Trainer:
         for sfx in self.trunks:
             for name in CONV_NAMES[1:]:
                 self.dg[name + sfx] = _tc_dgrad(self.tc[name + sfx + "/w"], 3)
-        for name in ("score_conv4", "score_conv5", "score_conv4_vertex", "score_conv5_vertex", "score", "vertex_pred"):
+        for name in SCORE_HEADS + ("score", "vertex_pred"):
             self.dg[name] = _tc_dgrad(self.tc[name + "/w"], 1)
         if self.rgbd:
             # score_conv4/5 read the concat [colour 512 | depth 512]: their input-gradient weights [1024][U] split into two
@@ -147,32 +168,15 @@ class Trainer:
             self.conv1_tc_p.zero_()
             self.conv1_tc_p[:, :27] = self.master["conv1_1_p/w"].to(torch.bfloat16)
 
+    def to_tf(self, name, t):
+        """A master-layout tensor of parameter `name` (a master, a gradient) -> the TF layout of its net.params entry."""
+        tf, kind, _ = self.layout[name]
+        return KINDS[kind].to_tf(t, self.net.params[tf].shape)
+
     def export_params(self):
         """Write the fp32 master weights back into net.params (TF layouts) and re-derive the inference copies."""
-        P, C = self.net.params, self.C
-        for sfx in self.trunks:
-            for layer in CONV_NAMES:
-                name = layer + sfx
-                shp = P[f"{name}/weights"].shape
-                if layer == "conv1_1":
-                    P[f"{name}/weights"] = self.master[name + "/w"].t().reshape(shp).contiguous()
-                else:
-                    P[f"{name}/weights"] = self.master[name + "/w"].view(shp[3], shp[0], shp[1], shp[2]).permute(1, 2, 3, 0).contiguous()
-                P[f"{name}/biases"] = self.master[name + "/b"].clone()
-        for name in ("score_conv4", "score_conv5", "score_conv4_vertex", "score_conv5_vertex"):
-            P[f"{name}/weights"] = self.master[name + "/w"].t().reshape(P[f"{name}/weights"].shape).contiguous()
-            P[f"{name}/biases"] = self.master[name + "/b"].clone()
-        P["score/weights"] = self.master["score/w"][:C].t().reshape(P["score/weights"].shape).contiguous()
-        P["score/biases"] = self.master["score/b"].clone()
-        P["vertex_pred/weights"] = self.master["vertex_pred/w"][:3 * C].t().reshape(P["vertex_pred/weights"].shape).contiguous()
-        P["vertex_pred/biases"] = self.master["vertex_pred/b"].clone()
-        for name in self.fc_names:
-            n_out = P[f"{name}/weights"].shape[1]
-            P[f"{name}/weights"] = self.master[name + "/w"][:n_out].t().contiguous()
-            P[f"{name}/biases"] = self.master[name + "/b"].clone()
-        if self.adapt:
-            P["domain_score/weights"] = self.master["domain_score/w"].t().contiguous()
-            P["domain_score/biases"] = self.master["domain_score/b"].clone()
+        for name, (tf, _, _) in self.layout.items():
+            self.net.params[tf] = self.to_tf(name, self.master[name])
         self.net.prepare()
 
     # ------------------------------------------------------------------ forward (training graph, activations kept)
@@ -329,15 +333,11 @@ class Trainer:
             dist.all_reduce(norm, op=dist.ReduceOp.SUM)
             A["cls_out"] = torch.stack([A["cls_out"][0] * local[0] / norm[0].clamp(min=1.0), norm[0]])     # this rank's share of the global mean
             A["vtx_out"] = torch.stack([A["vtx_out"][0] * local[1] / norm[1].clamp(min=1e-10), norm[1]])
-        rows_global = norm[2]
         # Averagedistance divides by the rows IT sees (capacity rows of this rank); the reference batch sees all of them
-        rows_g = float(rows)
-        if self.world == 1:
-            pose_scale = 1.0
-        elif self.adapt:
-            pose_scale, rows_g = torch.stack([float(rows) / rows_global, rows_global]).tolist()
+        if self.world > 1:
+            pose_scale, rows_g = torch.stack([float(rows) / norm[2], norm[2]]).tolist()         # one host read
         else:
-            pose_scale = (float(rows) / rows_global).item()
+            pose_scale, rows_g = 1.0, float(rows)
         A["loss_pose"] = A["loss_pose_raw"] * pose_scale
         if self.adapt:
             # domain branch, un-scaled pass: its gradient maximum is read with the pose chain's below
@@ -352,18 +352,15 @@ class Trainer:
                                         stream()))
         # dynamic loss scale: a power of two that puts the largest element of the chain's entry point at ~2^11 (one host read; the
         # un-scaled pass above is only used for its maximum, which fp16 represents well enough even when the small elements underflow)
-        if self.adapt:
-            amax, amax_d = torch.stack([dpre.float().abs().max(), dom["amax"][0]]).tolist()
-        else:
-            amax = float(dpre.float().abs().max().item())
+        amax = torch.stack([dpre.float().abs().max()] + ([dom["amax"][0]] if self.adapt else []))
         if self.world > 1:
-            t = torch.tensor([amax, amax_d] if self.adapt else [amax], device=dev); dist.all_reduce(t, op=dist.ReduceOp.MAX)
-            amax, amax_d = t.tolist() if self.adapt else (float(t.item()), None)
-        S = self._loss_scale(amax)
+            dist.all_reduce(amax, op=dist.ReduceOp.MAX)
+        amax = amax.tolist()
+        S = self._loss_scale(amax[0])
         self.pose_loss_scale = S
         if self.adapt:
             # the same dynamic power of two for fc9's backward GEMMs (d fc9 is ~1e-5: below fp16's normal range)
-            S_d = self._loss_scale(amax_d)
+            S_d = self._loss_scale(amax[1])
             self.domain_loss_scale = S_d
             dom = pose_head.domain_tail(A["fc9"], M["domain_score/w"], M["domain_score/b"], A["label_domain"], self.adapt_weight / rows_g, S_d)
             A["loss_domain"] = dom["loss"]
@@ -396,7 +393,7 @@ class Trainer:
         d_sc = torch.empty((B, h, w, 64), dtype=torch.bfloat16, device=dev)
         d_vt = torch.empty((B, h, w, 128), dtype=torch.bfloat16, device=dev)
         dbias = torch.empty((4 * C,), dtype=torch.float32, device=dev)
-        ws = workspace("up8_bwd", 4 * B * max(h * ((w + 15) // 16), ((w + 3) // 4) * ((h + 15) // 16)) * 4 * C, dev)
+        ws = workspace("up8_bwd", 4 * B * ((w + 3) // 4) * ((h + 15) // 16) * 4 * C, dev)
         check(lib().pcnn_up8_heads_bwd_ex(ptr(A["prob_normalized"]), ptr(A["score"]), ptr(gt_label_2d), ptr(A["cls_out"]), f32(1.0),
                                           f32(net.threshold_label), ptr(None), ptr(A["lowres"]), ptr(M["vertex_pred/b"]), ptr(centers),
                                           ptr(A["vtx_out"]), f32(self.vertex_w), f32(self.w_inside), f32(1.0), B, h, w, C, 64, 128, ptr(d_sc),
@@ -462,7 +459,7 @@ class Trainer:
             self._emit(grads, name + "/b", db)
             if layer == "conv1_1":
                 # Cin = 3: the weight gradient is the 1x1 tensor-core wgrad on the im2col view of the input (K = tap * 3 + c, the same
-                # bf16 (pixel - mean) values the forward MMA consumed); a CUDA-core kernel (pcnn_conv1_wgrad) took 2.6 ms at batch 16
+                # bf16 (pixel - mean) values the forward MMA consumed)
                 cols = im2col()                                                                 # [B,H,W,64] bf16, 27 columns used
                 self._emit(grads, name + "/w", bw.conv_wgrad(cols, dz, 1)[:, :27].contiguous())
                 break
@@ -481,7 +478,7 @@ class Trainer:
             assert g.shape == w.shape, (name, tuple(g.shape), tuple(w.shape))
             c16 = self.tc[name]
             check(lib().pcnn_sgd_momentum(ptr(w), ptr(self.accum[name]), ptr(g), ctypes.c_size_t(w.numel()), f32(self.lr), f32(self.mu), f32(self.wd),
-                                          f32(1.0), ptr(c16), int(self.kind[name]), stream()))
+                                          f32(1.0), ptr(c16), int(c16 is not None and c16.dtype == torch.float16), stream()))
         self._refresh_derived()
 
     def step(self, data, gt_label_2d, centers, meta_data, extents, gt_poses, points, symmetry, batch_global=None, batch_offset=0,

@@ -101,26 +101,6 @@ def test_conv_dgrad_through_forward_kernel(cuda, Cin, Cout, k):
     assert e < 5e-3, e                                                        # one bf16 rounding of the output
 
 
-def test_conv1_wgrad_cuda_cores(cuda):
-    """conv1_1 weight gradient (Cin = 3, input = uint8 image - mean) against autograd on the same bf16 dz."""
-    import ctypes
-    from posecnn_b200._lib import check, f32, lib, ptr, stream, workspace
-    g = torch.Generator().manual_seed(7)
-    B, H, W = 2, 20, 28
-    img = torch.randint(0, 256, (B, H, W, 3), generator=g, dtype=torch.uint8).to(cuda)
-    dz = (torch.randn(B, H, W, 64, generator=g) * 0.1).to(torch.bfloat16).to(cuda)
-    mean = (102.9801, 115.9465, 122.7717)
-    x = (img.float() - torch.tensor(mean, device=cuda)).permute(0, 3, 1, 2)
-    w = torch.zeros(64, 3, 3, 3, device=cuda, requires_grad=True)
-    F.conv2d(x, w, padding=1).backward(dz.float().permute(0, 3, 1, 2))
-    want = w.grad.permute(0, 2, 3, 1).reshape(64, 27)                       # [co][tap * 3 + c]
-    got = torch.empty((64, 27), device=cuda)
-    ws = workspace("conv1_wgrad", 4 * 132 * 4 * 64 * 27, cuda)
-    m = (ctypes.c_float * 3)(*mean)
-    check(lib().pcnn_conv1_wgrad(ptr(img), m, ptr(dz), B, H, W, f32(1.0), ptr(None), f32(0.0), ptr(got), ptr(ws), ctypes.c_size_t(ws.numel()), stream()))
-    assert rel_l2(got, want) < 1e-5
-
-
 def test_fc_dgrad_wgrad_and_pose_chain(cuda):
     """Fully connected backward GEMMs (fp16 operands) and the pose-loss chain against torch on the same operands."""
     import ctypes
@@ -196,7 +176,7 @@ def _up8_bwd(P, dense, thr=0.7, up_cls=1.0, up_vtx=2.0, w_in=10.0, sigma=1.0, co
     d_vt = torch.full((B, h, w, 128), 7.0, dtype=torch.bfloat16, device=dev)
     dbias = torch.empty((4 * C,), device=dev)
     cls_out, vtx_out = torch.tensor([0.5, count], device=dev), torch.tensor([0.25, sumw], device=dev)
-    ws = torch.empty(4 * B * max(h * ((w + 15) // 16), ((w + 3) // 4) * ((h + 15) // 16)) * 4 * C, dtype=torch.uint8, device=dev)
+    ws = torch.empty(4 * B * ((w + 3) // 4) * ((h + 15) // 16) * 4 * C, dtype=torch.uint8, device=dev)
     check(lib().pcnn_up8_heads_bwd_ex(ptr(P["prob"]), ptr(P["score"]), ptr(P["gt"]), ptr(cls_out), f32(up_cls), f32(thr),
                                       ptr(P["vertex"] if dense else None), ptr(None if dense else P["lowres"]), ptr(None if dense else P["bv"]),
                                       ptr(P["centers"]), ptr(vtx_out), f32(up_vtx), f32(w_in), f32(sigma), B, h, w, C, 64, 128, ptr(d_sc), ptr(d_vt),

@@ -60,6 +60,12 @@ def test_host_planning_without_gpu(native_lib):
     f1 = ctypes.c_float(1.0)
     assert native_lib.pcnn_up8_heads_bwd_ex(None, None, None, None, f1, f1, None, None, None, None, None, f1, f1, f1, 1, 8, 8, 22, 64, 128,
                                             None, None, None, None, ctypes.c_size_t(0), None) == -1
+    native_lib.pcnn_last_error.restype = ctypes.c_char_p
+    buf = ctypes.create_string_buffer(64)                      # any non-NULL host address: the checks fail before it is read
+    for C in (4, 7, 23, 52):                                   # the strip kernel's class counts: even, 6..50
+        assert native_lib.pcnn_up8_heads_bwd_ex(buf, buf, buf, buf, f1, f1, buf, None, None, buf, buf, f1, f1, f1, 1, 8, 8, C, 64, 160,
+                                                buf, buf, buf, buf, ctypes.c_size_t(1 << 20), None) == -1, C
+        assert b"C must be even" in native_lib.pcnn_last_error()
     assert native_lib.pcnn_vertex_loss_fused_lowres_fwd(None, None, None, None, 1, 64, 96, 22, ctypes.c_float(1.0), ctypes.c_float(1.0), None,
                                                         None, ctypes.c_size_t(0), None) == -1
 

@@ -3,31 +3,18 @@ the fused tail kernel, fc9's GEMMs at their shapes, the merge that applies the g
 fp32 autograd with the reversal restated as an autograd Function (identity forward, -lambda backward), invariants against the
 step without the branch, the dummy Hough row, inference and CUDA-graph capture, and two ranks."""
 import ctypes
-import os
-import socket
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 
-from oracle import oracle
-from posecnn_b200 import synth
-from tests import ref_network as R
-from tests.test_train_step_gpu import _ste, ad_loss_torch, rel_l2, to_tf_grad
+from tests.train_ref import (LAMBDA, bits, compare_grads, grads_of, limits_adapt, make_inputs, make_net, reference_grads, rel_l2,
+                             run_two_ranks, synthetic_pose_targets, train_worker)
 
 pytestmark = pytest.mark.gpu
 torch.backends.cudnn.allow_tf32 = False
 torch.backends.cuda.matmul.allow_tf32 = False
-MEANS = (102.9801, 115.9465, 122.7717)
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-LAMBDA = 0.01
-
-
-def _bits(t):
-    return t.contiguous().view(torch.int16 if t.element_size() == 2 else torch.int32)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -70,7 +57,7 @@ def test_domain_tail_against_float64(cuda, rows):
     if rows > 1:
         assert bool(dead.any()) and bool((~dead).any())
     for k in a:
-        assert torch.equal(_bits(a[k]), _bits(b[k])), k                     # run-to-run bit-identical
+        assert torch.equal(bits(a[k]), bits(b[k])), k                     # run-to-run bit-identical
     for k in ("domain_score", "domain_prob", "domain_label"):
         assert torch.equal(a[k], inf[k]), k
     assert torch.allclose(a["domain_score"].double(), z, rtol=1e-5, atol=1e-6)
@@ -141,7 +128,7 @@ def test_fc9_exact(cuda, M):
     lin = pool.double() @ w9.double() + b9.double()
     out = pose_head.fc(pool, w_tc, b9, "relu")
     torch.cuda.synchronize()
-    assert torch.equal(_bits(out), _bits(lin.clamp(min=0).float().to(torch.float16)))
+    assert torch.equal(bits(out), bits(lin.clamp(min=0).float().to(torch.float16)))
     # input gradient: dy [M,256] against the [25088][256] transposed copy, no mask (pool_score has none)
     dy = int_operands((M, N), -1, 1, g).to(torch.float16).to(cuda)
     wt = w_tc.t().contiguous()
@@ -151,7 +138,7 @@ def test_fc9_exact(cuda, M):
     ws = workspace("fc", nbytes.value, cuda)
     check(lib().pcnn_fc_dgrad_f16_tc(ptr(dy), ptr(wt), M, K, N, ptr(None), ptr(dx), K, ptr(ws), ctypes.c_size_t(ws.numel()), stream()))
     torch.cuda.synchronize()
-    assert torch.equal(_bits(dx), _bits((dy.double() @ wt.double().t()).float().to(torch.float16)))
+    assert torch.equal(bits(dx), bits((dy.double() @ wt.double().t()).float().to(torch.float16)))
     # weight gradient [256][25088] with a power-of-two scale
     dw = torch.empty((N, K), dtype=torch.float32, device=cuda)
     check(lib().pcnn_conv_wgrad_workspace_bytes(1, 1, M, K, N, 1, ctypes.byref(nbytes)))
@@ -191,180 +178,12 @@ def test_domain_grad_merge_bit_exact(cuda, rows):
     h2f = torch.empty(n, dtype=torch.float32, device=cuda)
     check(lib().pcnn_half_to_float(ptr(ad), ctypes.c_size_t(n), f32(sa), ptr(h2f), stream()))
     torch.cuda.synchronize()
-    assert torch.equal(_bits(zero.reshape(-1)), _bits(h2f))
+    assert torch.equal(bits(zero.reshape(-1)), bits(h2f))
 
 
 # ---------------------------------------------------------------------------------------------------------------------
 # 4-7. the training step
 # ---------------------------------------------------------------------------------------------------------------------
-def make_net(cuda, C=6, adaptation=True, fmt="COLOR", is_train=True, seed=0):
-    from posecnn_b200.networks.vgg16_convs import vgg16_convs
-    net = vgg16_convs(input_format=fmt, num_classes=C, device=cuda, is_train=is_train, fold_vertex_head=False,
-                      adaptation=adaptation).init_random(seed=seed, bias_std=0.02)
-    net.params["score/weights"] *= 0.02
-    net.params["vertex_pred/weights"] *= 0.02
-    net.params["fc8/weights"] *= 0.01
-    if adaptation:      # O(1) domain logits: a saturated softmax leaves only fp32 cancellation noise in the reference's gradient
-        net.params["domain_score/weights"] *= 0.05
-    net.prepare()
-    return net
-
-
-def make_inputs(cuda, B=2, H=64, W=96, C=6):
-    """The scene of tests/test_train_step_gpu.py make_problem, and its adapt form: labels -1 everywhere, no gt poses, no centres."""
-    rgb, depth = synth.make_images(B, H, W, seed=3)
-    sc = synth.make_scene(batch=B, height=H, width=W, num_classes=C, objects_per_image=3, seed=11, min_pixels=200)
-    centers = np.zeros((B, C, 3), np.float32)
-    for (b, cls, cx, cy, z) in sc["centers"]:
-        centers[b, cls] = (cx, cy, z)
-    T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(cuda)
-    labelled = (T(rgb), T(sc["label"]), T(centers), T(sc["meta"].reshape(B, 48)), T(sc["extents"]), T(sc["gt"]),
-                T(synth.make_model_points(C, 300)), torch.zeros(C, device=cuda))
-    adapt = (labelled[0], torch.full_like(labelled[1], -1), torch.zeros_like(labelled[2]), labelled[3], labelled[4],
-             torch.zeros((0, 13), device=cuda), labelled[6], labelled[7])
-    return labelled, adapt, T((depth * 1000.0).astype(np.float32))
-
-
-class GradReverse(torch.autograd.Function):
-    """gradient_reversal_op_gpu.cu.cc: identity forward, -lambda * grad backward."""
-    @staticmethod
-    def forward(ctx, x, lam):
-        ctx.lam = lam
-        return x.view_as(x)
-
-    @staticmethod
-    def backward(ctx, g):
-        return -ctx.lam * g, None
-
-
-def reference_grads_adapt(net, A, data, gt, centers, targets, weights, points, vertex_w, w_inside, margin, adapt_weight, sim16,
-                          domain_only=False, lam=LAMBDA):
-    """torch fp32 autograd of the colour graph with the domain branch (tests/test_train_step_gpu.py reference_grads plus
-    pool_score -> GradReverse -> fc9 -> ReLU -> domain_score -> ReLU -> cross entropy); ROI pooling gathers at OUR arg-max positions,
-    label_domain is Hough's.  domain_only: loss = loss_domain alone.  Returns the parameters (with .grad), the losses and the
-    gradient of pool_score."""
-    P = {k: v.detach().clone().requires_grad_(True) for k, v in net.params.items()}
-    C = net.num_classes
-    bf, hf = torch.bfloat16, torch.float16
-    r16 = (lambda y: _ste(y, bf)) if sim16 else (lambda y: y)
-    rh = (lambda y: _ste(y, hf)) if sim16 else (lambda y: y)
-    W = (lambda w: _ste(w, bf)) if sim16 else (lambda w: w)
-    Wh = (lambda w: _ste(w, hf)) if sim16 else (lambda w: w)
-    x = (data.float() - torch.tensor(MEANS, device=data.device)).permute(0, 3, 1, 2)
-    if sim16:
-        x = r16(x)
-    feats = {}
-    for item in R.VGG_CFG:
-        if isinstance(item, str):
-            x = F.max_pool2d(x, 2)
-        else:
-            x = r16(R.conv(x, W(P[f"{item[0]}/weights"]), P[f"{item[0]}/biases"]))
-            feats[item[0]] = x
-    c4, c5 = feats["conv4_3"], feats["conv5_3"]
-    if sim16:
-        s5 = r16(R.conv(c5, W(P["score_conv5/weights"]), P["score_conv5/biases"]))
-        s4 = r16(R.conv(c4, W(P["score_conv4/weights"]), P["score_conv4/biases"]))
-        v5 = r16(R.conv(c5, W(P["score_conv5_vertex/weights"]), P["score_conv5_vertex/biases"], False))
-        v4 = r16(R.conv(c4, W(P["score_conv4_vertex/weights"]), P["score_conv4_vertex/biases"], False))
-        add_s, add_v = r16(s4 + R.deconv(s5, 4, 2)), r16(v4 + R.deconv(v5, 4, 2))
-        zs, zv = torch.zeros(C, device=data.device), torch.zeros(3 * C, device=data.device)
-        lr_s = r16(R.conv(add_s, W(P["score/weights"]), zs, False))
-        lr_v = r16(R.conv(add_v, W(P["vertex_pred/weights"]), zv, False))
-        score = torch.relu(R.deconv(lr_s, 16, 8) + P["score/biases"][None, :, None, None])
-        vertex = R.deconv(lr_v, 16, 8) + P["vertex_pred/biases"][None, :, None, None]
-        prob = F.softmax(score, 1)
-    else:
-        score, label, prob, vertex = R.heads(P, c4, c5, C)
-    B = data.shape[0]
-    g = gt.long()
-    pg = prob.detach().gather(1, g.clamp(min=0)[:, None])[:, 0]
-    sel = (g >= 0) & ((g > 0) | (pg < net.threshold_label))
-    logp = F.log_softmax(score, 1).gather(1, g.clamp(min=0)[:, None])[:, 0]
-    loss_cls = -(logp * sel).sum() / (sel.sum() + 1e-10)
-    vt, vw = oracle.generate_vertex_targets(gt.cpu().numpy(), centers.cpu().numpy(), w_inside)
-    vt, vw = torch.from_numpy(vt).to(data.device).permute(0, 3, 1, 2), torch.from_numpy(vw).to(data.device).permute(0, 3, 1, 2)
-    diff = vw * (vertex - vt)
-    sl1 = torch.where(diff.abs() < 1, 0.5 * diff * diff, diff.abs() - 0.5)
-    loss_vertex = sl1.sum() / (vw.sum() + 1e-10)
-    rois = A["rois"]
-    n = rois.shape[0]
-
-    def pool(feat, arg):
-        f = feat.permute(0, 2, 3, 1).reshape(B, -1)
-        idx = arg.reshape(n, -1).long()
-        b = rois[:, 0].long()
-        return f[b[:, None], idx.clamp(min=0)] * (idx >= 0)
-    ps = rh(pool(c5, A["a5"]) + pool(c4, A["a4"]))
-    ps.retain_grad()
-    h6 = rh(torch.relu(ps @ Wh(P["fc6/weights"]) + P["fc6/biases"]))
-    h7 = rh(torch.relu(h6 @ Wh(P["fc7/weights"]) + P["fc7/biases"]))
-    th = torch.tanh(h7 @ Wh(P["fc8/weights"]) + P["fc8/biases"])
-    mul = th * weights
-    pred = mul / mul.pow(2).sum(1, keepdim=True).clamp(min=1e-12).sqrt()
-    loss_pose = ad_loss_torch(pred, targets, weights, points, margin)
-    h9 = rh(torch.relu(GradReverse.apply(ps, lam) @ Wh(P["fc9/weights"]) + P["fc9/biases"]))
-    z = torch.relu(h9 @ P["domain_score/weights"] + P["domain_score/biases"])
-    loss_domain = adapt_weight * F.cross_entropy(z, A["label_domain"].long())
-    loss = loss_domain if domain_only else loss_cls + vertex_w * loss_vertex + loss_pose + loss_domain
-    loss.backward()
-    return P, dict(loss_cls=loss_cls.item(), loss_vertex=(vertex_w * loss_vertex).item(), loss_pose=loss_pose.item(),
-                   loss_domain=loss_domain.item(), dpool=ps.grad.detach(), domain_score=z.detach())
-
-
-def synthetic_pose_targets(A, pts, sym, margin, C, cuda):
-    """Quaternion targets on the ROI rows' own classes, as tests/test_train_step_gpu.py sets them."""
-    from posecnn_b200.average_distance_loss import average_distance_loss_op
-    rows = A["rows"]
-    g = torch.Generator().manual_seed(5)
-    tw, wt = torch.zeros(rows, 4 * C), torch.zeros(rows, 4 * C)
-    for r in range(rows):
-        c = int(A["rois"][r, 1].item())
-        q = torch.randn(4, generator=g); q = q / q.norm()
-        tw[r, 4 * c:4 * c + 4] = q; wt[r, 4 * c:4 * c + 4] = 1.0
-    tw, wt = tw.to(cuda), wt.to(cuda)
-    mul = A["poses_tanh"] * wt
-    pred = (mul / mul.pow(2).sum(1, keepdim=True).clamp(min=1e-12).sqrt()).contiguous()
-    A["loss_pose_raw"], A["pose_diff"] = average_distance_loss_op.average_distance_loss(pred, tw, wt, pts, sym, margin)
-    A["poses_weight"], A["poses_target"] = wt, tw
-    return tw, wt
-
-
-def _limits(name):
-    """(16-bit-rounded, pure fp32) relative-L2 limits of tests/test_train_step_gpu.py; fc9 is held to fc6's, domain_score to the
-    heads' limits."""
-    layer = name.split("/")[0]
-    lim16 = 0.2 if name == "conv1_1/w" else (0.15 if layer in ("conv1_1", "conv1_2", "fc6", "fc7", "fc8", "fc9") else 6e-2)
-    lim32 = 0.3 if layer in ("conv1_1", "conv1_2") else (0.15 if layer in ("fc6", "fc7", "fc8", "fc9") else 0.1)
-    return lim16, lim32
-
-
-def _limits_adapt(name):
-    """The adapt batch's trunk gradients have one sparse source (the reversed domain gradient scattered by RoiPool at the ROI
-    maxima), and their weight gradients cancel more than the colour step's: the bf16 rounding of the propagated gradient shows
-    amplified further down.  Measured on this problem (16-bit-rounded / pure fp32 graph): 0.04-0.06 / 0.05-0.07 for conv5_x,
-    0.05-0.08 / 0.06-0.10 for conv4_x, 0.09-0.13 / 0.11-0.16 for conv3_x and 0.13-0.17 / 0.19-0.28 for conv1_x-conv2_x."""
-    block = name.split("/")[0][:5]
-    if block in ("conv5", "conv4"):
-        return 0.12, 0.15
-    return (0.2, 0.25) if block == "conv3" else (0.3, 0.4)
-
-
-def _compare(tr, grads, P, Pf, names, limits=_limits):
-    errs = {}
-    for name in names:
-        layer, kind = name.split("/")
-        key = f"{layer}/{'weights' if kind == 'w' else 'biases'}"
-        got = to_tf_grad(tr, name, grads[name])
-        assert got.shape == P[key].grad.shape, name
-        e16, e32 = rel_l2(got, P[key].grad), rel_l2(got, Pf[key].grad)
-        print(f"grad {name:22s} rel-L2 vs 16-bit-rounded graph {e16:.3e}   vs pure fp32 graph {e32:.3e}   |ref| {P[key].grad.norm().item():.3e}")
-        errs[name] = (e16, e32)
-    for name, (e16, e32) in errs.items():
-        lim16, lim32 = limits(name)
-        assert e16 < lim16, (name, e16, lim16)
-        assert e32 < lim32, (name, e32, lim32)
-
-
 def test_labelled_batch_matches_fp32_autograd(cuda):
     """Domain 0 (the batch has gt poses), ADAPT_WEIGHT = 1.0 as the shipped adaptation config: every gradient, the new ones
     included, against the 16-bit-rounded and the pure fp32 autograd graph.  The reversal itself is checked on pool_score's
@@ -372,7 +191,7 @@ def test_labelled_batch_matches_fp32_autograd(cuda):
     autograd of loss_domain alone — a wrong sign or lambda would be off by 2x or more."""
     from posecnn_b200.train import Trainer
     C, aw, margin = 6, 1.0, 0.01
-    net = make_net(cuda, C)
+    net = make_net(cuda, adaptation=True, C=C)
     args, _, _ = make_inputs(cuda, C=C)
     data, gt, centers, meta, ext, gtp, pts, sym = args
     tr = Trainer(net, lr=0.01, momentum=0.9, weight_decay=1e-4, vertex_w=1.0, vertex_w_inside=10.0, margin=margin, adapt_weight=aw)
@@ -381,7 +200,7 @@ def test_labelled_batch_matches_fp32_autograd(cuda):
     A = tr.forward(*args)
     assert A["rows"] >= 9
     assert not bool(A["label_domain"].any())
-    tw, wt = synthetic_pose_targets(A, pts, sym, margin, C, cuda)
+    tw, wt = synthetic_pose_targets(A, pts, sym, margin)
     tr.adapt_weight = 0.0
     tr.backward(A, gt, centers)
     dpool0 = A["dpool"].clone()
@@ -389,17 +208,17 @@ def test_labelled_batch_matches_fp32_autograd(cuda):
     grads = tr.backward(A, gt, centers)
     torch.cuda.synchronize()
     assert set(grads) == set(tr.master)
-    P, ref = reference_grads_adapt(net, A, data, gt, centers, tw, wt, pts, 1.0, 10.0, margin, aw, sim16=True)
-    Pf, reff = reference_grads_adapt(net, A, data, gt, centers, tw, wt, pts, 1.0, 10.0, margin, aw, sim16=False)
+    P, ref = reference_grads(net, A, args, tw, wt, True, 1.0, 10.0, margin, adapt_weight=aw)
+    Pf, reff = reference_grads(net, A, args, tw, wt, False, 1.0, 10.0, margin, adapt_weight=aw)
     for r_ in (ref, reff):
         assert abs(A["loss_domain"].item() - r_["loss_domain"]) < 3e-2 * abs(r_["loss_domain"]), (A["loss_domain"].item(), r_["loss_domain"])
         assert abs(A["loss_pose"].item() - r_["loss_pose"]) < 3e-2 * max(1e-3, abs(r_["loss_pose"]))
     print(f"loss_domain {A['loss_domain'].item():.6f} (16-bit graph {ref['loss_domain']:.6f}, fp32 {reff['loss_domain']:.6f}); "
           f"domain loss scale {tr.domain_loss_scale:g}")
-    _compare(tr, grads, P, Pf, sorted(grads))
+    compare_grads(tr, grads, P, Pf, sorted(grads))
     # the reversed domain gradient of pool_score
-    _, dref = reference_grads_adapt(net, A, data, gt, centers, tw, wt, pts, 1.0, 10.0, margin, aw, sim16=True, domain_only=True)
-    _, dreff = reference_grads_adapt(net, A, data, gt, centers, tw, wt, pts, 1.0, 10.0, margin, aw, sim16=False, domain_only=True)
+    _, dref = reference_grads(net, A, args, tw, wt, True, 1.0, 10.0, margin, adapt_weight=aw, domain_only=True)
+    _, dreff = reference_grads(net, A, args, tw, wt, False, 1.0, 10.0, margin, adapt_weight=aw, domain_only=True)
     ours = (A["dpool"] - dpool0).reshape(A["rows"], -1)
     e16, e32 = rel_l2(ours, dref["dpool"]), rel_l2(ours, dreff["dpool"])
     flipped = rel_l2(ours, -dref["dpool"])
@@ -430,9 +249,9 @@ def test_adapt_batch_isolates_the_reversal(cuda):
     match autograd."""
     from posecnn_b200.train import Trainer
     C = 6
-    net = make_net(cuda, C)
+    net = make_net(cuda, adaptation=True, C=C)
     _, args, _ = make_inputs(cuda, C=C)
-    data, gt, centers = args[0], args[1], args[2]
+    gt, centers = args[1], args[2]
     tr = Trainer(net, lr=0.01, adapt_weight=1.0)
     A = tr.forward(*args)
     grads = tr.backward(A, gt, centers)
@@ -446,47 +265,38 @@ def test_adapt_batch_isolates_the_reversal(cuda):
     assert len(zero) == 18
     for k in zero:
         assert not bool(grads[k].any()), k
-    P, ref = reference_grads_adapt(net, A, data, gt, centers, A["poses_target"], A["poses_weight"], args[6], 1.0, 10.0, 0.01, 1.0,
-                                   sim16=True)
-    Pf, reff = reference_grads_adapt(net, A, data, gt, centers, A["poses_target"], A["poses_weight"], args[6], 1.0, 10.0, 0.01, 1.0,
-                                     sim16=False)
+    P, ref = reference_grads(net, A, args, A["poses_target"], A["poses_weight"], True, adapt_weight=1.0)
+    Pf, reff = reference_grads(net, A, args, A["poses_target"], A["poses_weight"], False, adapt_weight=1.0)
     for r_ in (ref, reff):
         assert abs(A["loss_domain"].item() - r_["loss_domain"]) < 3e-2 * abs(r_["loss_domain"])
     trunk = sorted(k for k in grads if k.startswith("conv"))
-    _compare(tr, grads, P, Pf, trunk, _limits_adapt)
-    _compare(tr, grads, P, Pf, sorted(k for k in grads if k not in zero and k not in trunk))
+    compare_grads(tr, grads, P, Pf, trunk, limits_adapt)
+    compare_grads(tr, grads, P, Pf, sorted(k for k in grads if k not in zero and k not in trunk))
     # the same comparison against a graph whose reversal has the wrong sign fails by far
-    Pw, _ = reference_grads_adapt(net, A, data, gt, centers, A["poses_target"], A["poses_weight"], args[6], 1.0, 10.0, 0.01, 1.0,
-                                  sim16=True, lam=-LAMBDA)
-    e = rel_l2(to_tf_grad(tr, "conv5_3/w", grads["conv5_3/w"]), Pw["conv5_3/weights"].grad)
+    Pw, _ = reference_grads(net, A, args, A["poses_target"], A["poses_weight"], True, adapt_weight=1.0, lam=-LAMBDA)
+    e = rel_l2(tr.to_tf("conv5_3/w", grads["conv5_3/w"]), Pw["conv5_3/weights"].grad)
     print(f"conv5_3/w against the un-reversed graph: {e:.3e}")
     assert e > 1.5
 
 
-def _grads(tr, args, **kw):
-    A = tr.forward(*args, **kw)
-    g = tr.backward(A, args[1], args[2])
-    torch.cuda.synchronize()
-    return {k: v.clone() for k, v in g.items()}
-
-
 def _same(a, b, k, unfixed):
-    """Byte-identical, except the two bias gradients k_up8_bwd sums with shared-memory atomics (tests/test_train_rgbd_gpu.py)."""
+    """Byte-identical, except the score / vertex_pred bias gradients when two runs of one input already differ in them
+    (tests/test_train_rgbd_gpu.py)."""
     if k in unfixed:
         assert torch.allclose(a, b, rtol=1e-5, atol=1e-9), k
     else:
-        assert torch.equal(_bits(a), _bits(b)), k
+        assert torch.equal(bits(a), bits(b)), k
 
 
 def test_adapt_weight_zero_leaves_shared_gradients_unchanged(cuda):
     from posecnn_b200.train import Trainer
     args, _, _ = make_inputs(cuda)
-    base = Trainer(make_net(cuda, adaptation=False), lr=0.01)
-    a, a2 = _grads(base, args), _grads(base, args)
+    base = Trainer(make_net(cuda), lr=0.01)
+    a, a2 = grads_of(base, args), grads_of(base, args)
     unfixed = {k for k in a if not torch.equal(a[k], a2[k])}
     assert unfixed <= {"score/b", "vertex_pred/b"}
-    tr = Trainer(make_net(cuda), lr=0.01, adapt_weight=0.0)
-    b = _grads(tr, args)
+    tr = Trainer(make_net(cuda, adaptation=True), lr=0.01, adapt_weight=0.0)
+    b = grads_of(tr, args)
     assert set(b) == set(a) | {"fc9/w", "fc9/b", "domain_score/w", "domain_score/b"}
     for k in a:
         _same(a[k], b[k], k, unfixed)
@@ -499,14 +309,14 @@ def test_rgbd_depth_trunk_gradients_unchanged(cuda):
     byte-identical to the step without the branch."""
     from posecnn_b200.train import Trainer
     args, _, dm = make_inputs(cuda)
-    a = _grads(Trainer(make_net(cuda, adaptation=False, fmt="RGBD"), lr=0.01), args, depth=dm)
-    tr = Trainer(make_net(cuda, fmt="RGBD"), lr=0.01, adapt_weight=1.0)
-    b = _grads(tr, args, depth=dm)
+    a = grads_of(Trainer(make_net(cuda, "RGBD"), lr=0.01), args, depth=dm)
+    tr = Trainer(make_net(cuda, "RGBD", adaptation=True), lr=0.01, adapt_weight=1.0)
+    b = grads_of(tr, args, depth=dm)
     assert "fc9/w" in b and tr.domain_loss_scale > 1
     p = [k for k in a if k.split("/")[0].endswith("_p")]
     assert len(p) == 26
     for k in p:
-        assert torch.equal(_bits(a[k]), _bits(b[k])), k
+        assert torch.equal(bits(a[k]), bits(b[k])), k
     assert not torch.equal(a["conv5_3/w"], b["conv5_3/w"])
 
 
@@ -514,7 +324,7 @@ def test_dummy_row(cuda):
     """An all-background label map: Hough finds nothing, the pose head and the domain branch see the one all-zero dummy row,
     label_domain = 0 (also on an adapt batch), and the loss is finite and equals the restatement."""
     from posecnn_b200.train import Trainer
-    net = make_net(cuda)
+    net = make_net(cuda, adaptation=True)
     net.params["score/biases"][0] += 1000.0
     net.prepare()
     _, args, _ = make_inputs(cuda)
@@ -538,7 +348,7 @@ def test_inference_domain_outputs_and_graph(cuda):
     from posecnn_b200.networks.vgg16_convs import GraphedForward
     args, _, _ = make_inputs(cuda)
     data, meta, ext = args[0], args[3], args[4]
-    net = make_net(cuda, is_train=False)
+    net = make_net(cuda, adaptation=True, is_train=False)
     L = dict(net.forward(data, meta, ext))
     P = net.params
     n = L["rois"].shape[0]
@@ -565,7 +375,7 @@ def test_inference_domain_outputs_and_graph(cuda):
     for k in ("fc9", "domain_score", "domain_prob", "domain_label"):
         assert torch.equal(out[k], eager[k]), k
     assert torch.equal(eager["domain_label"][:n], L["domain_label"])
-    plain = make_net(cuda, adaptation=False, is_train=False)
+    plain = make_net(cuda, is_train=False)
     Lp = plain.forward(data, meta, ext)
     assert not any(k in Lp for k in ("fc9", "domain_score", "domain_prob", "domain_label", "label_domain"))
     assert "fc9/weights" not in plain.params
@@ -576,7 +386,7 @@ def test_training_losses_adds_loss_domain(cuda):
     from posecnn_b200.networks.vgg16_convs import training_losses
     args, _, _ = make_inputs(cuda)
     data, gt, centers, meta, ext, gtp, pts, sym = args
-    net = make_net(cuda)
+    net = make_net(cuda, adaptation=True)
     L = net.forward(data, meta, ext, poses=gtp, want_prob=True, want_score=True)
     out = training_losses(net, L, gt, None, None, pts, sym, centers=centers, adapt_weight=0.5)
     torch.cuda.synchronize()
@@ -590,66 +400,7 @@ def test_training_losses_adds_loss_domain(cuda):
 # ---------------------------------------------------------------------------------------------------------------------
 # 9. two ranks
 # ---------------------------------------------------------------------------------------------------------------------
-TRAIN_WORKER = r'''
-import os, sys
-import numpy as np, torch, torch.distributed as dist
-sys.path.insert(0, %r)
-from posecnn_b200 import parallel, synth
-from posecnn_b200.networks.vgg16_convs import vgg16_convs
-from posecnn_b200.train import Trainer
-rank, world = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"])
-torch.cuda.set_device(rank)
-dev = torch.device("cuda", rank)
-dist.init_process_group("nccl", device_id=dev)
-B, H, W, C = 4, 64, 96, 6
-def problem():
-    net = vgg16_convs(num_classes=C, device=dev, is_train=True, fold_vertex_head=False, adaptation=True).init_random(seed=0, bias_std=0.02)
-    net.params["score/weights"] *= 0.02; net.params["vertex_pred/weights"] *= 0.02; net.params["fc8/weights"] *= 0.01
-    net.prepare()
-    return net
-rgb, _ = synth.make_images(B, H, W, seed=3)
-sc = synth.make_scene(batch=B, height=H, width=W, num_classes=C, objects_per_image=3, seed=11, min_pixels=200)
-centers = np.zeros((B, C, 3), np.float32)
-for (b, cls, cx, cy, z) in sc["centers"]:
-    centers[b, cls] = (cx, cy, z)
-gt_np = sc["gt"][sc["gt"][:, 0] < 2]           # gt poses on the first shard's images only: rank 1 has none of its own
-T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
-data, gt, cen, meta, ext, gtp = T(rgb), T(sc["label"]), T(centers), T(sc["meta"].reshape(B, 48)), T(sc["extents"]), T(gt_np)
-pts, sym = T(synth.make_model_points(C, 300)), torch.zeros(C, device=dev)
-single = Trainer(problem(), lr=0.01, world=1, adapt_weight=1.0)
-ref = single.step(data, gt, cen, meta, ext, gtp, pts, sym)
-o, n = parallel.shard_range(B, rank, world)
-tr = Trainer(problem(), lr=0.01, world=world, adapt_weight=1.0)
-out = tr.step(data[o:o + n], gt[o:o + n], cen[o:o + n], meta[o:o + n], ext, gtp, pts, sym, batch_global=B, batch_offset=o)
-torch.cuda.synchronize()
-assert not bool(out["label_domain"].any())     # decided by the whole batch's gt count, on every rank
-assert set(out["grads"]) == set(ref["grads"]) == set(tr.master)
-worst = 0.0
-for name, g in out["grads"].items():
-    w = ref["grads"][name]
-    e = ((g - w).norm() / w.norm().clamp(min=1e-20)).item()
-    worst = max(worst, e)
-    assert e < 2e-3, (name, e)
-for name in tr.master:
-    assert torch.allclose(tr.master[name], single.master[name], rtol=1e-4, atol=1e-6), name
-tot = torch.stack([out["loss_cls"][0], out["loss_vertex"][0], out["loss_pose"][0], out["loss_domain"][0]])
-dist.all_reduce(tot)
-want = torch.stack([ref["loss_cls"][0], ref["loss_vertex"][0], ref["loss_pose"][0], ref["loss_domain"][0]])
-assert torch.allclose(tot, want, rtol=1e-4, atol=1e-6), (tot, want)
-dist.barrier()
-dist.destroy_process_group()
-print("TRAIN_RANK_OK", rank, worst)
-''' % ROOT
-
-
 def test_two_rank_adaptation_step_equals_single_gpu(tmp_path):
     """One adaptation step on image shards over 2 ranks == the step on the whole batch on one GPU; the second shard holds no gt
     pose of its own and still gets label_domain 0."""
-    if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs")
-    s = socket.socket(); s.bind(("127.0.0.1", 0)); port = s.getsockname()[1]; s.close()
-    script = tmp_path / "train_adapt_worker.py"
-    script.write_text(TRAIN_WORKER)
-    out = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2", "--master-addr", "127.0.0.1",
-                          "--master-port", str(port), str(script)], capture_output=True, text=True, timeout=900)
-    assert out.returncode == 0 and out.stdout.count("TRAIN_RANK_OK") == 2, (out.stdout[-2000:], out.stderr[-3000:])
+    run_two_ranks(tmp_path, train_worker(adaptation=True))
