@@ -389,6 +389,42 @@ int pcnn_vertex_loss_fused_lowres_fwd(const float* lowres, const float* bias_ver
                                       int H, int W, int C, float w_inside, float sigma, float* loss_out, void* workspace,
                                       size_t workspace_bytes, void* stream);
 
+/* ---------------------------------------------------------------------------------------
+ * Training image blobs (csrc/augment.cu): the image side of the synthetic-data loader, lib/gt_synthesize_layer/minibatch.py:147-200
+ * with lib/utils/blob.py:74-129 (chromatic_transform, add_noise), PIXEL_MEANS subtraction (minibatch.py:179-180).
+ * params [B, PCNN_AUG_PARAMS] f64 (device), one row per image, columns PCNN_AUG_*:
+ *   BACKGROUND  background pool index; -1 (or any value outside [0, N)) = none: alpha == 0 pixels become 0 (minibatch.py:160-168)
+ *   CHROMATIC   1 = run chromatic_transform with D_H / D_L / D_S, 0 = skip it
+ *   NOISE       0 none, 1 Gaussian (SIGMA), 2 motion blur (BLUR_SIZE odd in 3..15, BLUR_AXIS 0 = along the row, 1 = along the column)
+ * keys [B] u64: the image's Philox4x32-10 key; the Gaussian field g(pixel) = Box-Muller(Philox(key, pixel index)) belongs to the image,
+ * so any shard of a batch produces the same rows.  noise_field [B,H,W] f64 (optional) replaces g bit for bit.
+ *  pcnn_augment_color_fwd   rgba [B,H,W,channels] u8 (channels 4, or 3 = no alpha, no compositing), backgrounds [N,H,W,3] u8 ->
+ *      blob [B,H,W,3] f32, per pixel: composite; BGR->HLS (OpenCV's uint8 arithmetic), H' = trunc((h + d_h) mod 180), L' / S' =
+ *      trunc(clip(. + d, 0, 255)) in f64, HLS->BGR (OpenCV); Gaussian: clip(x + sigma g, 0, 255) in f64, one g for the three
+ *      channels; blur: round(sum_{|t| <= r} x[reflect101(p + t)] / size) on the uint8 image; f32(f64(f32(x)) - mean3).
+ *  pcnn_depth_blob_train_fwd   depth [B,H,W] u16 (depth_is_u16) or f32 -> depth_max [B] f32 = max(d) per image, blob [B,H,W,3]
+ *      f32 = f32(f32(d) / max) * 255 tiled x3 (minibatch.py:187-200), the same noise on float data (blur: the float64 sum of the
+ *      taps / size, rounded once), - mean3; its own params / keys (the reference draws add_noise again).  An all-zero image gives NaN
+ *      (0 / 0), as numpy does.
+ * mean3_host: 3 host doubles (PIXEL_MEANS, BGR).  A malformed params row never faults (unknown noise = none, size outside [1, 15]
+ * = 1 tap).  No allocation, no host synchronisation; CUDA-graph capturable.
+ */
+#define PCNN_AUG_BACKGROUND 0
+#define PCNN_AUG_CHROMATIC 1
+#define PCNN_AUG_DH 2
+#define PCNN_AUG_DL 3
+#define PCNN_AUG_DS 4
+#define PCNN_AUG_NOISE 5
+#define PCNN_AUG_SIGMA 6
+#define PCNN_AUG_BLUR_SIZE 7
+#define PCNN_AUG_BLUR_AXIS 8
+#define PCNN_AUG_PARAMS 9
+int pcnn_augment_color_fwd(const uint8_t* rgba, int channels, const uint8_t* backgrounds, int num_backgrounds, const double* params,
+                           const uint64_t* keys, const double* noise_field, int B, int H, int W, const double* mean3_host, float* blob,
+                           void* stream);
+int pcnn_depth_blob_train_fwd(const void* depth, int depth_is_u16, const double* params, const uint64_t* keys, const double* noise_field,
+                              int B, int H, int W, const double* mean3_host, float* depth_max, float* blob, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

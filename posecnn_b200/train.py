@@ -180,6 +180,10 @@ class Trainer:
         self.net.prepare()
 
     # ------------------------------------------------------------------ forward (training graph, activations kept)
+    @staticmethod
+    def _mean(data):
+        return PIXEL_MEANS if data.dtype == torch.uint8 else None
+
     def _trunk_fwd(self, A, x, sfx=""):
         """conv1_2 .. conv5_3 of one trunk on its conv1_1 output x; every activation is kept in A (the backward pass reads them)."""
         M, T = self.master, self.tc
@@ -199,7 +203,9 @@ class Trainer:
         net, C, M, T = self.net, self.C, self.master, self.tc
         B, H, W, _ = data.shape
         A = {}                                    # activations by layer name (bf16 NHWC), "<pool>" = pooled tensors
-        self._trunk_fwd(A, conv.conv1_fused(data, self.conv1_tc, M["conv1_1/b"], PIXEL_MEANS, True))
+        # data: [B,H,W,3] u8 BGR (PIXEL_MEANS subtracted in conv1_1's loader) or the f32 blob of augment.augment_color (means
+        # already subtracted), as vgg16_convs._trunk chooses
+        self._trunk_fwd(A, conv.conv1_fused(data, self.conv1_tc, M["conv1_1/b"], self._mean(data), True))
         c4, c5 = A["conv4_3"], A["conv5_3"]
         h4, h5 = c4, c5
         if self.rgbd:
@@ -425,7 +431,7 @@ class Trainer:
         g5 = bw.add_to_bf16(conv.conv_bf16(d_s5, self.dg["score_conv5"], z512, 1, False),
                             conv.conv_bf16(d_v5, self.dg["score_conv5_vertex"], z512, 1, False), g5_roi)
         # ---- trunk, top down
-        self._trunk_bwd(grads, A, g5, g4, "", lambda: conv.im2col_c3(data, PIXEL_MEANS))
+        self._trunk_bwd(grads, A, g5, g4, "", lambda: conv.im2col_c3(data, self._mean(data)))
         if self.rgbd:
             # the depth trunk's gradient enters through the depth half of the concat only (the vertex heads and RoiPool read
             # the colour trunk, vgg16_convs.py:151-182)
