@@ -230,8 +230,9 @@ int pcnn_add_to_bf16(const void* a_bf16, const void* b_bf16, const float* b_f32,
  *  pcnn_up8_heads_bwd_ex  gradient of loss_cls (Hardlabel-selected cross entropy through log-softmax and the ReLU of `score`) and of
  *                         loss_vertex (smooth L1 on the labelled pixels' own class) w.r.t. the low-resolution head tensor, formed from
  *                         the loss structure on the fly: d_sc [B,h,w,Cs], d_vt [B,h,w,Cv] bf16 (padding channels zero), dbias [4C]
- *                         (C even, 6..50); the labelled pixels' vertex values come from vertex_pred [B,H,W,3C], or with
- *                         vertex_pred == NULL from the low-resolution head tensor `lowres` [B,h,w,4C] + bias_vertex [3C]
+ *                         (C = 2, or C even in 6..50); the labelled pixels' vertex values come from vertex_pred [B,H,W,3C], or
+ *                         with vertex_pred == NULL from the low-resolution head tensor `lowres` [B,h,w,4C] + bias_vertex [3C];
+ *                         workspace >= 16 C B ceil(h / 16) ceil(w / S) bytes, S = 16 cells at C = 2 and 4 otherwise (4 C floats per CTA)
  *  pcnn_pose_chain_bwd    Averagedistance's bottom_diff through l2_normalize, * poses_weight and tanh -> d fc8 pre-activation (fp16)
  *  pcnn_sgd_momentum      accum = mu * accum + (gscale * grad + wd * w); w -= lr * accum; refreshed 16-bit tensor-core copy (kind 0 bf16, 1 fp16)
  *  pcnn_transpose16 / pcnn_half_to_float   layout / precision glue of the fully connected backward GEMMs

@@ -133,27 +133,33 @@ k_pack_lowres(const __nv_bfloat16* __restrict__ sc, int Cs, const __nv_bfloat16*
 // Outputs d lowres as TWO bf16 tensors in the layouts the 1x1 backward GEMMs read: d_sc [B,h,w,Cs] (first C channels,
 // rest zero) and d_vt [B,h,w,Cv] (first 3C channels), plus per-CTA partial sums of d bias (the up-sampling weights of a
 // pixel sum to the same value for bias: d b[ch] = sum_p d up[p, ch]).
-// Organised so that every byte of prob / score is read (nearly) once and every load is coalesced.  CTA = (image, strip of kSC low-resolution columns = 8 kSC + 8 output columns incl. the halo, band of `rb`
-// low-resolution rows).  Thread = (output column, channel PAIR): the CTA's threads read one contiguous run of
-// kCols * C floats per output row of prob and of score (64-bit loads).  The thread walks DOWN the band's 8 rb + 8 output
-// rows; a pixel row contributes to exactly two low-resolution rows (taps ky and ky + 8), so two running vertical sums per
-// channel live in registers and the finished one is handed to the horizontal pass every 8 rows.  The three vertex channels of a labelled pixel go to a
-// per-column shared-memory accumulator owned by thread (column, k).  Bias gradients: per-thread registers (fixed channel
-// pair) / per-column shared-memory cells, reduced over the columns in a fixed order (no atomics: run-to-run deterministic).
-// Redundant reads: (8 kSC + 8) / (8 kSC) x (8 rb + 8) / (8 rb) = 1.25 x 1.07 at kSC = 4, rb = 16.
+// Organised so that every byte of prob / score is read (nearly) once and every load is coalesced.  CTA = (image, strip of SC
+// low-resolution columns = 8 SC + 8 output columns incl. the halo, band of `rb` low-resolution rows).  Thread = (output column,
+// channel PAIR): the CTA's threads read one contiguous run of (8 SC + 8) * C floats per output row of prob and of score (64-bit
+// loads).  The thread walks DOWN the band's 8 rb + 8 output rows; a pixel row contributes to exactly two low-resolution rows (taps
+// ky and ky + 8), so two running vertical sums per channel live in registers and the finished one is handed to the horizontal pass
+// every 8 rows.  The three vertex channels of a labelled pixel go to a per-column shared-memory accumulator owned by the column's
+// vertex-role thread (t < 8 SC + 8, below).  Bias gradients: per-thread registers (fixed channel pair) / per-column shared-memory
+// cells, reduced over the columns in a fixed order (no atomics: run-to-run deterministic).
+// Strip width SC: 4 cells for C >= 6 (40 columns x C / 2 pairs = 120 .. 1000 threads).  At C = 2 a column is one thread, so a 4-cell
+// strip would be a 40-thread CTA; the two-class kernel takes 16 cells (136 threads), which also cuts the halo.
+// Redundant reads: (8 SC + 8) / (8 SC) x (8 rb + 8) / (8 rb) = 1.25 x 1.07 at SC = 4, 1.06 x 1.07 at SC = 16 (rb = 16).
 // ---------------------------------------------------------------------------------------------
-constexpr int kSC = 4;
-constexpr int kSCols = 8 * kSC + 8;                 // 40 output columns
+constexpr int kStrip = 4;                           // strip width (cells) of the C >= 6 kernels
+constexpr int kStrip2 = 16;                         // strip width (cells) of the C = 2 kernel
 
-template <int CT>
-__global__ void __launch_bounds__(CT ? kSCols * (CT / 2) : 1024, CT ? 2 : 1)
+// C = 2: 6 resident CTAs per SM caps the kernel at 64 registers without spills (-Xptxas -v); 8 would spill
+template <int CT, int SC>
+__global__ void __launch_bounds__(CT ? (8 * SC + 8) * (CT / 2) : 1024, CT == 2 ? 6 : (CT ? 2 : 1))
 k_up8_bwd_strip(const float* __restrict__ prob, const float* __restrict__ score, const int* __restrict__ gt, const float* __restrict__ cls_out,
                 float up_cls, float threshold, const float* __restrict__ vpred, const float* __restrict__ lowres,
                 const float* __restrict__ bias_v, const float* __restrict__ centers,
                 const float* __restrict__ vtx_out, float up_vtx, float w_inside, float sigma2, int h, int w, int rb, int C_rt, int Cs, int Cv,
                 __nv_bfloat16* __restrict__ d_sc, __nv_bfloat16* __restrict__ d_vt, float* __restrict__ dbias_partial /*[ctas][4C]*/)
 {
-    // C even, 6 <= C <= 50: channel pairs; threads (column, 0..2) own the three vertex channels; kSCols * C / 2 threads
+    // C == 2 or C even in 6..50: thread = (output column, channel pair), kSCols * C / 2 threads; threads t < kSCols also own the
+    // vertex channels of output column t (at C = 2 that is every thread)
+    constexpr int kSC = SC, kSCols = 8 * SC + 8;
     const int C = CT ? CT : C_rt;
     const int CP = C / 2, No = 4 * C, VC = 3 * C, NT = kSCols * CP;
     const int H = 8 * h, W = 8 * w;
@@ -242,8 +248,8 @@ k_up8_bwd_strip(const float* __restrict__ prob, const float* __restrict__ score,
         }
         // ---- vertex role: thread t < kSCols owns output column t of the strip (all three vertex channels of the pixel's class).
         // The target direction needs a double sqrt and two double divisions per labelled pixel (the reference forms it in float64,
-        // minibatch.py:582-594); keeping that on 40 densely packed lanes instead of three lanes of every column costs 1/7 of the
-        // double-precision issue slots (the (column, k) mapping made the whole kernel FP64-bound: 3.2 ms at batch 64).
+        // minibatch.py:582-594); keeping that on kSCols densely packed lanes instead of three lanes of every column costs 1/7 of the
+        // double-precision issue slots at C = 22 (the (column, k) mapping made the whole kernel FP64-bound: 3.2 ms at batch 64).
         if (t < kSCols) {
             const int gB = gB0;
             if (gB > 0 && gB < C) {
@@ -470,24 +476,31 @@ extern "C" int pcnn_up8_heads_bwd_ex(const float* prob, const float* score, cons
                      d_vt_bf16 && dbias && workspace,
                  "up8_heads_bwd: NULL tensor pointer");
     PCNN_REQUIRE(Cs >= C && Cv >= 3 * C && h <= 65535 && B <= 65535, "up8_heads_bwd: bad shape");
-    PCNN_REQUIRE(C % 2 == 0 && C >= 6 && C <= 50, "up8_heads_bwd: C must be even and in 6..50 (C = %d)", C);
+    PCNN_REQUIRE(C == 2 || (C % 2 == 0 && C >= 6 && C <= 50), "up8_heads_bwd: C must be even and 2 or in 6..50 (C = %d)", C);
     // coalesced strip kernel (see k_up8_bwd_strip); partial bias sums: one row of 4C floats per CTA
-    const int rb = 16, bands = (h + rb - 1) / rb, strips = (w + kSC - 1) / kSC;
+    const int sc = C == 2 ? kStrip2 : kStrip, cols = 8 * sc + 8;
+    const int rb = 16, bands = (h + rb - 1) / rb, strips = (w + sc - 1) / sc;
     const size_t need = sizeof(float) * (size_t)B * strips * bands * 4 * C;
     PCNN_REQUIRE(workspace_bytes >= need, "up8_heads_bwd: workspace too small (%zu < %zu)", workspace_bytes, need);
     PCNN_REQUIRE(bands <= 65535, "up8_heads_bwd: bad shape");
     cudaStream_t st = (cudaStream_t)stream;
-    const size_t smem = sizeof(float) * ((size_t)kSCols * 11 * C + C);
+    const size_t smem = sizeof(float) * ((size_t)cols * 11 * C + C);
     const dim3 grid(strips, bands, B);
     if (C == 22)
-        k_up8_bwd_strip<22><<<grid, kSCols * 11, smem, st>>>(prob, score, gt, cls_loss_out, upstream_cls, threshold, vertex_pred, lowres, bias_vertex,
-                                                            centers, vertex_loss_out, upstream_vertex, w_inside, sigma * sigma, h, w, rb, C, Cs, Cv,
-                                                            (__nv_bfloat16*)d_sc_bf16, (__nv_bfloat16*)d_vt_bf16, (float*)workspace);
+        k_up8_bwd_strip<22, kStrip><<<grid, cols * 11, smem, st>>>(prob, score, gt, cls_loss_out, upstream_cls, threshold, vertex_pred, lowres,
+                                                                  bias_vertex, centers, vertex_loss_out, upstream_vertex, w_inside, sigma * sigma, h,
+                                                                  w, rb, C, Cs, Cv, (__nv_bfloat16*)d_sc_bf16, (__nv_bfloat16*)d_vt_bf16,
+                                                                  (float*)workspace);
+    else if (C == 2)
+        k_up8_bwd_strip<2, kStrip2><<<grid, cols, smem, st>>>(prob, score, gt, cls_loss_out, upstream_cls, threshold, vertex_pred, lowres,
+                                                             bias_vertex, centers, vertex_loss_out, upstream_vertex, w_inside, sigma * sigma, h, w,
+                                                             rb, C, Cs, Cv, (__nv_bfloat16*)d_sc_bf16, (__nv_bfloat16*)d_vt_bf16, (float*)workspace);
     else {
-        PCNN_SMEM_OPTIN(k_up8_bwd_strip<0>, 100 * 1024, "up8_bwd_strip<0>");
-        k_up8_bwd_strip<0><<<grid, kSCols * (C / 2), smem, st>>>(prob, score, gt, cls_loss_out, upstream_cls, threshold, vertex_pred, lowres,
-                                                                bias_vertex, centers, vertex_loss_out, upstream_vertex, w_inside, sigma * sigma, h, w,
-                                                                rb, C, Cs, Cv, (__nv_bfloat16*)d_sc_bf16, (__nv_bfloat16*)d_vt_bf16, (float*)workspace);
+        PCNN_SMEM_OPTIN((k_up8_bwd_strip<0, kStrip>), 100 * 1024, "up8_bwd_strip<0>");
+        k_up8_bwd_strip<0, kStrip><<<grid, cols * (C / 2), smem, st>>>(prob, score, gt, cls_loss_out, upstream_cls, threshold, vertex_pred, lowres,
+                                                                      bias_vertex, centers, vertex_loss_out, upstream_vertex, w_inside, sigma * sigma,
+                                                                      h, w, rb, C, Cs, Cv, (__nv_bfloat16*)d_sc_bf16, (__nv_bfloat16*)d_vt_bf16,
+                                                                      (float*)workspace);
     }
     k_sum_partials<<<(4 * C + 31) / 32, 256, 0, st>>>((const float*)workspace, B * strips * bands, 4 * C, 1.f, nullptr, 0.f, dbias);
     return check_launch("up8_heads_bwd");

@@ -7,6 +7,10 @@ Reference: the training graph lib/networks/vgg16_convs.py:79-212 driven by lib/f
     loss_pose   = Averagedistance(l2_normalize(poses_tanh * poses_weight), poses_target, poses_weight, points, symmetry)
     optimizer   = tf.train.MomentumOptimizer(lr, 0.9) (train.py:633), l2_regularizer(WEIGHT_REG) on every conv / fc weight AND bias.
 This is the keep_prob = 1.0 graph (the reference trains with dropout 0.5; random masks cannot be compared, SURVEY App. A.7).
+A network built with pose_reg=False (the linemod_{benchvise,camera,iron,lamp,phone}.yml models) trains
+    loss = loss_cls + VERTEX_W * loss_vertex + l2 regularisation (train.py:517, vgg16_convs.py:128-163):
+no Hough voting, RoiPool or fc6-fc8 in the step, and no fc6-fc8 parameters in it.
+Every class count the kernels take trains: C = 2 (the single-object LINEMOD / YCB models) and even C in 6..50.
 input_format='RGBD' adds the depth trunk conv1_1_p .. conv5_3_p (vgg16_convs.py:99-126): score_conv4 / score_conv5 read the channel
 concat [colour | depth] of conv4_3 / conv5_3 (c_i = 1024), the vertex heads, Hough voting and RoiPool read the colour trunk only.
 A network built with adaptation=True adds the domain classifier (vgg16_convs.py:202-212) and
@@ -88,11 +92,13 @@ KINDS = {
 def param_layout(net) -> dict:
     """{master name: (TF parameter name, kind, master rows)} for every parameter the training step updates.  score / vertex_pred
     keep C / 3C rows zero-padded to 64 / 128: the channel counts of their 1x1 GEMMs, which pcnn_pack_lowres and the up8
-    backward read."""
+    backward read.  A pose_reg=False network has no fc6-fc8: the reference creates those variables only under POSE_REG
+    (vgg16_convs.py:175-200), so they are neither trained, decayed nor exported."""
     trunks = ("", "_p") if net.input_format == "RGBD" else ("",)
     weights = [(layer + sfx, "conv1_1" if layer == "conv1_1" else "conv", None) for sfx in trunks for layer in CONV_NAMES]
     weights += [(name, "conv", None) for name in SCORE_HEADS] + [("score", "conv", 64), ("vertex_pred", "conv", 128)]
-    weights += [(name, "fc", None) for name in ("fc6", "fc7", "fc8") + (("fc9",) if net.domain_branch else ())]
+    fc = (("fc6", "fc7", "fc8") if net.pose_reg else ()) + (("fc9",) if net.domain_branch else ())
+    weights += [(name, "fc", None) for name in fc]
     if net.domain_branch:
         weights.append(("domain_score", "domain_score", None))
     layout = {}
@@ -120,11 +126,14 @@ class Trainer:
         self.net, self.lr, self.mu, self.wd = net, float(lr), float(momentum), float(weight_decay)
         self.vertex_w, self.w_inside, self.margin, self.world = float(vertex_w), float(vertex_w_inside), float(margin), int(world)
         self.C = net.num_classes
+        # POSE_REG: Hough voting, RoiPool, fc6-fc8 and loss_pose (vgg16_convs.py:165-200).  Without it the step is the dense heads'
+        # loss_cls + VERTEX_W * loss_vertex (+ l2 regularisation) alone, as lib/fcn/train.py:517 trains it
+        self.pose_reg = bool(net.pose_reg)
         self.pose_loss_scale = 1.0               # last dynamic loss scale of the fp16 pose-head backward (see backward())
         self.adapt = net.domain_branch           # the domain classifier and loss_domain (ADAPT_WEIGHT, lib/fcn/config.py:95)
         self.adapt_weight = float(adapt_weight)
         self.domain_loss_scale = 1.0             # the same for the domain branch's fp16 backward
-        self.fc_names = ("fc6", "fc7", "fc8") + (("fc9",) if self.adapt else ())
+        self.fc_names = (("fc6", "fc7", "fc8") if self.pose_reg else ()) + (("fc9",) if self.adapt else ())
         self.comm = torch.cuda.Stream(device=net.device) if world > 1 else None
         P, dev = net.params, net.device
         self.layout = param_layout(net)
@@ -247,7 +256,9 @@ class Trainer:
         vtx_out = torch.empty((2,), dtype=torch.float32, device=data.device)
         check(lib().pcnn_vertex_loss_fused_lowres_fwd(ptr(lowres), ptr(M["vertex_pred/b"]), ptr(gt_label_2d), ptr(centers), B, H, W, C,
                                                       f32(self.w_inside), f32(1.0), ptr(vtx_out), ptr(ws), ctypes.c_size_t(ws.numel()), stream()))
-        A.update(cls_out=cls_out, vtx_out=vtx_out)
+        A.update(cls_out=cls_out, vtx_out=vtx_out, data=data)
+        if not self.pose_reg:
+            return A
         # Hough voting in train mode (9 jittered ROIs per maximum, quaternion targets from the gt poses)
         Bg = B if batch_global is None else int(batch_global)
         box, pose, target, weight, domain, num_rois, status = hough_voting_gpu_op.hough_voting_gpu_capacity(
@@ -271,7 +282,7 @@ class Trainer:
         pred = (mul / mul.pow(2).sum(1, keepdim=True).clamp(min=1e-12).sqrt()).contiguous()     # tf.nn.l2_normalize(dim=1)
         loss_pose, pose_diff = average_distance_loss_op.average_distance_loss(pred, tw, wt, points, symmetry, self.margin)
         A.update(rois=rl, num_rois=num_rois, a5=a5, a4=a4, pool=pool, fc6=f6, fc7=f7, poses_tanh=tanh, poses_weight=wt, poses_target=tw,
-                 pose_diff=pose_diff, loss_pose_raw=loss_pose, rows=rows, data=data)
+                 pose_diff=pose_diff, loss_pose_raw=loss_pose, rows=rows)
         if self.adapt:
             # the domain classifier on the same fp16 pool_score (gradient_reversal is the identity forward); label_domain = Hough's
             # top_domain, decided by the whole batch's gt count (every rank is given the whole gt array)
@@ -323,22 +334,79 @@ class Trainer:
         return out
 
     def backward(self, A, gt_label_2d, centers):
-        """All parameter gradients of loss = loss_cls + vertex_w * loss_vertex + loss_pose (weight decay is applied in the update).
-        Loss normalisers (selected-pixel count, vertex weight sum, ROI rows) are GLOBAL over the ranks."""
+        """All parameter gradients of loss = loss_cls + vertex_w * loss_vertex + loss_pose (weight decay is applied in the update);
+        without pose_reg, of loss_cls + vertex_w * loss_vertex.  Loss normalisers (selected-pixel count, vertex weight sum, ROI rows)
+        are GLOBAL over the ranks."""
         net, C, M, T = self.net, self.C, self.master, self.tc
         data = A["data"]
         B, H, W, _ = data.shape
         h, w = H // 8, W // 8
         dev = data.device
         grads = {}
-        rows = A["rows"]
-        # ---- global loss normalisers: one all-reduce of [count_cls, sum_w_vertex, rows]
-        norm = torch.stack([A["cls_out"][1], A["vtx_out"][1], torch.tensor(float(rows), device=dev)])
+        # ---- global loss normalisers: one all-reduce of [count_cls, sum_w_vertex(, rows)]
+        rows = [torch.tensor(float(A["rows"]), device=dev)] if self.pose_reg else []
+        norm = torch.stack([A["cls_out"][1], A["vtx_out"][1]] + rows)
         if self.world > 1:
             local = norm.clone()
             dist.all_reduce(norm, op=dist.ReduceOp.SUM)
             A["cls_out"] = torch.stack([A["cls_out"][0] * local[0] / norm[0].clamp(min=1.0), norm[0]])     # this rank's share of the global mean
             A["vtx_out"] = torch.stack([A["vtx_out"][0] * local[1] / norm[1].clamp(min=1e-10), norm[1]])
+        g5_roi = g4_roi = None                    # the RoiPool gradients of the pose head (and the domain branch)
+        if self.pose_reg:
+            g5_roi, g4_roi = self._pose_bwd(grads, A, norm)
+        # ---- FCN heads
+        d_sc = torch.empty((B, h, w, 64), dtype=torch.bfloat16, device=dev)
+        d_vt = torch.empty((B, h, w, 128), dtype=torch.bfloat16, device=dev)
+        dbias = torch.empty((4 * C,), dtype=torch.float32, device=dev)
+        # 4C floats per CTA of >= 4 columns x 16 rows: covers every strip width; the entry point checks its own requirement
+        ws = workspace("up8_bwd", 4 * B * ((w + 3) // 4) * ((h + 15) // 16) * 4 * C, dev)
+        check(lib().pcnn_up8_heads_bwd_ex(ptr(A["prob_normalized"]), ptr(A["score"]), ptr(gt_label_2d), ptr(A["cls_out"]), f32(1.0),
+                                          f32(net.threshold_label), ptr(None), ptr(A["lowres"]), ptr(M["vertex_pred/b"]), ptr(centers),
+                                          ptr(A["vtx_out"]), f32(self.vertex_w), f32(self.w_inside), f32(1.0), B, h, w, C, 64, 128, ptr(d_sc),
+                                          ptr(d_vt), ptr(dbias), ptr(ws), ctypes.c_size_t(ws.numel()), stream()))
+        self._emit(grads, "score/b", dbias[:C].contiguous())
+        self._emit(grads, "vertex_pred/b", dbias[C:].contiguous())
+        self._emit(grads, "score/w", bw.conv_wgrad(A["add_s"], d_sc, 1))
+        self._emit(grads, "vertex_pred/w", bw.conv_wgrad(A["add_v"], d_vt, 1))
+        d_add_s = conv.conv_bf16(d_sc, self.dg["score"], self.zero_bias[64], 1, False)
+        d_add_v = conv.conv_bf16(d_vt, self.dg["vertex_pred"], self.zero_bias[128], 1, False)
+        d_s4, db = bw.relu_bwd(d_add_s, A["s4"], True, want_bias=True)
+        self._emit(grads, "score_conv4/b", db)
+        d_s5 = torch.empty_like(A["s5"])
+        check(lib().pcnn_up2_bwd_bf16(ptr(d_add_s), ptr(A["s5"]), B, h, w, 64, ptr(d_s5), stream()))
+        self._emit(grads, "score_conv5/b", bw.relu_bwd(d_s5, None, False, want_bias=True, want_dz=False)[1])
+        self._emit(grads, "score_conv4_vertex/b", bw.relu_bwd(d_add_v, None, False, want_bias=True, want_dz=False)[1])
+        d_v5 = torch.empty_like(A["v5"])
+        check(lib().pcnn_up2_bwd_bf16(ptr(d_add_v), ptr(None), B, h, w, 128, ptr(d_v5), stream()))
+        self._emit(grads, "score_conv5_vertex/b", bw.relu_bwd(d_v5, None, False, want_bias=True, want_dz=False)[1])
+        c4, c5 = A["conv4_3"], A["conv5_3"]
+        # RGB-D: score_conv4/5 read the 1024-channel concat, so their weight gradient is one wgrad on it
+        self._emit(grads, "score_conv4/w", bw.conv_wgrad(A["concat_conv4"] if self.rgbd else c4, d_s4, 1))
+        self._emit(grads, "score_conv5/w", bw.conv_wgrad(A["concat_conv5"] if self.rgbd else c5, d_s5, 1))
+        self._emit(grads, "score_conv4_vertex/w", bw.conv_wgrad(c4, d_add_v, 1))
+        self._emit(grads, "score_conv5_vertex/w", bw.conv_wgrad(c5, d_v5, 1))
+        z512 = self.zero_bias[512]
+        g4 = bw.add_to_bf16(conv.conv_bf16(d_s4, self.dg["score_conv4"], z512, 1, False),
+                            conv.conv_bf16(d_add_v, self.dg["score_conv4_vertex"], z512, 1, False), g4_roi)
+        g5 = bw.add_to_bf16(conv.conv_bf16(d_s5, self.dg["score_conv5"], z512, 1, False),
+                            conv.conv_bf16(d_v5, self.dg["score_conv5_vertex"], z512, 1, False), g5_roi)
+        # ---- trunk, top down
+        self._trunk_bwd(grads, A, g5, g4, "", lambda: conv.im2col_c3(data, self._mean(data)))
+        if self.rgbd:
+            # the depth trunk's gradient enters through the depth half of the concat only (the vertex heads and RoiPool read
+            # the colour trunk, vgg16_convs.py:151-182)
+            g4_p = conv.conv_bf16(d_s4, self.dg["score_conv4_p"], z512, 1, False)
+            g5_p = conv.conv_bf16(d_s5, self.dg["score_conv5_p"], z512, 1, False)
+            x_p = A["depth_in"]
+            cols_p = (lambda: conv.im2col_depth(x_p, PIXEL_MEANS)) if x_p.dim() == 3 else (lambda: conv.im2col_c3(x_p, None))
+            self._trunk_bwd(grads, A, g5_p, g4_p, "_p", cols_p)
+        return grads
+
+    def _pose_bwd(self, grads, A, norm):
+        """Gradients of loss_pose (and loss_domain) through fc8 .. fc6 (and fc9) and RoiPool: emits the fc parameters' gradients and
+        returns the dense fp32 RoiPool gradients (g5_roi, g4_roi) that enter conv5_3 / conv4_3."""
+        C, M = self.C, self.master
+        dev, rows = A["data"].device, A["rows"]
         # Averagedistance divides by the rows IT sees (capacity rows of this rank); the reference batch sees all of them
         if self.world > 1:
             pose_scale, rows_g = torch.stack([float(rows) / norm[2], norm[2]]).tolist()         # one host read
@@ -395,52 +463,7 @@ class Trainer:
         A["dpool"] = dpool                                                                      # d loss / d pool_score (kept for inspection)
         g5_roi = roi_pooling_op.roi_pool_grad(A["conv5_3"], A["rois"], A["a5"], dpool, 7, 7, 1.0 / 16.0, 0)       # fp32 dense
         g4_roi = roi_pooling_op.roi_pool_grad(A["conv4_3"], A["rois"], A["a4"], dpool, 7, 7, 1.0 / 8.0, 0)
-        # ---- FCN heads
-        d_sc = torch.empty((B, h, w, 64), dtype=torch.bfloat16, device=dev)
-        d_vt = torch.empty((B, h, w, 128), dtype=torch.bfloat16, device=dev)
-        dbias = torch.empty((4 * C,), dtype=torch.float32, device=dev)
-        ws = workspace("up8_bwd", 4 * B * ((w + 3) // 4) * ((h + 15) // 16) * 4 * C, dev)
-        check(lib().pcnn_up8_heads_bwd_ex(ptr(A["prob_normalized"]), ptr(A["score"]), ptr(gt_label_2d), ptr(A["cls_out"]), f32(1.0),
-                                          f32(net.threshold_label), ptr(None), ptr(A["lowres"]), ptr(M["vertex_pred/b"]), ptr(centers),
-                                          ptr(A["vtx_out"]), f32(self.vertex_w), f32(self.w_inside), f32(1.0), B, h, w, C, 64, 128, ptr(d_sc),
-                                          ptr(d_vt), ptr(dbias), ptr(ws), ctypes.c_size_t(ws.numel()), stream()))
-        self._emit(grads, "score/b", dbias[:C].contiguous())
-        self._emit(grads, "vertex_pred/b", dbias[C:].contiguous())
-        self._emit(grads, "score/w", bw.conv_wgrad(A["add_s"], d_sc, 1))
-        self._emit(grads, "vertex_pred/w", bw.conv_wgrad(A["add_v"], d_vt, 1))
-        d_add_s = conv.conv_bf16(d_sc, self.dg["score"], self.zero_bias[64], 1, False)
-        d_add_v = conv.conv_bf16(d_vt, self.dg["vertex_pred"], self.zero_bias[128], 1, False)
-        d_s4, db = bw.relu_bwd(d_add_s, A["s4"], True, want_bias=True)
-        self._emit(grads, "score_conv4/b", db)
-        d_s5 = torch.empty_like(A["s5"])
-        check(lib().pcnn_up2_bwd_bf16(ptr(d_add_s), ptr(A["s5"]), B, h, w, 64, ptr(d_s5), stream()))
-        self._emit(grads, "score_conv5/b", bw.relu_bwd(d_s5, None, False, want_bias=True, want_dz=False)[1])
-        self._emit(grads, "score_conv4_vertex/b", bw.relu_bwd(d_add_v, None, False, want_bias=True, want_dz=False)[1])
-        d_v5 = torch.empty_like(A["v5"])
-        check(lib().pcnn_up2_bwd_bf16(ptr(d_add_v), ptr(None), B, h, w, 128, ptr(d_v5), stream()))
-        self._emit(grads, "score_conv5_vertex/b", bw.relu_bwd(d_v5, None, False, want_bias=True, want_dz=False)[1])
-        c4, c5 = A["conv4_3"], A["conv5_3"]
-        # RGB-D: score_conv4/5 read the 1024-channel concat, so their weight gradient is one wgrad on it
-        self._emit(grads, "score_conv4/w", bw.conv_wgrad(A["concat_conv4"] if self.rgbd else c4, d_s4, 1))
-        self._emit(grads, "score_conv5/w", bw.conv_wgrad(A["concat_conv5"] if self.rgbd else c5, d_s5, 1))
-        self._emit(grads, "score_conv4_vertex/w", bw.conv_wgrad(c4, d_add_v, 1))
-        self._emit(grads, "score_conv5_vertex/w", bw.conv_wgrad(c5, d_v5, 1))
-        z512 = self.zero_bias[512]
-        g4 = bw.add_to_bf16(conv.conv_bf16(d_s4, self.dg["score_conv4"], z512, 1, False),
-                            conv.conv_bf16(d_add_v, self.dg["score_conv4_vertex"], z512, 1, False), g4_roi)
-        g5 = bw.add_to_bf16(conv.conv_bf16(d_s5, self.dg["score_conv5"], z512, 1, False),
-                            conv.conv_bf16(d_v5, self.dg["score_conv5_vertex"], z512, 1, False), g5_roi)
-        # ---- trunk, top down
-        self._trunk_bwd(grads, A, g5, g4, "", lambda: conv.im2col_c3(data, self._mean(data)))
-        if self.rgbd:
-            # the depth trunk's gradient enters through the depth half of the concat only (the vertex heads and RoiPool read
-            # the colour trunk, vgg16_convs.py:151-182)
-            g4_p = conv.conv_bf16(d_s4, self.dg["score_conv4_p"], z512, 1, False)
-            g5_p = conv.conv_bf16(d_s5, self.dg["score_conv5_p"], z512, 1, False)
-            x_p = A["depth_in"]
-            cols_p = (lambda: conv.im2col_depth(x_p, PIXEL_MEANS)) if x_p.dim() == 3 else (lambda: conv.im2col_c3(x_p, None))
-            self._trunk_bwd(grads, A, g5_p, g4_p, "_p", cols_p)
-        return grads
+        return g5_roi, g4_roi
 
     @staticmethod
     def _loss_scale(amax):
@@ -489,10 +512,17 @@ class Trainer:
 
     def step(self, data, gt_label_2d, centers, meta_data, extents, gt_poses, points, symmetry, batch_global=None, batch_offset=0,
              depth=None, data_p=None):
+        """One forward, backward and update.  Returns loss_cls, loss_vertex, loss_pose, their sum `loss`, num_rois and the gradients
+        `grads` (master layouts), plus loss_domain, label_domain and domain_label with the domain branch.  A pose_reg=False network
+        returns no pose entries (loss_pose, num_rois): its loss is loss_cls + loss_vertex, and extents, gt_poses, points, symmetry,
+        meta_data, batch_global and batch_offset are not read."""
         A = self.forward(data, gt_label_2d, centers, meta_data, extents, gt_poses, points, symmetry, batch_global, batch_offset,
                          depth=depth, data_p=data_p)
         grads = self.backward(A, gt_label_2d, centers)
         self.update(grads)
+        if not self.pose_reg:
+            loss_cls, loss_vertex = A["cls_out"][0:1], self.vertex_w * A["vtx_out"][0:1]
+            return dict(loss_cls=loss_cls, loss_vertex=loss_vertex, loss=loss_cls + loss_vertex, grads=grads)
         loss_cls, loss_vertex, loss_pose = A["cls_out"][0:1], self.vertex_w * A["vtx_out"][0:1], A["loss_pose"]
         out = dict(loss_cls=loss_cls, loss_vertex=loss_vertex, loss_pose=loss_pose, loss=loss_cls + loss_vertex + loss_pose, num_rois=A["num_rois"],
                    grads=grads)

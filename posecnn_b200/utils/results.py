@@ -46,6 +46,17 @@ def segmentation_record(labels, rois, poses, poses_refined=None, poses_icp=None)
             "poses_icp": z(poses_icp)}
 
 
+def to_dataset_classes(labels, rois, cls_index):
+    """A two-class model's output in the dataset's class numbering, as test.py:1409-1414 hands it to the ICP refiner: every
+    label > 0 becomes cls_index and every ROI row's class column becomes cls_index (copies; the inputs are not changed).
+    The forward direction is posecnn_b200.single_class.single_class_view."""
+    labels = np.array(labels, dtype=np.int32, copy=True)
+    labels[labels > 0] = int(cls_index)
+    rois = np.array(rois, dtype=np.float32, copy=True).reshape(-1, 7)
+    rois[:, 1] = cls_index
+    return labels, rois
+
+
 def save_mat(filename, record):
     """lov.py:431-438: `scipy.io.savemat(filename, results, do_compression=True)`."""
     import scipy.io
