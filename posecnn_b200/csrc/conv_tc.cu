@@ -4,22 +4,21 @@
 // stride 1, bias add, optional ReLU) as wired by lib/networks/vgg16_convs.py:80-97, 128-163.
 // The reference runs tf.nn.conv2d -> cuDNN in fp32; here the convolution is an implicit GEMM
 //
-//      D[m, n] = sum_{tap, c} A_tap[m, c] * Wt[n, tap*Cin + c],      m = pixel of an 8x16 tile
+//      D[m, n] = sum_{tap, c} A_tap[m, c] * Wt[n, tap*Cin + c],      m = pixel of an 8x16 (or 16x16) tile
 //
 // with BF16 operands and FP32 accumulation (precision is stated with every number, DESIGN.md §4):
 //   * im2col is never materialised: for every filter tap the A operand of a tile is ONE 4-D TMA
-//     box {64 ch, 16 w, 8 h, 1 n} of the NHWC activation tensor at the tap's (dy, dx) offset;
-//     out-of-image coordinates are zero-filled by the TMA unit = SAME padding;
-//   * the box lands in shared memory as 128 rows x 128 B with the 128-byte swizzle, which is
+//     box {64 ch, 16 w, 8 h, 1 n} (256-pixel tile: {64, 16, 16, 1}) of the NHWC activation tensor at the tap's (dy, dx)
+//     offset; out-of-image coordinates are zero-filled by the TMA unit = SAME padding;
+//   * the box lands in shared memory as 128 (256) rows x 128 B with the 128-byte swizzle, which is
 //     exactly the canonical K-major wgmma operand layout, so wgmma reads it in place;
-//   * warp roles: warps 0-7 = two consumer warpgroups (pixel rows 0-63 / 64-127 of the tile): wgmma with the
+//   * warp roles: warps 0-7 = two consumer warpgroups (pixel rows 0-63 / 64-127 of each 128-pixel half): wgmma with the
 //     accumulators in registers, then the epilogue (bias, ReLU, bf16 pack, TMA store) from registers; warpgroup 2
 //     (warps 8-11) gives its registers to the consumers (setmaxnreg: 2 x 128 x 232 + 128 x 40 <= 64 K) and one thread of
 //     it is the TMA producer, which keeps filling the stage ring during the epilogue.  Persistent CTAs, one per SM,
 //     static round-robin tile schedule.
 #include <cuda.h>
 #include <cuda_bf16.h>
-#include <stdlib.h>
 
 #include <type_traits>
 
@@ -46,6 +45,7 @@ struct ConvParams {
     int tile_h, tile_w;       // k_conv_tc: pixel tile (tile_h * tile_w = 128; 8 x 16, or 16 x 8 when that wastes fewer pixels)
     int relu;
     int pool;                 // 1: the epilogue applies the 2x2 / stride-2 max pool and stores ONLY the pooled tensor
+    int kc_outer;             // k_conv_tc<BN, 256>: 1 = K steps chunk-outer (ks = c * taps + tap), 0 = tap-outer
     const float* bias;
 };
 
@@ -97,22 +97,29 @@ __device__ __forceinline__ void pool_staged(uint8_t* ob, int t)
     *reinterpret_cast<uint4*>(ob + p * 128 + ((piece ^ (p & 7)) << 4)) = *reinterpret_cast<const uint4*>(v);
 }
 
-template <int BN>
+// BM = pixels of a tile: 128 (8 x 16 or 16 x 8), or 256 (16 x 16 = two 8 x 16 halves, rows 0-127 = image rows h0 .. h0 + 7)
+template <int BN, int BM>
 struct SmemPlan {
+    static constexpr int kABytesT = BM * kKC * 2;
     static constexpr int kBBytes = BN * kKC * 2;
-    static constexpr int kStage = kABytes + kBBytes;
-    static constexpr int kStages = BN == 256 ? 4 : (BN == 128 ? 6 : 8);
+    static constexpr int kStage = kABytesT + kBBytes;
+    static constexpr int kStages = BN == 256 || BM == 256 ? 4 : (BN == 128 ? 6 : 8);
     static constexpr int kOutBufs = 2;
     static constexpr int kBarOff = kStages * kStage + kOutBufs * kStageBytes;
     static constexpr int kTotal = kBarOff + 256 + 1024;  // barriers + alignment slack
 };
 
-template <int BN>
+// BM = 128: consumer warpgroup g owns the m64 block g; K order tap-outer (ks = tap * kchunks + c).
+// BM = 256: warpgroup g owns the m64 blocks g and g + 2 (its rows of both 8 x 16 halves, one accumulator each); K order
+// chunk-outer (the order of row mode) or tap-outer as p.kc_outer says (conv_bf16_tc_impl).
+template <int BN, int BM>
 __global__ void __launch_bounds__(kThreadsConv, 1)
 k_conv_tc(const __grid_constant__ CUtensorMap map_in, const __grid_constant__ CUtensorMap map_w,
           const __grid_constant__ CUtensorMap map_out, const ConvParams p)  // map_out: box {64,16,8,1}, or {64,8,4,1} of the pooled tensor
 {
-    using Plan = SmemPlan<BN>;
+    static_assert(BM == 128 || (BM == 256 && BN <= 128), "k_conv_tc: BM = 256 needs BN <= 128 (accumulator registers)");
+    using Plan = SmemPlan<BN, BM>;
+    constexpr int kMB = BM / kTileM;                   // accumulators (8 x 16 halves) per consumer thread
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     uint8_t* out_stage = smem + Plan::kStages * Plan::kStage;
@@ -148,13 +155,15 @@ k_conv_tc(const __grid_constant__ CUtensorMap map_in, const __grid_constant__ CU
                 const int pad = p.ksize / 2;
 #pragma unroll 1   // the producer runs on 40 registers
                 for (int ks = 0; ks < ksteps; ks++) {
-                    const int tap = ks / kchunks, c0 = (ks % kchunks) * kKC;
+                    const bool kc_outer = BM == 256 && p.kc_outer;
+                    const int tap = kc_outer ? ks % p.taps : ks / kchunks;
+                    const int c0 = (kc_outer ? ks / p.taps : ks % kchunks) * kKC;
                     const int dy = tap / p.ksize - pad, dx = tap % p.ksize - pad;
                     mbar_wait(&empty[stage], phase ^ 1);
                     uint8_t* sa = smem + stage * Plan::kStage;
                     mbar_arrive_expect_tx(&full[stage], Plan::kStage);
                     tma_load_4d(sa, &map_in, &full[stage], c0, w0 + dx, h0 + dy, img);
-                    tma_load_2d(sa + kABytes, &map_w, &full[stage], tap * p.Cin + c0, n0);
+                    tma_load_2d(sa + Plan::kABytesT, &map_w, &full[stage], tap * p.Cin + c0, n0);
                     if (++stage == Plan::kStages) { stage = 0; phase ^= 1; }
                 }
             }
@@ -163,8 +172,8 @@ k_conv_tc(const __grid_constant__ CUtensorMap map_in, const __grid_constant__ CU
         // ===================== consumer warpgroups: MMA + epilogue =====================
         setmaxnreg_inc<kConsumerRegs>();
         const int wg = warp >> 2, wq = warp & 3;
-        const int row = wg * 64 + wq * 16 + (lane >> 2);   // first of the two tile rows (pixels) this thread holds
-        float acc[BN / 2];
+        const int row = wg * 64 + wq * 16 + (lane >> 2);   // first of the two rows (pixels) of a 128-pixel half this thread holds
+        float acc[kMB][BN / 2];                            // acc[h]: the thread's rows of half h
         int stage = 0, obuf = 0;
         uint32_t phase = 0;
         for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
@@ -178,13 +187,20 @@ k_conv_tc(const __grid_constant__ CUtensorMap map_in, const __grid_constant__ CU
             for (int ks = 0; ks < ksteps; ks++) {
                 mbar_wait(&full[stage], phase);
                 const uint32_t sa = smem_u32(smem + stage * Plan::kStage);
-                const uint64_t da = make_desc(sa + wg * 64 * 128), db = make_desc(sa + kABytes);
-                acc_fence<BN / 2>(acc);
+                const uint64_t db = make_desc(sa + Plan::kABytesT);
+#pragma unroll
+                for (int h = 0; h < kMB; h++) acc_fence<BN / 2>(acc[h]);
                 wgmma_fence();
 #pragma unroll
-                for (int k = 0; k < kKC / 16; k++) wgmma<BN, 0, 0, 0>(acc, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (ks | k) != 0);
+                for (int h = 0; h < kMB; h++) {
+                    const uint64_t da = make_desc(sa + (h * 2 + wg) * 64 * 128);   // m64 block wg of half h
+#pragma unroll
+                    for (int k = 0; k < kKC / 16; k++)
+                        wgmma<BN, 0, 0, 0>(acc[h], da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (ks | k) != 0);
+                }
                 wgmma_commit();
-                acc_fence<BN / 2>(acc);
+#pragma unroll
+                for (int h = 0; h < kMB; h++) acc_fence<BN / 2>(acc[h]);
                 if (prev >= 0) {   // the previous stage's MMAs are complete: its slot may be refilled
                     wgmma_wait<1>();
                     release(&empty[prev], lane);
@@ -193,27 +209,33 @@ k_conv_tc(const __grid_constant__ CUtensorMap map_in, const __grid_constant__ CU
                 if (++stage == Plan::kStages) { stage = 0; phase ^= 1; }
             }
             wgmma_wait<0>();
-            acc_fence<BN / 2>(acc);
+#pragma unroll
+            for (int h = 0; h < kMB; h++) acc_fence<BN / 2>(acc[h]);
             release(&empty[prev], lane);
 #pragma unroll
-            for (int g = 0; g < BN / 64; g++) {
-                // staging buffer obuf must have been read out by the TMA store issued two groups ago
-                if (threadIdx.x == 0) tma_store_wait_read<1>();
-                consumer_sync();
-                uint8_t* ob = out_stage + obuf * kStageBytes;
-                stage_rows(ob, acc + g * 32, p.bias + n0 + g * 64, p.relu, row, lane & 3);
-                if (p.pool) {
+            for (int h = 0; h < kMB; h++) {
+                // a second half wholly below the image has nothing to store (the condition is uniform over the CTA)
+                if (h > 0 && h0 + 8 * h >= p.H) break;
+#pragma unroll
+                for (int g = 0; g < BN / 64; g++) {
+                    // staging buffer obuf must have been read out by the TMA store issued two groups ago
+                    if (threadIdx.x == 0) tma_store_wait_read<1>();
                     consumer_sync();
-                    pool_staged(ob, threadIdx.x);
+                    uint8_t* ob = out_stage + obuf * kStageBytes;
+                    stage_rows(ob, acc[h] + g * 32, p.bias + n0 + g * 64, p.relu, row, lane & 3);
+                    if (p.pool) {
+                        consumer_sync();
+                        pool_staged(ob, threadIdx.x);
+                    }
+                    fence_proxy_async();
+                    consumer_sync();
+                    if (threadIdx.x == 0) {   // half h: image rows h0 + 8 h .. h0 + 8 h + 7 (pooled: 4 rows from h0 / 2 + 4 h)
+                        if (!p.pool) tma_store_4d(&map_out, ob, n0 + g * 64, w0, h0 + 8 * h, img);
+                        else tma_store_4d(&map_out, ob, n0 + g * 64, w0 >> 1, (h0 >> 1) + 4 * h, img);
+                        tma_store_commit();
+                    }
+                    obuf ^= 1;
                 }
-                fence_proxy_async();
-                consumer_sync();
-                if (threadIdx.x == 0) {
-                    if (!p.pool) tma_store_4d(&map_out, ob, n0 + g * 64, w0, h0, img);
-                    else tma_store_4d(&map_out, ob, n0 + g * 64, w0 >> 1, h0 >> 1, img);
-                    tma_store_commit();
-                }
-                obuf ^= 1;
             }
         }
         if (threadIdx.x == 0) tma_store_wait_all();
@@ -857,14 +879,14 @@ static int make_map_nhwc(CUtensorMap* m, const void* ptr, int B, int H, int W, i
     return PCNN_OK;
 }
 
-template <int BN>
+template <int BN, int BM = kTileM>
 static int launch_conv(const CUtensorMap& mi, const CUtensorMap& mw, const CUtensorMap& mo, const ConvParams& p, int num_sms,
                        cudaStream_t st)
 {
-    using Plan = SmemPlan<BN>;
-    PCNN_SMEM_OPTIN(k_conv_tc<BN>, Plan::kTotal, "conv_tc");
+    using Plan = SmemPlan<BN, BM>;
+    PCNN_SMEM_OPTIN((k_conv_tc<BN, BM>), Plan::kTotal, "conv_tc");
     int grid = p.total_tiles < num_sms ? p.total_tiles : num_sms;
-    k_conv_tc<BN><<<grid, kThreadsConv, Plan::kTotal, st>>>(mi, mw, mo, p);
+    k_conv_tc<BN, BM><<<grid, kThreadsConv, Plan::kTotal, st>>>(mi, mw, mo, p);
     return check_launch("conv_tc");
 }
 
@@ -924,14 +946,17 @@ static int conv_bf16_tc_impl(const void* in, const void* weights, const float* b
     cudaStream_t st = (cudaStream_t)stream;
     CUtensorMap mi, mw, mo;
     int rc;
-    // row mode (two output rows x 128 px per work item, A patch reused by all nine taps) for the K-small layers
-    static const bool row_mode_on = getenv("PCNN_CONV_ROWMODE") == nullptr || atoi(getenv("PCNN_CONV_ROWMODE")) != 0;
-    if (row_mode_on && block_n == 0 && ksize == 3 && Cin <= 128 && Cout <= 128 && H % 2 == 0 && W >= kRowPx) {
-        // conv1_2 shape (Cin = Cout = 64): the nine 8-KB weight slices stay resident in shared memory.  The N tile is 64
-        // channels (two N tiles for conv2_x) so that both rows' accumulators fit the 168 registers of a thread.  Measured on
-        // the H100 at batch 32 (tools/bench_conv.py): conv1_2 1.19 ms here vs 1.94 on the tile kernel, but conv2_1 / conv2_2
-        // 0.75 / 1.33 ms vs 0.65 / 1.16 on the tile kernel with BN = 128
-        const bool resb = Cin == 64 && Cout == 64;
+    // The K-small 3x3 layers (Cin <= 128) take one of two kernels chosen from the shape alone; an explicit block_n always runs
+    // the 128-pixel tile kernel at that N tile.
+    //   Cout = 128 (conv2_1, conv2_2 (+ pool2), conv2_2's input gradient): the 256-pixel tile (16 x 16) at BN = 128, below.
+    //     Batch 32, one H100 SXM at a 400 W power limit (tools/bench_trunk.py): conv2_1 0.758 ms, conv2_2 + pool2 1.334 ms,
+    //     against 0.849 / 1.527 ms on the 128-pixel tile at BN = 128 and 0.922 / 1.959 ms in row mode (N = 64).
+    //   Cout = 64 (conv1_2, conv2_1's input gradient): row mode (two output rows x 128 px per work item, one A patch per
+    //     64-channel chunk reused by all nine taps); conv1_2 keeps its nine 8-KB weight slices resident in shared memory
+    //     (conv1_2 + pool1 at batch 32: 1.371 ms, same card and run).
+    const bool tile256 = block_n == 0 && ksize == 3 && Cin <= 128 && Cout == 128;
+    if (block_n == 0 && ksize == 3 && Cin <= 128 && Cout == 64 && H % 2 == 0 && W >= kRowPx) {
+        const bool resb = Cin == 64;
         bn = 64;
         rc = make_map_nhwc(&mi, in, B, H, W, Cin, kKC, kPatchW, kPatchH);
         if (rc) return rc;
@@ -946,21 +971,23 @@ static int conv_bf16_tc_impl(const void* in, const void* weights, const float* b
         p.tiles_w = (W + kRowPx - 1) / kRowPx;
         p.n_tiles_n = Cout / bn;
         p.total_tiles = B * p.tiles_h * p.tiles_w * p.n_tiles_n;
-        p.relu = relu; p.pool = pool; p.bias = bias;
+        p.relu = relu; p.pool = pool; p.bias = bias; p.kc_outer = 0;
         if (resb && p.total_tiles >= p.n_tiles_n) return launch_conv_row2<64, true>(mi, mw, mo, p, sms, st);
         return launch_conv_row2<64, false>(mi, mw, mo, p, sms, st);
     }
-    // pixel tile: 8 x 16, or 16 x 8 when that covers the map with fewer tiles (conv5: 30 x 40 -> 10 tiles instead of 12).
-    // The tile's pixel order is whatever the TMA box says (row = h * tile_w + w for load and store alike), so only
-    // the box shape and the tile origin change; the fused pool epilogue is written for 8 x 16.
+    // pixel tile: 8 x 16, or 16 x 8 when that covers the map with fewer tiles (conv5: 30 x 40 -> 10 tiles instead of 12);
+    // 16 x 16 for the 256-pixel tile.  The tile's pixel order is whatever the TMA box says (row = h * tile_w + w for load
+    // and store alike), so only the box shape and the tile origin change; the epilogue stores (and pools) one 128-pixel
+    // half at a time, and the fused pool is written for 8 x 16 halves.
     int tile_h = kTileH, tile_w = kTileW;
-    if (!pool && ((H + 15) / 16) * ((W + 7) / 8) < ((H + 7) / 8) * ((W + 15) / 16)) { tile_h = 16; tile_w = 8; }
+    if (tile256) tile_h = 2 * kTileH;
+    else if (!pool && ((H + 15) / 16) * ((W + 7) / 8) < ((H + 7) / 8) * ((W + 15) / 16)) { tile_h = 16; tile_w = 8; }
     rc = make_map_nhwc(&mi, in, B, H, W, Cin, kKC, tile_w, tile_h);
     if (rc) return rc;
     rc = make_map_weights(&mw, weights, ksize * ksize * Cin, Cout, bn);
     if (rc) return rc;
     rc = pool ? make_map_nhwc(&mo, out, B, H / 2, W / 2, Cout, 64, kTileW / 2, kTileH / 2)
-              : make_map_nhwc(&mo, out, B, H, W, Cout, 64, tile_w, tile_h);
+              : make_map_nhwc(&mo, out, B, H, W, Cout, 64, tile_w, tile256 ? kTileH : tile_h);
     if (rc) return rc;
     ConvParams p;
     p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.Cout = Cout;
@@ -973,6 +1000,11 @@ static int conv_bf16_tc_impl(const void* in, const void* weights, const float* b
     p.relu = relu;
     p.pool = pool;
     p.bias = bias;
+    // 256-pixel tile: chunk-outer where these shapes ran in row mode before (even H, W >= 128: every conv2_x shape of a
+    // 480 x 640 input), tap-outer where they ran on the 128-pixel tile, so that every call sums in the order it did then and
+    // gives the same bits (for Cin = 64 the two orders coincide)
+    p.kc_outer = tile256 && H % 2 == 0 && W >= kRowPx;
+    if (tile256) return launch_conv<128, 256>(mi, mw, mo, p, sms, st);
     if (bn == 256) return launch_conv<256>(mi, mw, mo, p, sms, st);
     if (bn == 128) return launch_conv<128>(mi, mw, mo, p, sms, st);
     return launch_conv<64>(mi, mw, mo, p, sms, st);
@@ -1070,7 +1102,7 @@ static int conv1_fused_impl(const void* in, int in_kind, const float* mean3_host
     p.tiles_w = (W + kTileW - 1) / kTileW;
     p.n_tiles_n = 1;
     p.total_tiles = B * p.tiles_h * p.tiles_w;
-    p.relu = relu; p.pool = 0; p.bias = bias;
+    p.relu = relu; p.pool = 0; p.bias = bias; p.kc_outer = 0;
     int dev = 0, sms = kNumSMs;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);

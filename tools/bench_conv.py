@@ -36,7 +36,7 @@ for name, H, W, Cin, Cout in layers:
     best = min(res.items(), key=lambda kv: kv[1][0])
     mult = {"conv1_2": 1, "conv2_1": 1, "conv2_2": 1, "conv3_1": 1, "conv3_2": 2, "conv4_1": 1, "conv4_2": 2, "conv5_1": 3}[name]
     tot_t += best[1][0] * mult; tot_f += 2.0 * B * H * W * 9 * Cin * Cout * mult
-    print(name, f"M={B*H*W} K={9*Cin} N={Cout}", " ".join(f"{'row-mode' if bn == 0 else 'bn%d' % bn}: {ms:.3f} ms {tf:.0f} TFLOP/s ({tf/peaks['bf16_tflops']*100:.0f}%)" for bn, (ms, tf) in res.items()))
+    print(name, f"M={B*H*W} K={9*Cin} N={Cout}", " ".join(f"{('row-mode' if Cout == 64 else 'tile256') if bn == 0 else 'bn%d' % bn}: {ms:.3f} ms {tf:.0f} TFLOP/s ({tf/peaks['bf16_tflops']*100:.0f}%)" for bn, (ms, tf) in res.items()))
 print(f"stack (12 tensor-core layers, best tile each): {tot_t:.2f} ms, {tot_f/tot_t/1e9:.0f} TFLOP/s = {tot_f/tot_t/1e9/peaks['bf16_tflops']*100:.0f}% of measured bf16 peak {peaks['bf16_tflops']}")
 x = torch.randn((B, 480, 640, 3), device=dev); w = torch.randn((3, 3, 3, 64), device=dev) * 0.1; b = torch.zeros(64, device=dev)
 for _ in range(2): y = conv.conv3x3_small_cin(x, w, b)

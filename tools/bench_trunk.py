@@ -1,11 +1,13 @@
 """Per-launch timing of the convolution trunk (net._trunk) at batch 32, 640x480 uint8 input, launch by launch as the trunk
-issues it: conv1_1 fused from uint8, the row-mode layers, the pooled conv1_2 / conv2_2 / conv3_3, pool4 and every
-tile-kernel layer with the N tile (BN) the dispatcher picks.  Layers with Cout >= 256 are also timed at the other BN
-(128 / 256).  CUDA events around each launch, L2 flushed (256 MB write) before each one; median of --reps.
+issues it: conv1_1 fused from uint8, the row-mode layer, the pooled conv1_2 / conv2_2 / conv3_3, pool4 and every
+tile-kernel layer with the pixel tile and N tile (BN) the dispatcher picks.  Layers with Cout >= 256 are also timed at the
+other BN (128 / 256), and the Cout = 128 layers (256-pixel tile) on the 128-pixel tile at BN = 128 (explicit block_n).
+CUDA events around each launch, L2 flushed (256 MB write) before each one; median of --reps.
 
 For the wgmma layers the table gives the operand bytes the CTAs request from L2 and their rate (bytes / time):
-  tile kernel: work items x K steps x (A box 16 KB + B box BN x 128 B)
-  row mode:    work items x 64-channel chunks x (A patch 65 KB + 9 weight slices of BN x 128 B unless they stay resident)
+  tile kernel:  work items x K steps x (A box 16 KB + B box BN x 128 B)
+  256-px tile:  work items x K steps x (A box 32 KB + B box BN x 128 B)
+  row mode:     work items x 64-channel chunks x (A patch 65 KB + 9 weight slices of BN x 128 B unless they stay resident)
 If a kernel were bound by L2 -> SM operand delivery, its layers would show the same rate at BN = 128 and BN = 256.
 
     python tools/bench_trunk.py [--batch 32] [--reps 10] [--json FILE]
@@ -24,8 +26,11 @@ PATCH_BYTES = 130 * 4 * 128   # row mode: one {64 ch, 130 px, 4 rows} patch
 
 def plan(B, H, W, Cin, Cout, block_n, pool):
     """Kernel, BN and L2 operand bytes of one pcnn_conv_bf16_tc / pcnn_conv_pool_bf16_tc call (the dispatcher's rule)."""
-    if block_n == 0 and Cin <= 128 and Cout <= 128 and H % 2 == 0 and W >= 128:
-        resb = Cin == 64 and Cout == 64
+    if block_n == 0 and Cin <= 128 and Cout == 128:
+        items = B * math.ceil(H / 16) * math.ceil(W / 16)
+        return "tile256", 128, items * (9 * Cin // KC) * (2 * A_BYTES + 128 * 128)
+    if block_n == 0 and Cin <= 128 and Cout == 64 and H % 2 == 0 and W >= 128:
+        resb = Cin == 64
         items = B * (H // 2) * math.ceil(W / 128) * (Cout // 64)
         per_chunk = PATCH_BYTES + (0 if resb else 9 * 64 * 128)
         return ("row_resb" if resb else "row"), 64, items * (Cin // KC) * per_chunk
@@ -89,8 +94,8 @@ def main():
         ms, y = timed(lambda: call(0))
         label = name + ("+" + cfg[i + 1] if pool else "")
         rows.append(dict(layer=label, kernel=kern, bn=bn, ms=ms, flop=fl, operand_bytes=nbytes, in_trunk=True))
-        if co >= 256:
-            alt = 128 if bn == 256 else 256
+        if co >= 256 or kern == "tile256":
+            alt = 128 if bn == 256 or kern == "tile256" else 256
             _, _, nb_alt = plan(B, h, w, ci, co, alt, pool)
             ms_alt, _ = timed(lambda: call(alt))
             rows.append(dict(layer=label, kernel="tile", bn=alt, ms=ms_alt, flop=fl, operand_bytes=nb_alt, in_trunk=False))
@@ -108,11 +113,11 @@ def main():
         tf = r["flop"] / r["ms"] / 1e9 if r["flop"] else None
         tbs = r["operand_bytes"] / r["ms"] / 1e9 if r["operand_bytes"] else None
         r["tflops"], r["operand_tbs"] = tf, tbs
-        print(f"{r['layer'] if r['in_trunk'] else '  (other BN)':<16}{r['kernel']:<10}{r['bn'] or '-':>5}{r['ms']:>9.3f}"
+        print(f"{r['layer'] if r['in_trunk'] else '  (other tile)':<16}{r['kernel']:<10}{r['bn'] or '-':>5}{r['ms']:>9.3f}"
               f"{(f'{tf:.0f}' if tf else '-'):>9}{(f'{r['operand_bytes'] / 1e9:.2f}' if r['operand_bytes'] else '-'):>11}{(f'{tbs:.2f}' if tbs else '-'):>7}")
     sum_ms = sum(r["ms"] for r in rows if r["in_trunk"])
-    tile_ms = sum(r["ms"] for r in rows if r["in_trunk"] and r["kernel"] == "tile")
-    tile_fl = sum(r["flop"] for r in rows if r["in_trunk"] and r["kernel"] == "tile")
+    tile_ms = sum(r["ms"] for r in rows if r["in_trunk"] and r["kernel"].startswith("tile"))
+    tile_fl = sum(r["flop"] for r in rows if r["in_trunk"] and r["kernel"].startswith("tile"))
     print(f"sum of the trunk's launches: {sum_ms:.3f} ms; tile-kernel layers {tile_ms:.3f} ms at {tile_fl / tile_ms / 1e9:.0f} TFLOP/s; "
           f"net._trunk as one call: {trunk_ms:.3f} ms")
     if args.json:
