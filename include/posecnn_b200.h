@@ -426,6 +426,24 @@ int pcnn_augment_color_fwd(const uint8_t* rgba, int channels, const uint8_t* bac
 int pcnn_depth_blob_train_fwd(const void* depth, int depth_is_u16, const double* params, const uint64_t* keys, const double* noise_field,
                               int B, int H, int W, const double* mean3_host, float* depth_max, float* blob, void* stream);
 
+/* ---------------------------------------------------------------------------------------
+ * Pose refinement with depth (csrc/pose_refine.cu, DESIGN.md 12): the ICP stage of lib/fcn/test.py:1314-1351
+ * (Synthesizer::icp_python / solveICP) on the model point table, batched over every ROI row of a batch.
+ *  label [B,H,W] int32, depth [B,H,W] f32 raw sensor units (z = depth / depth_factor), meta [B, num_meta] (fx = m[0],
+ *  px = m[2], fy = m[4], py = m[5]), rois / poses [cap,7] (image = rois[r,0] - batch_offset, class = rois[r,1]),
+ *  num_rows: device int32 (NULL = cap), points [C,P,3] (P <= 4096).
+ *  -> poses_refined [cap,7] (depth re-centring along the ray), poses_icp [cap,7] (best of 8 depth hypotheses after `iterations`
+ *  point-to-plane Gauss-Newton steps), info [cap,4] = (class pixels, chosen hypothesis, score, inliers at its final pose),
+ *  trace [cap, 8, iterations + 1, 8] (nullable) = per hypothesis and step the pose (7) and its inlier count.
+ *  Rows with class <= 0 or >= C, image outside [0,B), r >= *num_rows or fewer than min_pixels class pixels are zero (info[0] =
+ *  the class pixel count).  workspace: pcnn_pose_refine_workspace_bytes.  Deterministic, no host synchronisation. */
+int pcnn_pose_refine_workspace_bytes(int B, int C, size_t* bytes);
+int pcnn_pose_refine_fwd(const int32_t* label, const float* depth, const float* meta, int num_meta, const float* rois,
+                         const float* poses, const int32_t* num_rows, int cap, const float* points, int C, int P, int B, int H, int W,
+                         int batch_offset, float depth_factor, float znear, float zfar, float max_error, int min_pixels,
+                         int iterations, float* poses_refined, float* poses_icp, float* info, float* trace, void* workspace,
+                         size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

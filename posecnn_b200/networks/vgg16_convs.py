@@ -209,7 +209,8 @@ class vgg16_convs:
         return feats
 
     def forward(self, data, meta_data, extents, poses=None, data_p=None, want_prob=False, sync_rois=True, want_score=False,
-                dense_vertex=True, batch_global=None, batch_offset=0, depth=None):
+                dense_vertex=True, batch_global=None, batch_offset=0, depth=None, refine_depth=None, refine_points=None,
+                depth_factor=10000.0):
         """Inference / forward pass.  data [B,H,W,3] (u8 BGR or pre-processed f32), H, W multiples of 16
         (pad_im, lib/utils/blob.py:48-58).  Returns self.layers with the reference's layer names.
 
@@ -217,8 +218,14 @@ class vgg16_convs:
         reference for visualisation, lib/fcn/test.py:587-599) is not materialised; Houghvotinggpu samples the vertex
         head on demand from the 1/8-resolution head tensor (bit-identical ROIs, pcnn_hough_vote_fwd_ex).
         batch_global / batch_offset: this call is the image shard [batch_offset, batch_offset + B) of a batch of
-        batch_global images (SURVEY.md §8(e)): ROI budget 128 // batch_global per image, global batch indices."""
+        batch_global images (SURVEY.md §8(e)): ROI budget 128 // batch_global per image, global batch indices.
+        refine_depth [B,H,W] f32 raw depth (sensor units, z = depth / depth_factor) + refine_points [C,P,3] (the model point
+        table in this network's class numbering): at test time, refine the detections against the depth (pose_refine.py,
+        TEST.POSE_REFINE) -> detections_poses_refined / detections_poses_icp / detections_icp_info, capacity-shaped like the
+        other detections_* outputs.  Without refine_depth nothing else runs."""
         C = self.num_classes
+        if refine_depth is not None and (self.is_train or not (self.vertex_reg_2d and self.pose_reg)):
+            raise ValueError("refine_depth refines the test-time detections: it needs is_train=False, vertex_reg_2d and pose_reg")
         L = self.layers = {}
         P, T = self.params, self._tc
         B, H, W, _ = data.shape
@@ -303,6 +310,14 @@ class vgg16_convs:
             keep, d_rois, d_poses, d_n = dev_nms.nms_pose_capacity(rois, L["poses_init"], L.get("poses_tanh"), num_rois,
                                                                    self.nms_thresh, per_image=True, num_classes=C)
             L["detections_keep"], L["detections_rois"], L["detections_poses"], L["num_detections"] = keep, d_rois, d_poses, d_n
+            if refine_depth is not None:
+                if refine_points is None:
+                    raise ValueError("refine_depth needs refine_points (the [C,P,3] model point table)")
+                from ..pose_refine import refine_poses
+                ref = refine_poses(label, refine_depth, meta_data, d_rois, d_poses, refine_points, num_rows=d_n,
+                                   factor_depth=depth_factor, batch_offset=batch_offset)
+                L["detections_poses_refined"], L["detections_poses_icp"] = ref["poses_refined"], ref["poses_icp"]
+                L["detections_icp_info"] = ref["icp_info"]
         if sync_rois:
             host = torch.cat([num_rois, status[:2]]).tolist()  # the one host read the op's data-dependent shape requires
             n = max(1, host[0])
@@ -392,6 +407,10 @@ class GraphedForward:
                 from .. import parallel
                 L["records"] = parallel.pack_detections(L)
             return L
+        # refine_depth is a static input like data: replays read the copy that __call__ makes
+        self.s_depth = kw["refine_depth"].clone() if kw.get("refine_depth") is not None else None
+        if self.s_depth is not None:
+            kw["refine_depth"] = self.s_depth
         self.s_data = data.clone()
         self.s_meta = meta_data.clone()
         self.s_ext = extents.clone()
@@ -406,9 +425,13 @@ class GraphedForward:
         with torch.cuda.graph(self.graph):
             self.layers = run()
 
-    def __call__(self, data: torch.Tensor, meta_data: torch.Tensor | None = None):
+    def __call__(self, data: torch.Tensor, meta_data: torch.Tensor | None = None, refine_depth: torch.Tensor | None = None):
         self.s_data.copy_(data, non_blocking=True)
         if meta_data is not None:
             self.s_meta.copy_(meta_data, non_blocking=True)
+        if refine_depth is not None:
+            if self.s_depth is None:
+                raise ValueError("this graph was captured without refine_depth")
+            self.s_depth.copy_(refine_depth, non_blocking=True)
         self.graph.replay()
         return self.layers

@@ -190,6 +190,87 @@ def make_model_points(num_classes: int = 22, num_points: int = 2620, seed: int =
     return pts
 
 
+def quat_to_rot(q) -> np.ndarray:
+    """(w, x, y, z) unit quaternion -> 3x3 rotation matrix."""
+    w, x, y, z = (float(v) for v in q)
+    return np.array([[1 - 2 * (y * y + z * z), 2 * (x * y - w * z), 2 * (x * z + w * y)],
+                     [2 * (x * y + w * z), 1 - 2 * (x * x + z * z), 2 * (y * z - w * x)],
+                     [2 * (x * z - w * y), 2 * (y * z + w * x), 1 - 2 * (x * x + y * y)]])
+
+
+def perturb_pose(q, t, rng, angle_deg: float = 3.0, lateral: float = 0.005, depth: float = 0.025):
+    """A pose off by `angle_deg` about a random axis (applied in the camera frame), `lateral` metres in a random direction of the
+    image plane and `depth` metres along z.  Returns (q [4], t [3]) float64."""
+    axis = rng.normal(size=3)
+    axis /= np.linalg.norm(axis)
+    h = 0.5 * np.deg2rad(angle_deg)
+    dq = np.r_[np.cos(h), np.sin(h) * axis]
+    w0, v0 = dq[0], dq[1:]
+    w1, v1 = float(q[0]), np.asarray(q[1:], np.float64)
+    qn = np.r_[w0 * w1 - v0 @ v1, w0 * v1 + w1 * v0 + np.cross(v0, v1)]
+    phi = rng.uniform(0, 2 * np.pi)
+    tn = np.asarray(t, np.float64) + np.array([lateral * np.cos(phi), lateral * np.sin(phi), depth])
+    return qn, tn
+
+
+def make_refine_scene(batch: int = 1, height: int = 480, width: int = 640, num_classes: int = 22, objects_per_image: int = 3,
+                      seed: int = 5, noise_m: float = 0.0, factor_depth: float = 10000.0, num_points: int = 2620,
+                      background_z: float = 1.8, min_pixels: int = 1500):
+    """Depth scenes for the pose refiner: the ellipsoids of make_model_points (semi-axes extents / 2), posed, rendered
+    analytically by ray-ellipsoid intersection with a z-buffer in front of a fronto-parallel background plane (label 0).
+
+    Returns a dict of numpy arrays:
+      label  [B,H,W] int32   class of the nearest surface
+      depth  [B,H,W] f32     raw sensor units (metres * factor_depth), + N(0, noise_m) metres if noise_m > 0
+      meta   [B,48]  f32     make_meta of the scaled YCB camera
+      points [C,P,3] f32     make_model_points(num_classes, num_points)
+      poses  [N,9]   f64     (b, cls, qw, qx, qy, qz, tx, ty, tz) of every object with >= min_pixels visible pixels
+    """
+    C = num_classes
+    K = intrinsics(height, width)
+    fx, fy, px, py = K[0, 0], K[1, 1], K[0, 2], K[1, 2]
+    ext = extents_for(C)
+    pts = make_model_points(C, num_points)
+    vv, uu = np.mgrid[0:height, 0:width].astype(np.float64)
+    rays = np.stack([(uu - px) / fx, (vv - py) / fy, np.ones_like(uu)], -1)
+    label = np.zeros((batch, height, width), np.int32)
+    depth = np.zeros((batch, height, width), np.float32)
+    meta = np.zeros((batch, 48), np.float32)
+    rows = []
+    for b in range(batch):
+        rng = np.random.default_rng(seed + 1000 * b)
+        meta[b] = make_meta(K)
+        zbuf = np.full((height, width), background_z)
+        lab = np.zeros((height, width), np.int32)
+        k = min(objects_per_image, C - 1)
+        placed = []
+        for cls in rng.choice(np.arange(1, C), size=k, replace=False):
+            q = _rand_quat(rng)
+            z = rng.uniform(0.6, 1.1)
+            cx, cy = rng.uniform(0.25 * width, 0.75 * width), rng.uniform(0.25 * height, 0.75 * height)
+            t = z * np.array([(cx - px) / fx, (cy - py) / fy, 1.0])
+            R = quat_to_rot(q)
+            inv_a = 1.0 / (0.5 * ext[cls].astype(np.float64))
+            A = (rays @ R) * inv_a                     # R^T d, scaled
+            Bv = -(R.T @ t) * inv_a
+            aa = np.sum(A * A, -1)
+            ab = A @ Bv
+            disc = ab * ab - aa * (Bv @ Bv - 1.0)
+            s = np.where(disc > 0, (-ab - np.sqrt(np.maximum(disc, 0))) / aa, np.inf)
+            hit = (disc > 0) & (s > 0) & (s < zbuf)
+            zbuf = np.where(hit, s, zbuf)
+            lab[hit] = cls
+            placed.append((int(cls), q, t))
+        if noise_m > 0:
+            zbuf = zbuf + rng.normal(0.0, noise_m, zbuf.shape)
+        label[b] = lab
+        depth[b] = (zbuf * factor_depth).astype(np.float32)
+        for cls, q, t in placed:
+            if int((lab == cls).sum()) >= min_pixels:
+                rows.append([b, cls, *q, *t])
+    return dict(label=label, depth=depth, meta=meta, points=pts, poses=np.array(rows, np.float64).reshape(-1, 9))
+
+
 def make_pose_batch(num_rois: int, num_classes: int = 22, seed: int = 11, noise: float = 0.15):
     """prediction/target/weight [N,4C] for Averagedistance (vgg16_convs.py:195-200)."""
     rng = np.random.default_rng(seed)

@@ -36,7 +36,7 @@ def icp_parameters(intrinsic_matrix, factor_depth, im_scale=1.0):
 
 def segmentation_record(labels, rois, poses, poses_refined=None, poses_icp=None):
     """The per-image dictionary of test.py:1415-1419 (VERTEX_REG_2D): refined / ICP poses default to zeros [n,7]
-    (test.py:1324-1325) until a refiner fills them."""
+    (test.py:1324-1325); posecnn_b200.pose_refine fills them."""
     rois = np.ascontiguousarray(rois, dtype=np.float32).reshape(-1, 7)
     poses = np.ascontiguousarray(poses, dtype=np.float32).reshape(-1, 7)
     if rois.shape[0] != poses.shape[0]:
