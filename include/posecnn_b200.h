@@ -444,6 +444,33 @@ int pcnn_pose_refine_fwd(const int32_t* label, const float* depth, const float* 
                          int iterations, float* poses_refined, float* poses_icp, float* info, float* trace, void* workspace,
                          size_t workspace_bytes, void* stream);
 
+/* ---------------------------------------------------------------------------------------
+ * Pose estimation from object coordinates and depth (csrc/coord_pose.cu, DESIGN.md 13): the VERTEX_REG_3D test path,
+ * Synthesizer::estimatePose3D (lib/synthesize/synthesize.cpp:1769-1966), batched.
+ *  label [B,H,W] int32; object coordinates scaled into [0,1] by the class extents from the dense vertex [B,H,W,3C], or (vertex
+ *  NULL) evaluated at the sampled pixels from lowres [B,H/8,W/8,4C] + bias_vertex [3C] like the Hough entry; depth [B,H,W] f32 raw
+ *  sensor units (0 = hole, z = depth / depth_factor); meta [B, num_meta] (fx = m[0], px = m[2], fy = m[4], py = m[5]); extents
+ *  [C,3]; keys [B]: the per-image Philox4x32-10 keys.  2 <= C <= 128.
+ *  -> poses [B,C,3,4] ([R | t] per class, zero where no pose was found; class 0 unused), info [B,C,6] = (class pixels,
+ *  hypotheses drawn for the class, inliers of the survivor at its last count, final energy or -1, hypotheses of the image that
+ *  hit the attempt cap, survivor's hypothesis index or -1).  trace_hyp [B,256,13] (nullable) = per hypothesis (class or 0,
+ *  attempts, three pixel indices or -1, inlier count in each of the 8 rounds or -1); trace_round [B,C,8,4] (nullable) = per
+ *  class and round (pixels taken, their index sum mod 2^32, best hypothesis, its inliers).  workspace:
+ *  pcnn_coord_pose3d_workspace_bytes.  Deterministic, no host synchronisation.  There is no batch_offset: an image's result
+ *  depends only on its own inputs and keys[b], so a shard of a batch passes the slices of the inputs and of the keys (the offset
+ *  only numbers the records, pcnn_coord_pose3d_records).
+ * pcnn_coord_pose3d_records: the detection records of lib/fcn/test.py:1383-1399 from poses [B,C,3,4]: for every image and class
+ *  j >= 1 with t_z > 0, in (image, class) order, rois [B*(C-1),6] = (image + batch_offset, j, _get_bb2D(extent, pose, K) *
+ *  im_scale) with K = the meta intrinsics / im_scale (meta holds K * im_scale), poses [B*(C-1),7] = (mat2quat(R), t); rows after
+ *  the last are zero, *num_rows (device int32) = the row count. */
+int pcnn_coord_pose3d_workspace_bytes(int B, int H, int W, int C, size_t* bytes);
+int pcnn_coord_pose3d_fwd(const int32_t* label, const float* vertex, const float* lowres, const float* bias_vertex, const float* depth,
+                          const float* meta, int num_meta, const float* extents, const uint64_t* keys, int B, int H, int W, int C,
+                          float depth_factor, float* poses, float* info, int32_t* trace_hyp, int32_t* trace_round, void* workspace,
+                          size_t workspace_bytes, void* stream);
+int pcnn_coord_pose3d_records(const float* poses, const float* extents, const float* meta, int num_meta, int B, int C, int batch_offset,
+                              float im_scale, float* rois, float* out_poses, int32_t* num_rows, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

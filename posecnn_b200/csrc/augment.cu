@@ -51,16 +51,9 @@ __device__ __forceinline__ Params load_params(const double* __restrict__ p, int 
 // on two 53-bit uniforms: u1 in (0, 1], u2 in [0, 1).
 __device__ __forceinline__ double philox_normal(uint64_t key, uint64_t pix)
 {
-    uint32_t c0 = (uint32_t)pix, c1 = (uint32_t)(pix >> 32), c2 = 0u, c3 = 0u;
-    uint32_t k0 = (uint32_t)key, k1 = (uint32_t)(key >> 32);
-#pragma unroll
-    for (int i = 0; i < 10; i++) {
-        if (i) { k0 += 0x9E3779B9u; k1 += 0xBB67AE85u; }
-        const uint32_t hi0 = __umulhi(0xD2511F53u, c0), lo0 = 0xD2511F53u * c0;
-        const uint32_t hi1 = __umulhi(0xCD9E8D57u, c2), lo1 = 0xCD9E8D57u * c2;
-        const uint32_t n0 = hi1 ^ c1 ^ k0, n2 = hi0 ^ c3 ^ k1;
-        c0 = n0; c1 = lo1; c2 = n2; c3 = lo0;
-    }
+    uint32_t w[4];
+    philox4x32_10(key, pix, w);
+    const uint32_t c0 = w[0], c1 = w[1], c2 = w[2], c3 = w[3];
     const double u1 = (double)(((((uint64_t)c0 << 32) | c1) >> 11) + 1) * 0x1p-53;
     const double u2 = (double)((((uint64_t)c2 << 32) | c3) >> 11) * 0x1p-53;
     return __dmul_rn(sqrt(__dmul_rn(-2.0, log(u1))), cos(__dmul_rn(6.283185307179586, u2)));

@@ -15,6 +15,7 @@
 
 #include "common.cuh"
 #include "heads_common.cuh"
+#include "pose_common.cuh"
 
 namespace pcnn {
 
@@ -243,53 +244,8 @@ k_vertex_targets_instances(const int* __restrict__ label, const int* __restrict_
 // pose blob and meta_data packing of the data layer (minibatch.py:440-451, 474-492):
 //   pose_blob rows [image, cls, 0, 0, 0, 0, mat2quat(R) (w, x, y, z), T] for every listed instance, images in order;
 //   meta_data[48]: K * im_scale with K[2][2] = 1 in [0:9], its (pseudo-)inverse in [9:18], zeros elsewhere, FLIP_X signs.
-// mat2quat is transforms3d's (Bar-Itzhack): eigenvector of the largest eigenvalue of the symmetric 4x4 K matrix, here
-// by cyclic Jacobi rotations in double, w made non-negative.
+// mat2quat_d: pose_common.cuh.
 // ---------------------------------------------------------------------------------------------
-__device__ void mat2quat_d(const float* __restrict__ rt /*3x4 row-major*/, float q[4])
-{
-    // transforms3d: `Qxx, Qyx, Qzx, Qxy, Qyy, Qzy, Qxz, Qyz, Qzz = M.flat` (row-major flat order: Qyx = M[0][1], Qxy = M[1][0], ...)
-    const double Qxx = rt[0], Qyx = rt[1], Qzx = rt[2], Qxy = rt[4], Qyy = rt[5], Qzy = rt[6], Qxz = rt[8], Qyz = rt[9], Qzz = rt[10];
-    double A[4][4] = {{Qxx - Qyy - Qzz, Qyx + Qxy, Qzx + Qxz, Qyz - Qzy},
-                      {Qyx + Qxy, Qyy - Qxx - Qzz, Qzy + Qyz, Qzx - Qxz},
-                      {Qzx + Qxz, Qzy + Qyz, Qzz - Qxx - Qyy, Qxy - Qyx},
-                      {Qyz - Qzy, Qzx - Qxz, Qxy - Qyx, Qxx + Qyy + Qzz}};
-    double V[4][4] = {{1, 0, 0, 0}, {0, 1, 0, 0}, {0, 0, 1, 0}, {0, 0, 0, 1}};
-    for (int i = 0; i < 4; i++)
-        for (int j = 0; j < 4; j++) A[i][j] /= 3.0;
-    for (int sweep = 0; sweep < 30; sweep++) {
-        double off = 0;
-        for (int i = 0; i < 4; i++)
-            for (int j = i + 1; j < 4; j++) off += A[i][j] * A[i][j];
-        if (off < 1e-30) break;
-        for (int pI = 0; pI < 3; pI++)
-            for (int qI = pI + 1; qI < 4; qI++) {
-                if (fabs(A[pI][qI]) < 1e-300) continue;
-                const double theta = (A[qI][qI] - A[pI][pI]) / (2.0 * A[pI][qI]);
-                const double t = (theta >= 0 ? 1.0 : -1.0) / (fabs(theta) + sqrt(theta * theta + 1.0));
-                const double c = 1.0 / sqrt(t * t + 1.0), sn = t * c;
-                for (int k = 0; k < 4; k++) {
-                    const double akp = A[k][pI], akq = A[k][qI];
-                    A[k][pI] = c * akp - sn * akq; A[k][qI] = sn * akp + c * akq;
-                }
-                for (int k = 0; k < 4; k++) {
-                    const double apk = A[pI][k], aqk = A[qI][k];
-                    A[pI][k] = c * apk - sn * aqk; A[qI][k] = sn * apk + c * aqk;
-                }
-                for (int k = 0; k < 4; k++) {
-                    const double vkp = V[k][pI], vkq = V[k][qI];
-                    V[k][pI] = c * vkp - sn * vkq; V[k][qI] = sn * vkp + c * vkq;
-                }
-            }
-    }
-    int best = 0;
-    for (int k = 1; k < 4; k++)
-        if (A[k][k] > A[best][best]) best = k;
-    double w = V[3][best], x = V[0][best], y = V[1][best], z = V[2][best];   // vecs[[3, 0, 1, 2], argmax]
-    if (w < 0) { w = -w; x = -x; y = -y; z = -z; }
-    q[0] = (float)w; q[1] = (float)x; q[2] = (float)y; q[3] = (float)z;
-}
-
 __global__ void __launch_bounds__(256)
 k_pack_pose_meta(const float* __restrict__ poses /*[B,I,12]*/, const int* __restrict__ cls /*[B,I], < 0 = unused*/,
                  const float* __restrict__ intr /*[B,9]*/, int B, int I, float im_scale, int flip_x, float* __restrict__ pose_blob /*[B*I,13]*/,

@@ -48,6 +48,8 @@ class vgg16_convs:
         self.threshold_label = threshold_label
         self.vertex_reg = vertex_reg_2d or vertex_reg_3d
         self.vertex_reg_2d = vertex_reg_2d
+        self.vertex_reg_3d = vertex_reg_3d
+        self.scales = tuple(float(v) for v in scales)
         self.pose_reg = pose_reg
         # domain classifier on pool_score (vgg16_convs.py:202-212); built only where the reference builds it
         self.adaptation = bool(adaptation)
@@ -210,7 +212,7 @@ class vgg16_convs:
 
     def forward(self, data, meta_data, extents, poses=None, data_p=None, want_prob=False, sync_rois=True, want_score=False,
                 dense_vertex=True, batch_global=None, batch_offset=0, depth=None, refine_depth=None, refine_points=None,
-                depth_factor=10000.0):
+                depth_factor=10000.0, estimate_depth=None, estimate_keys=None):
         """Inference / forward pass.  data [B,H,W,3] (u8 BGR or pre-processed f32), H, W multiples of 16
         (pad_im, lib/utils/blob.py:48-58).  Returns self.layers with the reference's layer names.
 
@@ -222,8 +224,16 @@ class vgg16_convs:
         refine_depth [B,H,W] f32 raw depth (sensor units, z = depth / depth_factor) + refine_points [C,P,3] (the model point
         table in this network's class numbering): at test time, refine the detections against the depth (pose_refine.py,
         TEST.POSE_REFINE) -> detections_poses_refined / detections_poses_icp / detections_icp_info, capacity-shaped like the
-        other detections_* outputs.  Without refine_depth nothing else runs."""
+        other detections_* outputs.  Without refine_depth nothing else runs.
+        estimate_depth [B,H,W] f32 raw depth at the network's resolution (+ estimate_keys [B] int64 Philox keys, default the global
+        image indices): on a vertex_reg_3d network at test time, estimate the poses from the object coordinates of the
+        1/8-resolution head and the depth (coord_pose.py, lib/fcn/test.py:1381-1399) -> estimate_poses [B,C,3,4], estimate_info
+        [B,C,6] and the records detections_rois [B*(C-1),6] / detections_poses [B*(C-1),7] / num_detections [1] (im_scale =
+        scales[0]).  Without estimate_depth nothing else runs."""
         C = self.num_classes
+        if estimate_depth is not None and (self.is_train or self.vertex_reg_2d or not self.vertex_reg_3d):
+            raise ValueError("estimate_depth estimates poses from object coordinates: it needs is_train=False and vertex_reg_3d "
+                             "without vertex_reg_2d")
         if refine_depth is not None and (self.is_train or not (self.vertex_reg_2d and self.pose_reg)):
             raise ValueError("refine_depth refines the test-time detections: it needs is_train=False, vertex_reg_2d and pose_reg")
         L = self.layers = {}
@@ -271,6 +281,15 @@ class vgg16_convs:
         if want_score:
             L["score"] = score
         if not self.vertex_reg_2d:
+            if estimate_depth is not None:
+                from ..coord_pose import assemble_records, estimate_poses_3d
+                keys = estimate_keys if estimate_keys is not None else \
+                    torch.arange(batch_offset, batch_offset + B, dtype=torch.int64, device=data.device)
+                est = estimate_poses_3d(label, estimate_depth, meta_data, extents, keys, lowres=lowres, bias_vertex=P["vertex_pred/biases"],
+                                        factor_depth=depth_factor)
+                L["estimate_poses"], L["estimate_info"] = est["poses"], est["info"]
+                L["detections_rois"], L["detections_poses"], L["num_detections"] = assemble_records(
+                    est["poses"], extents, meta_data, self.scales[0], batch_offset)
             return L
         Bg = B if batch_global is None else int(batch_global)
         box, pose, target, weight, domain, num_rois, status = hough_voting_gpu_op.hough_voting_gpu_capacity(
@@ -407,10 +426,13 @@ class GraphedForward:
                 from .. import parallel
                 L["records"] = parallel.pack_detections(L)
             return L
-        # refine_depth is a static input like data: replays read the copy that __call__ makes
+        # refine_depth / estimate_depth are static inputs like data: replays read the copies that __call__ makes
         self.s_depth = kw["refine_depth"].clone() if kw.get("refine_depth") is not None else None
         if self.s_depth is not None:
             kw["refine_depth"] = self.s_depth
+        self.s_est_depth = kw["estimate_depth"].clone() if kw.get("estimate_depth") is not None else None
+        if self.s_est_depth is not None:
+            kw["estimate_depth"] = self.s_est_depth
         self.s_data = data.clone()
         self.s_meta = meta_data.clone()
         self.s_ext = extents.clone()
@@ -425,7 +447,8 @@ class GraphedForward:
         with torch.cuda.graph(self.graph):
             self.layers = run()
 
-    def __call__(self, data: torch.Tensor, meta_data: torch.Tensor | None = None, refine_depth: torch.Tensor | None = None):
+    def __call__(self, data: torch.Tensor, meta_data: torch.Tensor | None = None, refine_depth: torch.Tensor | None = None,
+                 estimate_depth: torch.Tensor | None = None):
         self.s_data.copy_(data, non_blocking=True)
         if meta_data is not None:
             self.s_meta.copy_(meta_data, non_blocking=True)
@@ -433,5 +456,9 @@ class GraphedForward:
             if self.s_depth is None:
                 raise ValueError("this graph was captured without refine_depth")
             self.s_depth.copy_(refine_depth, non_blocking=True)
+        if estimate_depth is not None:
+            if self.s_est_depth is None:
+                raise ValueError("this graph was captured without estimate_depth")
+            self.s_est_depth.copy_(estimate_depth, non_blocking=True)
         self.graph.replay()
         return self.layers

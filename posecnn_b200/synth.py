@@ -271,6 +271,47 @@ def make_refine_scene(batch: int = 1, height: int = 480, width: int = 640, num_c
     return dict(label=label, depth=depth, meta=meta, points=pts, poses=np.array(rows, np.float64).reshape(-1, 9))
 
 
+def make_coordinate_scene(batch: int = 1, height: int = 480, width: int = 640, num_classes: int = 22, objects_per_image: int = 3,
+                          seed: int = 5, coord_noise_m: float = 0.0, outlier_fraction: float = 0.0, factor_depth: float = 10000.0):
+    """Object-coordinate scenes for the VERTEX_REG_3D pose estimator, on the analytic ellipsoid scenes of make_refine_scene: the
+    visible surface point X of a pixel is its ray scaled to the rendered depth, its object coordinate is R^T (X - t).  Coordinates
+    get N(0, coord_noise_m) noise per component, and a fraction `outlier_fraction` of each object's pixels gets a coordinate drawn
+    uniformly in the class's extent box.  The coordinates are then scaled into [0,1] by the extents
+    (lib/gt_synthesize_layer/minibatch.py:605-616) into the class's three channels of a [B,H,W,3C] tensor, zero elsewhere.
+
+    Returns make_refine_scene's dict (label, depth, meta, points, poses [N,9]: every placed object) plus
+      coords  [B,H,W,3] f32  unscaled object coordinate of the labelled object (zero on the background)
+      vertex  [B,H,W,3C] f32 scaled coordinates
+      extents [C,3] f32"""
+    C = num_classes
+    sc = make_refine_scene(batch=batch, height=height, width=width, num_classes=C, objects_per_image=objects_per_image, seed=seed,
+                           factor_depth=factor_depth, min_pixels=1)
+    K = intrinsics(height, width)
+    fx, fy, px, py = K[0, 0], K[1, 1], K[0, 2], K[1, 2]
+    ext = extents_for(C)
+    vv, uu = np.mgrid[0:height, 0:width].astype(np.float64)
+    coords = np.zeros((batch, height, width, 3), np.float32)
+    vertex = np.zeros((batch, height, width, 3 * C), np.float32)
+    for row in sc["poses"]:
+        b, cls = int(row[0]), int(row[1])
+        R, t = quat_to_rot(row[2:6]), row[6:9]
+        mask = sc["label"][b] == cls
+        z = sc["depth"][b][mask].astype(np.float64) / factor_depth
+        X = np.stack([(uu[mask] - px) / fx * z, (vv[mask] - py) / fy * z, z], -1)
+        obj = (X - t) @ R
+        rng = np.random.default_rng(seed + 7919 * b + cls)
+        if coord_noise_m > 0:
+            obj = obj + rng.normal(0.0, coord_noise_m, obj.shape)
+        if outlier_fraction > 0:
+            bad = rng.random(obj.shape[0]) < outlier_fraction
+            obj[bad] = (rng.random((int(bad.sum()), 3)) - 0.5) * ext[cls]
+        coords[b][mask] = obj
+        vmin, vmax = -ext[cls].astype(np.float64) / 2, ext[cls].astype(np.float64) / 2
+        vertex[b][mask, 3 * cls:3 * cls + 3] = (obj - vmin) / (vmax - vmin)
+    sc.update(coords=coords, vertex=vertex, extents=ext)
+    return sc
+
+
 def make_pose_batch(num_rois: int, num_classes: int = 22, seed: int = 11, noise: float = 0.15):
     """prediction/target/weight [N,4C] for Averagedistance (vgg16_convs.py:195-200)."""
     rng = np.random.default_rng(seed)
