@@ -245,6 +245,14 @@ int pcnn_up8_heads_bwd_ex(const float* prob, const float* score, const int32_t* 
                           const float* vertex_loss_out, float upstream_vertex, float w_inside, float sigma, int B, int h, int w, int C,
                           int Cs, int Cv, void* d_sc_bf16, void* d_vt_bf16, float* dbias, void* workspace, size_t workspace_bytes,
                           void* stream);
+/* pcnn_up8_heads_bwd_coord  the same adjoint for the VERTEX_REG_3D networks: the vertex target of a weighted pixel (label c in 1..C-1,
+ *      centers[b, c, 2] > 0) is its object coordinate vertmap [B,8h,8w,3] f32 scaled by extents [C,3] f32 (as
+ *      pcnn_vertex_targets_3d_fwd); every other argument, check, output and the workspace are those of pcnn_up8_heads_bwd_ex. */
+int pcnn_up8_heads_bwd_coord(const float* prob, const float* score, const int32_t* gt, const float* cls_loss_out, float upstream_cls,
+                             float threshold, const float* vertex_pred, const float* lowres, const float* bias_vertex, const float* vertmap,
+                             const float* centers, const float* extents, const float* vertex_loss_out, float upstream_vertex, float w_inside,
+                             float sigma, int B, int h, int w, int C, int Cs, int Cv, void* d_sc_bf16, void* d_vt_bf16, float* dbias,
+                             void* workspace, size_t workspace_bytes, void* stream);
 int pcnn_pose_chain_bwd(const float* bottom_diff, const float* poses_tanh, const float* poses_weight, int N, int D, float upstream,
                         void* dpre_f16, int ld, void* stream);
 int pcnn_sgd_momentum(float* w, float* accum, const float* grad, size_t n, float lr, float mu, float wd, float gscale, void* copy16,
@@ -389,6 +397,22 @@ int pcnn_vertex_loss_fused_fwd(const float* pred, const int32_t* label, const fl
 int pcnn_vertex_loss_fused_lowres_fwd(const float* lowres, const float* bias_vertex, const int32_t* label, const float* centers, int B,
                                       int H, int W, int C, float w_inside, float sigma, float* loss_out, void* workspace,
                                       size_t workspace_bytes, void* stream);
+/* VERTEX_REG_3D targets (the 3-D branch of _generate_vertex_targets, minibatch.py:595-600, and _scale_vertmap, :605-616):
+ *  pcnn_vertex_targets_3d_fwd   label [B,H,W] int32, vertmap [B,H,W,3] f32 (the object coordinate of each pixel, metres in the model
+ *      frame), centers [B,C,3] (only z > 0 is read: the class is listed in the frame), extents [C,3] f32 -> vertex_targets /
+ *      vertex_weights [B,H,W,3C] f32: for a pixel labelled c in 1..C-1 with a listed class, channel 3c+k = a_k * v_k + b_k with
+ *      vmin = -e_k / 2, vmax = e_k / 2, a_k = 1 / (vmax - vmin), b_k = -vmin / (vmax - vmin) (a_k = b_k = 0 where vmax - vmin <= 0),
+ *      all in float32 with the product rounded before the sum; weight w_inside on those channels; zero elsewhere.
+ *  pcnn_vertex_loss_coord_fwd / pcnn_vertex_loss_coord_lowres_fwd   pcnn_vertex_loss_fused_fwd / _lowres_fwd on that target, without
+ *      materialising it (same outputs, workspace and gradient convention). */
+int pcnn_vertex_targets_3d_fwd(const int32_t* label, const float* vertmap, const float* centers, const float* extents, int B, int H, int W,
+                               int C, float w_inside, float* targets, float* weights, void* stream);
+int pcnn_vertex_loss_coord_fwd(const float* pred, const int32_t* label, const float* vertmap, const float* centers, const float* extents,
+                               int B, int H, int W, int C, float w_inside, float sigma, float* loss_out, float upstream, float* grad_pred,
+                               void* workspace, size_t workspace_bytes, void* stream);
+int pcnn_vertex_loss_coord_lowres_fwd(const float* lowres, const float* bias_vertex, const int32_t* label, const float* vertmap,
+                                      const float* centers, const float* extents, int B, int H, int W, int C, float w_inside, float sigma,
+                                      float* loss_out, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * Training image blobs (csrc/augment.cu): the image side of the synthetic-data loader, lib/gt_synthesize_layer/minibatch.py:147-200

@@ -44,4 +44,22 @@ __device__ __forceinline__ float up8_value(const float* __restrict__ lr, int n, 
     return up8_hblend(wa, va, wb, vb, bias);
 }
 
+// _scale_vertmap (minibatch.py:605-616), the VERTEX_REG_3D target of one class, shared by the fused loss (train_targets.cu) and the
+// up-sampling adjoint (train_bwd.cu).  The reference works in float32 (extents and vertmap are float32 arrays), so vmin = -e / 2,
+// vmax = e / 2, a = 1 / (vmax - vmin), b = -1 * vmin / (vmax - vmin) are float32 operations (a = b = 0 where vmax - vmin <= 0), and
+// the target of an object coordinate v is a * v rounded, then + b rounded: no contraction into an FMA.  ab = (a_0, b_0, a_1, ..).
+__device__ __forceinline__ void coord_scale(const float* ext /*[3]*/, float ab[6])
+{
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+        const float e = ext[k];
+        const float vmin = -e / 2.f, vmax = e / 2.f, span = vmax - vmin;
+        const bool ok = span > 0.f;
+        ab[2 * k] = ok ? 1.f / span : 0.f;
+        ab[2 * k + 1] = ok ? (-1.f * vmin) / span : 0.f;
+    }
+}
+
+__device__ __forceinline__ float coord_target(float a, float b, float v) { return __fadd_rn(__fmul_rn(a, v), b); }
+
 }  // namespace pcnn

@@ -148,14 +148,19 @@ k_pack_lowres(const __nv_bfloat16* __restrict__ sc, int Cs, const __nv_bfloat16*
 constexpr int kStrip = 4;                           // strip width (cells) of the C >= 6 kernels
 constexpr int kStrip2 = 16;                         // strip width (cells) of the C = 2 kernel
 
+// Target mode kCoord (VERTEX_REG_3D): the vertex target is the pixel's object coordinate vertmap [B,H,W,3] scaled by its class's
+// extents (coord_scale / coord_target, heads_common.cuh) instead of the 2-D centre direction + log z.  The per-class (a_k, b_k) sit in
+// shared memory after the per-class listed flags (where the 2-D mode keeps log z: 6 C more floats), and the vertex-role thread loads
+// a pixel's three vertmap floats one row ahead, together with the label it already prefetches, and only for weighted pixels.
 // C = 2: 6 resident CTAs per SM caps the kernel at 64 registers without spills (-Xptxas -v); 8 would spill
-template <int CT, int SC>
+template <int CT, int SC, bool kCoord = false>
 __global__ void __launch_bounds__(CT ? (8 * SC + 8) * (CT / 2) : 1024, CT == 2 ? 6 : (CT ? 2 : 1))
 k_up8_bwd_strip(const float* __restrict__ prob, const float* __restrict__ score, const int* __restrict__ gt, const float* __restrict__ cls_out,
                 float up_cls, float threshold, const float* __restrict__ vpred, const float* __restrict__ lowres,
                 const float* __restrict__ bias_v, const float* __restrict__ centers,
                 const float* __restrict__ vtx_out, float up_vtx, float w_inside, float sigma2, int h, int w, int rb, int C_rt, int Cs, int Cv,
-                __nv_bfloat16* __restrict__ d_sc, __nv_bfloat16* __restrict__ d_vt, float* __restrict__ dbias_partial /*[ctas][4C]*/)
+                __nv_bfloat16* __restrict__ d_sc, __nv_bfloat16* __restrict__ d_vt, float* __restrict__ dbias_partial /*[ctas][4C]*/,
+                const float* __restrict__ vertmap, const float* __restrict__ extents)
 {
     // C == 2 or C even in 6..50: thread = (output column, channel pair), kSCols * C / 2 threads; threads t < kSCols also own the
     // vertex channels of output column t (at C = 2 that is every thread)
@@ -174,10 +179,17 @@ k_up8_bwd_strip(const float* __restrict__ prob, const float* __restrict__ score,
     float* bs = vacc + 2 * kSCols * VC;              // [kSCols][C]       bias-gradient sums (score), per column
     float* bv = bs + kSCols * C;                     // [kSCols][VC]      bias-gradient sums (vertex), per column
     float* logz = bv + kSCols * VC;                  // [C]               log of the listed centre depth of each class of this image
+                                                     //                   (kCoord: 1 if the class is listed, else 0)
+    float* ab = logz + C;                            // [C][6]            kCoord: (a_0, b_0, a_1, b_1, a_2, b_2) of each class
     const int t = threadIdx.x, col = t / CP, j = t - col * CP;
     for (int i = t; i < C; i += NT) {
         const float z = centers[((size_t)n * C + i) * 3 + 2];
-        logz[i] = z > 0.f ? (float)log((double)z) : 0.f;
+        if constexpr (kCoord) {
+            logz[i] = z > 0.f ? 1.f : 0.f;
+            coord_scale(extents + 3 * i, ab + 6 * i);
+        } else {
+            logz[i] = z > 0.f ? (float)log((double)z) : 0.f;
+        }
     }
     for (int i = t; i < 2 * kSCols * VC; i += NT) vacc[i] = 0.f;
     for (int i = t; i < kSCols * VC; i += NT) bv[i] = 0.f;
@@ -222,6 +234,14 @@ k_up8_bwd_strip(const float* __restrict__ prob, const float* __restrict__ score,
         if (y_first <= y_last) gB0 = __ldg(gtB_c + r0);
         if (y_first + 1 <= y_last) gB1 = __ldg(gtB_c + r0 + W);
     }
+    // kCoord: object coordinate of the vertex-role pixel of the current row, loaded one row ahead for weighted pixels only
+    float vB[3] = {0.f, 0.f, 0.f};
+    if constexpr (kCoord) {
+        if (gB0 > 0 && gB0 < C && logz[gB0] > 0.f) {
+            const float* vp = vertmap + (img + r0 + xB) * 3;
+            vB[0] = __ldg(vp); vB[1] = __ldg(vp + 1); vB[2] = __ldg(vp + 2);
+        }
+    }
     int g0 = -1, g1 = -1, g2;
     float q0 = 0.f, q1 = 0.f, q2;
     float2 sv0 = make_float2(0.f, 0.f), pv0 = sv0, sv1 = sv0, pv1 = sv0;
@@ -254,11 +274,18 @@ k_up8_bwd_strip(const float* __restrict__ prob, const float* __restrict__ score,
             const int gB = gB0;
             if (gB > 0 && gB < C) {
                 const float* cen = centers + ((size_t)n * C + gB) * 3;
-                if (cen[2] > 0.f) {
+                if (kCoord ? logz[gB] > 0.f : cen[2] > 0.f) {
                     const bool ownB = ownB_x && y >= own_lo && y < own_hi;
-                    const double dx = (double)cen[0] - (double)xB, dy = (double)cen[1] - (double)y;
-                    const double nrm = sqrt(dx * dx + dy * dy) + 1e-10;
-                    const float tg[3] = {(float)(dx / nrm), (float)(dy / nrm), logz[gB]};
+                    float tg[3];
+                    if constexpr (kCoord) {
+                        const float* s = ab + 6 * gB;
+#pragma unroll
+                        for (int k = 0; k < 3; k++) tg[k] = coord_target(s[2 * k], s[2 * k + 1], vB[k]);
+                    } else {
+                        const double dx = (double)cen[0] - (double)xB, dy = (double)cen[1] - (double)y;
+                        const double nrm = sqrt(dx * dx + dy * dy) + 1e-10;
+                        tg[0] = (float)(dx / nrm); tg[1] = (float)(dy / nrm); tg[2] = logz[gB];
+                    }
                     const size_t pB = img + (size_t)y * W + xB;
                     float* a_lo = vacc + ((size_t)slot_lo * kSCols + t) * VC + 3 * gB;
                     float* a_hi = vacc + ((size_t)(slot_lo ^ 1) * kSCols + t) * VC + 3 * gB;
@@ -280,6 +307,12 @@ k_up8_bwd_strip(const float* __restrict__ prob, const float* __restrict__ score,
             gB0 = gB1;
             gB1 = (xinB && y + 2 <= y_last) ? __ldg(gpB2) : -1;
             gpB2 += W;
+            if constexpr (kCoord) {
+                if (gB0 > 0 && gB0 < C && logz[gB0] > 0.f) {   // a label >= 0 is only ever loaded for rows <= y_last
+                    const float* vp = vertmap + (img + (size_t)(y + 1) * W + xB) * 3;
+                    vB[0] = __ldg(vp); vB[1] = __ldg(vp + 1); vB[2] = __ldg(vp + 2);
+                }
+            }
         }
         g0 = g1; q0 = q1; s0 = s1; sv0 = sv1; pv0 = pv1; g1 = g2; q1 = q2;
         if (kh == 7) {
@@ -466,44 +499,71 @@ extern "C" int pcnn_pack_lowres(const void* sc, int Cs, const void* vt, int Cv, 
     return check_launch("pack_lowres");
 }
 
+// the adjoint in either target mode (kCoord: vertmap + extents give the vertex target); `what` names the entry point in messages
+template <bool kCoord>
+static int up8_heads_bwd(const char* what, const float* prob, const float* score, const int32_t* gt, const float* cls_loss_out,
+                         float upstream_cls, float threshold, const float* vertex_pred, const float* lowres, const float* bias_vertex,
+                         const float* vertmap, const float* centers, const float* extents, const float* vertex_loss_out, float upstream_vertex,
+                         float w_inside, float sigma, int B, int h, int w, int C, int Cs, int Cv, void* d_sc_bf16, void* d_vt_bf16, float* dbias,
+                         void* workspace, size_t workspace_bytes, void* stream)
+{
+    PCNN_REQUIRE(prob && score && gt && cls_loss_out && (vertex_pred || (lowres && bias_vertex)) && centers && vertex_loss_out && d_sc_bf16 &&
+                     d_vt_bf16 && dbias && workspace && (!kCoord || (vertmap && extents)),
+                 "%s: NULL tensor pointer", what);
+    PCNN_REQUIRE(Cs >= C && Cv >= 3 * C && h <= 65535 && B <= 65535, "%s: bad shape", what);
+    PCNN_REQUIRE(C == 2 || (C % 2 == 0 && C >= 6 && C <= 50), "%s: C must be even and 2 or in 6..50 (C = %d)", what, C);
+    // coalesced strip kernel (see k_up8_bwd_strip); partial bias sums: one row of 4C floats per CTA
+    const int sc = C == 2 ? kStrip2 : kStrip, cols = 8 * sc + 8;
+    const int rb = 16, bands = (h + rb - 1) / rb, strips = (w + sc - 1) / sc;
+    const size_t need = sizeof(float) * (size_t)B * strips * bands * 4 * C;
+    PCNN_REQUIRE(workspace_bytes >= need, "%s: workspace too small (%zu < %zu)", what, workspace_bytes, need);
+    PCNN_REQUIRE(bands <= 65535, "%s: bad shape", what);
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t smem = sizeof(float) * ((size_t)cols * 11 * C + C + (kCoord ? 6 * C : 0));
+    const dim3 grid(strips, bands, B);
+    if (C == 22)
+        k_up8_bwd_strip<22, kStrip, kCoord><<<grid, cols * 11, smem, st>>>(prob, score, gt, cls_loss_out, upstream_cls, threshold, vertex_pred, lowres,
+                                                                          bias_vertex, centers, vertex_loss_out, upstream_vertex, w_inside,
+                                                                          sigma * sigma, h, w, rb, C, Cs, Cv, (__nv_bfloat16*)d_sc_bf16,
+                                                                          (__nv_bfloat16*)d_vt_bf16, (float*)workspace, vertmap, extents);
+    else if (C == 2)
+        k_up8_bwd_strip<2, kStrip2, kCoord><<<grid, cols, smem, st>>>(prob, score, gt, cls_loss_out, upstream_cls, threshold, vertex_pred, lowres,
+                                                                     bias_vertex, centers, vertex_loss_out, upstream_vertex, w_inside, sigma * sigma, h,
+                                                                     w, rb, C, Cs, Cv, (__nv_bfloat16*)d_sc_bf16, (__nv_bfloat16*)d_vt_bf16,
+                                                                     (float*)workspace, vertmap, extents);
+    else {
+        PCNN_SMEM_OPTIN((k_up8_bwd_strip<0, kStrip, kCoord>), 100 * 1024, kCoord ? "up8_bwd_strip<0, coord>" : "up8_bwd_strip<0>");
+        k_up8_bwd_strip<0, kStrip, kCoord><<<grid, cols * (C / 2), smem, st>>>(prob, score, gt, cls_loss_out, upstream_cls, threshold, vertex_pred,
+                                                                              lowres, bias_vertex, centers, vertex_loss_out, upstream_vertex, w_inside,
+                                                                              sigma * sigma, h, w, rb, C, Cs, Cv, (__nv_bfloat16*)d_sc_bf16,
+                                                                              (__nv_bfloat16*)d_vt_bf16, (float*)workspace, vertmap, extents);
+    }
+    k_sum_partials<<<(4 * C + 31) / 32, 256, 0, st>>>((const float*)workspace, B * strips * bands, 4 * C, 1.f, nullptr, 0.f, dbias);
+    return check_launch(what);
+}
+
 extern "C" int pcnn_up8_heads_bwd_ex(const float* prob, const float* score, const int32_t* gt, const float* cls_loss_out, float upstream_cls,
                                      float threshold, const float* vertex_pred, const float* lowres, const float* bias_vertex, const float* centers,
                                      const float* vertex_loss_out, float upstream_vertex, float w_inside, float sigma, int B, int h, int w, int C,
                                      int Cs, int Cv, void* d_sc_bf16, void* d_vt_bf16, float* dbias, void* workspace, size_t workspace_bytes,
                                      void* stream)
 {
-    PCNN_REQUIRE(prob && score && gt && cls_loss_out && (vertex_pred || (lowres && bias_vertex)) && centers && vertex_loss_out && d_sc_bf16 &&
-                     d_vt_bf16 && dbias && workspace,
-                 "up8_heads_bwd: NULL tensor pointer");
-    PCNN_REQUIRE(Cs >= C && Cv >= 3 * C && h <= 65535 && B <= 65535, "up8_heads_bwd: bad shape");
-    PCNN_REQUIRE(C == 2 || (C % 2 == 0 && C >= 6 && C <= 50), "up8_heads_bwd: C must be even and 2 or in 6..50 (C = %d)", C);
-    // coalesced strip kernel (see k_up8_bwd_strip); partial bias sums: one row of 4C floats per CTA
-    const int sc = C == 2 ? kStrip2 : kStrip, cols = 8 * sc + 8;
-    const int rb = 16, bands = (h + rb - 1) / rb, strips = (w + sc - 1) / sc;
-    const size_t need = sizeof(float) * (size_t)B * strips * bands * 4 * C;
-    PCNN_REQUIRE(workspace_bytes >= need, "up8_heads_bwd: workspace too small (%zu < %zu)", workspace_bytes, need);
-    PCNN_REQUIRE(bands <= 65535, "up8_heads_bwd: bad shape");
-    cudaStream_t st = (cudaStream_t)stream;
-    const size_t smem = sizeof(float) * ((size_t)cols * 11 * C + C);
-    const dim3 grid(strips, bands, B);
-    if (C == 22)
-        k_up8_bwd_strip<22, kStrip><<<grid, cols * 11, smem, st>>>(prob, score, gt, cls_loss_out, upstream_cls, threshold, vertex_pred, lowres,
-                                                                  bias_vertex, centers, vertex_loss_out, upstream_vertex, w_inside, sigma * sigma, h,
-                                                                  w, rb, C, Cs, Cv, (__nv_bfloat16*)d_sc_bf16, (__nv_bfloat16*)d_vt_bf16,
-                                                                  (float*)workspace);
-    else if (C == 2)
-        k_up8_bwd_strip<2, kStrip2><<<grid, cols, smem, st>>>(prob, score, gt, cls_loss_out, upstream_cls, threshold, vertex_pred, lowres,
-                                                             bias_vertex, centers, vertex_loss_out, upstream_vertex, w_inside, sigma * sigma, h, w,
-                                                             rb, C, Cs, Cv, (__nv_bfloat16*)d_sc_bf16, (__nv_bfloat16*)d_vt_bf16, (float*)workspace);
-    else {
-        PCNN_SMEM_OPTIN((k_up8_bwd_strip<0, kStrip>), 100 * 1024, "up8_bwd_strip<0>");
-        k_up8_bwd_strip<0, kStrip><<<grid, cols * (C / 2), smem, st>>>(prob, score, gt, cls_loss_out, upstream_cls, threshold, vertex_pred, lowres,
-                                                                      bias_vertex, centers, vertex_loss_out, upstream_vertex, w_inside, sigma * sigma,
-                                                                      h, w, rb, C, Cs, Cv, (__nv_bfloat16*)d_sc_bf16, (__nv_bfloat16*)d_vt_bf16,
-                                                                      (float*)workspace);
-    }
-    k_sum_partials<<<(4 * C + 31) / 32, 256, 0, st>>>((const float*)workspace, B * strips * bands, 4 * C, 1.f, nullptr, 0.f, dbias);
-    return check_launch("up8_heads_bwd");
+    return up8_heads_bwd<false>("up8_heads_bwd", prob, score, gt, cls_loss_out, upstream_cls, threshold, vertex_pred, lowres, bias_vertex, nullptr,
+                                centers, nullptr, vertex_loss_out, upstream_vertex, w_inside, sigma, B, h, w, C, Cs, Cv, d_sc_bf16, d_vt_bf16, dbias,
+                                workspace, workspace_bytes, stream);
+}
+
+// VERTEX_REG_3D: the same adjoint with the object-coordinate target (vertmap [B,8h,8w,3] f32, extents [C,3] f32); centers stays the
+// presence table (a class's pixels are weighted iff centers[b, c, 2] > 0)
+extern "C" int pcnn_up8_heads_bwd_coord(const float* prob, const float* score, const int32_t* gt, const float* cls_loss_out, float upstream_cls,
+                                        float threshold, const float* vertex_pred, const float* lowres, const float* bias_vertex, const float* vertmap,
+                                        const float* centers, const float* extents, const float* vertex_loss_out, float upstream_vertex,
+                                        float w_inside, float sigma, int B, int h, int w, int C, int Cs, int Cv, void* d_sc_bf16, void* d_vt_bf16,
+                                        float* dbias, void* workspace, size_t workspace_bytes, void* stream)
+{
+    return up8_heads_bwd<true>("up8_heads_bwd_coord", prob, score, gt, cls_loss_out, upstream_cls, threshold, vertex_pred, lowres, bias_vertex,
+                               vertmap, centers, extents, vertex_loss_out, upstream_vertex, w_inside, sigma, B, h, w, C, Cs, Cv, d_sc_bf16, d_vt_bf16,
+                               dbias, workspace, workspace_bytes, stream);
 }
 
 extern "C" int pcnn_pose_chain_bwd(const float* bottom_diff, const float* poses_tanh, const float* poses_weight, int N, int D, float upstream,

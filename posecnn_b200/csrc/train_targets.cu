@@ -6,6 +6,9 @@
 //   pcnn_loss_cls_hard_fwd       lib/fcn/train.py:455-465 (loss_cross_entropy_single_frame) applied to the Hardlabel mask
 //                                (hard_label_op_gpu.cu.cc:16-29) WITHOUT materialising the [B,H,W,C] mask
 //   pcnn_smooth_l1_vertex_fwd    lib/fcn/train.py:564-573 (smooth_l1_loss_vertex)
+//   pcnn_vertex_targets_3d_fwd   the VERTEX_REG_3D branch of _generate_vertex_targets (minibatch.py:595-600, _scale_vertmap :605-616):
+//                                the pixel's object coordinate scaled into [0, 1] by its class's extents; pcnn_vertex_loss_coord_fwd /
+//                                _lowres_fwd: the fused loss on that target
 // Losses: fixed 592-CTA grid, per-CTA partial sums in double, last CTA to finish reduces them in index order
 // (run-to-run deterministic), optional gradient pass w.r.t. the first input.
 #include <cuda_runtime.h>
@@ -197,6 +200,33 @@ __device__ __forceinline__ bool pixel_targets(const int* __restrict__ label, con
     return true;
 }
 
+// VERTEX_REG_3D target (minibatch.py:595-600 with _scale_vertmap, :605-616; coord_scale / coord_target: heads_common.cuh): the pixel's
+// object coordinate vertmap [.., 3] scaled into [0, 1] by its class's extents.  Weighted pixels are those of pixel_targets: label l in
+// 1..C-1 with a listed centre (centers[b, l, 2] > 0), so `centers` stays the presence table.
+__device__ __forceinline__ bool pixel_targets_3d(const int* __restrict__ label, const float* __restrict__ vertmap, const float* __restrict__ centers,
+                                                 const float* __restrict__ extents, unsigned pix, int HW, int C, int& cls, float t[3])
+{
+    const int l = __ldg(label + pix);
+    if (l <= 0 || l >= C) return false;
+    const int b = pix / HW;
+    if (!(centers[((size_t)b * C + l) * 3 + 2] > 0.f)) return false;
+    float ab[6];
+    coord_scale(extents + 3 * l, ab);
+#pragma unroll
+    for (int k = 0; k < 3; k++) t[k] = coord_target(ab[2 * k], ab[2 * k + 1], __ldg(vertmap + (size_t)pix * 3 + k));
+    cls = l;
+    return true;
+}
+
+// the target of either mode: 2-D centre direction + log z (kCoord = false) or the scaled object coordinate (kCoord = true)
+template <bool kCoord>
+__device__ __forceinline__ bool vertex_target(const int* __restrict__ label, const float* __restrict__ centers, const float* __restrict__ vertmap,
+                                              const float* __restrict__ extents, unsigned pix, int HW, int W, int C, int& cls, float t[3])
+{
+    if constexpr (kCoord) return pixel_targets_3d(label, vertmap, centers, extents, pix, HW, C, cls, t);
+    else return pixel_targets(label, centers, pix, HW, W, C, cls, t);
+}
+
 // materialised targets / weights (drop-in for the data layer's blobs): the tensors are >97 % zeros, so they are
 // cleared with two memset nodes and only the three channels of each labelled pixel's own class are written
 __global__ void __launch_bounds__(256)
@@ -207,6 +237,22 @@ k_vertex_targets_sparse(const int* __restrict__ label, const float* __restrict__
         int cls;
         float t[3];
         if (!pixel_targets(label, centers, pix, HW, W, C, cls, t)) continue;
+        const size_t o = (size_t)pix * 3 * C + 3 * cls;
+#pragma unroll
+        for (int k = 0; k < 3; k++) { targets[o + k] = t[k]; weights[o + k] = w_inside; }
+    }
+}
+
+// the same for the VERTEX_REG_3D target (pixel_targets_3d)
+__global__ void __launch_bounds__(256)
+k_vertex_targets_3d_sparse(const int* __restrict__ label, const float* __restrict__ vertmap, const float* __restrict__ centers,
+                           const float* __restrict__ extents, unsigned npix, int HW, int C, float w_inside, float* __restrict__ targets,
+                           float* __restrict__ weights)
+{
+    for (unsigned pix = blockIdx.x * blockDim.x + threadIdx.x; pix < npix; pix += gridDim.x * blockDim.x) {
+        int cls;
+        float t[3];
+        if (!pixel_targets_3d(label, vertmap, centers, extents, pix, HW, C, cls, t)) continue;
         const size_t o = (size_t)pix * 3 * C + 3 * cls;
 #pragma unroll
         for (int k = 0; k < 3; k++) { targets[o + k] = t[k]; weights[o + k] = w_inside; }
@@ -292,11 +338,13 @@ k_pack_pose_meta(const float* __restrict__ poses /*[B,I,12]*/, const int* __rest
     }
 }
 
+// kCoord: the VERTEX_REG_3D target (vertmap + extents, pixel_targets_3d); otherwise the 2-D one (vertmap / extents unused)
+template <bool kCoord>
 __global__ void __launch_bounds__(kLossThreads)
 k_vertex_loss_fused(const float* __restrict__ pred, const float* __restrict__ lowres, const float* __restrict__ bias_v,
                     const int* __restrict__ label, const float* __restrict__ centers, unsigned npix, int HW,
                     int W, int C, float w_inside, float sigma2, double* __restrict__ partial, unsigned* __restrict__ ticket,
-                    float* __restrict__ out)
+                    float* __restrict__ out, const float* __restrict__ vertmap, const float* __restrict__ extents)
 {
     // pred == NULL: the labelled pixels' three vertex values are formed on demand from the 1/8-resolution head tensor with
     // k_up8_heads' own operation sequence (heads_common.cuh) — bit-identical to reading the dense vertex_pred
@@ -305,7 +353,7 @@ k_vertex_loss_fused(const float* __restrict__ pred, const float* __restrict__ lo
     for (unsigned pix = blockIdx.x * blockDim.x + threadIdx.x; pix < npix; pix += gridDim.x * blockDim.x) {
         int cls;
         float t[3], d;
-        if (!pixel_targets(label, centers, pix, HW, W, C, cls, t)) continue;
+        if (!vertex_target<kCoord>(label, centers, vertmap, extents, pix, HW, W, C, cls, t)) continue;
         if (pred) {
             const float* pp = pred + (size_t)pix * 3 * C + 3 * cls;
 #pragma unroll
@@ -327,16 +375,17 @@ k_vertex_loss_fused(const float* __restrict__ pred, const float* __restrict__ lo
     }
 }
 
+template <bool kCoord>
 __global__ void __launch_bounds__(256)
 k_vertex_loss_fused_grad(const float* __restrict__ pred, const int* __restrict__ label, const float* __restrict__ centers, unsigned npix,
                          int HW, int W, int C, float w_inside, float sigma2, const float* __restrict__ loss_out, float upstream,
-                         float* __restrict__ grad /*zero-filled*/)
+                         float* __restrict__ grad /*zero-filled*/, const float* __restrict__ vertmap, const float* __restrict__ extents)
 {
     const float scale = upstream / (loss_out[1] + 1e-10f);
     for (unsigned pix = blockIdx.x * blockDim.x + threadIdx.x; pix < npix; pix += gridDim.x * blockDim.x) {
         int cls;
         float t[3], d;
-        if (!pixel_targets(label, centers, pix, HW, W, C, cls, t)) continue;
+        if (!vertex_target<kCoord>(label, centers, vertmap, extents, pix, HW, W, C, cls, t)) continue;
         const size_t o = (size_t)pix * 3 * C + 3 * cls;
 #pragma unroll
         for (int k = 0; k < 3; k++) {
@@ -350,28 +399,46 @@ k_vertex_loss_fused_grad(const float* __restrict__ pred, const int* __restrict__
 
 using namespace pcnn;
 
-extern "C" int pcnn_vertex_loss_fused_fwd(const float* pred, const int32_t* label, const float* centers, int B, int H, int W, int C,
-                                          float w_inside, float sigma, float* loss_out, float upstream, float* grad_pred,
-                                          void* workspace, size_t workspace_bytes, void* stream)
+// the fused vertex loss of either target mode: vertex values from the dense `pred` (grad_pred optional), or with pred == NULL from
+// `lowres` + `bias_vertex` (no gradient); `what` names the entry point in error messages
+template <bool kCoord>
+static int vertex_loss_fused(const char* what, const float* pred, const float* lowres, const float* bias_vertex, const int32_t* label,
+                             const float* vertmap, const float* centers, const float* extents, int B, int H, int W, int C, float w_inside,
+                             float sigma, float* loss_out, float upstream, float* grad_pred, void* workspace, size_t workspace_bytes,
+                             void* stream)
 {
-    PCNN_REQUIRE(pred && label && centers && loss_out && workspace, "vertex_loss_fused: NULL tensor pointer");
-    PCNN_REQUIRE(sigma > 0.f && B >= 1 && H >= 1 && W >= 1 && C >= 1, "vertex_loss_fused: bad arguments");
-    PCNN_REQUIRE((unsigned long long)B * H * W < 0xffffffffULL, "vertex_loss_fused: too many pixels");
+    PCNN_REQUIRE((pred || (lowres && bias_vertex)) && label && centers && loss_out && workspace && (!kCoord || (vertmap && extents)),
+                 "%s: NULL tensor pointer", what);
+    if (pred)
+        PCNN_REQUIRE(sigma > 0.f && B >= 1 && H >= 1 && W >= 1 && C >= 1, "%s: bad arguments", what);
+    else
+        PCNN_REQUIRE(sigma > 0.f && B >= 1 && H >= 8 && W >= 8 && H % 8 == 0 && W % 8 == 0 && C >= 1, "%s: bad arguments", what);
+    PCNN_REQUIRE((unsigned long long)B * H * W < 0xffffffffULL, "%s: too many pixels", what);
     size_t need = 0;
     pcnn_train_loss_workspace_bytes(&need);
-    PCNN_REQUIRE(workspace_bytes >= need, "vertex_loss_fused: workspace too small (%zu < %zu)", workspace_bytes, need);
+    PCNN_REQUIRE(workspace_bytes >= need, "%s: workspace too small (%zu < %zu)", what, workspace_bytes, need);
     double* partial = (double*)workspace;
     unsigned* ticket = (unsigned*)(partial + 2 * kLossBlocks);
     const unsigned npix = (unsigned)B * H * W;
     cudaStream_t st = (cudaStream_t)stream;
-    k_vertex_loss_fused<<<kLossBlocks, kLossThreads, 0, st>>>(pred, nullptr, nullptr, label, centers, npix, H * W, W, C, w_inside, sigma * sigma,
-                                                               partial, ticket, loss_out);
-    if (grad_pred) {
+    k_vertex_loss_fused<kCoord><<<kLossBlocks, kLossThreads, 0, st>>>(pred, pred ? nullptr : lowres, pred ? nullptr : bias_vertex, label, centers,
+                                                                       npix, H * W, W, C, w_inside, sigma * sigma, partial, ticket, loss_out,
+                                                                       vertmap, extents);
+    if (pred && grad_pred) {
         cudaMemsetAsync(grad_pred, 0, sizeof(float) * (size_t)npix * 3 * C, st);
-        k_vertex_loss_fused_grad<<<kNumSMs * 16, 256, 0, st>>>(pred, label, centers, npix, H * W, W, C, w_inside, sigma * sigma, loss_out,
-                                                                upstream, grad_pred);
+        k_vertex_loss_fused_grad<kCoord><<<kNumSMs * 16, 256, 0, st>>>(pred, label, centers, npix, H * W, W, C, w_inside, sigma * sigma, loss_out,
+                                                                        upstream, grad_pred, vertmap, extents);
     }
-    return check_launch("vertex_loss_fused");
+    return check_launch(what);
+}
+
+extern "C" int pcnn_vertex_loss_fused_fwd(const float* pred, const int32_t* label, const float* centers, int B, int H, int W, int C,
+                                          float w_inside, float sigma, float* loss_out, float upstream, float* grad_pred,
+                                          void* workspace, size_t workspace_bytes, void* stream)
+{
+    PCNN_REQUIRE(pred, "vertex_loss_fused: NULL tensor pointer");
+    return vertex_loss_fused<false>("vertex_loss_fused", pred, nullptr, nullptr, label, nullptr, centers, nullptr, B, H, W, C, w_inside, sigma,
+                                    loss_out, upstream, grad_pred, workspace, workspace_bytes, stream);
 }
 
 // the same loss with the vertex head given as the 1/8-resolution head tensor `lowres` [B,H/8,W/8,4C] (channels C.. = vertex) + the
@@ -380,17 +447,28 @@ extern "C" int pcnn_vertex_loss_fused_lowres_fwd(const float* lowres, const floa
                                                  int H, int W, int C, float w_inside, float sigma, float* loss_out, void* workspace,
                                                  size_t workspace_bytes, void* stream)
 {
-    PCNN_REQUIRE(lowres && bias_vertex && label && centers && loss_out && workspace, "vertex_loss_fused_lowres: NULL tensor pointer");
-    PCNN_REQUIRE(sigma > 0.f && B >= 1 && H >= 8 && W >= 8 && H % 8 == 0 && W % 8 == 0 && C >= 1, "vertex_loss_fused_lowres: bad arguments");
-    PCNN_REQUIRE((unsigned long long)B * H * W < 0xffffffffULL, "vertex_loss_fused_lowres: too many pixels");
-    size_t need = 0;
-    pcnn_train_loss_workspace_bytes(&need);
-    PCNN_REQUIRE(workspace_bytes >= need, "vertex_loss_fused_lowres: workspace too small (%zu < %zu)", workspace_bytes, need);
-    double* partial = (double*)workspace;
-    unsigned* ticket = (unsigned*)(partial + 2 * kLossBlocks);
-    k_vertex_loss_fused<<<kLossBlocks, kLossThreads, 0, (cudaStream_t)stream>>>(nullptr, lowres, bias_vertex, label, centers, (unsigned)B * H * W, H * W,
-                                                                                 W, C, w_inside, sigma * sigma, partial, ticket, loss_out);
-    return check_launch("vertex_loss_fused_lowres");
+    PCNN_REQUIRE(lowres && bias_vertex, "vertex_loss_fused_lowres: NULL tensor pointer");
+    return vertex_loss_fused<false>("vertex_loss_fused_lowres", nullptr, lowres, bias_vertex, label, nullptr, centers, nullptr, B, H, W, C,
+                                    w_inside, sigma, loss_out, 0.f, nullptr, workspace, workspace_bytes, stream);
+}
+
+// VERTEX_REG_3D: the same two losses on the scaled object-coordinate target (pixel_targets_3d)
+extern "C" int pcnn_vertex_loss_coord_fwd(const float* pred, const int32_t* label, const float* vertmap, const float* centers, const float* extents,
+                                          int B, int H, int W, int C, float w_inside, float sigma, float* loss_out, float upstream,
+                                          float* grad_pred, void* workspace, size_t workspace_bytes, void* stream)
+{
+    PCNN_REQUIRE(pred, "vertex_loss_coord: NULL tensor pointer");
+    return vertex_loss_fused<true>("vertex_loss_coord", pred, nullptr, nullptr, label, vertmap, centers, extents, B, H, W, C, w_inside, sigma,
+                                   loss_out, upstream, grad_pred, workspace, workspace_bytes, stream);
+}
+
+extern "C" int pcnn_vertex_loss_coord_lowres_fwd(const float* lowres, const float* bias_vertex, const int32_t* label, const float* vertmap,
+                                                 const float* centers, const float* extents, int B, int H, int W, int C, float w_inside,
+                                                 float sigma, float* loss_out, void* workspace, size_t workspace_bytes, void* stream)
+{
+    PCNN_REQUIRE(lowres && bias_vertex, "vertex_loss_coord_lowres: NULL tensor pointer");
+    return vertex_loss_fused<true>("vertex_loss_coord_lowres", nullptr, lowres, bias_vertex, label, vertmap, centers, extents, B, H, W, C,
+                                   w_inside, sigma, loss_out, 0.f, nullptr, workspace, workspace_bytes, stream);
 }
 
 extern "C" int pcnn_train_loss_workspace_bytes(size_t* bytes)
@@ -412,6 +490,20 @@ extern "C" int pcnn_vertex_targets_fwd(const int32_t* label, const float* center
     cudaMemsetAsync(weights, 0, sizeof(float) * (size_t)npix * 3 * C, st);
     k_vertex_targets_sparse<<<kNumSMs * 16, 256, 0, st>>>(label, centers, npix, H * W, W, C, w_inside, targets, weights);
     return check_launch("vertex_targets");
+}
+
+extern "C" int pcnn_vertex_targets_3d_fwd(const int32_t* label, const float* vertmap, const float* centers, const float* extents, int B, int H,
+                                          int W, int C, float w_inside, float* targets, float* weights, void* stream)
+{
+    PCNN_REQUIRE(label && vertmap && centers && extents && targets && weights, "vertex_targets_3d: NULL tensor pointer");
+    PCNN_REQUIRE(B >= 1 && H >= 1 && W >= 1 && C >= 1, "vertex_targets_3d: bad shape");
+    PCNN_REQUIRE((unsigned long long)B * H * W < 0xffffffffULL, "vertex_targets_3d: too many pixels");
+    const unsigned npix = (unsigned)B * H * W;
+    cudaStream_t st = (cudaStream_t)stream;
+    cudaMemsetAsync(targets, 0, sizeof(float) * (size_t)npix * 3 * C, st);
+    cudaMemsetAsync(weights, 0, sizeof(float) * (size_t)npix * 3 * C, st);
+    k_vertex_targets_3d_sparse<<<kNumSMs * 16, 256, 0, st>>>(label, vertmap, centers, extents, npix, H * W, C, w_inside, targets, weights);
+    return check_launch("vertex_targets_3d");
 }
 
 extern "C" int pcnn_loss_cls_hard_fwd(const float* score, const float* prob, const int32_t* gt, int B, int H, int W, int C, float threshold,

@@ -27,7 +27,9 @@ def single_class_view(cls_index: int, gt_label_2d: torch.Tensor, centers: torch.
                                     same row as linemod.py's extents_all[cls_index - 1] of extents.txt)
     points      [C,P,3]          -> [2,P,3]: row 0 zero, row 1 = the object's points
     symmetry    [C]              -> [0, symmetry[cls_index]]
-    The label remap is one element-wise pass on the device; everything else is a row selection."""
+    The label remap is one element-wise pass on the device; everything else is a row selection.  The object-coordinate map of a
+    VERTEX_REG_3D batch (Trainer.step's vertmap [B,H,W,3]) needs no view: it is per pixel, not indexed by class, and the two-row
+    extents above already scale the object's coordinates."""
     c = int(cls_index)
     if not 1 <= c < centers.shape[1]:
         raise ValueError(f"cls_index must be a foreground class of the {centers.shape[1]}-class tables (got {c})")

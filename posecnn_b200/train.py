@@ -11,6 +11,10 @@ A network built with pose_reg=False (the linemod_{benchvise,camera,iron,lamp,pho
     loss = loss_cls + VERTEX_W * loss_vertex + l2 regularisation (train.py:517, vgg16_convs.py:128-163):
 no Hough voting, RoiPool or fc6-fc8 in the step, and no fc6-fc8 parameters in it.
 Every class count the kernels take trains: C = 2 (the single-object LINEMOD / YCB models) and even C in 6..50.
+A network built with vertex_reg_2d=False, vertex_reg_3d=True (the object-coordinate models linemod_*_3d.yml, lov_color_3d.yml) trains
+its vertex head on 3-D targets (minibatch.py:595-600, 605-616): a labelled pixel of a listed class regresses its object coordinate
+vertmap [B,H,W,3] scaled into [0, 1] by the class's extents.  Its graph has no pose head whatever pose_reg says (vgg16_convs.py:165-200
+builds Hough voting, RoiPool and fc6-fc8 only under vertex_reg_2d), so it trains loss_cls + VERTEX_W * loss_vertex (+ l2).
 input_format='RGBD' adds the depth trunk conv1_1_p .. conv5_3_p (vgg16_convs.py:99-126): score_conv4 / score_conv5 read the channel
 concat [colour | depth] of conv4_3 / conv5_3 (c_i = 1024), the vertex heads, Hough voting and RoiPool read the colour trunk only.
 A network built with adaptation=True adds the domain classifier (vgg16_convs.py:202-212) and
@@ -89,15 +93,21 @@ KINDS = {
 }
 
 
+def trains_coords(net) -> bool:
+    """True for the object-coordinate (VERTEX_REG_3D) training graph: 3-D vertex targets and no pose head."""
+    return bool(net.vertex_reg_3d) and not bool(net.vertex_reg_2d)
+
+
 def param_layout(net) -> dict:
     """{master name: (TF parameter name, kind, master rows)} for every parameter the training step updates.  score / vertex_pred
     keep C / 3C rows zero-padded to 64 / 128: the channel counts of their 1x1 GEMMs, which pcnn_pack_lowres and the up8
     backward read.  A pose_reg=False network has no fc6-fc8: the reference creates those variables only under POSE_REG
-    (vgg16_convs.py:175-200), so they are neither trained, decayed nor exported."""
+    (vgg16_convs.py:175-200), so they are neither trained, decayed nor exported.  Neither has an object-coordinate network, whose
+    pose head sits under vertex_reg_2d in the reference graph."""
     trunks = ("", "_p") if net.input_format == "RGBD" else ("",)
     weights = [(layer + sfx, "conv1_1" if layer == "conv1_1" else "conv", None) for sfx in trunks for layer in CONV_NAMES]
     weights += [(name, "conv", None) for name in SCORE_HEADS] + [("score", "conv", 64), ("vertex_pred", "conv", 128)]
-    fc = (("fc6", "fc7", "fc8") if net.pose_reg else ()) + (("fc9",) if net.domain_branch else ())
+    fc = (("fc6", "fc7", "fc8") if net.pose_reg and not trains_coords(net) else ()) + (("fc9",) if net.domain_branch else ())
     weights += [(name, "fc", None) for name in fc]
     if net.domain_branch:
         weights.append(("domain_score", "domain_score", None))
@@ -127,8 +137,10 @@ class Trainer:
         self.vertex_w, self.w_inside, self.margin, self.world = float(vertex_w), float(vertex_w_inside), float(margin), int(world)
         self.C = net.num_classes
         # POSE_REG: Hough voting, RoiPool, fc6-fc8 and loss_pose (vgg16_convs.py:165-200).  Without it the step is the dense heads'
-        # loss_cls + VERTEX_W * loss_vertex (+ l2 regularisation) alone, as lib/fcn/train.py:517 trains it
-        self.pose_reg = bool(net.pose_reg)
+        # loss_cls + VERTEX_W * loss_vertex (+ l2 regularisation) alone, as lib/fcn/train.py:517 trains it.  The object-coordinate
+        # graph (3-D vertex targets) never has the pose head
+        self.coord = trains_coords(net)
+        self.pose_reg = bool(net.pose_reg) and not self.coord
         self.pose_loss_scale = 1.0               # last dynamic loss scale of the fp16 pose-head backward (see backward())
         self.adapt = net.domain_branch           # the domain classifier and loss_domain (ADAPT_WEIGHT, lib/fcn/config.py:95)
         self.adapt_weight = float(adapt_weight)
@@ -205,12 +217,25 @@ class Trainer:
                 x = conv.maxpool2x2(x)
                 A[name + "/pool"] = x
 
+    def _require_vertmap(self, vertmap, data):
+        B, H, W = data.shape[:3]
+        if vertmap is None:
+            raise ValueError("an object-coordinate (vertex_reg_3d) network trains on 3-D targets: pass vertmap= [B,H,W,3] f32")
+        if vertmap.dtype != torch.float32 or tuple(vertmap.shape) != (B, H, W, 3) or vertmap.device != data.device:
+            raise ValueError(f"vertmap must be a [{B},{H},{W},3] float32 tensor on {data.device}")
+        return vertmap.contiguous()
+
     def forward(self, data, gt_label_2d, centers, meta_data, extents, gt_poses, points, symmetry, batch_global=None, batch_offset=0,
-                depth=None, data_p=None):
+                depth=None, data_p=None, vertmap=None):
         """RGBD: the depth trunk reads depth= (a raw [B,H,W] f32 depth image, sensor units; its blob is formed in conv1_1_p's loader)
-        or data_p= (the pre-processed blob [B,H,W,3] f32), as vgg16_convs.forward does."""
+        or data_p= (the pre-processed blob [B,H,W,3] f32), as vgg16_convs.forward does.  An object-coordinate network reads
+        vertmap= [B,H,W,3] f32 (each pixel's object coordinate, metres in the model frame) and extents [C,3]; other networks ignore
+        vertmap."""
         net, C, M, T = self.net, self.C, self.master, self.tc
         B, H, W, _ = data.shape
+        if self.coord:
+            vertmap = self._require_vertmap(vertmap, data)
+            extents = extents.contiguous()
         A = {}                                    # activations by layer name (bf16 NHWC), "<pool>" = pooled tensors
         # data: [B,H,W,3] u8 BGR (PIXEL_MEANS subtracted in conv1_1's loader) or the f32 blob of augment.augment_color (means
         # already subtracted), as vgg16_convs._trunk chooses
@@ -254,8 +279,14 @@ class Trainer:
         check(lib().pcnn_loss_cls_hard_raw_fwd(ptr(score), ptr(prob), ptr(gt_label_2d), B, H, W, C, f32(net.threshold_label), ptr(cls_out), ptr(ws),
                                                ctypes.c_size_t(ws.numel()), stream()))
         vtx_out = torch.empty((2,), dtype=torch.float32, device=data.device)
-        check(lib().pcnn_vertex_loss_fused_lowres_fwd(ptr(lowres), ptr(M["vertex_pred/b"]), ptr(gt_label_2d), ptr(centers), B, H, W, C,
-                                                      f32(self.w_inside), f32(1.0), ptr(vtx_out), ptr(ws), ctypes.c_size_t(ws.numel()), stream()))
+        if self.coord:
+            check(lib().pcnn_vertex_loss_coord_lowres_fwd(ptr(lowres), ptr(M["vertex_pred/b"]), ptr(gt_label_2d), ptr(vertmap), ptr(centers),
+                                                          ptr(extents), B, H, W, C, f32(self.w_inside), f32(1.0), ptr(vtx_out), ptr(ws),
+                                                          ctypes.c_size_t(ws.numel()), stream()))
+            A.update(extents=extents)
+        else:
+            check(lib().pcnn_vertex_loss_fused_lowres_fwd(ptr(lowres), ptr(M["vertex_pred/b"]), ptr(gt_label_2d), ptr(centers), B, H, W, C,
+                                                          f32(self.w_inside), f32(1.0), ptr(vtx_out), ptr(ws), ctypes.c_size_t(ws.numel()), stream()))
         A.update(cls_out=cls_out, vtx_out=vtx_out, data=data)
         if not self.pose_reg:
             return A
@@ -333,10 +364,10 @@ class Trainer:
                                          ctypes.c_size_t(ws.numel()), stream()))
         return out
 
-    def backward(self, A, gt_label_2d, centers):
+    def backward(self, A, gt_label_2d, centers, vertmap=None):
         """All parameter gradients of loss = loss_cls + vertex_w * loss_vertex + loss_pose (weight decay is applied in the update);
         without pose_reg, of loss_cls + vertex_w * loss_vertex.  Loss normalisers (selected-pixel count, vertex weight sum, ROI rows)
-        are GLOBAL over the ranks."""
+        are GLOBAL over the ranks.  An object-coordinate network needs the forward's vertmap= again (its extents are kept in A)."""
         net, C, M, T = self.net, self.C, self.master, self.tc
         data = A["data"]
         B, H, W, _ = data.shape
@@ -360,10 +391,18 @@ class Trainer:
         dbias = torch.empty((4 * C,), dtype=torch.float32, device=dev)
         # 4C floats per CTA of >= 4 columns x 16 rows: covers every strip width; the entry point checks its own requirement
         ws = workspace("up8_bwd", 4 * B * ((w + 3) // 4) * ((h + 15) // 16) * 4 * C, dev)
-        check(lib().pcnn_up8_heads_bwd_ex(ptr(A["prob_normalized"]), ptr(A["score"]), ptr(gt_label_2d), ptr(A["cls_out"]), f32(1.0),
-                                          f32(net.threshold_label), ptr(None), ptr(A["lowres"]), ptr(M["vertex_pred/b"]), ptr(centers),
-                                          ptr(A["vtx_out"]), f32(self.vertex_w), f32(self.w_inside), f32(1.0), B, h, w, C, 64, 128, ptr(d_sc),
-                                          ptr(d_vt), ptr(dbias), ptr(ws), ctypes.c_size_t(ws.numel()), stream()))
+        if self.coord:
+            vm = self._require_vertmap(vertmap, data)
+            check(lib().pcnn_up8_heads_bwd_coord(ptr(A["prob_normalized"]), ptr(A["score"]), ptr(gt_label_2d), ptr(A["cls_out"]), f32(1.0),
+                                                 f32(net.threshold_label), ptr(None), ptr(A["lowres"]), ptr(M["vertex_pred/b"]), ptr(vm),
+                                                 ptr(centers), ptr(A["extents"]), ptr(A["vtx_out"]), f32(self.vertex_w), f32(self.w_inside),
+                                                 f32(1.0), B, h, w, C, 64, 128, ptr(d_sc), ptr(d_vt), ptr(dbias), ptr(ws),
+                                                 ctypes.c_size_t(ws.numel()), stream()))
+        else:
+            check(lib().pcnn_up8_heads_bwd_ex(ptr(A["prob_normalized"]), ptr(A["score"]), ptr(gt_label_2d), ptr(A["cls_out"]), f32(1.0),
+                                              f32(net.threshold_label), ptr(None), ptr(A["lowres"]), ptr(M["vertex_pred/b"]), ptr(centers),
+                                              ptr(A["vtx_out"]), f32(self.vertex_w), f32(self.w_inside), f32(1.0), B, h, w, C, 64, 128, ptr(d_sc),
+                                              ptr(d_vt), ptr(dbias), ptr(ws), ctypes.c_size_t(ws.numel()), stream()))
         self._emit(grads, "score/b", dbias[:C].contiguous())
         self._emit(grads, "vertex_pred/b", dbias[C:].contiguous())
         self._emit(grads, "score/w", bw.conv_wgrad(A["add_s"], d_sc, 1))
@@ -511,14 +550,15 @@ class Trainer:
         self._refresh_derived()
 
     def step(self, data, gt_label_2d, centers, meta_data, extents, gt_poses, points, symmetry, batch_global=None, batch_offset=0,
-             depth=None, data_p=None):
+             depth=None, data_p=None, vertmap=None):
         """One forward, backward and update.  Returns loss_cls, loss_vertex, loss_pose, their sum `loss`, num_rois and the gradients
         `grads` (master layouts), plus loss_domain, label_domain and domain_label with the domain branch.  A pose_reg=False network
         returns no pose entries (loss_pose, num_rois): its loss is loss_cls + loss_vertex, and extents, gt_poses, points, symmetry,
-        meta_data, batch_global and batch_offset are not read."""
+        meta_data, batch_global and batch_offset are not read.  An object-coordinate (vertex_reg_3d) network steps the same way
+        whatever its pose_reg, and reads vertmap= [B,H,W,3] f32 and extents [C,3]."""
         A = self.forward(data, gt_label_2d, centers, meta_data, extents, gt_poses, points, symmetry, batch_global, batch_offset,
-                         depth=depth, data_p=data_p)
-        grads = self.backward(A, gt_label_2d, centers)
+                         depth=depth, data_p=data_p, vertmap=vertmap)
+        grads = self.backward(A, gt_label_2d, centers, vertmap=vertmap)
         self.update(grads)
         if not self.pose_reg:
             loss_cls, loss_vertex = A["cls_out"][0:1], self.vertex_w * A["vtx_out"][0:1]

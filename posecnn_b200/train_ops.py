@@ -33,6 +33,34 @@ def generate_vertex_targets(im_label, centers, w_inside=1.0):
     return targets, weights
 
 
+def _coord_inputs(im_label, vertmap, centers, extents):
+    lab = require_cuda("im_label", im_label, torch.int32, 3)
+    vm = require_cuda("vertmap", vertmap, torch.float32, 4)
+    cen = require_cuda("centers", centers, torch.float32, 3)
+    ext = require_cuda("extents", extents, torch.float32, 2)
+    B, H, W = lab.shape
+    C = cen.shape[1]
+    if tuple(vm.shape) != (B, H, W, 3) or cen.shape[0] != B or cen.shape[2] != 3 or tuple(ext.shape) != (C, 3):
+        raise ValueError("vertmap must be [B,H,W,3], centers [B,C,3] and extents [C,3]")
+    return lab, vm, cen, ext
+
+
+def generate_vertex_targets_3d(im_label, vertmap, centers, extents, w_inside=1.0):
+    """The VERTEX_REG_3D branch of _generate_vertex_targets (minibatch.py:595-600, _scale_vertmap :605-616): im_label [B,H,W] int32,
+    vertmap [B,H,W,3] f32 (each pixel's object coordinate, metres in the model frame), centers [B,C,3] f32 (only z > 0 is read: the
+    class is listed in the frame), extents [C,3] f32.  A pixel of a listed class c in 1..C-1 gets (vertmap - vmin) / (vmax - vmin)
+    per axis in channels 3c..3c+2 (the reference's float32 a * v + b) and weight w_inside there.  Returns (vertex_targets,
+    vertex_weights) [B,H,W,3C] f32."""
+    lab, vm, cen, ext = _coord_inputs(im_label, vertmap, centers, extents)
+    B, H, W = lab.shape
+    C = cen.shape[1]
+    targets = torch.empty((B, H, W, 3 * C), dtype=torch.float32, device=lab.device)
+    weights = torch.empty_like(targets)
+    check(lib().pcnn_vertex_targets_3d_fwd(ptr(lab), ptr(vm), ptr(cen), ptr(ext), B, H, W, C, f32(w_inside), ptr(targets), ptr(weights),
+                                           stream()))
+    return targets, weights
+
+
 def generate_vertex_targets_instances(im_label, mask, instances, num_classes, w_inside=1.0):
     """Multi-instance branch of _generate_vertex_targets (minibatch.py:549-573): im_label / mask [B,H,W] int32 (instance
     mask image), instances [B,I,5] f32 = (cls, mask id = cls_indexes_old + 1, cx, cy, z), z <= 0 = unused slot."""
@@ -111,4 +139,33 @@ def vertex_loss_from_centers(vertex_pred, im_label, centers, w_inside=1.0, sigma
     ws = _workspace(p.device)
     check(lib().pcnn_vertex_loss_fused_fwd(ptr(p), ptr(lab), ptr(cen), B, H, W, C, f32(w_inside), f32(sigma), ptr(out), f32(upstream),
                                            ptr(grad), ptr(ws), ctypes.c_size_t(ws.numel()), stream()))
+    return (out[0:1], out[1:2], grad) if want_grad else (out[0:1], out[1:2])
+
+
+def vertex_loss_from_coords(vertex_pred, im_label, vertmap, centers, extents, w_inside=1.0, sigma=1.0, want_grad=False, upstream=1.0,
+                            bias_vertex=None):
+    """smooth_l1_loss_vertex(vertex_pred, *generate_vertex_targets_3d(im_label, vertmap, centers, extents, w_inside)) in one pass that
+    never builds the target / weight tensors.  vertex_pred is the dense [B,H,W,3C] tensor, or with bias_vertex [3C] given, the
+    1/8-resolution head tensor [B,H/8,W/8,4C] whose vertex values are formed on demand (bit-identical; no gradient then).
+    Returns (loss [1], sum of weights [1][, grad wrt vertex_pred])."""
+    lab, vm, cen, ext = _coord_inputs(im_label, vertmap, centers, extents)
+    B, H, W = lab.shape
+    C = cen.shape[1]
+    p = require_cuda("vertex_pred", vertex_pred, torch.float32, 4)
+    out = torch.empty((2,), dtype=torch.float32, device=p.device)
+    ws = _workspace(p.device)
+    if bias_vertex is not None:
+        if want_grad:
+            raise ValueError("the low-resolution source has no gradient output")
+        bv = require_cuda("bias_vertex", bias_vertex, torch.float32, 1)
+        if tuple(p.shape) != (B, H // 8, W // 8, 4 * C) or bv.numel() != 3 * C:
+            raise ValueError("the low-resolution source must be [B,H/8,W/8,4C] with a [3C] bias")
+        check(lib().pcnn_vertex_loss_coord_lowres_fwd(ptr(p), ptr(bv), ptr(lab), ptr(vm), ptr(cen), ptr(ext), B, H, W, C, f32(w_inside),
+                                                      f32(sigma), ptr(out), ptr(ws), ctypes.c_size_t(ws.numel()), stream()))
+        return out[0:1], out[1:2]
+    if tuple(p.shape) != (B, H, W, 3 * C):
+        raise ValueError("vertex_pred must be [B,H,W,3C]")
+    grad = torch.empty_like(p) if want_grad else None
+    check(lib().pcnn_vertex_loss_coord_fwd(ptr(p), ptr(lab), ptr(vm), ptr(cen), ptr(ext), B, H, W, C, f32(w_inside), f32(sigma), ptr(out),
+                                           f32(upstream), ptr(grad), ptr(ws), ctypes.c_size_t(ws.numel()), stream()))
     return (out[0:1], out[1:2], grad) if want_grad else (out[0:1], out[1:2])
