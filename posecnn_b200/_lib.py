@@ -1,5 +1,10 @@
 """ctypes binding of libposecnn_b200.so (include/posecnn_b200.h).
 
+The Python side binds from the header: when the library is loaded, every `pcnn_*` prototype of include/posecnn_b200.h
+sets the `argtypes` / `restype` of its entry point, so a call with the wrong number of arguments, or a tensor where a pointer
+belongs, raises in Python before C is entered, and plain Python numbers reach C as the declared int / float / size_t.
+Pointers travel as ints (`ptr(t)`, `stream()`); ctypes values (c_void_p, c_float, c_size_t, byref, host arrays) are accepted too.
+
 There is NO fallback: if the shared object is missing or a call fails, the ops raise.
 PyTorch is used only for device memory and streams.
 """
@@ -7,15 +12,43 @@ from __future__ import annotations
 
 import ctypes
 import os
+import re
 
 import torch
 
-from .build import LIB
+from .build import HEADER, LIB
 
 _lib = None
 _ws = {}
 
-c_fp = ctypes.c_void_p  # device pointers travel as void*
+_SCALARS = {"int": ctypes.c_int, "float": ctypes.c_float, "double": ctypes.c_double, "size_t": ctypes.c_size_t,
+            "int8_t": ctypes.c_int8, "uint8_t": ctypes.c_uint8, "int16_t": ctypes.c_int16, "uint16_t": ctypes.c_uint16,
+            "int32_t": ctypes.c_int32, "uint32_t": ctypes.c_uint32, "int64_t": ctypes.c_int64, "uint64_t": ctypes.c_uint64}
+_RETURNS = {"int": ctypes.c_int, "const char*": ctypes.c_char_p}
+
+
+def prototypes(text: str) -> dict:
+    """{name: (restype, [argtypes])} for every `pcnn_*` prototype of a C header; any pointer is c_void_p.  A return or
+    parameter type outside the table raises, naming the function, so no entry point is ever bound in a wrong way."""
+    text = re.sub(r"/\*.*?\*/|//[^\n]*", " ", text, flags=re.S)
+    text = re.sub(r"^[ \t]*#[^\n]*", " ", text, flags=re.M)          # preprocessor lines
+    protos = {}
+    for ret, name, params in re.findall(r"([^;{}]*?)\b(pcnn_\w+)\s*\(([^)]*)\)\s*;", text):
+        ret = re.sub(r"\s*\*", "*", " ".join(ret.split()))
+        if ret not in _RETURNS:
+            raise TypeError(f"{name}: return type {ret!r} has no ctypes binding")
+        argtypes = []
+        for p in params.split(","):
+            p = " ".join(p.split())
+            if "*" in p:
+                argtypes.append(ctypes.c_void_p)
+            elif p not in ("", "void"):
+                t = re.sub(r"^const ", "", p).rsplit(" ", 1)[0]
+                if t not in _SCALARS:
+                    raise TypeError(f"{name}: parameter {p!r} has no ctypes binding")
+                argtypes.append(_SCALARS[t])
+        protos[name] = (_RETURNS[ret], argtypes)
+    return protos
 
 
 def lib():
@@ -25,8 +58,12 @@ def lib():
             raise RuntimeError(
                 f"{LIB} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
                 "(posecnn_b200 has no CPU or PyTorch fallback)")
-        _lib = ctypes.CDLL(LIB)
-        _lib.pcnn_last_error.restype = ctypes.c_char_p
+        handle = ctypes.CDLL(LIB)
+        with open(HEADER) as f:
+            for name, (restype, argtypes) in prototypes(f.read()).items():
+                fn = getattr(handle, name)
+                fn.restype, fn.argtypes = restype, argtypes
+        _lib = handle
     return _lib
 
 
@@ -36,16 +73,16 @@ def check(rc: int):
 
 
 def ptr(t):
-    if t is None:
-        return c_fp(0)
-    return c_fp(t.data_ptr())
+    return None if t is None else t.data_ptr()
 
 
 def stream():
-    return c_fp(torch.cuda.current_stream().cuda_stream)
+    return torch.cuda.current_stream().cuda_stream
 
 
 def f32(x: float):
+    """A float argument as ctypes.c_float.  Not needed with the header binding (a plain number converts the same way), and
+    kept so that callers written against the untyped binding keep working: the bound entry points accept it unchanged."""
     return ctypes.c_float(float(x))
 
 

@@ -11,9 +11,9 @@ import ctypes
 import torch
 
 try:
-    from .._lib import check, f32, lib, ptr, require_cuda, stream, workspace
+    from .._lib import check, lib, ptr, require_cuda, stream, workspace
 except ImportError:
-    from posecnn_b200._lib import check, f32, lib, ptr, require_cuda, stream, workspace
+    from posecnn_b200._lib import check, lib, ptr, require_cuda, stream, workspace
 
 
 def average_distance_loss(bottom_prediction, bottom_target, bottom_weight, bottom_point, bottom_symmetry, margin,
@@ -32,9 +32,8 @@ def average_distance_loss(bottom_prediction, bottom_target, bottom_weight, botto
     nbytes = ctypes.c_size_t(0)
     check(lib().pcnn_average_distance_workspace_bytes(N, ctypes.byref(nbytes)))
     ws = workspace("avgdist", nbytes.value, pred.device)
-    check(lib().pcnn_average_distance_fwd(ptr(pred), ptr(target), ptr(weight), ptr(point), ptr(symmetry), N, C, P,
-                                          f32(margin), ptr(loss), ptr(diff), ptr(ws), ctypes.c_size_t(ws.numel()),
-                                          stream()))
+    check(lib().pcnn_average_distance_fwd(ptr(pred), ptr(target), ptr(weight), ptr(point), ptr(symmetry), N, C, P, margin, ptr(loss),
+                                          ptr(diff), ptr(ws), ws.numel(), stream()))
     return loss, diff
 
 

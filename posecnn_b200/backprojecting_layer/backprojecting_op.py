@@ -10,9 +10,9 @@ from __future__ import annotations
 import torch
 
 try:
-    from .._lib import check, f32, lib, ptr, require_cuda, stream
+    from .._lib import check, lib, ptr, require_cuda, stream
 except ImportError:
-    from posecnn_b200._lib import check, f32, lib, ptr, require_cuda, stream
+    from posecnn_b200._lib import check, lib, ptr, require_cuda, stream
 
 
 def backproject(bottom_data, bottom_label, bottom_depth, bottom_meta_data, bottom_label_3d, grid_size, kernel_size,
@@ -29,9 +29,8 @@ def backproject(bottom_data, bottom_label, bottom_depth, bottom_meta_data, botto
     top_data = torch.empty((B, G, G, G, Cf), dtype=torch.float32, device=dev)
     top_label = torch.empty((B, G, G, G, C), dtype=torch.float32, device=dev)
     top_flag = torch.empty((B, G, G, G, Cf), dtype=torch.float32, device=dev)
-    check(lib().pcnn_backproject_fwd(ptr(data), ptr(label), ptr(depth), ptr(meta), ptr(label_3d), B, H, W, Cf, C,
-                                     meta.shape[-1], G, int(kernel_size), f32(threshold), ptr(top_data),
-                                     ptr(top_label), ptr(top_flag), stream()))
+    check(lib().pcnn_backproject_fwd(ptr(data), ptr(label), ptr(depth), ptr(meta), ptr(label_3d), B, H, W, Cf, C, meta.shape[-1], G,
+                                     int(kernel_size), threshold, ptr(top_data), ptr(top_label), ptr(top_flag), stream()))
     return top_data, top_label, top_flag
 
 
@@ -43,6 +42,5 @@ def backproject_grad(bottom_data, bottom_depth, bottom_meta_data, grad, grid_siz
     grad = require_cuda("grad", grad, torch.float32, 5)
     B, H, W, Cf = data.shape
     out = torch.empty_like(data)
-    check(lib().pcnn_backproject_bwd(ptr(grad), ptr(depth), ptr(meta), B, H, W, Cf, meta.shape[-1], int(grid_size),
-                                     ptr(out), stream()))
+    check(lib().pcnn_backproject_bwd(ptr(grad), ptr(depth), ptr(meta), B, H, W, Cf, meta.shape[-1], int(grid_size), ptr(out), stream()))
     return out

@@ -6,7 +6,7 @@ import ctypes
 
 import torch
 
-from ._lib import check, f32, lib, ptr, stream, workspace
+from ._lib import check, lib, ptr, stream, workspace
 
 
 def conv_wgrad(x: torch.Tensor, dz: torch.Tensor, ksize: int, scale: float = 1.0, w_master: torch.Tensor | None = None,
@@ -22,8 +22,8 @@ def conv_wgrad(x: torch.Tensor, dz: torch.Tensor, ksize: int, scale: float = 1.0
     nbytes = ctypes.c_size_t(0)
     check(lib().pcnn_conv_wgrad_workspace_bytes(B, H, W, Cin, Cout, int(ksize), ctypes.byref(nbytes)))
     ws = workspace("wgrad", nbytes.value, x.device)
-    check(lib().pcnn_conv_wgrad_bf16_tc(ptr(x), ptr(dz), B, H, W, Cin, Cout, int(ksize), f32(scale), ptr(w_master), f32(decay), ptr(out),
-                                        ptr(ws), ctypes.c_size_t(ws.numel()), stream()))
+    check(lib().pcnn_conv_wgrad_bf16_tc(ptr(x), ptr(dz), B, H, W, Cin, Cout, int(ksize), scale, ptr(w_master), decay, ptr(out),
+                                        ptr(ws), ws.numel(), stream()))
     return out
 
 
@@ -42,8 +42,8 @@ def relu_bwd(g: torch.Tensor, y: torch.Tensor | None, has_relu: bool = True, wan
     dz = torch.empty_like(g) if want_dz else None
     db = torch.empty((C,), dtype=torch.float32, device=g.device) if want_bias else None
     ws = _bias_ws(C, g.device) if want_bias else None
-    check(lib().pcnn_relu_bwd_bf16(ptr(g), ptr(y), ctypes.c_size_t(npix), C, int(bool(has_relu)), ptr(dz), f32(scale), ptr(bias), f32(decay),
-                                   ptr(db), ptr(ws), ctypes.c_size_t(ws.numel() if ws is not None else 0), stream()))
+    check(lib().pcnn_relu_bwd_bf16(ptr(g), ptr(y), npix, C, int(bool(has_relu)), ptr(dz), scale, ptr(bias), decay,
+                                   ptr(db), ptr(ws), ws.numel() if ws is not None else 0, stream()))
     return (dz, db) if want_bias else dz
 
 
@@ -56,8 +56,8 @@ def maxpool_relu_bwd(g: torch.Tensor, y: torch.Tensor, want_bias: bool = False, 
     dz = torch.empty_like(y)
     db = torch.empty((C,), dtype=torch.float32, device=g.device) if want_bias else None
     ws = _bias_ws(C, g.device) if want_bias else None
-    check(lib().pcnn_maxpool_relu_bwd_bf16(ptr(g), ptr(y), B, H, W, C, ptr(dz), f32(scale), ptr(bias), f32(decay), ptr(db), ptr(ws),
-                                           ctypes.c_size_t(ws.numel() if ws is not None else 0), stream()))
+    check(lib().pcnn_maxpool_relu_bwd_bf16(ptr(g), ptr(y), B, H, W, C, ptr(dz), scale, ptr(bias), decay, ptr(db), ptr(ws),
+                                           ws.numel() if ws is not None else 0, stream()))
     return (dz, db) if want_bias else dz
 
 
@@ -65,5 +65,5 @@ def add_to_bf16(a: torch.Tensor, b: torch.Tensor | None = None, b_f32: torch.Ten
     """a + b (+ b_f32) -> bf16 (gradient fan-in of conv4_3 / conv5_3)."""
     assert a.is_cuda and a.dtype == torch.bfloat16 and a.is_contiguous() and a.numel() % 8 == 0
     out = torch.empty_like(a)
-    check(lib().pcnn_add_to_bf16(ptr(a), ptr(b), ptr(b_f32), ctypes.c_size_t(a.numel()), ptr(out), stream()))
+    check(lib().pcnn_add_to_bf16(ptr(a), ptr(b), ptr(b_f32), a.numel(), ptr(out), stream()))
     return out

@@ -13,6 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT_DIR = os.path.join(HERE, "_build")
 LIB = os.path.join(OUT_DIR, "libposecnn_b200.so")
+HEADER = os.path.join(os.path.dirname(HERE), "include", "posecnn_b200.h")
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
@@ -35,8 +36,7 @@ def needs_build() -> bool:
     if not os.path.exists(LIB):
         return True
     t = os.path.getmtime(LIB)
-    deps = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(HERE, "..", "include", "posecnn_b200.h"),
-                                                                  os.path.abspath(__file__)]  # the flags live here
+    deps = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [HEADER, os.path.abspath(__file__)]  # the flags live here
     return any(os.path.getmtime(d) > t for d in deps)
 
 

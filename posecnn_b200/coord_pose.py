@@ -12,7 +12,7 @@ import ctypes
 import numpy as np
 import torch
 
-from ._lib import check, f32, lib, ptr, require_cuda, stream, workspace
+from ._lib import check, lib, ptr, require_cuda, stream, workspace
 
 NUM_HYPOTHESES = 256
 NUM_ROUNDS = 8
@@ -62,9 +62,8 @@ def estimate_poses_3d(label, depth, meta_data, extents, keys, vertex=None, lowre
     nbytes = ctypes.c_size_t(0)
     check(lib().pcnn_coord_pose3d_workspace_bytes(B, H, W, C, ctypes.byref(nbytes)))
     ws = workspace("coord_pose3d", nbytes.value, dev)
-    check(lib().pcnn_coord_pose3d_fwd(ptr(lab), ptr(v), ptr(lr), ptr(bv), ptr(dep), ptr(meta), meta.shape[1], ptr(ext), ptr(k), B, H,
-                                      W, C, f32(factor_depth), ptr(poses), ptr(info), ptr(th), ptr(tr), ptr(ws),
-                                      ctypes.c_size_t(ws.numel()), stream()))
+    check(lib().pcnn_coord_pose3d_fwd(ptr(lab), ptr(v), ptr(lr), ptr(bv), ptr(dep), ptr(meta), meta.shape[1], ptr(ext), ptr(k), B, H, W, C,
+                                      factor_depth, ptr(poses), ptr(info), ptr(th), ptr(tr), ptr(ws), ws.numel(), stream()))
     out = {"poses": poses, "info": info}
     if trace:
         out["trace_hyp"], out["trace_round"] = th, tr
@@ -86,7 +85,7 @@ def assemble_records(poses, extents, meta_data, im_scale=1.0, batch_offset=0):
     rois = torch.empty((B * (C - 1), 6), dtype=torch.float32, device=dev)
     out = torch.empty((B * (C - 1), 7), dtype=torch.float32, device=dev)
     num = torch.empty((1,), dtype=torch.int32, device=dev)
-    check(lib().pcnn_coord_pose3d_records(ptr(p), ptr(ext), ptr(meta), meta.shape[1], B, C, int(batch_offset), f32(im_scale), ptr(rois),
+    check(lib().pcnn_coord_pose3d_records(ptr(p), ptr(ext), ptr(meta), meta.shape[1], B, C, int(batch_offset), im_scale, ptr(rois),
                                           ptr(out), ptr(num), stream()))
     return rois, out, num
 

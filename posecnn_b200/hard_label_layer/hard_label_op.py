@@ -9,9 +9,9 @@ from __future__ import annotations
 import torch
 
 try:
-    from .._lib import check, f32, lib, ptr, require_cuda, stream
+    from .._lib import check, lib, ptr, require_cuda, stream
 except ImportError:
-    from posecnn_b200._lib import check, f32, lib, ptr, require_cuda, stream
+    from posecnn_b200._lib import check, lib, ptr, require_cuda, stream
 
 
 def hard_label(bottom_prob, bottom_gt, threshold, name=None):
@@ -21,7 +21,7 @@ def hard_label(bottom_prob, bottom_gt, threshold, name=None):
     if tuple(gt.shape) != (B, H, W):
         raise ValueError("bottom_gt must be [B,H,W] matching bottom_prob")
     top = torch.empty_like(prob)
-    check(lib().pcnn_hard_label_fwd(ptr(prob), ptr(gt), B, H, W, C, f32(threshold), ptr(top), stream()))
+    check(lib().pcnn_hard_label_fwd(ptr(prob), ptr(gt), B, H, W, C, threshold, ptr(top), stream()))
     return top
 
 

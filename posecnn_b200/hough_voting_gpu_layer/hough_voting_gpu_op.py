@@ -13,9 +13,9 @@ import ctypes
 import torch
 
 try:
-    from .._lib import check, f32, lib, ptr, require_cuda, stream, workspace
+    from .._lib import check, lib, ptr, require_cuda, stream, workspace
 except ImportError:  # posecnn_b200/ itself on sys.path (reference-style imports)
-    from posecnn_b200._lib import check, f32, lib, ptr, require_cuda, stream, workspace
+    from posecnn_b200._lib import check, lib, ptr, require_cuda, stream, workspace
 
 MAX_ROWS = 128 * 9          # hough_voting_gpu_op.cc:94
 INLIER_THRESHOLD = 0.9      # hough_voting_gpu_op.cc:356
@@ -71,14 +71,12 @@ def hough_voting_gpu_capacity(bottom_label, bottom_vertex, bottom_extents, botto
     num_rois = torch.empty((1,), dtype=torch.int32, device=dev)
     status = torch.empty((4,), dtype=torch.int32, device=dev)
     nbytes = ctypes.c_size_t(0)
-    check(lib().pcnn_hough_vote_workspace_bytes(B, H, W, C, int(skip_pixels), f32(threshold_vote), ctypes.byref(nbytes)))
+    check(lib().pcnn_hough_vote_workspace_bytes(B, H, W, C, int(skip_pixels), threshold_vote, ctypes.byref(nbytes)))
     ws = workspace("hough", nbytes.value, dev)
-    check(lib().pcnn_hough_vote_fwd_ex(
-        ptr(label), ptr(vertex), ptr(lowres), ptr(bias_vertex), ptr(extents), ptr(meta), ptr(gt), B, bg, int(batch_offset),
-        H, W, C, num_gt, num_meta, int(is_train),
-        f32(inlier_threshold), int(label_threshold), f32(threshold_vote), f32(threshold_percentage), int(skip_pixels),
-        ptr(box), ptr(pose), ptr(target), ptr(weight), ptr(domain), ptr(num_rois), ptr(status), ptr(ws),
-        ctypes.c_size_t(ws.numel()), stream()))
+    check(lib().pcnn_hough_vote_fwd_ex(ptr(label), ptr(vertex), ptr(lowres), ptr(bias_vertex), ptr(extents), ptr(meta), ptr(gt), B, bg,
+                                       int(batch_offset), H, W, C, num_gt, num_meta, int(is_train), inlier_threshold, int(label_threshold),
+                                       threshold_vote, threshold_percentage, int(skip_pixels), ptr(box), ptr(pose), ptr(target),
+                                       ptr(weight), ptr(domain), ptr(num_rois), ptr(status), ptr(ws), ws.numel(), stream()))
     return box, pose, target, weight, domain, num_rois, status
 
 
@@ -133,9 +131,8 @@ def hough_vote_planes(bottom_label, bottom_vertex, bottom_extents, bottom_meta_d
     C = vertex.shape[3] // 3
     votes = torch.empty((B, C, H, W), dtype=torch.float32, device=label.device)
     nbytes = ctypes.c_size_t(0)
-    check(lib().pcnn_hough_vote_workspace_bytes(B, H, W, C, int(skip_pixels), f32(-1.0), ctypes.byref(nbytes)))
+    check(lib().pcnn_hough_vote_workspace_bytes(B, H, W, C, int(skip_pixels), -1.0, ctypes.byref(nbytes)))
     ws = workspace("hough", nbytes.value, label.device)
-    check(lib().pcnn_hough_vote_planes(ptr(label), ptr(vertex), ptr(extents), ptr(meta), B, H, W, C, meta.shape[-1],
-                                       f32(inlier_threshold), int(label_threshold), int(skip_pixels), ptr(votes),
-                                       ptr(ws), ctypes.c_size_t(ws.numel()), stream()))
+    check(lib().pcnn_hough_vote_planes(ptr(label), ptr(vertex), ptr(extents), ptr(meta), B, H, W, C, meta.shape[-1], inlier_threshold,
+                                       int(label_threshold), int(skip_pixels), ptr(votes), ptr(ws), ws.numel(), stream()))
     return votes

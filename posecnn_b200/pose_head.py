@@ -7,7 +7,7 @@ import ctypes
 
 import torch
 
-from ._lib import check, f32, lib, ptr, stream, workspace
+from ._lib import check, lib, ptr, stream, workspace
 
 
 def fc_weights_to_tc(w_in_out: torch.Tensor, dtype=torch.float16) -> torch.Tensor:
@@ -30,7 +30,7 @@ def roi_pool_pair(f5: torch.Tensor, f4: torch.Tensor, rois: torch.Tensor, pooled
     n = rois.shape[0]
     out = torch.empty((n, pooled_h * pooled_w * C), dtype=torch.float16, device=f5.device)
     check(lib().pcnn_roi_pool_pair_f16(ptr(f5), H5, W5, ptr(f4), H4, W4, C, B, int(batch_offset), ptr(rois), n, rois.shape[1],
-                                        int(pooled_h), int(pooled_w), f32(scale5), f32(scale4), ptr(out), stream()))
+                                        int(pooled_h), int(pooled_w), scale5, scale4, ptr(out), stream()))
     return out
 
 
@@ -49,12 +49,10 @@ def fc(a: torch.Tensor, w_tc: torch.Tensor, bias: torch.Tensor, act: str = "relu
     code = {"none": 0, "relu": 1, "tanh": 2}[act]
     if out_dtype == torch.float16:
         out = torch.empty((M, N), dtype=torch.float16, device=a.device)
-        check(lib().pcnn_fc_f16_tc(ptr(a), ptr(w_tc), ptr(bias), M, N, K, nv, code, ptr(out), N, ptr(None), ptr(ws),
-                                    ctypes.c_size_t(ws.numel()), stream()))
+        check(lib().pcnn_fc_f16_tc(ptr(a), ptr(w_tc), ptr(bias), M, N, K, nv, code, ptr(out), N, ptr(None), ptr(ws), ws.numel(), stream()))
     else:
         out = torch.empty((M, nv), dtype=torch.float32, device=a.device)
-        check(lib().pcnn_fc_f16_tc(ptr(a), ptr(w_tc), ptr(bias), M, N, K, nv, code, ptr(None), 0, ptr(out), ptr(ws),
-                                    ctypes.c_size_t(ws.numel()), stream()))
+        check(lib().pcnn_fc_f16_tc(ptr(a), ptr(w_tc), ptr(bias), M, N, K, nv, code, ptr(None), 0, ptr(out), ptr(ws), ws.numel(), stream()))
     return out
 
 
@@ -78,7 +76,7 @@ def domain_tail(h9: torch.Tensor, w10: torch.Tensor, b10: torch.Tensor, label_do
                    dw10=torch.empty((2, 256), dtype=torch.float32, device=dev), db10=torch.empty((2,), dtype=torch.float32, device=dev),
                    db9=torch.empty((256,), dtype=torch.float32, device=dev), dpre9=torch.empty((rows, ld), dtype=torch.float16, device=dev))
     g = lambda k: ptr(out.get(k))
-    check(lib().pcnn_domain_tail(ptr(h9), rows, ld, ptr(w10), ptr(b10), ptr(label_domain), f32(loss_scale), f32(grad_scale),
+    check(lib().pcnn_domain_tail(ptr(h9), rows, ld, ptr(w10), ptr(b10), ptr(label_domain), loss_scale, grad_scale,
                                  g("domain_score"), g("domain_prob"), g("domain_label"), g("loss"), g("amax"), g("dw10"), g("db10"),
                                  g("db9"), g("dpre9"), stream()))
     return out
@@ -90,5 +88,5 @@ def domain_grad_merge(a: torch.Tensor, scale_a: float, b: torch.Tensor, scale_b:
     assert a.dtype == b.dtype == torch.float16 and a.is_contiguous() and b.is_contiguous() and a.numel() == b.numel()
     out = torch.empty(shape, dtype=torch.float32, device=a.device)
     assert out.numel() == a.numel()
-    check(lib().pcnn_domain_grad_merge(ptr(a), f32(scale_a), ptr(b), f32(scale_b), ctypes.c_size_t(a.numel()), ptr(out), stream()))
+    check(lib().pcnn_domain_grad_merge(ptr(a), scale_a, ptr(b), scale_b, a.numel(), ptr(out), stream()))
     return out

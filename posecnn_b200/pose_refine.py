@@ -12,7 +12,7 @@ import ctypes
 import numpy as np
 import torch
 
-from ._lib import check, f32, lib, ptr, require_cuda, stream, workspace
+from ._lib import check, lib, ptr, require_cuda, stream, workspace
 from .utils.results import ICP_ERROR_THRESHOLD, ZFAR, ZNEAR
 
 NUM_HYPOTHESES = 8
@@ -49,10 +49,9 @@ def refine_poses(label, depth, meta_data, rois, poses, points, num_rows=None, fa
     nbytes = ctypes.c_size_t(0)
     check(lib().pcnn_pose_refine_workspace_bytes(B, max(C, 2), ctypes.byref(nbytes)))
     ws = workspace("pose_refine", nbytes.value, dev)
-    check(lib().pcnn_pose_refine_fwd(ptr(lab), ptr(dep), ptr(meta), meta.shape[1], ptr(r), ptr(p), ptr(nr), cap, ptr(pts), C, P, B, H,
-                                     W, int(batch_offset), f32(factor_depth), f32(znear), f32(zfar), f32(max_error), int(min_pixels),
-                                     int(iterations), ptr(out_r), ptr(out_i), ptr(info), ptr(tr), ptr(ws), ctypes.c_size_t(ws.numel()),
-                                     stream()))
+    check(lib().pcnn_pose_refine_fwd(ptr(lab), ptr(dep), ptr(meta), meta.shape[1], ptr(r), ptr(p), ptr(nr), cap, ptr(pts), C, P, B, H, W,
+                                     int(batch_offset), factor_depth, znear, zfar, max_error, int(min_pixels), int(iterations), ptr(out_r),
+                                     ptr(out_i), ptr(info), ptr(tr), ptr(ws), ws.numel(), stream()))
     out = {"poses_refined": out_r, "poses_icp": out_i, "icp_info": info}
     if tr is not None:
         out["icp_trace"] = tr

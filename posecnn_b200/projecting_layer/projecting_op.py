@@ -8,9 +8,9 @@ from __future__ import annotations
 import torch
 
 try:
-    from .._lib import check, f32, lib, ptr, require_cuda, stream
+    from .._lib import check, lib, ptr, require_cuda, stream
 except ImportError:
-    from posecnn_b200._lib import check, f32, lib, ptr, require_cuda, stream
+    from posecnn_b200._lib import check, lib, ptr, require_cuda, stream
 
 
 def project(bottom_data, bottom_depth, bottom_meta_data, kernel_size, threshold, name=None):
@@ -35,5 +35,5 @@ def project_grad(bottom_data, bottom_depth, bottom_meta_data, grad, kernel_size,
     H, W = depth.shape[1], depth.shape[2]
     out = torch.empty_like(data)
     check(lib().pcnn_project_bwd(ptr(grad), ptr(depth), ptr(meta), B, H, W, Cf, meta.shape[-1], G, int(kernel_size),
-                                 f32(threshold), ptr(out), stream()))
+                                 threshold, ptr(out), stream()))
     return out

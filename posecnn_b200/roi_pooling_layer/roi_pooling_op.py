@@ -9,9 +9,9 @@ from __future__ import annotations
 import torch
 
 try:
-    from .._lib import check, f32, lib, ptr, require_cuda, stream
+    from .._lib import check, lib, ptr, require_cuda, stream
 except ImportError:
-    from posecnn_b200._lib import check, f32, lib, ptr, require_cuda, stream
+    from posecnn_b200._lib import check, lib, ptr, require_cuda, stream
 
 
 def roi_pool(bottom_data, bottom_rois, pooled_height, pooled_width, spatial_scale, pool_channel=0, name=None):
@@ -24,7 +24,7 @@ def roi_pool(bottom_data, bottom_rois, pooled_height, pooled_width, spatial_scal
         top = torch.empty((N, pooled_height, pooled_width, C), dtype=torch.float32, device=data.device)
         argmax = torch.empty((N, pooled_height, pooled_width, C), dtype=torch.int32, device=data.device)
         check(lib().pcnn_roi_pool_fwd_bf16(ptr(data), ptr(rois), N, cr, B, H, W, C, int(pooled_height), int(pooled_width),
-                                           f32(spatial_scale), ptr(top), ptr(argmax), stream()))
+                                           spatial_scale, ptr(top), ptr(argmax), stream()))
         return top, argmax
     data = require_cuda("bottom_data", bottom_data, torch.float32, 4)   # roi_pooling_op.cc:297-298
     rois = require_cuda("bottom_rois", bottom_rois, torch.float32, 2)   # roi_pooling_op.cc:301-302
@@ -34,7 +34,7 @@ def roi_pool(bottom_data, bottom_rois, pooled_height, pooled_width, spatial_scal
     top = torch.empty((N, pooled_height, pooled_width, co), dtype=torch.float32, device=data.device)
     argmax = torch.empty((N, pooled_height, pooled_width, co), dtype=torch.int32, device=data.device)
     check(lib().pcnn_roi_pool_fwd(ptr(data), ptr(rois), N, cr, B, H, W, C, int(pooled_height), int(pooled_width),
-                                  f32(spatial_scale), int(pool_channel), ptr(top), ptr(argmax), stream()))
+                                  spatial_scale, int(pool_channel), ptr(top), ptr(argmax), stream()))
     return top, argmax
 
 
@@ -51,5 +51,5 @@ def roi_pool_grad(bottom_data, bottom_rois, argmax, grad, pooled_height, pooled_
     N, cr = rois.shape
     out = torch.empty((B, H, W, C), dtype=torch.float32, device=bottom_data.device)
     check(lib().pcnn_roi_pool_bwd(ptr(grad), ptr(argmax), ptr(rois), B, N, cr, H, W, C, int(pooled_height),
-                                  int(pooled_width), f32(spatial_scale), int(pool_channel), ptr(out), stream()))
+                                  int(pooled_width), spatial_scale, int(pool_channel), ptr(out), stream()))
     return out

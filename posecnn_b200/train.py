@@ -45,7 +45,7 @@ import torch.distributed as dist
 
 from . import backward as bw
 from . import conv, pose_head, train_ops
-from ._lib import check, f32, lib, ptr, stream, workspace
+from ._lib import check, lib, ptr, stream, workspace
 from .average_distance_loss import average_distance_loss_op
 from .hough_voting_gpu_layer import hough_voting_gpu_op
 from .networks.vgg16_convs import PIXEL_MEANS, VGG_CFG
@@ -276,17 +276,17 @@ class Trainer:
         # losses on the dense heads (fused kernels; the masks / targets are never materialised)
         ws = train_ops._workspace(data.device)
         cls_out = torch.empty((2,), dtype=torch.float32, device=data.device)
-        check(lib().pcnn_loss_cls_hard_raw_fwd(ptr(score), ptr(prob), ptr(gt_label_2d), B, H, W, C, f32(net.threshold_label), ptr(cls_out), ptr(ws),
-                                               ctypes.c_size_t(ws.numel()), stream()))
+        check(lib().pcnn_loss_cls_hard_raw_fwd(ptr(score), ptr(prob), ptr(gt_label_2d), B, H, W, C, net.threshold_label, ptr(cls_out), ptr(ws),
+                                               ws.numel(), stream()))
         vtx_out = torch.empty((2,), dtype=torch.float32, device=data.device)
         if self.coord:
             check(lib().pcnn_vertex_loss_coord_lowres_fwd(ptr(lowres), ptr(M["vertex_pred/b"]), ptr(gt_label_2d), ptr(vertmap), ptr(centers),
-                                                          ptr(extents), B, H, W, C, f32(self.w_inside), f32(1.0), ptr(vtx_out), ptr(ws),
-                                                          ctypes.c_size_t(ws.numel()), stream()))
+                                                          ptr(extents), B, H, W, C, self.w_inside, 1.0, ptr(vtx_out), ptr(ws),
+                                                          ws.numel(), stream()))
             A.update(extents=extents)
         else:
             check(lib().pcnn_vertex_loss_fused_lowres_fwd(ptr(lowres), ptr(M["vertex_pred/b"]), ptr(gt_label_2d), ptr(centers), B, H, W, C,
-                                                          f32(self.w_inside), f32(1.0), ptr(vtx_out), ptr(ws), ctypes.c_size_t(ws.numel()), stream()))
+                                                          self.w_inside, 1.0, ptr(vtx_out), ptr(ws), ws.numel(), stream()))
         A.update(cls_out=cls_out, vtx_out=vtx_out, data=data)
         if not self.pose_reg:
             return A
@@ -350,7 +350,7 @@ class Trainer:
         nbytes = ctypes.c_size_t(0)
         check(lib().pcnn_fc_workspace_bytes(M_, N, K, ctypes.byref(nbytes)))
         ws = workspace("fc", nbytes.value, dy.device)
-        check(lib().pcnn_fc_dgrad_f16_tc(ptr(dy), ptr(wt), M_, N, K, ptr(mask), ptr(out), N, ptr(ws), ctypes.c_size_t(ws.numel()), stream()))
+        check(lib().pcnn_fc_dgrad_f16_tc(ptr(dy), ptr(wt), M_, N, K, ptr(mask), ptr(out), N, ptr(ws), ws.numel(), stream()))
         return out
 
     def _fc_wgrad(self, x, dy, scale=1.0):
@@ -360,8 +360,7 @@ class Trainer:
         nbytes = ctypes.c_size_t(0)
         check(lib().pcnn_conv_wgrad_workspace_bytes(1, 1, rows, Cin, Cout, 1, ctypes.byref(nbytes)))
         ws = workspace("wgrad", nbytes.value, x.device)
-        check(lib().pcnn_fc_wgrad_f16_tc(ptr(x), ptr(dy), rows, Cin, Cout, f32(scale), ptr(None), f32(0.0), ptr(out), ptr(ws),
-                                         ctypes.c_size_t(ws.numel()), stream()))
+        check(lib().pcnn_fc_wgrad_f16_tc(ptr(x), ptr(dy), rows, Cin, Cout, scale, ptr(None), 0.0, ptr(out), ptr(ws), ws.numel(), stream()))
         return out
 
     def backward(self, A, gt_label_2d, centers, vertmap=None):
@@ -393,16 +392,15 @@ class Trainer:
         ws = workspace("up8_bwd", 4 * B * ((w + 3) // 4) * ((h + 15) // 16) * 4 * C, dev)
         if self.coord:
             vm = self._require_vertmap(vertmap, data)
-            check(lib().pcnn_up8_heads_bwd_coord(ptr(A["prob_normalized"]), ptr(A["score"]), ptr(gt_label_2d), ptr(A["cls_out"]), f32(1.0),
-                                                 f32(net.threshold_label), ptr(None), ptr(A["lowres"]), ptr(M["vertex_pred/b"]), ptr(vm),
-                                                 ptr(centers), ptr(A["extents"]), ptr(A["vtx_out"]), f32(self.vertex_w), f32(self.w_inside),
-                                                 f32(1.0), B, h, w, C, 64, 128, ptr(d_sc), ptr(d_vt), ptr(dbias), ptr(ws),
-                                                 ctypes.c_size_t(ws.numel()), stream()))
+            check(lib().pcnn_up8_heads_bwd_coord(ptr(A["prob_normalized"]), ptr(A["score"]), ptr(gt_label_2d), ptr(A["cls_out"]), 1.0,
+                                                 net.threshold_label, ptr(None), ptr(A["lowres"]), ptr(M["vertex_pred/b"]), ptr(vm),
+                                                 ptr(centers), ptr(A["extents"]), ptr(A["vtx_out"]), self.vertex_w, self.w_inside, 1.0, B,
+                                                 h, w, C, 64, 128, ptr(d_sc), ptr(d_vt), ptr(dbias), ptr(ws), ws.numel(), stream()))
         else:
-            check(lib().pcnn_up8_heads_bwd_ex(ptr(A["prob_normalized"]), ptr(A["score"]), ptr(gt_label_2d), ptr(A["cls_out"]), f32(1.0),
-                                              f32(net.threshold_label), ptr(None), ptr(A["lowres"]), ptr(M["vertex_pred/b"]), ptr(centers),
-                                              ptr(A["vtx_out"]), f32(self.vertex_w), f32(self.w_inside), f32(1.0), B, h, w, C, 64, 128, ptr(d_sc),
-                                              ptr(d_vt), ptr(dbias), ptr(ws), ctypes.c_size_t(ws.numel()), stream()))
+            check(lib().pcnn_up8_heads_bwd_ex(ptr(A["prob_normalized"]), ptr(A["score"]), ptr(gt_label_2d), ptr(A["cls_out"]), 1.0,
+                                              net.threshold_label, ptr(None), ptr(A["lowres"]), ptr(M["vertex_pred/b"]), ptr(centers),
+                                              ptr(A["vtx_out"]), self.vertex_w, self.w_inside, 1.0, B, h, w, C, 64, 128, ptr(d_sc),
+                                              ptr(d_vt), ptr(dbias), ptr(ws), ws.numel(), stream()))
         self._emit(grads, "score/b", dbias[:C].contiguous())
         self._emit(grads, "vertex_pred/b", dbias[C:].contiguous())
         self._emit(grads, "score/w", bw.conv_wgrad(A["add_s"], d_sc, 1))
@@ -461,7 +459,7 @@ class Trainer:
         # where it leaves (weight gradients, bias sums, the RoiPool gradient); conversions saturate at +-65504.
         D = 4 * C
         dpre = torch.empty((rows, 128), dtype=torch.float16, device=dev)
-        check(lib().pcnn_pose_chain_bwd(ptr(A["pose_diff"]), ptr(A["poses_tanh"]), ptr(A["poses_weight"]), rows, D, f32(pose_scale), ptr(dpre), 128,
+        check(lib().pcnn_pose_chain_bwd(ptr(A["pose_diff"]), ptr(A["poses_tanh"]), ptr(A["poses_weight"]), rows, D, pose_scale, ptr(dpre), 128,
                                         stream()))
         # dynamic loss scale: a power of two that puts the largest element of the chain's entry point at ~2^11 (one host read; the
         # un-scaled pass above is only used for its maximum, which fp16 represents well enough even when the small elements underflow)
@@ -482,7 +480,7 @@ class Trainer:
             self._emit(grads, "fc9/w", self._fc_wgrad(A["pool"], dom["dpre9"], 1.0 / S_d))
             self._emit(grads, "fc9/b", dom["db9"])
             d9 = self._fc_dgrad(dom["dpre9"], "fc9", None)                                    # [rows, 25088], scaled by S_d
-        check(lib().pcnn_pose_chain_bwd(ptr(A["pose_diff"]), ptr(A["poses_tanh"]), ptr(A["poses_weight"]), rows, D, f32(pose_scale * S), ptr(dpre), 128,
+        check(lib().pcnn_pose_chain_bwd(ptr(A["pose_diff"]), ptr(A["poses_tanh"]), ptr(A["poses_weight"]), rows, D, pose_scale * S, ptr(dpre), 128,
                                         stream()))
         self._emit(grads, "fc8/w", self._fc_wgrad(A["fc7"], dpre, 1.0 / S))
         self._emit(grads, "fc8/b", dpre[:, :D].float().sum(0) / S)
@@ -498,7 +496,7 @@ class Trainer:
             dpool = pose_head.domain_grad_merge(dpool16, 1.0 / S, d9, -GRL_LAMBDA / S_d, (rows, 7, 7, 512))
         else:
             dpool = torch.empty((rows, 7, 7, 512), dtype=torch.float32, device=dev)
-            check(lib().pcnn_half_to_float(ptr(dpool16), ctypes.c_size_t(dpool16.numel()), f32(1.0 / S), ptr(dpool), stream()))
+            check(lib().pcnn_half_to_float(ptr(dpool16), dpool16.numel(), 1.0 / S, ptr(dpool), stream()))
         A["dpool"] = dpool                                                                      # d loss / d pool_score (kept for inspection)
         g5_roi = roi_pooling_op.roi_pool_grad(A["conv5_3"], A["rois"], A["a5"], dpool, 7, 7, 1.0 / 16.0, 0)       # fp32 dense
         g4_roi = roi_pooling_op.roi_pool_grad(A["conv4_3"], A["rois"], A["a4"], dpool, 7, 7, 1.0 / 8.0, 0)
@@ -545,8 +543,8 @@ class Trainer:
             w = self.master[name]
             assert g.shape == w.shape, (name, tuple(g.shape), tuple(w.shape))
             c16 = self.tc[name]
-            check(lib().pcnn_sgd_momentum(ptr(w), ptr(self.accum[name]), ptr(g), ctypes.c_size_t(w.numel()), f32(self.lr), f32(self.mu), f32(self.wd),
-                                          f32(1.0), ptr(c16), int(c16 is not None and c16.dtype == torch.float16), stream()))
+            check(lib().pcnn_sgd_momentum(ptr(w), ptr(self.accum[name]), ptr(g), w.numel(), self.lr, self.mu, self.wd,
+                                          1.0, ptr(c16), int(c16 is not None and c16.dtype == torch.float16), stream()))
         self._refresh_derived()
 
     def step(self, data, gt_label_2d, centers, meta_data, extents, gt_poses, points, symmetry, batch_global=None, batch_offset=0,

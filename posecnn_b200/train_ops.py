@@ -10,7 +10,7 @@ import ctypes
 
 import torch
 
-from ._lib import check, f32, lib, ptr, require_cuda, stream, workspace
+from ._lib import check, lib, ptr, require_cuda, stream, workspace
 
 def _workspace(device):
     n = ctypes.c_size_t(0)
@@ -29,7 +29,7 @@ def generate_vertex_targets(im_label, centers, w_inside=1.0):
         raise ValueError("centers must be [B,C,3]")
     targets = torch.empty((B, H, W, 3 * C), dtype=torch.float32, device=lab.device)
     weights = torch.empty_like(targets)
-    check(lib().pcnn_vertex_targets_fwd(ptr(lab), ptr(cen), B, H, W, C, f32(w_inside), ptr(targets), ptr(weights), stream()))
+    check(lib().pcnn_vertex_targets_fwd(ptr(lab), ptr(cen), B, H, W, C, w_inside, ptr(targets), ptr(weights), stream()))
     return targets, weights
 
 
@@ -56,7 +56,7 @@ def generate_vertex_targets_3d(im_label, vertmap, centers, extents, w_inside=1.0
     C = cen.shape[1]
     targets = torch.empty((B, H, W, 3 * C), dtype=torch.float32, device=lab.device)
     weights = torch.empty_like(targets)
-    check(lib().pcnn_vertex_targets_3d_fwd(ptr(lab), ptr(vm), ptr(cen), ptr(ext), B, H, W, C, f32(w_inside), ptr(targets), ptr(weights),
+    check(lib().pcnn_vertex_targets_3d_fwd(ptr(lab), ptr(vm), ptr(cen), ptr(ext), B, H, W, C, w_inside, ptr(targets), ptr(weights),
                                            stream()))
     return targets, weights
 
@@ -73,7 +73,7 @@ def generate_vertex_targets_instances(im_label, mask, instances, num_classes, w_
     C = int(num_classes)
     targets = torch.empty((B, H, W, 3 * C), dtype=torch.float32, device=lab.device)
     weights = torch.empty_like(targets)
-    check(lib().pcnn_vertex_targets_instances_fwd(ptr(lab), ptr(msk), ptr(ins), B, H, W, C, ins.shape[1], f32(w_inside), ptr(targets),
+    check(lib().pcnn_vertex_targets_instances_fwd(ptr(lab), ptr(msk), ptr(ins), B, H, W, C, ins.shape[1], w_inside, ptr(targets),
                                                   ptr(weights), stream()))
     return targets, weights
 
@@ -89,7 +89,7 @@ def pack_pose_meta(poses, cls, intrinsics, im_scale=1.0, flip_x=False):
     blob = torch.empty((B * I, 13), dtype=torch.float32, device=po.device)
     nrows = torch.empty((1,), dtype=torch.int32, device=po.device)
     meta = torch.empty((B, 1, 1, 48), dtype=torch.float32, device=po.device)
-    check(lib().pcnn_pack_pose_meta_fwd(ptr(po), ptr(cl), ptr(kk), B, I, f32(im_scale), int(bool(flip_x)), ptr(blob), ptr(nrows), ptr(meta),
+    check(lib().pcnn_pack_pose_meta_fwd(ptr(po), ptr(cl), ptr(kk), B, I, im_scale, int(bool(flip_x)), ptr(blob), ptr(nrows), ptr(meta),
                                         stream()))
     return blob, nrows, meta
 
@@ -104,8 +104,8 @@ def loss_cross_entropy_hard(scores, prob, gt_label, threshold, want_grad=False, 
     out = torch.empty((2,), dtype=torch.float32, device=sc.device)
     grad = torch.empty_like(sc) if want_grad else None
     ws = _workspace(sc.device)
-    check(lib().pcnn_loss_cls_hard_fwd(ptr(sc), ptr(pr), ptr(gt), B, H, W, C, f32(threshold), ptr(out), f32(upstream), ptr(grad),
-                                       ptr(ws), ctypes.c_size_t(ws.numel()), stream()))
+    check(lib().pcnn_loss_cls_hard_fwd(ptr(sc), ptr(pr), ptr(gt), B, H, W, C, threshold, ptr(out), upstream, ptr(grad),
+                                       ptr(ws), ws.numel(), stream()))
     return (out[0:1], out[1:2], grad) if want_grad else (out[0:1], out[1:2])
 
 
@@ -119,8 +119,8 @@ def smooth_l1_loss_vertex(vertex_pred, vertex_targets, vertex_weights, sigma=1.0
     out = torch.empty((2,), dtype=torch.float32, device=p.device)
     grad = torch.empty_like(p) if want_grad else None
     ws = _workspace(p.device)
-    check(lib().pcnn_smooth_l1_vertex_fwd(ptr(p), ptr(t), ptr(w), ctypes.c_size_t(p.numel()), f32(sigma), ptr(out), f32(upstream),
-                                          ptr(grad), ptr(ws), ctypes.c_size_t(ws.numel()), stream()))
+    check(lib().pcnn_smooth_l1_vertex_fwd(ptr(p), ptr(t), ptr(w), p.numel(), sigma, ptr(out), upstream,
+                                          ptr(grad), ptr(ws), ws.numel(), stream()))
     return (out[0:1], out[1:2], grad) if want_grad else (out[0:1], out[1:2])
 
 
@@ -137,8 +137,8 @@ def vertex_loss_from_centers(vertex_pred, im_label, centers, w_inside=1.0, sigma
     out = torch.empty((2,), dtype=torch.float32, device=p.device)
     grad = torch.empty_like(p) if want_grad else None
     ws = _workspace(p.device)
-    check(lib().pcnn_vertex_loss_fused_fwd(ptr(p), ptr(lab), ptr(cen), B, H, W, C, f32(w_inside), f32(sigma), ptr(out), f32(upstream),
-                                           ptr(grad), ptr(ws), ctypes.c_size_t(ws.numel()), stream()))
+    check(lib().pcnn_vertex_loss_fused_fwd(ptr(p), ptr(lab), ptr(cen), B, H, W, C, w_inside, sigma, ptr(out), upstream,
+                                           ptr(grad), ptr(ws), ws.numel(), stream()))
     return (out[0:1], out[1:2], grad) if want_grad else (out[0:1], out[1:2])
 
 
@@ -160,12 +160,12 @@ def vertex_loss_from_coords(vertex_pred, im_label, vertmap, centers, extents, w_
         bv = require_cuda("bias_vertex", bias_vertex, torch.float32, 1)
         if tuple(p.shape) != (B, H // 8, W // 8, 4 * C) or bv.numel() != 3 * C:
             raise ValueError("the low-resolution source must be [B,H/8,W/8,4C] with a [3C] bias")
-        check(lib().pcnn_vertex_loss_coord_lowres_fwd(ptr(p), ptr(bv), ptr(lab), ptr(vm), ptr(cen), ptr(ext), B, H, W, C, f32(w_inside),
-                                                      f32(sigma), ptr(out), ptr(ws), ctypes.c_size_t(ws.numel()), stream()))
+        check(lib().pcnn_vertex_loss_coord_lowres_fwd(ptr(p), ptr(bv), ptr(lab), ptr(vm), ptr(cen), ptr(ext), B, H, W, C, w_inside,
+                                                      sigma, ptr(out), ptr(ws), ws.numel(), stream()))
         return out[0:1], out[1:2]
     if tuple(p.shape) != (B, H, W, 3 * C):
         raise ValueError("vertex_pred must be [B,H,W,3C]")
     grad = torch.empty_like(p) if want_grad else None
-    check(lib().pcnn_vertex_loss_coord_fwd(ptr(p), ptr(lab), ptr(vm), ptr(cen), ptr(ext), B, H, W, C, f32(w_inside), f32(sigma), ptr(out),
-                                           f32(upstream), ptr(grad), ptr(ws), ctypes.c_size_t(ws.numel()), stream()))
+    check(lib().pcnn_vertex_loss_coord_fwd(ptr(p), ptr(lab), ptr(vm), ptr(cen), ptr(ext), B, H, W, C, w_inside, sigma, ptr(out),
+                                           upstream, ptr(grad), ptr(ws), ws.numel(), stream()))
     return (out[0:1], out[1:2], grad) if want_grad else (out[0:1], out[1:2])

@@ -9,9 +9,9 @@ from __future__ import annotations
 import torch
 
 try:
-    from .._lib import check, f32, lib, ptr, require_cuda, stream
+    from .._lib import check, lib, ptr, require_cuda, stream
 except ImportError:
-    from posecnn_b200._lib import check, f32, lib, ptr, require_cuda, stream
+    from posecnn_b200._lib import check, lib, ptr, require_cuda, stream
 
 
 def nms_pose_capacity(rois, poses_init, poses_pred=None, num_rois=None, thresh=0.5, per_image=True, num_classes=None):
@@ -34,7 +34,7 @@ def nms_pose_capacity(rois, poses_init, poses_pred=None, num_rois=None, thresh=0
     out_r = torch.empty_like(r)
     out_p = torch.empty_like(pi)
     nk = torch.empty((1,), dtype=torch.int32, device=r.device)
-    check(lib().pcnn_nms_pose_fwd(ptr(r), ptr(pi), ptr(pp), ptr(nr), cap, cap, C, f32(thresh), 1 if per_image else 0,
+    check(lib().pcnn_nms_pose_fwd(ptr(r), ptr(pi), ptr(pp), ptr(nr), cap, cap, C, thresh, 1 if per_image else 0,
                                   ptr(keep), ptr(out_r), ptr(out_p), ptr(nk), stream()))
     return keep, out_r, out_p, nk
 

@@ -137,7 +137,6 @@ def test_draw_params_ranges():
 
 
 def test_augment_entries_reject_bad_arguments_without_gpu(native_lib):
-    native_lib.pcnn_last_error.restype = ctypes.c_char_p
     mean = (ctypes.c_double * 3)(102.9801, 115.9465, 122.7717)
     buf = ctypes.create_string_buffer(64)                      # any non-NULL host address: the checks fail before it is read
     f = native_lib.pcnn_augment_color_fwd

@@ -105,7 +105,7 @@ def test_fc_dgrad_wgrad_and_pose_chain(cuda):
     """Fully connected backward GEMMs (fp16 operands) and the pose-loss chain against torch on the same operands."""
     import ctypes
     from posecnn_b200 import pose_head
-    from posecnn_b200._lib import check, f32, lib, ptr, stream, workspace
+    from posecnn_b200._lib import check, lib, ptr, stream, workspace
     g = torch.Generator().manual_seed(11)
     rows, Kin, Nout = 45, 4096, 256
     x = torch.relu(torch.randn(rows, Kin, generator=g)).to(torch.float16).to(cuda)          # stored output of the layer below (ReLU)
@@ -120,14 +120,14 @@ def test_fc_dgrad_wgrad_and_pose_chain(cuda):
     nbytes = ctypes.c_size_t(0)
     check(lib().pcnn_fc_workspace_bytes(rows, Kin, Nout, ctypes.byref(nbytes)))
     ws = workspace("fc", nbytes.value, cuda)
-    check(lib().pcnn_fc_dgrad_f16_tc(ptr(dy), ptr(w_t), rows, Kin, Nout, ptr(x), ptr(out), Kin, ptr(ws), ctypes.c_size_t(ws.numel()), stream()))
+    check(lib().pcnn_fc_dgrad_f16_tc(ptr(dy), ptr(w_t), rows, Kin, Nout, ptr(x), ptr(out), Kin, ptr(ws), ws.numel(), stream()))
     want = (dy.float() @ w_tc.float()) * (x.float() > 0)
     assert rel_l2(out.float(), want) < 2e-3
     # weight gradient [out][in] with a scale
     dw = torch.empty((Nout, Kin), dtype=torch.float32, device=cuda)
     check(lib().pcnn_conv_wgrad_workspace_bytes(1, 1, rows, Kin, Nout, 1, ctypes.byref(nbytes)))
     ws2 = workspace("wgrad", nbytes.value, cuda)
-    check(lib().pcnn_fc_wgrad_f16_tc(ptr(x), ptr(dy), rows, Kin, Nout, f32(0.25), ptr(None), f32(0.0), ptr(dw), ptr(ws2), ctypes.c_size_t(ws2.numel()), stream()))
+    check(lib().pcnn_fc_wgrad_f16_tc(ptr(x), ptr(dy), rows, Kin, Nout, 0.25, ptr(None), 0.0, ptr(dw), ptr(ws2), ws2.numel(), stream()))
     assert rel_l2(dw, 0.25 * dy.float().t() @ x.float()) < 1e-4
     # pose chain: d pre-activation of fc8 from d loss / d poses_pred, poses_pred = l2_normalize(tanh(pre) * weight)
     N, D = 19, 24
@@ -139,7 +139,7 @@ def test_fc_dgrad_wgrad_and_pose_chain(cuda):
     pred = mul / mul.pow(2).sum(1, keepdim=True).clamp(min=1e-12).sqrt()
     (pred * gup).sum().backward()
     dpre = torch.empty((N, 128), dtype=torch.float16, device=cuda)
-    check(lib().pcnn_pose_chain_bwd(ptr(gup), ptr(th.detach().contiguous()), ptr(wt), N, D, f32(1.0), ptr(dpre), 128, stream()))
+    check(lib().pcnn_pose_chain_bwd(ptr(gup), ptr(th.detach().contiguous()), ptr(wt), N, D, 1.0, ptr(dpre), 128, stream()))
     assert rel_l2(dpre[:, :D].float(), pre.grad) < 2e-3 and float(dpre[:, D:].float().abs().max()) == 0.0
 
 
@@ -168,8 +168,7 @@ def _up8_problem(cuda, B, h, w, C, seed):
 
 
 def _up8_bwd(P, dense, thr=0.7, up_cls=1.0, up_vtx=2.0, w_in=10.0, sigma=1.0, count=937.0, sumw=411.0):
-    import ctypes
-    from posecnn_b200._lib import check, f32, lib, ptr, stream
+    from posecnn_b200._lib import check, lib, ptr, stream
     B, h, w, C = P["B"], P["h"], P["w"], P["C"]
     dev = P["lowres"].device
     d_sc = torch.full((B, h, w, 64), 7.0, dtype=torch.bfloat16, device=dev)
@@ -177,10 +176,10 @@ def _up8_bwd(P, dense, thr=0.7, up_cls=1.0, up_vtx=2.0, w_in=10.0, sigma=1.0, co
     dbias = torch.empty((4 * C,), device=dev)
     cls_out, vtx_out = torch.tensor([0.5, count], device=dev), torch.tensor([0.25, sumw], device=dev)
     ws = torch.empty(4 * B * ((w + 3) // 4) * ((h + 15) // 16) * 4 * C, dtype=torch.uint8, device=dev)
-    check(lib().pcnn_up8_heads_bwd_ex(ptr(P["prob"]), ptr(P["score"]), ptr(P["gt"]), ptr(cls_out), f32(up_cls), f32(thr),
+    check(lib().pcnn_up8_heads_bwd_ex(ptr(P["prob"]), ptr(P["score"]), ptr(P["gt"]), ptr(cls_out), up_cls, thr,
                                       ptr(P["vertex"] if dense else None), ptr(None if dense else P["lowres"]), ptr(None if dense else P["bv"]),
-                                      ptr(P["centers"]), ptr(vtx_out), f32(up_vtx), f32(w_in), f32(sigma), B, h, w, C, 64, 128, ptr(d_sc), ptr(d_vt),
-                                      ptr(dbias), ptr(ws), ctypes.c_size_t(ws.numel()), stream()))
+                                      ptr(P["centers"]), ptr(vtx_out), up_vtx, w_in, sigma, B, h, w, C, 64, 128, ptr(d_sc), ptr(d_vt),
+                                      ptr(dbias), ptr(ws), ws.numel(), stream()))
     return d_sc, d_vt, dbias
 
 
@@ -341,7 +340,7 @@ def test_fc_wgrad_exact(cuda, name, Cin, Cout, rows):
     """pcnn_fc_wgrad_f16_tc at the fc6 / fc7 shapes with 600 ROI rows (direct mode, ten 64-row K tiles, the last ragged) and
     at Cin = 192 / 384 (one / two 64-channel B blocks), with a power-of-two scale: exact against the float64 product."""
     import ctypes
-    from posecnn_b200._lib import check, f32, lib, ptr, stream, workspace
+    from posecnn_b200._lib import check, lib, ptr, stream, workspace
     from tests.util import int_operands, wgrad_batch_for_coverage, wgrad_plan
     if rows == 0:
         rows, plan = wgrad_batch_for_coverage(1, 1, Cin, Cout, 1)
@@ -357,8 +356,7 @@ def test_fc_wgrad_exact(cuda, name, Cin, Cout, rows):
     nbytes = ctypes.c_size_t(0)
     check(lib().pcnn_conv_wgrad_workspace_bytes(1, 1, rows, Cin, Cout, 1, ctypes.byref(nbytes)))
     ws = workspace("wgrad", nbytes.value, cuda)
-    check(lib().pcnn_fc_wgrad_f16_tc(ptr(x), ptr(dy), rows, Cin, Cout, f32(0.25), ptr(None), f32(0.0), ptr(dw), ptr(ws),
-                                     ctypes.c_size_t(ws.numel()), stream()))
+    check(lib().pcnn_fc_wgrad_f16_tc(ptr(x), ptr(dy), rows, Cin, Cout, 0.25, ptr(None), 0.0, ptr(dw), ptr(ws), ws.numel(), stream()))
     want = (dy.double().t() @ x.double()).float() * 0.25
     torch.cuda.synchronize()
     bad = dw != want

@@ -67,7 +67,6 @@ def test_kabsch_and_rodrigues_closed_forms():
 def test_abi_argument_validation_without_gpu(native_lib):
     nbytes = ctypes.c_size_t(0)
     lib = native_lib
-    lib.pcnn_last_error.restype = ctypes.c_char_p
     assert lib.pcnn_coord_pose3d_workspace_bytes(2, 480, 640, 22, ctypes.byref(nbytes)) == 0 and nbytes.value > 0
     assert lib.pcnn_coord_pose3d_workspace_bytes(2, 480, 640, 1, ctypes.byref(nbytes)) == -1
     assert b"C = 1" in lib.pcnn_last_error()
@@ -75,15 +74,14 @@ def test_abi_argument_validation_without_gpu(native_lib):
     assert lib.pcnn_coord_pose3d_workspace_bytes(2, 480, 640, 22, None) == -1
     p = ctypes.c_void_p(16)
     args = lambda **kw: dict(dict(label=p, vertex=p, lowres=None, bias=None, depth=p, meta=p, num_meta=48, ext=p, keys=p, B=1, H=480,
-                                  W=640, C=22, factor=ctypes.c_float(10000.0), poses=p, info=p, th=None, tr=None, ws=p,
-                                  nbytes=ctypes.c_size_t(1 << 40), stream=None), **kw)
+                                  W=640, C=22, factor=10000.0, poses=p, info=p, th=None, tr=None, ws=p, nbytes=1 << 40, stream=None), **kw)
     call = lambda a: lib.pcnn_coord_pose3d_fwd(*a.values())
     assert call(args(label=None)) == -1
     assert call(args(vertex=None)) == -1 and b"lowres" in lib.pcnn_last_error()
     assert call(args(vertex=None, lowres=p, bias=p, H=481)) == -1 and b"multiples of 8" in lib.pcnn_last_error()
     assert call(args(num_meta=5)) == -1
-    assert call(args(factor=ctypes.c_float(0.0))) == -1
-    assert call(args(nbytes=ctypes.c_size_t(16))) == -1 and b"workspace" in lib.pcnn_last_error()
+    assert call(args(factor=0.0)) == -1
+    assert call(args(nbytes=16)) == -1 and b"workspace" in lib.pcnn_last_error()
 
 
 def golden_record_cases():

@@ -26,16 +26,15 @@ def test_abi_exports_every_declared_symbol(native_lib):
 def test_abi_argument_validation_without_gpu(native_lib):
     # validation happens before any CUDA call, so these are safe on a CPU-only box
     nbytes = ctypes.c_size_t(0)
-    assert native_lib.pcnn_hough_vote_workspace_bytes(1, 480, 640, 22, 10, ctypes.c_float(-1.0), ctypes.byref(nbytes)) == 0
+    assert native_lib.pcnn_hough_vote_workspace_bytes(1, 480, 640, 22, 10, -1.0, ctypes.byref(nbytes)) == 0
     assert nbytes.value > 0
     small = nbytes.value
-    assert native_lib.pcnn_hough_vote_workspace_bytes(32, 480, 640, 22, 10, ctypes.c_float(-1.0), ctypes.byref(nbytes)) == 0
+    assert native_lib.pcnn_hough_vote_workspace_bytes(32, 480, 640, 22, 10, -1.0, ctypes.byref(nbytes)) == 0
     assert nbytes.value > small
-    assert native_lib.pcnn_hough_vote_workspace_bytes(1, 480, 640, 1, 10, ctypes.c_float(-1.0), ctypes.byref(nbytes)) == -1
-    native_lib.pcnn_last_error.restype = ctypes.c_char_p
+    assert native_lib.pcnn_hough_vote_workspace_bytes(1, 480, 640, 1, 10, -1.0, ctypes.byref(nbytes)) == -1
     assert b"C >= 2" in native_lib.pcnn_last_error()
-    assert native_lib.pcnn_hough_vote_workspace_bytes(1, 480, 640, 22, 0, ctypes.c_float(-1.0), ctypes.byref(nbytes)) == -1
-    assert native_lib.pcnn_roi_pool_fwd(None, None, 1, 5, 1, 4, 4, 4, 7, 7, ctypes.c_float(1.0), 0, None, None, None) == -1
+    assert native_lib.pcnn_hough_vote_workspace_bytes(1, 480, 640, 22, 0, -1.0, ctypes.byref(nbytes)) == -1
+    assert native_lib.pcnn_roi_pool_fwd(None, None, 1, 5, 1, 4, 4, 4, 7, 7, 1.0, 0, None, None, None) == -1
 
 
 def test_host_planning_without_gpu(native_lib):
@@ -44,7 +43,7 @@ def test_host_planning_without_gpu(native_lib):
     nbytes = ctypes.c_size_t(0)
     ws = {}
     for B in (1, 2, 4, 8, 16, 32, 64):
-        assert native_lib.pcnn_hough_vote_workspace_bytes(B, 480, 640, 22, 10, ctypes.c_float(-1.0), ctypes.byref(nbytes)) == 0
+        assert native_lib.pcnn_hough_vote_workspace_bytes(B, 480, 640, 22, 10, -1.0, ctypes.byref(nbytes)) == 0
         ws[B] = nbytes.value
     assert all(ws[a] < ws[b] for a, b in zip((1, 2, 4, 8, 16, 32), (2, 4, 8, 16, 32, 64)))      # monotone in the batch size
     # 8-row bands below ~16 items per resident CTA (B <= 8 at C = 22, H = 480), 16 rows above: the per-image band table doubles
@@ -57,17 +56,15 @@ def test_host_planning_without_gpu(native_lib):
         splits = nbytes.value // per_split
         assert 1 <= splits <= 2 * 132                                                              # at most two waves of work items on 132 SMs
     assert native_lib.pcnn_conv_wgrad_workspace_bytes(1, 8, 8, 48, 64, 3, ctypes.byref(nbytes)) == -1  # Cin % 64
-    f1 = ctypes.c_float(1.0)
+    f1 = 1.0
     assert native_lib.pcnn_up8_heads_bwd_ex(None, None, None, None, f1, f1, None, None, None, None, None, f1, f1, f1, 1, 8, 8, 22, 64, 128,
-                                            None, None, None, None, ctypes.c_size_t(0), None) == -1
-    native_lib.pcnn_last_error.restype = ctypes.c_char_p
+                                            None, None, None, None, 0, None) == -1
     buf = ctypes.create_string_buffer(64)                      # any non-NULL host address: the checks fail before it is read
     for C in (4, 7, 23, 52):                                   # the strip kernel's class counts: even, 6..50
         assert native_lib.pcnn_up8_heads_bwd_ex(buf, buf, buf, buf, f1, f1, buf, None, None, buf, buf, f1, f1, f1, 1, 8, 8, C, 64, 160,
-                                                buf, buf, buf, buf, ctypes.c_size_t(1 << 20), None) == -1, C
+                                                buf, buf, buf, buf, 1 << 20, None) == -1, C
         assert b"C must be even" in native_lib.pcnn_last_error()
-    assert native_lib.pcnn_vertex_loss_fused_lowres_fwd(None, None, None, None, 1, 64, 96, 22, ctypes.c_float(1.0), ctypes.c_float(1.0), None,
-                                                        None, ctypes.c_size_t(0), None) == -1
+    assert native_lib.pcnn_vertex_loss_fused_lowres_fwd(None, None, None, None, 1, 64, 96, 22, 1.0, 1.0, None, None, 0, None) == -1
 
 
 def test_ops_refuse_cpu_tensors(native_lib):

@@ -213,7 +213,7 @@ def test_fc_dgrad_exact_at_fc6(cuda, M):
     nbytes = ctypes.c_size_t(0)
     check(lib().pcnn_fc_workspace_bytes(M, N, K, ctypes.byref(nbytes)))
     ws = workspace("fc", nbytes.value, cuda)
-    check(lib().pcnn_fc_dgrad_f16_tc(ptr(dy), ptr(wt), M, N, K, ptr(mask), ptr(out), N, ptr(ws), ctypes.c_size_t(ws.numel()), stream()))
+    check(lib().pcnn_fc_dgrad_f16_tc(ptr(dy), ptr(wt), M, N, K, ptr(mask), ptr(out), N, ptr(ws), ws.numel(), stream()))
     want = ((dy.double() @ wt.double().t()) * (mask > 0)).float().to(torch.float16)
     torch.cuda.synchronize()
     assert torch.equal(out, want), int((out != want).sum())

@@ -202,17 +202,15 @@ def test_ties_pick_the_first_hypothesis():
 
 def test_abi_argument_validation(native_lib):
     L = native_lib
-    L.pcnn_last_error.restype = ctypes.c_char_p
     nbytes = ctypes.c_size_t(0)
     assert L.pcnn_pose_refine_workspace_bytes(4, 22, ctypes.byref(nbytes)) == 0 and nbytes.value >= 4 * 22 * 4
     assert L.pcnn_pose_refine_workspace_bytes(4, 1, ctypes.byref(nbytes)) == -1
     buf = ctypes.c_void_p(16)       # never dereferenced: validation rejects the call first
-    F = ctypes.c_float
 
     def call(C=22, P=2620, iterations=8, factor=10000.0, znear=0.25, zfar=6.0, null=False):
         lab = None if null else buf
-        return L.pcnn_pose_refine_fwd(lab, buf, buf, 48, buf, buf, None, 4, buf, C, P, 2, 48, 64, 0, F(factor), F(znear), F(zfar),
-                                      F(0.01), 400, iterations, buf, buf, buf, None, buf, ctypes.c_size_t(1 << 20), None)
+        return L.pcnn_pose_refine_fwd(lab, buf, buf, 48, buf, buf, None, 4, buf, C, P, 2, 48, 64, 0, factor, znear, zfar, 0.01, 400,
+                                      iterations, buf, buf, buf, None, buf, 1 << 20, None)
     for kw, msg in ((dict(P=4097), b"P = 4097"), (dict(iterations=-1), b"iterations"), (dict(null=True), b"NULL"),
                     (dict(C=1), b"C = 1"), (dict(factor=0.0), b"depth_factor"), (dict(znear=6.0, zfar=6.0), b"znear < zfar")):
         assert call(**kw) == -1, kw

@@ -11,17 +11,16 @@ GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "sin
 
 
 def test_up8_backward_accepts_two_classes(native_lib):
-    native_lib.pcnn_last_error.restype = ctypes.c_char_p
-    f1 = ctypes.c_float(1.0)
+    f1 = 1.0
     buf = ctypes.create_string_buffer(64)                      # any non-NULL host address: the checks fail before it is read
     # C = 2 passes the class-count check and stops at the workspace check (the 60 x 80 problem needs 5 x 4 CTAs x 8 floats)
     assert native_lib.pcnn_up8_heads_bwd_ex(buf, buf, buf, buf, f1, f1, buf, None, None, buf, buf, f1, f1, f1, 1, 60, 80, 2, 64, 128,
-                                            buf, buf, buf, buf, ctypes.c_size_t(16), None) == -1
+                                            buf, buf, buf, buf, 16, None) == -1
     err = native_lib.pcnn_last_error()
     assert b"C must be even" not in err and b"workspace too small (16 < 640)" in err, err
     for C in (4, 7, 23, 52):                                   # no reference configuration uses them: still rejected
         assert native_lib.pcnn_up8_heads_bwd_ex(buf, buf, buf, buf, f1, f1, buf, None, None, buf, buf, f1, f1, f1, 1, 8, 8, C, 64, 160,
-                                                buf, buf, buf, buf, ctypes.c_size_t(1 << 20), None) == -1, C
+                                                buf, buf, buf, buf, 1 << 20, None) == -1, C
         assert b"C must be even" in native_lib.pcnn_last_error()
 
 

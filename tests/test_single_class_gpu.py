@@ -2,7 +2,6 @@
 two-class kernel, the network's forward at 480 x 640, Hough voting in train mode, the training step with and without pose_reg,
 the domain branch and two ranks.  Every comparison is against the same references and within the same stated limits as the
 C = 6 / 22 tests (tests/train_ref.py, oracle/ref_network.py, the C oracle); every measured error is printed."""
-import ctypes
 
 import numpy as np
 import pytest
@@ -70,7 +69,7 @@ def _up8_problem(cuda, B, h, w, seed):
 
 
 def _up8_bwd(P, dense, thr, up_vtx=2.0, w_in=10.0, count=937.0, sumw=411.0):
-    from posecnn_b200._lib import check, f32, lib, ptr, stream
+    from posecnn_b200._lib import check, lib, ptr, stream
     B, h, w = P["B"], P["h"], P["w"]
     dev = P["lowres"].device
     d_sc = torch.full((B, h, w, 64), 7.0, dtype=torch.bfloat16, device=dev)             # padding channels must be written as 0
@@ -78,10 +77,10 @@ def _up8_bwd(P, dense, thr, up_vtx=2.0, w_in=10.0, count=937.0, sumw=411.0):
     dbias = torch.empty((4 * C,), device=dev)
     cls_out, vtx_out = torch.tensor([0.5, count], device=dev), torch.tensor([0.25, sumw], device=dev)
     ws = torch.empty(4 * B * ((w + 15) // 16) * ((h + 15) // 16) * 4 * C, dtype=torch.uint8, device=dev)    # 16-cell strips
-    check(lib().pcnn_up8_heads_bwd_ex(ptr(P["prob"]), ptr(P["score"]), ptr(P["gt"]), ptr(cls_out), f32(1.0), f32(thr),
+    check(lib().pcnn_up8_heads_bwd_ex(ptr(P["prob"]), ptr(P["score"]), ptr(P["gt"]), ptr(cls_out), 1.0, thr,
                                       ptr(P["vertex"] if dense else None), ptr(None if dense else P["lowres"]), ptr(None if dense else P["bv"]),
-                                      ptr(P["centers"]), ptr(vtx_out), f32(up_vtx), f32(w_in), f32(1.0), B, h, w, C, 64, 128, ptr(d_sc), ptr(d_vt),
-                                      ptr(dbias), ptr(ws), ctypes.c_size_t(ws.numel()), stream()))
+                                      ptr(P["centers"]), ptr(vtx_out), up_vtx, w_in, 1.0, B, h, w, C, 64, 128, ptr(d_sc), ptr(d_vt),
+                                      ptr(dbias), ptr(ws), ws.numel(), stream()))
     return d_sc, d_vt, dbias
 
 

@@ -9,12 +9,11 @@ MAX_ROWS = 128 * 9
 
 def _tail(lib, buf, rows=9, ld=256, fc9=True, w10=True, b10=True, labels=None, grads=True, outs=True, gscale=1.0):
     p = lambda on: buf if on else None
-    return lib.pcnn_domain_tail(p(fc9), rows, ld, p(w10), p(b10), labels, ctypes.c_float(0.1 / max(rows, 1)), ctypes.c_float(gscale),
+    return lib.pcnn_domain_tail(p(fc9), rows, ld, p(w10), p(b10), labels, 0.1 / max(rows, 1), gscale,
                                 p(outs), p(outs), p(outs), p(grads), p(grads), p(grads), p(grads), p(grads), p(grads), None)
 
 
 def test_domain_tail_rejects_bad_arguments_without_gpu(native_lib):
-    native_lib.pcnn_last_error.restype = ctypes.c_char_p
     buf = ctypes.create_string_buffer(64)                      # any non-NULL host address: the checks fail before it is read
     for kw in (dict(fc9=False), dict(w10=False), dict(b10=False), dict(outs=False)):
         assert _tail(native_lib, buf, **kw) == -1, kw
@@ -33,14 +32,13 @@ def test_domain_tail_rejects_bad_arguments_without_gpu(native_lib):
 
 
 def test_domain_grad_merge_rejects_bad_arguments_without_gpu(native_lib):
-    native_lib.pcnn_last_error.restype = ctypes.c_char_p
     buf = ctypes.create_string_buffer(64)
-    f = ctypes.c_float(1.0)
+    f = 1.0
     for a, b, d in ((None, buf, buf), (buf, None, buf), (buf, buf, None)):
-        assert native_lib.pcnn_domain_grad_merge(a, f, b, f, ctypes.c_size_t(8), d, None) == -1
+        assert native_lib.pcnn_domain_grad_merge(a, f, b, f, 8, d, None) == -1
         assert b"NULL" in native_lib.pcnn_last_error()
     for n in (0, 4, 12):
-        assert native_lib.pcnn_domain_grad_merge(buf, f, buf, f, ctypes.c_size_t(n), buf, None) == -1, n
+        assert native_lib.pcnn_domain_grad_merge(buf, f, buf, f, n, buf, None) == -1, n
         assert b"multiple of 8" in native_lib.pcnn_last_error()
 
 

@@ -108,7 +108,7 @@ def test_fc9_exact(cuda, M):
     K chunks; the input gradient's K = 256 is four 64-wide chunks, all of which every item runs; the weight gradient's items
     run >= 8 of its 64-row K tiles where the rows hold that many (M = 128 has 2)."""
     from posecnn_b200 import pose_head
-    from posecnn_b200._lib import check, f32, lib, ptr, stream, workspace
+    from posecnn_b200._lib import check, lib, ptr, stream, workspace
     from tests.util import fc_plan, int_operands, wgrad_plan
     K, N = 25088, 256
     g = torch.Generator().manual_seed(M + 9)
@@ -136,15 +136,14 @@ def test_fc9_exact(cuda, M):
     nbytes = ctypes.c_size_t(0)
     check(lib().pcnn_fc_workspace_bytes(M, K, N, ctypes.byref(nbytes)))
     ws = workspace("fc", nbytes.value, cuda)
-    check(lib().pcnn_fc_dgrad_f16_tc(ptr(dy), ptr(wt), M, K, N, ptr(None), ptr(dx), K, ptr(ws), ctypes.c_size_t(ws.numel()), stream()))
+    check(lib().pcnn_fc_dgrad_f16_tc(ptr(dy), ptr(wt), M, K, N, ptr(None), ptr(dx), K, ptr(ws), ws.numel(), stream()))
     torch.cuda.synchronize()
     assert torch.equal(bits(dx), bits((dy.double() @ wt.double().t()).float().to(torch.float16)))
     # weight gradient [256][25088] with a power-of-two scale
     dw = torch.empty((N, K), dtype=torch.float32, device=cuda)
     check(lib().pcnn_conv_wgrad_workspace_bytes(1, 1, M, K, N, 1, ctypes.byref(nbytes)))
     ws = workspace("wgrad", nbytes.value, cuda)
-    check(lib().pcnn_fc_wgrad_f16_tc(ptr(pool), ptr(dy), M, K, N, f32(0.25), ptr(None), f32(0.0), ptr(dw), ptr(ws),
-                                     ctypes.c_size_t(ws.numel()), stream()))
+    check(lib().pcnn_fc_wgrad_f16_tc(ptr(pool), ptr(dy), M, K, N, 0.25, ptr(None), 0.0, ptr(dw), ptr(ws), ws.numel(), stream()))
     torch.cuda.synchronize()
     want = (dy.double().t() @ pool.double()).float() * 0.25
     bad = dw != want
@@ -159,7 +158,7 @@ def test_domain_grad_merge_bit_exact(cuda, rows):
     """dst = (s_a * a) + (s_b * b) in float32, each product rounded: bit-exact against numpy; with b = 0 it is
     pcnn_half_to_float(a, s_a) bit for bit (signed zeros included)."""
     from posecnn_b200 import pose_head
-    from posecnn_b200._lib import check, f32, lib, ptr, stream
+    from posecnn_b200._lib import check, lib, ptr, stream
     g = torch.Generator().manual_seed(rows)
     n = rows * 25088
     a = (torch.randn(n, generator=g) * torch.exp2(torch.randint(-20, 12, (n,), generator=g).float())).to(torch.float16)
@@ -176,7 +175,7 @@ def test_domain_grad_merge_bit_exact(cuda, rows):
     ad = a.to(cuda)
     zero = pose_head.domain_grad_merge(ad, sa, torch.zeros_like(ad), sb, (rows, 7, 7, 512))
     h2f = torch.empty(n, dtype=torch.float32, device=cuda)
-    check(lib().pcnn_half_to_float(ptr(ad), ctypes.c_size_t(n), f32(sa), ptr(h2f), stream()))
+    check(lib().pcnn_half_to_float(ptr(ad), n, sa, ptr(h2f), stream()))
     torch.cuda.synchronize()
     assert torch.equal(bits(zero.reshape(-1)), bits(h2f))
 

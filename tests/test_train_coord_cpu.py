@@ -32,56 +32,49 @@ def test_restatement_equals_reference_golden():
     assert len({int(c) for c in np.unique(lab[1]) if c > 0}) >= 3
 
 
-def _err(native_lib):
-    native_lib.pcnn_last_error.restype = ctypes.c_char_p
-    return native_lib.pcnn_last_error()
-
-
 def test_coord_entry_points_check_arguments(native_lib):
-    f1 = ctypes.c_float(1.0)
+    f1 = 1.0
     buf = ctypes.create_string_buffer(64)                      # any non-NULL host address: the checks fail before it is read
-    ws = ctypes.c_size_t(1 << 20)
+    ws = 1 << 20
     # targets: every tensor is required; shapes positive
     assert native_lib.pcnn_vertex_targets_3d_fwd(buf, None, buf, buf, 1, 8, 8, 6, f1, buf, buf, None) == -1
-    assert b"vertex_targets_3d: NULL tensor pointer" in _err(native_lib)
+    assert b"vertex_targets_3d: NULL tensor pointer" in native_lib.pcnn_last_error()
     assert native_lib.pcnn_vertex_targets_3d_fwd(buf, buf, buf, buf, 1, 0, 8, 6, f1, buf, buf, None) == -1
-    assert b"vertex_targets_3d: bad shape" in _err(native_lib)
+    assert b"vertex_targets_3d: bad shape" in native_lib.pcnn_last_error()
     assert native_lib.pcnn_vertex_targets_3d_fwd(buf, buf, buf, buf, 65536, 256, 256, 6, f1, buf, buf, None) == -1
-    assert b"too many pixels" in _err(native_lib)
+    assert b"too many pixels" in native_lib.pcnn_last_error()
     # fused losses: vertmap and extents are required on top of the 2-D twin's tensors; sigma > 0; lowres needs H, W % 8 == 0
     assert native_lib.pcnn_vertex_loss_coord_fwd(buf, buf, None, buf, buf, 1, 8, 8, 6, f1, f1, buf, f1, None, buf, ws, None) == -1
-    assert b"vertex_loss_coord: NULL tensor pointer" in _err(native_lib)
+    assert b"vertex_loss_coord: NULL tensor pointer" in native_lib.pcnn_last_error()
     assert native_lib.pcnn_vertex_loss_coord_fwd(buf, buf, buf, buf, None, 1, 8, 8, 6, f1, f1, buf, f1, None, buf, ws, None) == -1
-    assert b"vertex_loss_coord: NULL tensor pointer" in _err(native_lib)
-    assert native_lib.pcnn_vertex_loss_coord_fwd(buf, buf, buf, buf, buf, 1, 8, 8, 6, f1, ctypes.c_float(0.0), buf, f1, None, buf, ws,
-                                                 None) == -1
-    assert b"vertex_loss_coord: bad arguments" in _err(native_lib)
-    assert native_lib.pcnn_vertex_loss_coord_fwd(buf, buf, buf, buf, buf, 1, 8, 8, 6, f1, f1, buf, f1, None, buf, ctypes.c_size_t(16),
-                                                 None) == -1
-    assert b"vertex_loss_coord: workspace too small" in _err(native_lib)
+    assert b"vertex_loss_coord: NULL tensor pointer" in native_lib.pcnn_last_error()
+    assert native_lib.pcnn_vertex_loss_coord_fwd(buf, buf, buf, buf, buf, 1, 8, 8, 6, f1, 0.0, buf, f1, None, buf, ws, None) == -1
+    assert b"vertex_loss_coord: bad arguments" in native_lib.pcnn_last_error()
+    assert native_lib.pcnn_vertex_loss_coord_fwd(buf, buf, buf, buf, buf, 1, 8, 8, 6, f1, f1, buf, f1, None, buf, 16, None) == -1
+    assert b"vertex_loss_coord: workspace too small" in native_lib.pcnn_last_error()
     assert native_lib.pcnn_vertex_loss_coord_lowres_fwd(buf, None, buf, buf, buf, buf, 1, 64, 96, 22, f1, f1, buf, buf, ws, None) == -1
-    assert b"vertex_loss_coord_lowres: NULL tensor pointer" in _err(native_lib)
+    assert b"vertex_loss_coord_lowres: NULL tensor pointer" in native_lib.pcnn_last_error()
     assert native_lib.pcnn_vertex_loss_coord_lowres_fwd(buf, buf, buf, None, buf, buf, 1, 64, 96, 22, f1, f1, buf, buf, ws, None) == -1
-    assert b"vertex_loss_coord_lowres: NULL tensor pointer" in _err(native_lib)
+    assert b"vertex_loss_coord_lowres: NULL tensor pointer" in native_lib.pcnn_last_error()
     assert native_lib.pcnn_vertex_loss_coord_lowres_fwd(buf, buf, buf, buf, buf, buf, 1, 60, 96, 22, f1, f1, buf, buf, ws, None) == -1
-    assert b"vertex_loss_coord_lowres: bad arguments" in _err(native_lib)
+    assert b"vertex_loss_coord_lowres: bad arguments" in native_lib.pcnn_last_error()
 
 
 def test_coord_adjoint_checks_arguments(native_lib):
-    f1 = ctypes.c_float(1.0)
+    f1 = 1.0
     buf = ctypes.create_string_buffer(64)
 
     def call(vertmap, extents, C, h=8, w=8, ws=1 << 20):
         return native_lib.pcnn_up8_heads_bwd_coord(buf, buf, buf, buf, f1, f1, buf, None, None, vertmap, buf, extents, buf, f1, f1, f1, 1, h,
-                                                   w, C, 64, 160, buf, buf, buf, buf, ctypes.c_size_t(ws), None)
-    assert call(None, buf, 22) == -1 and b"up8_heads_bwd_coord: NULL tensor pointer" in _err(native_lib)
-    assert call(buf, None, 22) == -1 and b"up8_heads_bwd_coord: NULL tensor pointer" in _err(native_lib)
+                                                   w, C, 64, 160, buf, buf, buf, buf, ws, None)
+    assert call(None, buf, 22) == -1 and b"up8_heads_bwd_coord: NULL tensor pointer" in native_lib.pcnn_last_error()
+    assert call(buf, None, 22) == -1 and b"up8_heads_bwd_coord: NULL tensor pointer" in native_lib.pcnn_last_error()
     for C in (4, 7, 23, 52):                                   # the class counts of the 2-D entry, no others
         assert call(buf, buf, C) == -1, C
-        assert b"C must be even" in _err(native_lib)
+        assert b"C must be even" in native_lib.pcnn_last_error()
     # C = 2 (16-cell strips: 5 x 4 CTAs x 8 floats at 60 x 80) passes the class-count check and stops at the workspace check
     assert call(buf, buf, 2, 60, 80, 16) == -1
-    err = _err(native_lib)
+    err = native_lib.pcnn_last_error()
     assert b"C must be even" not in err and b"workspace too small (16 < 640)" in err, err
 
 

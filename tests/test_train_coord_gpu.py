@@ -2,7 +2,6 @@
 loss (dense and 1/8-resolution sources) against smooth_l1_loss_vertex on the materialised blobs, the up-sampling adjoint's 3-D mode
 against torch, the training step against the autograd graph, its contents, a short training run whose weights then estimate poses
 on an inference network, and two ranks.  Every measured error is printed."""
-import ctypes
 
 import numpy as np
 import pytest
@@ -134,7 +133,7 @@ def _up8_problem(cuda, B, h, w, C, seed):
 
 
 def _up8_bwd(P, dense, coord, thr=0.7, up_vtx=2.0, w_in=10.0, count=937.0, sumw=411.0):
-    from posecnn_b200._lib import check, f32, lib, ptr, stream
+    from posecnn_b200._lib import check, lib, ptr, stream
     B, h, w, C = P["B"], P["h"], P["w"], P["C"]
     dev = P["lowres"].device
     d_sc = torch.full((B, h, w, 64), 7.0, dtype=torch.bfloat16, device=dev)             # padding channels must be written as 0
@@ -143,9 +142,9 @@ def _up8_bwd(P, dense, coord, thr=0.7, up_vtx=2.0, w_in=10.0, count=937.0, sumw=
     cls_out, vtx_out = torch.tensor([0.5, count], device=dev), torch.tensor([0.25, sumw], device=dev)
     ws = torch.empty(4 * B * ((w + 3) // 4) * ((h + 15) // 16) * 4 * C, dtype=torch.uint8, device=dev)
     src = (ptr(P["vertex"] if dense else None), ptr(None if dense else P["lowres"]), ptr(None if dense else P["bv"]))
-    head = (ptr(P["prob"]), ptr(P["score"]), ptr(P["gt"]), ptr(cls_out), f32(1.0), f32(thr)) + src
-    tail = (ptr(vtx_out), f32(up_vtx), f32(w_in), f32(1.0), B, h, w, C, 64, 128, ptr(d_sc), ptr(d_vt), ptr(dbias), ptr(ws),
-            ctypes.c_size_t(ws.numel()), stream())
+    head = (ptr(P["prob"]), ptr(P["score"]), ptr(P["gt"]), ptr(cls_out), 1.0, thr) + src
+    tail = (ptr(vtx_out), up_vtx, w_in, 1.0, B, h, w, C, 64, 128, ptr(d_sc), ptr(d_vt), ptr(dbias), ptr(ws),
+            ws.numel(), stream())
     if coord:
         check(lib().pcnn_up8_heads_bwd_coord(*head, ptr(P["vertmap"]), ptr(P["centers"]), ptr(P["ext"]), *tail))
     else:

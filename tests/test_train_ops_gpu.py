@@ -227,9 +227,8 @@ def test_pack_pose_meta_matches_data_layer_restatement(cuda):
 def test_vertex_loss_from_lowres_equals_dense(cuda):
     """pcnn_vertex_loss_fused_lowres_fwd (vertex values formed on demand from the 1/8-resolution head tensor) == the fused loss on
     the dense vertex_pred produced by pcnn_up8_heads from the same tensor: the training step needs no dense vertex_pred."""
-    import ctypes
     from posecnn_b200 import synth, train_ops
-    from posecnn_b200._lib import check, f32, lib, ptr, stream
+    from posecnn_b200._lib import check, lib, ptr, stream
     B, H, W, C = 2, 96, 128, 22
     sc = synth.make_scene(batch=B, height=H, width=W, num_classes=C, seed=5, objects_per_image=4, min_pixels=100)
     g = torch.Generator().manual_seed(9)
@@ -246,7 +245,7 @@ def test_vertex_loss_from_lowres_equals_dense(cuda):
         l0, w0 = train_ops.vertex_loss_from_centers(vertex, lab, cen, 10.0, sigma, want_grad=False)
         out = torch.empty((2,), device=cuda)
         ws = train_ops._workspace(cuda)
-        check(lib().pcnn_vertex_loss_fused_lowres_fwd(ptr(lowres), ptr(bv), ptr(lab), ptr(cen), B, H, W, C, f32(10.0), f32(sigma), ptr(out), ptr(ws),
-                                                      ctypes.c_size_t(ws.numel()), stream()))
+        check(lib().pcnn_vertex_loss_fused_lowres_fwd(ptr(lowres), ptr(bv), ptr(lab), ptr(cen), B, H, W, C, 10.0, sigma, ptr(out), ptr(ws),
+                                                      ws.numel(), stream()))
         assert float(w0.item()) == float(out[1].item()) > 0
         assert float(l0.item()) == float(out[0].item())

@@ -4,7 +4,6 @@ import ctypes
 
 
 def test_im2col_depth_rejects_bad_arguments_without_gpu(native_lib):
-    native_lib.pcnn_last_error.restype = ctypes.c_char_p
     mean = (ctypes.c_float * 3)(102.9801, 115.9465, 122.7717)
     buf = ctypes.create_string_buffer(64)                      # any non-NULL host address: the checks fail before it is read
     assert native_lib.pcnn_im2col_depth(None, mean, buf, 1, 8, 8, None) == -1

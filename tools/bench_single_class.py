@@ -14,7 +14,6 @@ The card name and power limit are read in the same run with a read-only nvidia-s
     python tools/bench_single_class.py [--batch 64] [--steps 10] [--warmup 3] [--runs 3]
 """
 import argparse
-import ctypes
 import json
 import os
 import statistics
@@ -26,7 +25,7 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from bench_train_rgbd import H, W, gpu_info, make_inputs           # noqa: E402
-from posecnn_b200._lib import check, f32, lib, ptr, stream        # noqa: E402
+from posecnn_b200._lib import check, lib, ptr, stream        # noqa: E402
 from posecnn_b200.networks.vgg16_convs import GraphedForward, vgg16_convs   # noqa: E402
 from posecnn_b200.single_class import single_class_view           # noqa: E402
 from posecnn_b200.train import Trainer                             # noqa: E402
@@ -92,9 +91,9 @@ def up8_problem(dev, B, C, gt):
     ws = torch.empty(4 * B * ((w + 3) // 4) * ((h + 15) // 16) * 4 * C, dtype=torch.uint8, device=dev)
 
     def run():
-        check(lib().pcnn_up8_heads_bwd_ex(ptr(prob), ptr(score), ptr(lab), ptr(cls_out), f32(1.0), f32(0.7), ptr(None), ptr(lowres), ptr(bv),
-                                          ptr(centers), ptr(vtx_out), f32(1.0), f32(10.0), f32(1.0), B, h, w, C, 64, 128, ptr(d_sc), ptr(d_vt),
-                                          ptr(dbias), ptr(ws), ctypes.c_size_t(ws.numel()), stream()))
+        check(lib().pcnn_up8_heads_bwd_ex(ptr(prob), ptr(score), ptr(lab), ptr(cls_out), 1.0, 0.7, ptr(None), ptr(lowres), ptr(bv),
+                                          ptr(centers), ptr(vtx_out), 1.0, 10.0, 1.0, B, h, w, C, 64, 128, ptr(d_sc), ptr(d_vt),
+                                          ptr(dbias), ptr(ws), ws.numel(), stream()))
     return run
 
 

@@ -12,7 +12,6 @@ The card name and power limit are read in the same run with a read-only nvidia-s
     python tools/bench_train_coord.py [--batch 64] [--steps 10] [--warmup 3] [--runs 3]
 """
 import argparse
-import ctypes
 import json
 import os
 import statistics
@@ -25,7 +24,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from bench_single_class import timed, timed_steps, two_class_inputs   # noqa: E402
 from bench_train_rgbd import H, W, gpu_info, make_inputs           # noqa: E402
-from posecnn_b200._lib import check, f32, lib, ptr, stream        # noqa: E402
+from posecnn_b200._lib import check, lib, ptr, stream        # noqa: E402
 from posecnn_b200.networks.vgg16_convs import vgg16_convs         # noqa: E402
 from posecnn_b200.train import Trainer                             # noqa: E402
 
@@ -61,9 +60,9 @@ def up8_problem(dev, B, C, gt, centers, vertmap, ext):
     d_vt = torch.empty((B, h, w, 128), dtype=torch.bfloat16, device=dev)
     dbias = torch.empty((4 * C,), device=dev)
     ws = torch.empty(4 * B * ((w + 3) // 4) * ((h + 15) // 16) * 4 * C, dtype=torch.uint8, device=dev)
-    head = lambda: (ptr(prob), ptr(score), ptr(gt), ptr(cls_out), f32(1.0), f32(0.7), ptr(None), ptr(lowres), ptr(bv))
-    tail = lambda: (ptr(vtx_out), f32(1.0), f32(10.0), f32(1.0), B, h, w, C, 64, 128, ptr(d_sc), ptr(d_vt), ptr(dbias), ptr(ws),
-                    ctypes.c_size_t(ws.numel()), stream())
+    head = lambda: (ptr(prob), ptr(score), ptr(gt), ptr(cls_out), 1.0, 0.7, ptr(None), ptr(lowres), ptr(bv))
+    tail = lambda: (ptr(vtx_out), 1.0, 10.0, 1.0, B, h, w, C, 64, 128, ptr(d_sc), ptr(d_vt), ptr(dbias), ptr(ws),
+                    ws.numel(), stream())
 
     def run_2d():
         check(lib().pcnn_up8_heads_bwd_ex(*head(), ptr(centers), *tail()))
