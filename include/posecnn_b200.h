@@ -495,6 +495,18 @@ int pcnn_coord_pose3d_fwd(const int32_t* label, const float* vertex, const float
 int pcnn_coord_pose3d_records(const float* poses, const float* extents, const float* meta, int num_meta, int B, int C, int batch_offset,
                               float im_scale, float* rois, float* out_poses, int32_t* num_rows, void* stream);
 
+/* Colour-only pose estimation from object coordinates (csrc/coord_pose.cu, DESIGN.md 13): Synthesizer::estimatePose2D
+ * (lib/synthesize/synthesize.cpp:1571-1767), batched; the arguments of pcnn_coord_pose3d_fwd without depth and depth_factor.
+ *  Hypotheses from four pixels by P3P, inliers within 10 px of the projection; the survivor keeps its P3P pose (no refit, no
+ *  Nelder-Mead, as the reference behaves).  -> poses [B,C,3,4], info [B,C,6] as pcnn_coord_pose3d_fwd with energy = -1;
+ *  trace_hyp [B,256,14] (nullable) = per hypothesis (class or 0, attempts, four pixel indices or -1, inlier count in each of the
+ *  8 rounds or -1); trace_round [B,C,8,4] (nullable) as pcnn_coord_pose3d_fwd.  workspace: pcnn_coord_pose2d_workspace_bytes.
+ *  The records come from pcnn_coord_pose3d_records.  Deterministic, no host synchronisation. */
+int pcnn_coord_pose2d_workspace_bytes(int B, int H, int W, int C, size_t* bytes);
+int pcnn_coord_pose2d_fwd(const int32_t* label, const float* vertex, const float* lowres, const float* bias_vertex, const float* meta,
+                          int num_meta, const float* extents, const uint64_t* keys, int B, int H, int W, int C, float* poses, float* info,
+                          int32_t* trace_hyp, int32_t* trace_round, void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

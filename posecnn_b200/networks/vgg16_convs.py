@@ -212,7 +212,7 @@ class vgg16_convs:
 
     def forward(self, data, meta_data, extents, poses=None, data_p=None, want_prob=False, sync_rois=True, want_score=False,
                 dense_vertex=True, batch_global=None, batch_offset=0, depth=None, refine_depth=None, refine_points=None,
-                depth_factor=10000.0, estimate_depth=None, estimate_keys=None):
+                depth_factor=10000.0, estimate_depth=None, estimate_keys=None, estimate_rgb=False):
         """Inference / forward pass.  data [B,H,W,3] (u8 BGR or pre-processed f32), H, W multiples of 16
         (pad_im, lib/utils/blob.py:48-58).  Returns self.layers with the reference's layer names.
 
@@ -229,13 +229,24 @@ class vgg16_convs:
         image indices): on a vertex_reg_3d network at test time, estimate the poses from the object coordinates of the
         1/8-resolution head and the depth (coord_pose.py, lib/fcn/test.py:1381-1399) -> estimate_poses [B,C,3,4], estimate_info
         [B,C,6] and the records detections_rois [B*(C-1),6] / detections_poses [B*(C-1),7] / num_detections [1] (im_scale =
-        scales[0]).  Without estimate_depth nothing else runs."""
+        scales[0]).  Without estimate_depth nothing else runs.
+        estimate_rgb=True: on the same networks, the colour-only estimate from the object coordinates alone (coord_pose.py
+        estimate_poses_2d, lib/fcn/test.py:1362-1380, keys as for estimate_depth) -> estimate_poses_rgb, estimate_info_rgb,
+        detections_rois_rgb, detections_poses_rgb, num_detections_rgb, shaped like the depth estimate's outputs.
+        On a vertex_reg_3d network, refine_depth + refine_points refine the depth estimate's detections_* records (test.py:1403-1416;
+        for C = 2 pass refine_points in the dataset's numbering and map the outputs with utils/results.py::to_dataset_classes)."""
         C = self.num_classes
-        if estimate_depth is not None and (self.is_train or self.vertex_reg_2d or not self.vertex_reg_3d):
+        coord_net = not self.is_train and self.vertex_reg_3d and not self.vertex_reg_2d
+        if estimate_depth is not None and not coord_net:
             raise ValueError("estimate_depth estimates poses from object coordinates: it needs is_train=False and vertex_reg_3d "
                              "without vertex_reg_2d")
-        if refine_depth is not None and (self.is_train or not (self.vertex_reg_2d and self.pose_reg)):
-            raise ValueError("refine_depth refines the test-time detections: it needs is_train=False, vertex_reg_2d and pose_reg")
+        if estimate_rgb and not coord_net:
+            raise ValueError("estimate_rgb estimates poses from object coordinates: it needs is_train=False and vertex_reg_3d "
+                             "without vertex_reg_2d")
+        if refine_depth is not None and not (coord_net and estimate_depth is not None) and \
+                (self.is_train or not (self.vertex_reg_2d and self.pose_reg)):
+            raise ValueError("refine_depth refines the test-time detections: it needs is_train=False and vertex_reg_2d with pose_reg, "
+                             "or vertex_reg_3d with estimate_depth")
         L = self.layers = {}
         P, T = self.params, self._tc
         B, H, W, _ = data.shape
@@ -281,15 +292,24 @@ class vgg16_convs:
         if want_score:
             L["score"] = score
         if not self.vertex_reg_2d:
+            if not estimate_rgb and estimate_depth is None:
+                return L
+            from ..coord_pose import assemble_records, estimate_poses_2d, estimate_poses_3d
+            keys = estimate_keys if estimate_keys is not None else \
+                torch.arange(batch_offset, batch_offset + B, dtype=torch.int64, device=data.device)
+            if estimate_rgb:
+                est = estimate_poses_2d(label, meta_data, extents, keys, lowres=lowres, bias_vertex=P["vertex_pred/biases"])
+                L["estimate_poses_rgb"], L["estimate_info_rgb"] = est["poses"], est["info"]
+                L["detections_rois_rgb"], L["detections_poses_rgb"], L["num_detections_rgb"] = assemble_records(
+                    est["poses"], extents, meta_data, self.scales[0], batch_offset)
             if estimate_depth is not None:
-                from ..coord_pose import assemble_records, estimate_poses_3d
-                keys = estimate_keys if estimate_keys is not None else \
-                    torch.arange(batch_offset, batch_offset + B, dtype=torch.int64, device=data.device)
                 est = estimate_poses_3d(label, estimate_depth, meta_data, extents, keys, lowres=lowres, bias_vertex=P["vertex_pred/biases"],
                                         factor_depth=depth_factor)
                 L["estimate_poses"], L["estimate_info"] = est["poses"], est["info"]
                 L["detections_rois"], L["detections_poses"], L["num_detections"] = assemble_records(
                     est["poses"], extents, meta_data, self.scales[0], batch_offset)
+                if refine_depth is not None:
+                    self._refine(L, label, refine_depth, meta_data, refine_points, depth_factor, batch_offset)
             return L
         Bg = B if batch_global is None else int(batch_global)
         box, pose, target, weight, domain, num_rois, status = hough_voting_gpu_op.hough_voting_gpu_capacity(
@@ -330,13 +350,7 @@ class vgg16_convs:
                                                                    self.nms_thresh, per_image=True, num_classes=C)
             L["detections_keep"], L["detections_rois"], L["detections_poses"], L["num_detections"] = keep, d_rois, d_poses, d_n
             if refine_depth is not None:
-                if refine_points is None:
-                    raise ValueError("refine_depth needs refine_points (the [C,P,3] model point table)")
-                from ..pose_refine import refine_poses
-                ref = refine_poses(label, refine_depth, meta_data, d_rois, d_poses, refine_points, num_rows=d_n,
-                                   factor_depth=depth_factor, batch_offset=batch_offset)
-                L["detections_poses_refined"], L["detections_poses_icp"] = ref["poses_refined"], ref["poses_icp"]
-                L["detections_icp_info"] = ref["icp_info"]
+                self._refine(L, label, refine_depth, meta_data, refine_points, depth_factor, batch_offset)
         if sync_rois:
             host = torch.cat([num_rois, status[:2]]).tolist()  # the one host read the op's data-dependent shape requires
             n = max(1, host[0])
@@ -350,6 +364,20 @@ class vgg16_convs:
                 if k in L:
                     L[k] = L[k][:n]
         return L
+
+
+    def _refine(self, L, label, refine_depth, meta_data, refine_points, depth_factor, batch_offset):
+        """TEST.POSE_REFINE on L's detections_* records -> detections_poses_refined / _icp / detections_icp_info."""
+        if refine_points is None:
+            raise ValueError("refine_depth needs refine_points (the [C,P,3] model point table)")
+        from ..pose_refine import refine_poses
+        rois = L["detections_rois"]
+        if rois.shape[1] == 6:          # the object-coordinate records have no score column
+            rois = torch.nn.functional.pad(rois, (0, 1))
+        ref = refine_poses(label, refine_depth, meta_data, rois, L["detections_poses"], refine_points, num_rows=L["num_detections"],
+                           factor_depth=depth_factor, batch_offset=batch_offset)
+        L["detections_poses_refined"], L["detections_poses_icp"] = ref["poses_refined"], ref["poses_icp"]
+        L["detections_icp_info"] = ref["icp_info"]
 
 
 def training_losses(net: vgg16_convs, layers: dict, gt_label_2d, vertex_targets, vertex_weights, points, symmetry,
