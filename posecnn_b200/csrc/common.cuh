@@ -56,6 +56,10 @@ __device__ __forceinline__ void philox4x32_10(uint64_t key, uint64_t ctr, uint32
     out[0] = c0; out[1] = c1; out[2] = c2; out[3] = c3;
 }
 
+// Saturate to the fp16 range before a float -> half conversion: finite overflow and +-inf go to +-65504, NaN stays NaN
+// (fminf / fmaxf alone would return the non-NaN operand and turn a NaN into -65504)
+__device__ __forceinline__ float sat_f16(float v) { return v != v ? v : fminf(fmaxf(v, -65504.f), 65504.f); }
+
 // streaming (read-once) 128-bit load / store: keep L1 for data that is actually reused
 __device__ __forceinline__ float4 ld_stream_f4(const float4* p)
 {

@@ -22,8 +22,6 @@ constexpr int kWarps = 16;
 constexpr int kThreads = kWarps * 32;
 constexpr int kPer = kHid / 32;            // hidden units per lane: k = kPer * lane + j
 
-__device__ __forceinline__ float sat_f16(float v) { return fminf(fmaxf(v, -65504.f), 65504.f); }
-
 // the fixed-order sum over warps of one [kHid] partial held as v[kPer] by every lane -> dst[kHid]
 __device__ __forceinline__ void reduce_warps(const float (&v)[kPer], float (*red)[kHid], int warp, int k0, float* __restrict__ dst)
 {

@@ -110,9 +110,6 @@ k_fc_tc(const __grid_constant__ CUtensorMap map_a /*[M][K] f16, box {64, 128}*/,
     }
 }
 
-// fp16 activations saturate instead of overflowing to inf (|x| <= 65504)
-__device__ __forceinline__ float sat_f16(float v) { return fminf(fmaxf(v, -65504.f), 65504.f); }
-
 // out[m][n] = act(bias[n] + sum_s partial[s][m][n]) for n < n_valid; act: 0 none, 1 ReLU, 2 tanh.
 // out_f16 (row stride ld_out, the next layer's A operand) and / or out_f32 (row stride n_valid).
 __global__ void __launch_bounds__(256)

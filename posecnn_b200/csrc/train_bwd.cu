@@ -415,7 +415,7 @@ k_pose_chain_bwd(const float* __restrict__ g, const float* __restrict__ tanhv, c
             const float du = clamped ? gg * inv : (gg - u * inv * (sg * inv)) * inv;
             d = du * wv * (1.f - t * t);
         }
-        dpre[(size_t)row * ld + j] = __float2half_rn(fminf(fmaxf(d, -65504.f), 65504.f));
+        dpre[(size_t)row * ld + j] = __float2half_rn(sat_f16(d));
     }
 }
 
@@ -427,7 +427,7 @@ __device__ __forceinline__ T16 to16(float v);
 template <>
 __device__ __forceinline__ __nv_bfloat16 to16<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
 template <>
-__device__ __forceinline__ __half to16<__half>(float v) { return __float2half_rn(fminf(fmaxf(v, -65504.f), 65504.f)); }
+__device__ __forceinline__ __half to16<__half>(float v) { return __float2half_rn(sat_f16(v)); }
 
 template <typename T16>
 __global__ void __launch_bounds__(256)

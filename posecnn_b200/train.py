@@ -457,9 +457,10 @@ class Trainer:
         # The head's backward GEMMs run on FP16 operands like its forward.  The pose-loss gradients are tiny (a mean over rows x points:
         # 1e-6 .. 1e-4 per element, below fp16's normal range), so the chain is LOSS-SCALED by a dynamic power of two S where it enters fp16 and un-scaled
         # where it leaves (weight gradients, bias sums, the RoiPool gradient); conversions saturate at +-65504.
-        D = 4 * C
-        dpre = torch.empty((rows, 128), dtype=torch.float16, device=dev)
-        check(lib().pcnn_pose_chain_bwd(ptr(A["pose_diff"]), ptr(A["poses_tanh"]), ptr(A["poses_weight"]), rows, D, pose_scale, ptr(dpre), 128,
+        # dpre's row stride is fc8's output count padded to a multiple of 128 (its fp16 weight copy's rows): 128 up to C = 32, 256 above
+        D, ld = 4 * C, self.tc["fc8/w"].shape[0]
+        dpre = torch.empty((rows, ld), dtype=torch.float16, device=dev)
+        check(lib().pcnn_pose_chain_bwd(ptr(A["pose_diff"]), ptr(A["poses_tanh"]), ptr(A["poses_weight"]), rows, D, pose_scale, ptr(dpre), ld,
                                         stream()))
         # dynamic loss scale: a power of two that puts the largest element of the chain's entry point at ~2^11 (one host read; the
         # un-scaled pass above is only used for its maximum, which fp16 represents well enough even when the small elements underflow)
@@ -480,7 +481,7 @@ class Trainer:
             self._emit(grads, "fc9/w", self._fc_wgrad(A["pool"], dom["dpre9"], 1.0 / S_d))
             self._emit(grads, "fc9/b", dom["db9"])
             d9 = self._fc_dgrad(dom["dpre9"], "fc9", None)                                    # [rows, 25088], scaled by S_d
-        check(lib().pcnn_pose_chain_bwd(ptr(A["pose_diff"]), ptr(A["poses_tanh"]), ptr(A["poses_weight"]), rows, D, pose_scale * S, ptr(dpre), 128,
+        check(lib().pcnn_pose_chain_bwd(ptr(A["pose_diff"]), ptr(A["poses_tanh"]), ptr(A["poses_weight"]), rows, D, pose_scale * S, ptr(dpre), ld,
                                         stream()))
         self._emit(grads, "fc8/w", self._fc_wgrad(A["fc7"], dpre, 1.0 / S))
         self._emit(grads, "fc8/b", dpre[:, :D].float().sum(0) / S)
