@@ -274,19 +274,11 @@ class Trainer:
                                    ptr(score), stream()))
         A.update(s4=s4, s5=s5, v4=v4, v5=v5, add_s=add_s, add_v=add_v, label_2d=label, lowres=lowres, prob_normalized=prob, score=score)
         # losses on the dense heads (fused kernels; the masks / targets are never materialised)
-        ws = train_ops._workspace(data.device)
-        cls_out = torch.empty((2,), dtype=torch.float32, device=data.device)
-        check(lib().pcnn_loss_cls_hard_raw_fwd(ptr(score), ptr(prob), ptr(gt_label_2d), B, H, W, C, net.threshold_label, ptr(cls_out), ptr(ws),
-                                               ws.numel(), stream()))
-        vtx_out = torch.empty((2,), dtype=torch.float32, device=data.device)
+        cls_out = train_ops.loss_cls(score, prob, gt_label_2d, net.threshold_label)
+        vtx_out = train_ops.loss_vertex(lowres, M["vertex_pred/b"], gt_label_2d, centers, self.w_inside, 1.0,
+                                        vertmap if self.coord else None, extents if self.coord else None)
         if self.coord:
-            check(lib().pcnn_vertex_loss_coord_lowres_fwd(ptr(lowres), ptr(M["vertex_pred/b"]), ptr(gt_label_2d), ptr(vertmap), ptr(centers),
-                                                          ptr(extents), B, H, W, C, self.w_inside, 1.0, ptr(vtx_out), ptr(ws),
-                                                          ws.numel(), stream()))
             A.update(extents=extents)
-        else:
-            check(lib().pcnn_vertex_loss_fused_lowres_fwd(ptr(lowres), ptr(M["vertex_pred/b"]), ptr(gt_label_2d), ptr(centers), B, H, W, C,
-                                                          self.w_inside, 1.0, ptr(vtx_out), ptr(ws), ws.numel(), stream()))
         A.update(cls_out=cls_out, vtx_out=vtx_out, data=data)
         if not self.pose_reg:
             return A

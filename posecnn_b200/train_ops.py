@@ -1,8 +1,9 @@
-"""Training-side target generation and fused losses on the device (SURVEY.md §8(f) rank 3).
+"""Training-side target generation and the training step's fused losses on the device (SURVEY.md §8(f) rank 3).
 
-Names follow the reference: `_generate_vertex_targets` (lib/gt_synthesize_layer/minibatch.py:543-602),
-`loss_cross_entropy_single_frame` on the Hardlabel mask (lib/fcn/train.py:455-465, network.py:340) and
-`smooth_l1_loss_vertex` (lib/fcn/train.py:564-573).  All tensors are CUDA torch tensors; no host synchronisation.
+Targets follow the reference's `_generate_vertex_targets` (lib/gt_synthesize_layer/minibatch.py:543-602); `loss_cls` is
+`loss_cross_entropy_single_frame` on the Hardlabel mask (lib/fcn/train.py:455-465, network.py:340) and `loss_vertex` is
+`smooth_l1_loss_vertex` (lib/fcn/train.py:564-573), each the launch Trainer.forward runs.  All tensors are CUDA torch tensors;
+no host synchronisation.
 """
 from __future__ import annotations
 
@@ -94,78 +95,44 @@ def pack_pose_meta(poses, cls, intrinsics, im_scale=1.0, flip_x=False):
     return blob, nrows, meta
 
 
-def loss_cross_entropy_hard(scores, prob, gt_label, threshold, want_grad=False, upstream=1.0):
-    """-sum(hard_label(prob, gt, threshold) * scores) / (sum(mask) + 1e-10) with scores = log-softmax [B,H,W,C];
-    the mask is never materialised.  Returns (loss [1] view, count [1] view[, grad wrt scores])."""
-    sc = require_cuda("scores", scores, torch.float32, 4)
+def loss_cls(score, prob, gt_label, threshold):
+    """The training step's loss_cls: loss_cross_entropy_single_frame (lib/fcn/train.py:455-465) of log_softmax(score) over the
+    pixels Hardlabel(prob, gt_label, threshold) selects (network.py:340), from the raw score [B,H,W,C]; neither the log-softmax
+    nor the mask is materialised.  prob [B,H,W,C] f32, gt_label [B,H,W] int32.  Returns the [2] buffer (loss, count) that the
+    backward pass reads."""
+    sc = require_cuda("score", score, torch.float32, 4)
     pr = require_cuda("prob", prob, torch.float32, 4)
     gt = require_cuda("gt_label", gt_label, torch.int32, 3)
     B, H, W, C = sc.shape
+    if pr.shape != sc.shape or tuple(gt.shape) != (B, H, W):
+        raise ValueError("prob must match score [B,H,W,C] and gt_label must be [B,H,W]")
     out = torch.empty((2,), dtype=torch.float32, device=sc.device)
-    grad = torch.empty_like(sc) if want_grad else None
     ws = _workspace(sc.device)
-    check(lib().pcnn_loss_cls_hard_fwd(ptr(sc), ptr(pr), ptr(gt), B, H, W, C, threshold, ptr(out), upstream, ptr(grad),
-                                       ptr(ws), ws.numel(), stream()))
-    return (out[0:1], out[1:2], grad) if want_grad else (out[0:1], out[1:2])
+    check(lib().pcnn_loss_cls_hard_raw_fwd(ptr(sc), ptr(pr), ptr(gt), B, H, W, C, threshold, ptr(out), ptr(ws), ws.numel(), stream()))
+    return out
 
 
-def smooth_l1_loss_vertex(vertex_pred, vertex_targets, vertex_weights, sigma=1.0, want_grad=False, upstream=1.0):
-    """lib/fcn/train.py:564-573.  Returns (loss [1], sum of weights [1][, grad wrt vertex_pred])."""
-    p = require_cuda("vertex_pred", vertex_pred, torch.float32, vertex_pred.dim())
-    t = require_cuda("vertex_targets", vertex_targets, torch.float32, vertex_pred.dim())
-    w = require_cuda("vertex_weights", vertex_weights, torch.float32, vertex_pred.dim())
-    if t.shape != p.shape or w.shape != p.shape:
-        raise ValueError("vertex_pred, vertex_targets and vertex_weights must have the same shape")
-    out = torch.empty((2,), dtype=torch.float32, device=p.device)
-    grad = torch.empty_like(p) if want_grad else None
-    ws = _workspace(p.device)
-    check(lib().pcnn_smooth_l1_vertex_fwd(ptr(p), ptr(t), ptr(w), p.numel(), sigma, ptr(out), upstream,
-                                          ptr(grad), ptr(ws), ws.numel(), stream()))
-    return (out[0:1], out[1:2], grad) if want_grad else (out[0:1], out[1:2])
-
-
-def vertex_loss_from_centers(vertex_pred, im_label, centers, w_inside=1.0, sigma=1.0, want_grad=False, upstream=1.0):
-    """smooth_l1_loss_vertex(vertex_pred, *generate_vertex_targets(im_label, centers, w_inside)) in one pass that never
-    builds the target / weight tensors.  Returns (loss [1], sum of weights [1][, grad wrt vertex_pred])."""
-    p = require_cuda("vertex_pred", vertex_pred, torch.float32, 4)
+def loss_vertex(lowres, bias_vertex, im_label, centers, w_inside, sigma=1.0, vertmap=None, extents=None):
+    """The training step's loss_vertex: smooth_l1_loss_vertex (lib/fcn/train.py:564-573) of vertex_pred against the targets of
+    generate_vertex_targets(im_label, centers, w_inside), or with vertmap [B,H,W,3] and extents [C,3] given, of
+    generate_vertex_targets_3d(im_label, vertmap, centers, extents, w_inside); the targets and weights are never built.  The
+    vertex values come from the 1/8-resolution head tensor lowres [B,H/8,W/8,4C] + bias_vertex [3C] (bit-identical to the dense
+    vertex_pred that pcnn_up8_heads writes from them).  Returns the [2] buffer (loss, sum of weights) that the backward pass reads."""
     lab = require_cuda("im_label", im_label, torch.int32, 3)
     cen = require_cuda("centers", centers, torch.float32, 3)
+    lr = require_cuda("lowres", lowres, torch.float32, 4)
+    bv = require_cuda("bias_vertex", bias_vertex, torch.float32, 1)
     B, H, W = lab.shape
     C = cen.shape[1]
-    if tuple(p.shape) != (B, H, W, 3 * C) or cen.shape[0] != B or cen.shape[2] != 3:
-        raise ValueError("vertex_pred must be [B,H,W,3C] and centers [B,C,3]")
-    out = torch.empty((2,), dtype=torch.float32, device=p.device)
-    grad = torch.empty_like(p) if want_grad else None
-    ws = _workspace(p.device)
-    check(lib().pcnn_vertex_loss_fused_fwd(ptr(p), ptr(lab), ptr(cen), B, H, W, C, w_inside, sigma, ptr(out), upstream,
-                                           ptr(grad), ptr(ws), ws.numel(), stream()))
-    return (out[0:1], out[1:2], grad) if want_grad else (out[0:1], out[1:2])
-
-
-def vertex_loss_from_coords(vertex_pred, im_label, vertmap, centers, extents, w_inside=1.0, sigma=1.0, want_grad=False, upstream=1.0,
-                            bias_vertex=None):
-    """smooth_l1_loss_vertex(vertex_pred, *generate_vertex_targets_3d(im_label, vertmap, centers, extents, w_inside)) in one pass that
-    never builds the target / weight tensors.  vertex_pred is the dense [B,H,W,3C] tensor, or with bias_vertex [3C] given, the
-    1/8-resolution head tensor [B,H/8,W/8,4C] whose vertex values are formed on demand (bit-identical; no gradient then).
-    Returns (loss [1], sum of weights [1][, grad wrt vertex_pred])."""
-    lab, vm, cen, ext = _coord_inputs(im_label, vertmap, centers, extents)
-    B, H, W = lab.shape
-    C = cen.shape[1]
-    p = require_cuda("vertex_pred", vertex_pred, torch.float32, 4)
-    out = torch.empty((2,), dtype=torch.float32, device=p.device)
-    ws = _workspace(p.device)
-    if bias_vertex is not None:
-        if want_grad:
-            raise ValueError("the low-resolution source has no gradient output")
-        bv = require_cuda("bias_vertex", bias_vertex, torch.float32, 1)
-        if tuple(p.shape) != (B, H // 8, W // 8, 4 * C) or bv.numel() != 3 * C:
-            raise ValueError("the low-resolution source must be [B,H/8,W/8,4C] with a [3C] bias")
-        check(lib().pcnn_vertex_loss_coord_lowres_fwd(ptr(p), ptr(bv), ptr(lab), ptr(vm), ptr(cen), ptr(ext), B, H, W, C, w_inside,
-                                                      sigma, ptr(out), ptr(ws), ws.numel(), stream()))
-        return out[0:1], out[1:2]
-    if tuple(p.shape) != (B, H, W, 3 * C):
-        raise ValueError("vertex_pred must be [B,H,W,3C]")
-    grad = torch.empty_like(p) if want_grad else None
-    check(lib().pcnn_vertex_loss_coord_fwd(ptr(p), ptr(lab), ptr(vm), ptr(cen), ptr(ext), B, H, W, C, w_inside, sigma, ptr(out),
-                                           upstream, ptr(grad), ptr(ws), ws.numel(), stream()))
-    return (out[0:1], out[1:2], grad) if want_grad else (out[0:1], out[1:2])
+    if cen.shape[0] != B or cen.shape[2] != 3 or tuple(lr.shape) != (B, H // 8, W // 8, 4 * C) or bv.numel() != 3 * C:
+        raise ValueError("lowres must be [B,H/8,W/8,4C] with a [3C] bias, and centers [B,C,3]")
+    out = torch.empty((2,), dtype=torch.float32, device=lr.device)
+    ws = _workspace(lr.device)
+    if vertmap is None:
+        check(lib().pcnn_vertex_loss_fused_lowres_fwd(ptr(lr), ptr(bv), ptr(lab), ptr(cen), B, H, W, C, w_inside, sigma, ptr(out), ptr(ws),
+                                                      ws.numel(), stream()))
+    else:
+        lab, vm, cen, ext = _coord_inputs(lab, vertmap, cen, extents)
+        check(lib().pcnn_vertex_loss_coord_lowres_fwd(ptr(lr), ptr(bv), ptr(lab), ptr(vm), ptr(cen), ptr(ext), B, H, W, C, w_inside, sigma,
+                                                      ptr(out), ptr(ws), ws.numel(), stream()))
+    return out

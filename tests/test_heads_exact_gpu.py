@@ -227,29 +227,19 @@ def test_up8_heads_exact(cuda, C):
 # ---------------------------------------------------------------------------------------------------------------------
 # 6. the classification loss of the training step (k_loss_cls_hard_raw)
 # ---------------------------------------------------------------------------------------------------------------------
-def _loss(fn, score, prob, gt, thr, ws):
-    from posecnn_b200._lib import check, lib, ptr, stream
-    B, H, W, C = score.shape
-    out = torch.full((2,), 7.0, device=score.device)
-    if fn == "raw":
-        check(lib().pcnn_loss_cls_hard_raw_fwd(ptr(score), ptr(prob), ptr(gt), B, H, W, C, thr, ptr(out), ptr(ws), ws.numel(), stream()))
-    else:
-        check(lib().pcnn_loss_cls_hard_fwd(ptr(score), ptr(prob), ptr(gt), B, H, W, C, thr, ptr(out), 1.0, ptr(None), ptr(ws), ws.numel(),
-                                           stream()))
-    return out
-
-
-@pytest.mark.parametrize("C", [2, 22, 50])
-def test_loss_cls_hard_raw(cuda, C):
-    """pcnn_loss_cls_hard_raw_fwd (the step's loss_cls) at 2 x 480 x 640: count exact, loss within the bound derived from
-    fp32 expf / logf (heads_ref.loss_cls_hard_raw) of the float64 log-softmax reference, also with raw scores of +-80 where an
-    unshifted exp overflows; two launches bit-identical; an all-ignore batch gives 0 and 0; and pcnn_loss_cls_hard_fwd fed the
-    reference log-softmax rounded to fp32 agrees within the sum of the two kernels' bounds."""
-    from posecnn_b200 import train_ops
-    B, H, W, thr = 2, 480, 640, 0.5
+@pytest.mark.parametrize("C,thr", [pytest.param(C, 0.5, id=str(C)) for C in (2, 22, 50)] +
+                         [pytest.param(C, t, id=f"{C}-thr{t}") for t in (1.0, 0.4) for C in (2, 22, 50)])
+def test_loss_cls_hard_raw(cuda, C, thr):
+    """train_ops.loss_cls (pcnn_loss_cls_hard_raw_fwd, the step's loss_cls) at 2 x 480 x 640: count exact, loss within the bound
+    derived from fp32 expf / logf (heads_ref.loss_cls_hard_raw) of the float64 log-softmax reference, also with raw scores of +-80
+    where an unshifted exp overflows; two launches bit-identical; an all-ignore batch gives 0 and 0; and the un-fused composition
+    through the Hardlabel op (its mask times the float64 log-softmax) selects the same pixels and agrees within 1e-5 relative."""
+    from posecnn_b200.hard_label_layer import hard_label_op
+    from posecnn_b200.train_ops import loss_cls
+    B, H, W = 2, 480, 640
     npix = B * H * W
     blocks = R.NUM_SMS * 4
-    print(f"C={C}: {npix} pixels on {blocks} x 256 threads, {-(-npix // (blocks * 256))} grid-stride iterations")
+    print(f"C={C}, threshold {thr}: {npix} pixels on {blocks} x 256 threads, {-(-npix // (blocks * 256))} grid-stride iterations")
     g = torch.Generator().manual_seed(300 + C)
     score = R.dyadic((B, H, W, C), -8, 8, 0.125, g)
     hot = R.int_operands((B, H, W), 0, 19, g) == 0                          # 5 % of the pixels: one channel +80, one -80
@@ -259,20 +249,18 @@ def test_loss_cls_hard_raw(cuda, C):
     prob = R.dyadic((B, H, W, C), 0, 1, 0.125, g)
     gt = R.int_operands((B, H, W), -2, C, g).to(torch.int32)                # -2 and C: out of range, ignored like -1
     score, prob, gt, hot = score.to(cuda), prob.to(cuda), gt.to(cuda), hot.to(cuda)
-    ws = train_ops._workspace(cuda)
-    a = _loss("raw", score, prob, gt, thr, ws)
-    b = _loss("raw", score, prob, gt, thr, ws)
+    a = loss_cls(score, prob, gt, thr)
+    b = loss_cls(score, prob, gt, thr)
     loss, n, bound, logsm = R.loss_cls_hard_raw(score, prob, gt, thr)
-    hard = _loss("hard", logsm.float(), prob, gt, thr, ws)
     sel = ((gt >= 0) & (gt < C) & ((gt > 0) | (prob[..., 0] < thr)))
     assert bool((sel & hot & (score.gather(-1, gt.clamp(0, C - 1).long()[..., None])[..., 0] == -80)).any())
-    t = logsm.gather(-1, gt.clamp(0, C - 1).long()[..., None])[..., 0]
-    bound_hard = float((R.ulp32(t) * sel).sum() / n) + 2.0 ** -23 * abs(loss)
     print(f"  loss {a[0].item():.9f} ref {loss:.9f} |err| {abs(a[0].item() - loss):.3e} bound {bound:.3e}; count {int(a[1].item())}")
     assert torch.equal(bits(a), bits(b)), "two launches differ"
     assert a[1].item() == n
     assert abs(a[0].item() - loss) <= bound
-    assert hard[1].item() == n
-    assert abs(a[0].item() - hard[0].item()) <= bound + bound_hard
-    none = _loss("raw", score, prob, torch.full_like(gt, -1), thr, ws)
+    m = hard_label_op.hard_label(prob, gt, thr).double()
+    comp = float(-(m * logsm).sum() / (m.sum() + 1e-10))
+    assert m.sum().item() == n
+    assert abs(a[0].item() - comp) <= 1e-5 * abs(comp)
+    none = loss_cls(score, prob, torch.full_like(gt, -1), thr)
     assert none.tolist() == [0.0, 0.0]

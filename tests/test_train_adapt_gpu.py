@@ -380,18 +380,21 @@ def test_inference_domain_outputs_and_graph(cuda):
     assert "fc9/weights" not in plain.params
 
 
-def test_training_losses_adds_loss_domain(cuda):
-    """training_losses() on an is_train network's forward: loss_domain = adapt_weight * mean cross entropy of the rows."""
-    from posecnn_b200.networks.vgg16_convs import training_losses
+def test_step_adds_loss_domain(cuda):
+    """The adaptation step's loss_domain = adapt_weight * mean cross entropy of Trainer.forward's domain_score rows against
+    label_domain (0 on a labelled batch), and step() adds it to the other three losses."""
+    from posecnn_b200.train import Trainer
     args, _, _ = make_inputs(cuda)
-    data, gt, centers, meta, ext, gtp, pts, sym = args
-    net = make_net(cuda, adaptation=True)
-    L = net.forward(data, meta, ext, poses=gtp, want_prob=True, want_score=True)
-    out = training_losses(net, L, gt, None, None, pts, sym, centers=centers, adapt_weight=0.5)
+    gt, centers = args[1], args[2]
+    tr = Trainer(make_net(cuda, adaptation=True), lr=0.01, adapt_weight=0.5)
+    A = tr.forward(*args)
+    tr.backward(A, gt, centers)
     torch.cuda.synchronize()
-    z, lab = L["domain_score"].double(), L["label_domain"].long()
+    z, lab = A["domain_score"].double(), A["label_domain"].long()
     want = 0.5 * (torch.logsumexp(z, 1) - z.gather(1, lab[:, None])[:, 0]).mean().item()
     assert not bool(lab.any())
+    assert abs(A["loss_domain"].item() - want) < 1e-5 * max(1.0, want)
+    out = tr.step(*args)
     assert abs(out["loss_domain"].item() - want) < 1e-5 * max(1.0, want)
     assert torch.allclose(out["loss"], out["loss_cls"] + out["loss_vertex"] + out["loss_pose"] + out["loss_domain"])
 

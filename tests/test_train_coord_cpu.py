@@ -32,7 +32,7 @@ def test_restatement_equals_reference_golden():
     assert len({int(c) for c in np.unique(lab[1]) if c > 0}) >= 3
 
 
-def test_coord_entry_points_check_arguments(native_lib):
+def test_coord_target_and_loss_entries_check_arguments(native_lib):
     f1 = 1.0
     buf = ctypes.create_string_buffer(64)                      # any non-NULL host address: the checks fail before it is read
     ws = 1 << 20
@@ -43,19 +43,17 @@ def test_coord_entry_points_check_arguments(native_lib):
     assert b"vertex_targets_3d: bad shape" in native_lib.pcnn_last_error()
     assert native_lib.pcnn_vertex_targets_3d_fwd(buf, buf, buf, buf, 65536, 256, 256, 6, f1, buf, buf, None) == -1
     assert b"too many pixels" in native_lib.pcnn_last_error()
-    # fused losses: vertmap and extents are required on top of the 2-D twin's tensors; sigma > 0; lowres needs H, W % 8 == 0
-    assert native_lib.pcnn_vertex_loss_coord_fwd(buf, buf, None, buf, buf, 1, 8, 8, 6, f1, f1, buf, f1, None, buf, ws, None) == -1
-    assert b"vertex_loss_coord: NULL tensor pointer" in native_lib.pcnn_last_error()
-    assert native_lib.pcnn_vertex_loss_coord_fwd(buf, buf, buf, buf, None, 1, 8, 8, 6, f1, f1, buf, f1, None, buf, ws, None) == -1
-    assert b"vertex_loss_coord: NULL tensor pointer" in native_lib.pcnn_last_error()
-    assert native_lib.pcnn_vertex_loss_coord_fwd(buf, buf, buf, buf, buf, 1, 8, 8, 6, f1, 0.0, buf, f1, None, buf, ws, None) == -1
-    assert b"vertex_loss_coord: bad arguments" in native_lib.pcnn_last_error()
-    assert native_lib.pcnn_vertex_loss_coord_fwd(buf, buf, buf, buf, buf, 1, 8, 8, 6, f1, f1, buf, f1, None, buf, 16, None) == -1
-    assert b"vertex_loss_coord: workspace too small" in native_lib.pcnn_last_error()
+    # fused loss: vertmap and extents are required on top of the 2-D twin's tensors; sigma > 0; H, W % 8 == 0; workspace size
     assert native_lib.pcnn_vertex_loss_coord_lowres_fwd(buf, None, buf, buf, buf, buf, 1, 64, 96, 22, f1, f1, buf, buf, ws, None) == -1
     assert b"vertex_loss_coord_lowres: NULL tensor pointer" in native_lib.pcnn_last_error()
     assert native_lib.pcnn_vertex_loss_coord_lowres_fwd(buf, buf, buf, None, buf, buf, 1, 64, 96, 22, f1, f1, buf, buf, ws, None) == -1
     assert b"vertex_loss_coord_lowres: NULL tensor pointer" in native_lib.pcnn_last_error()
+    assert native_lib.pcnn_vertex_loss_coord_lowres_fwd(buf, buf, buf, buf, buf, None, 1, 64, 96, 22, f1, f1, buf, buf, ws, None) == -1
+    assert b"vertex_loss_coord_lowres: NULL tensor pointer" in native_lib.pcnn_last_error()
+    assert native_lib.pcnn_vertex_loss_coord_lowres_fwd(buf, buf, buf, buf, buf, buf, 1, 64, 96, 22, f1, 0.0, buf, buf, ws, None) == -1
+    assert b"vertex_loss_coord_lowres: bad arguments" in native_lib.pcnn_last_error()
+    assert native_lib.pcnn_vertex_loss_coord_lowres_fwd(buf, buf, buf, buf, buf, buf, 1, 64, 96, 22, f1, f1, buf, buf, 16, None) == -1
+    assert b"vertex_loss_coord_lowres: workspace too small" in native_lib.pcnn_last_error()
     assert native_lib.pcnn_vertex_loss_coord_lowres_fwd(buf, buf, buf, buf, buf, buf, 1, 60, 96, 22, f1, f1, buf, buf, ws, None) == -1
     assert b"vertex_loss_coord_lowres: bad arguments" in native_lib.pcnn_last_error()
 

@@ -1,5 +1,5 @@
 """Object-coordinate (VERTEX_REG_3D) training on the GPU: the materialised 3-D targets against the reference's own lines, the fused
-loss (dense and 1/8-resolution sources) against smooth_l1_loss_vertex on the materialised blobs, the up-sampling adjoint's 3-D mode
+loss (1/8-resolution source) against the oracle's smooth_l1_loss_vertex on the 3-D targets, the up-sampling adjoint's 3-D mode
 against torch, the training step against the autograd graph, its contents, a short training run whose weights then estimate poses
 on an inference network, and two ranks.  Every measured error is printed."""
 
@@ -8,6 +8,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from oracle import oracle
 from posecnn_b200 import synth
 from tests.test_train_coord_cpu import load_golden
 from tests.train_coord_ref import vertex_targets_3d
@@ -74,9 +75,13 @@ def test_targets_3d_equal_reference_golden(cuda):
 # 2. fused loss
 # ---------------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("C", [2, 22])
-def test_fused_coord_loss_equals_materialised(cuda, C):
-    """vertex_loss_from_coords (dense vertex_pred, with gradient; and the 1/8-resolution source) == smooth_l1_loss_vertex on the
-    materialised blobs: loss within 1e-6 relative, gradient identical; dense and low-resolution sources bit-identical."""
+def test_coord_loss_vertex_against_oracle(cuda, C):
+    """train_ops.loss_vertex with vertmap / extents (the step's 3-D loss_vertex from the 1/8-resolution head tensor) against
+    oracle.smooth_l1_loss_vertex on the dense vertex_pred that pcnn_up8_heads writes from the same tensor and the 3-D targets of
+    tests/train_coord_ref.vertex_targets_3d (bit-exact to the reference's), sigma 1 and 2.5: sum of weights exact, two launches
+    bit-identical, loss within 1e-6 relative.  That bound is the one the fused kernel was held to against smooth L1 on the
+    materialised blobs: vertex values and targets are bit-identical, each term is the same fp32 expression, and the float64 sums
+    differ only in order, so the quotient's fp32 rounding (2^-24 relative) dominates."""
     from posecnn_b200 import train_ops
     from posecnn_b200._lib import check, lib, ptr, stream
     B, H, W = 2, 240, 320
@@ -87,19 +92,18 @@ def test_fused_coord_loss_equals_materialised(cuda, C):
     label = torch.empty((B, H, W), dtype=torch.int32, device=cuda)
     vertex = torch.empty((B, H, W, 3 * C), device=cuda)
     check(lib().pcnn_up8_heads(ptr(lowres), ptr(bs), ptr(bv), B, H // 8, W // 8, C, ptr(label), ptr(vertex), ptr(None), ptr(None), stream()))
+    vp = vertex.cpu().numpy()
+    vt, vw = vertex_targets_3d(sc["label"], sc["coords"], cen, sc["extents"], 10.0)
     lab, vm, cn, ext = T(sc["label"], cuda), T(sc["coords"], cuda), T(cen, cuda), T(sc["extents"], cuda)
     for sigma in (1.0, 2.5):
-        vt, vw = train_ops.generate_vertex_targets_3d(lab, vm, cn, ext, 10.0)
-        l0, w0, g0 = train_ops.smooth_l1_loss_vertex(vertex, vt, vw, sigma, want_grad=True, upstream=0.7)
-        l1, w1, g1 = train_ops.vertex_loss_from_coords(vertex, lab, vm, cn, ext, 10.0, sigma, want_grad=True, upstream=0.7)
-        l2, w2 = train_ops.vertex_loss_from_coords(lowres, lab, vm, cn, ext, 10.0, sigma, bias_vertex=bv)
-        torch.cuda.synchronize()
-        print(f"C = {C}, sigma {sigma}: sum w {w0.item():.0f}, loss {l0.item():.6f} materialised / {l1.item():.6f} fused "
-              f"(rel {abs(l0.item() - l1.item()) / abs(l0.item()):.2e})")
-        assert float(w0.item()) == float(w1.item()) == float(w2.item()) > 0
-        assert abs(float(l0.item()) - float(l1.item())) <= 1e-6 * abs(float(l0.item()))
-        assert torch.equal(g0, g1)
-        assert float(l1.item()) == float(l2.item())
+        out = train_ops.loss_vertex(lowres, bv, lab, cn, 10.0, sigma, vertmap=vm, extents=ext)
+        again = train_ops.loss_vertex(lowres, bv, lab, cn, 10.0, sigma, vertmap=vm, extents=ext)
+        want, _ = oracle.smooth_l1_loss_vertex(vp, vt, vw, sigma)
+        print(f"C = {C}, sigma {sigma}: sum w {out[1].item():.0f}, loss {out[0].item():.7f} / oracle {want:.7f} "
+              f"(rel {abs(out[0].item() - want) / abs(want):.2e})")
+        assert float(out[1].item()) == float(vw.astype(np.float64).sum()) > 0
+        assert abs(float(out[0].item()) - want) <= 1e-6 * abs(want)
+        assert torch.equal(out, again)
     # the unlisted object's pixels carry no weight
     c0 = int(sc["poses"][0][1])
     assert (sc["label"][0] == c0).any() and not bool(vw[0, ..., 3 * c0:3 * c0 + 3].any())
