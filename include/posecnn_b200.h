@@ -495,6 +495,34 @@ int pcnn_coord_pose2d_fwd(const int32_t* label, const float* vertex, const float
                           int num_meta, const float* extents, const uint64_t* keys, int B, int H, int W, int C, float* poses, float* info,
                           int32_t* trace_hyp, int32_t* trace_round, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---------------------------------------------------------------------------------------
+ * Evaluation of the test-time records (csrc/evaluate.cu, DESIGN.md 14): the scorer of lib/datasets/lov.py:397-680 and
+ * linemod.py:626-760 on the device.  Every output accumulates (the caller zeroes it once); counts are int64; 2 <= C <= 128.
+ *  pcnn_eval_confusion   gt_label, label [num_pixels] int32 -> hist [C,C] += the confusion matrix of fast_hist
+ *      (datasets/imdb.py:123-125): row = gt, column = prediction; a pixel counts only when 0 <= gt < C.  A prediction outside
+ *      [0, C) is an argument error: it is not counted, and status[0] += the number of such pixels.
+ *  pcnn_eval_pose_errors   scores 1 to 4 pose sets (poses0..3 [cap,7] = (qw,qx,qy,qz, tx,ty,tz), sharing rois [cap, roi_stride]
+ *      with image = rois[:,0], class = rois[:,1]) against gt_rows [num_gt,14] = (image, class, [R | t] 3x4 row-major).
+ *      Rows k < *num_rows (NULL = cap; a value outside [0, cap] is clamped and counts in status[1]).  Pairing as lov.py:576-628:
+ *      every gt j with 0 < class < C counts once in counts[s][0][class] (count_all) and pairs with every row of the same image and
+ *      class; pairs are gt-major, rows ascending, so duplicate detections each form a pair.  A gt of a foreground class whose
+ *      image - batch_offset is outside [0, B) is not scored and counts in status[1].
+ *      Per pair p < *num_pairs: pairs [num_gt*cap, 2] = (j, k); per set s: errors [s][p] = (re deg, te, ADD or ADD-S, reproj px)
+ *      f64, flags [s][p] = bit0 error < threshold[class] (counts[s][1][class] += 1), bit1 reproj < 5 px (counts[s][2][class] += 1),
+ *      bit2 the eggbox flip was applied.  symmetric [C] > 0: ADD-S (adi); flip_z [C] > 0: an estimate more than 90 degrees off is
+ *      scored for reprojection as R diag(-1,-1,1) (linemod.py:727-733).  K = meta[image - batch_offset, 0:9]; points [C,P,3],
+ *      P <= 4096; num_gt <= 4096.  counts [num_sets,3,C].  Deterministic, no host synchronisation, CUDA-graph capturable.
+ *  pcnn_eval_gt_rows_from_blob   pose_blob [n,13] (image, class, box, qw,qx,qy,qz, tx,ty,tz) -> gt_rows [n,14], R by quat2mat.
+ */
+int pcnn_eval_confusion(const int32_t* gt_label, const int32_t* label, size_t num_pixels, int C, int64_t* hist, int64_t* status,
+                        void* stream);
+int pcnn_eval_pose_errors(const float* gt_rows, int num_gt, const float* rois, int roi_stride, int cap, const int32_t* num_rows,
+                          const float* poses0, const float* poses1, const float* poses2, const float* poses3, int num_sets,
+                          const float* meta, int num_meta, int B, int batch_offset, const float* points, int C, int P,
+                          const float* symmetric, const float* threshold, const float* flip_z, int32_t* pairs, double* errors,
+                          int32_t* flags, int32_t* num_pairs, int64_t* counts, int64_t* status, void* stream);
+int pcnn_eval_gt_rows_from_blob(const float* pose_blob, int n, float* gt_rows, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
