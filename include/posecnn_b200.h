@@ -230,7 +230,7 @@ int pcnn_add_to_bf16(const void* a_bf16, const void* b_bf16, const float* b_f32,
  *  pcnn_up8_heads_bwd_ex  gradient of loss_cls (Hardlabel-selected cross entropy through log-softmax and the ReLU of `score`) and of
  *                         loss_vertex (smooth L1 on the labelled pixels' own class) w.r.t. the low-resolution head tensor, formed from
  *                         the loss structure on the fly: d_sc [B,h,w,Cs], d_vt [B,h,w,Cv] bf16 (padding channels zero), dbias [4C]
- *                         (C = 2, or C even in 6..50); the labelled pixels' vertex values come from vertex_pred [B,H,W,3C], or
+ *                         (C = 2, C even in 6..50, or C = 9); the labelled pixels' vertex values come from vertex_pred [B,H,W,3C], or
  *                         with vertex_pred == NULL from the low-resolution head tensor `lowres` [B,h,w,4C] + bias_vertex [3C];
  *                         workspace >= 16 C B ceil(h / 16) ceil(w / S) bytes, S = 16 cells at C = 2 and 4 otherwise (4 C floats per CTA)
  *  pcnn_pose_chain_bwd    Averagedistance's bottom_diff through l2_normalize, * poses_weight and tanh -> d fc8 pre-activation (fp16)
@@ -327,7 +327,8 @@ int pcnn_domain_grad_merge(const void* a_f16, float scale_a, const void* b_f16, 
 int pcnn_lowres_heads(const void* score4, const void* score5, const void* vert4, const void* vert5,
                       const float* w_score, const float* w_vertex, int B, int h, int w, int Cs, int Cv, int C,
                       float* lowres, void* stream);
-/* vertex == NULL: label-only mode (label_2d / prob / score only; see pcnn_hough_vote_fwd_ex for the consumer) */
+/* 2 <= C <= 128, either parity.  vertex == NULL: label-only mode (label_2d / prob / score only; see pcnn_hough_vote_fwd_ex for the
+ * consumer) */
 int pcnn_up8_heads(const float* lowres, const float* bias_score, const float* bias_vertex, int B, int h, int w,
                    int C, int32_t* label, float* vertex, float* prob, float* score, void* stream);
 /* depthwise bilinear conv2d_transpose (k x k, stride s, SAME) on f32 NHWC — un-fused reference path */

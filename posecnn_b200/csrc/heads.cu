@@ -223,15 +223,19 @@ k_lowres_heads(const __nv_bfloat16* __restrict__ s4 /*[B,h,w,Cs]*/, const __nv_b
 // instructions, 24 % of them IMAD address math, before the change).
 // Thread roles: threads [0, nv) own one vertex channel pair of one cell phase (consecutive lanes = consecutive channel
 // pairs -> contiguous 8-byte stores), threads [nv, nv + ns) own one score channel pair.
+// CPT = channels per thread.  2: C even, the roles above.  1: C odd, where a pixel's score row, its vertex row and the vertex
+// part of a low-resolution row are not 8-byte aligned: a role owns ONE channel (4-byte loads and stores, consecutive lanes still
+// on consecutive channels), so a cell phase takes 4C roles; at C >= 65 that exceeds the CTA and a thread loops over the roles
+// with stride 256.
 // ---------------------------------------------------------------------------------------------
-template <int CT>
+template <int CT, int CPT>
 __global__ void __launch_bounds__(256)
 k_up8_heads(const float* __restrict__ lr /*[B,h,w,4C]*/, const float* __restrict__ bias_s /*[C]*/,
             const float* __restrict__ bias_v /*[3C]*/, int h, int w, int C_rt, int seg_cells, int* __restrict__ label /*[B,8h,8w]*/,
             float* __restrict__ vertex /*[B,8h,8w,3C]*/, float* __restrict__ prob /*[B,8h,8w,C] or null*/,
             float* __restrict__ score_out /*[B,8h,8w,C] or null*/)
 {
-    // C even: every channel pair is one 8-byte vector (vertex rows are 3C floats = 8-byte aligned).
+    // CPT = 2, C even: every channel pair is one 8-byte vector (vertex rows are 3C floats = 8-byte aligned).
     extern __shared__ float smem_f[];
     const int C = CT ? CT : C_rt;
     const int No = 4 * C, W = 8 * w, H = 8 * h, N2 = No / 2, C2 = C / 2, V2 = 3 * C2;
@@ -248,7 +252,19 @@ k_up8_heads(const float* __restrict__ lr /*[B,h,w,4C]*/, const float* __restrict
     const float wy1 = (iy1 >= 0 && iy1 < h) ? deconv_w(y - 8 * iy1 + 4, 16) : 0.f;
     const float2* r0 = reinterpret_cast<const float2*>(lr + ((size_t)n * h + min(max(iy0, 0), h - 1)) * w * No);
     const float2* r1 = reinterpret_cast<const float2*>(lr + ((size_t)n * h + min(max(iy1, 0), h - 1)) * w * No);
-    if (vertex) {
+    if constexpr (CPT == 1) {
+        float* rows = smem_f - (size_t)s_lo * No;                                   // [s_lo, s_hi) x No scalars
+        const float* q0 = reinterpret_cast<const float*>(r0);
+        const float* q1 = reinterpret_cast<const float*>(r1);
+        if (vertex) {
+            for (int i = s_lo * No + t; i < s_hi * No; i += 256) rows[i] = up8_vblend(wy0, __ldg(q0 + i), wy1, __ldg(q1 + i));
+        } else {
+            for (int j = t; j < (s_hi - s_lo) * C; j += 256) {
+                const int i = (s_lo + j / C) * No + j % C;
+                rows[i] = up8_vblend(wy0, __ldg(q0 + i), wy1, __ldg(q1 + i));
+            }
+        }
+    } else if (vertex) {
         for (int i = s_lo * N2 + t; i < s_hi * N2; i += 256) {
             const float2 a = __ldg(r0 + i), b = __ldg(r1 + i);
             rowi[i] = make_float2(up8_vblend(wy0, a.x, wy1, b.x), up8_vblend(wy0, a.y, wy1, b.y));
@@ -269,66 +285,107 @@ k_up8_heads(const float* __restrict__ lr /*[B,h,w,4C]*/, const float* __restrict
     const float2 a = tx < 4 ? vl : vc, b = tx < 4 ? vc : vr;                                                   \
     float v0 = up8_hblend(wa, a.x, wb, b.x, bb.x);                                                             \
     float v1 = up8_hblend(wa, a.y, wb, b.y, bb.y);
-    // cell phases; vertex threads [0, gv*V2), score threads [gv*V2, gv*N2); label-only mode: all threads on scores
-    const int gv = vertex ? 256 / N2 : min(256 / C2, seg_cells);
-    const int nv = vertex ? gv * V2 : 0;
-    if (t < nv) {
-        const int g = t / V2, c2 = t - g * V2;                   // vertex channel pair c2 (channels C + 2 c2, +1 of a lowres cell)
-        const float2 bb = make_float2(bias_v[2 * c2], bias_v[2 * c2 + 1]);
-        const float2* src = rowi + C2 + c2;
-        float* vp = vertex + (rowbase + 8 * (size_t)(c_lo + g)) * 3 * C + 2 * c2;
-        const int vstep = gv * 8 * 3 * C;
-        for (int mx = c_lo + g; mx < c_hi; mx += gv, vp += vstep) {
-            const float2 vl = mx > 0 ? src[(mx - 1) * N2] : zero;
-            const float2 vc = src[mx * N2];
-            const float2 vr = mx + 1 < w ? src[(mx + 1) * N2] : zero;
+    if constexpr (CPT == 1) {
+        // one channel per role: vertex roles [0, gv 3C), score roles [gv 3C, gv 4C); label-only mode: score roles only
+        const float* rows = smem_f - (size_t)s_lo * No;
+        const int gv = vertex ? max(256 / No, 1) : min(256 / C, seg_cells);
+        const int nv = vertex ? gv * 3 * C : 0;
+        for (int u = t; u < nv + gv * C; u += 256) {
+            const bool vrole = u < nv;
+            const int uc = vrole ? u : u - nv, Cr = vrole ? 3 * C : C;
+            const int g = uc / Cr, c = uc - g * Cr;
+            const float bb = vrole ? bias_v[c] : bias_s[c];
+            const float* src = rows + (vrole ? C : 0) + c;
+            float* op = vrole ? vertex + (rowbase + 8 * (size_t)(c_lo + g)) * 3 * C + c : sc + 8 * (c_lo + g) * C + c;
+            float* gp = !vrole && score_out ? score_out + (rowbase + 8 * (size_t)(c_lo + g)) * C + c : nullptr;
+            for (int mx = c_lo + g; mx < c_hi; mx += gv, op += gv * 8 * Cr) {
+                const float vl = mx > 0 ? src[(mx - 1) * No] : 0.f;
+                const float vc = src[mx * No];
+                const float vr = mx + 1 < w ? src[(mx + 1) * No] : 0.f;
 #pragma unroll
-            for (int tx = 0; tx < 8; tx++) {
-                PCNN_UP8_BLEND(tx, v0, v1)
-                __stcs(reinterpret_cast<float2*>(vp + tx * 3 * C), make_float2(v0, v1));
+                for (int tx = 0; tx < 8; tx++) {
+                    const float wa = deconv_w(tx < 4 ? tx + 12 : tx + 4, 16), wb = deconv_w(tx < 4 ? tx + 4 : tx - 4, 16);
+                    const float v = up8_hblend(wa, tx < 4 ? vl : vc, wb, tx < 4 ? vc : vr, bb);
+                    if (vrole) {
+                        __stcs(op + tx * 3 * C, v);
+                    } else {
+                        op[tx * C] = fmaxf(v, 0.f);                       // `score` has a ReLU
+                        if (gp) gp[tx * C] = fmaxf(v, 0.f);
+                    }
+                }
+                if (gp) gp += gv * 8 * C;
             }
         }
-    } else if (t < nv + gv * C2) {
-        const int u = t - nv;
-        const int g = u / C2, c2 = u - g * C2;                   // score channel pair
-        const float2 bb = make_float2(bias_s[2 * c2], bias_s[2 * c2 + 1]);
-        const float2* src = rowi + c2;
-        float* sp = sc + 8 * (c_lo + g) * C + 2 * c2;
-        float* gp = score_out ? score_out + (rowbase + 8 * (size_t)(c_lo + g)) * C + 2 * c2 : nullptr;
-        for (int mx = c_lo + g; mx < c_hi; mx += gv, sp += gv * 8 * C) {
-            const float2 vl = mx > 0 ? src[(mx - 1) * N2] : zero;
-            const float2 vc = src[mx * N2];
-            const float2 vr = mx + 1 < w ? src[(mx + 1) * N2] : zero;
+    } else {
+        // cell phases; vertex threads [0, gv*V2), score threads [gv*V2, gv*N2); label-only mode: all threads on scores
+        const int gv = vertex ? 256 / N2 : min(256 / C2, seg_cells);
+        const int nv = vertex ? gv * V2 : 0;
+        if (t < nv) {
+            const int g = t / V2, c2 = t - g * V2;                   // vertex channel pair c2 (channels C + 2 c2, +1 of a lowres cell)
+            const float2 bb = make_float2(bias_v[2 * c2], bias_v[2 * c2 + 1]);
+            const float2* src = rowi + C2 + c2;
+            float* vp = vertex + (rowbase + 8 * (size_t)(c_lo + g)) * 3 * C + 2 * c2;
+            const int vstep = gv * 8 * 3 * C;
+            for (int mx = c_lo + g; mx < c_hi; mx += gv, vp += vstep) {
+                const float2 vl = mx > 0 ? src[(mx - 1) * N2] : zero;
+                const float2 vc = src[mx * N2];
+                const float2 vr = mx + 1 < w ? src[(mx + 1) * N2] : zero;
 #pragma unroll
-            for (int tx = 0; tx < 8; tx++) {
-                PCNN_UP8_BLEND(tx, v0, v1)
-                v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f);        // `score` has a ReLU (vgg16_convs.py:141, network.py:160)
-                *reinterpret_cast<float2*>(sp + tx * C) = make_float2(v0, v1);
-                if (gp) *reinterpret_cast<float2*>(gp + tx * C) = make_float2(v0, v1);
+                for (int tx = 0; tx < 8; tx++) {
+                    PCNN_UP8_BLEND(tx, v0, v1)
+                    __stcs(reinterpret_cast<float2*>(vp + tx * 3 * C), make_float2(v0, v1));
+                }
             }
-            if (gp) gp += gv * 8 * C;
+        } else if (t < nv + gv * C2) {
+            const int u = t - nv;
+            const int g = u / C2, c2 = u - g * C2;                   // score channel pair
+            const float2 bb = make_float2(bias_s[2 * c2], bias_s[2 * c2 + 1]);
+            const float2* src = rowi + c2;
+            float* sp = sc + 8 * (c_lo + g) * C + 2 * c2;
+            float* gp = score_out ? score_out + (rowbase + 8 * (size_t)(c_lo + g)) * C + 2 * c2 : nullptr;
+            for (int mx = c_lo + g; mx < c_hi; mx += gv, sp += gv * 8 * C) {
+                const float2 vl = mx > 0 ? src[(mx - 1) * N2] : zero;
+                const float2 vc = src[mx * N2];
+                const float2 vr = mx + 1 < w ? src[(mx + 1) * N2] : zero;
+#pragma unroll
+                for (int tx = 0; tx < 8; tx++) {
+                    PCNN_UP8_BLEND(tx, v0, v1)
+                    v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f);        // `score` has a ReLU (vgg16_convs.py:141, network.py:160)
+                    *reinterpret_cast<float2*>(sp + tx * C) = make_float2(v0, v1);
+                    if (gp) *reinterpret_cast<float2*>(gp + tx * C) = make_float2(v0, v1);
+                }
+                if (gp) gp += gv * 8 * C;
+            }
         }
     }
 #undef PCNN_UP8_BLEND
     __syncthreads();
     // arg-max over classes, lowest index wins ties (tf.argmax); softmax for prob_normalized (network.py:474-488)
     for (int x = 8 * c_lo + t; x < 8 * c_hi; x += 256) {
-        const float2* s2 = reinterpret_cast<const float2*>(sc + x * C);
-        float best = s2[0].x;
+        float best;
         int bi = 0;
-        if (s2[0].y > best) { best = s2[0].y; bi = 1; }
+        if constexpr (CPT == 1) {
+            const float* s1 = sc + x * C;
+            best = s1[0];
+            for (int c = 1; c < C; c++)
+                if (s1[c] > best) { best = s1[c]; bi = c; }
+        } else {
+            const float2* s2 = reinterpret_cast<const float2*>(sc + x * C);
+            best = s2[0].x;
+            if (s2[0].y > best) { best = s2[0].y; bi = 1; }
 #pragma unroll
-        for (int c = 1; c < (CT ? CT / 2 : 1); c++) {
-            const float2 v = s2[c];
-            if (v.x > best) { best = v.x; bi = 2 * c; }
-            if (v.y > best) { best = v.y; bi = 2 * c + 1; }
-        }
-        if (!CT)
-            for (int c = 1; c < C2; c++) {
+            for (int c = 1; c < (CT ? CT / 2 : 1); c++) {
                 const float2 v = s2[c];
                 if (v.x > best) { best = v.x; bi = 2 * c; }
                 if (v.y > best) { best = v.y; bi = 2 * c + 1; }
             }
+            if (!CT)
+                for (int c = 1; c < C2; c++) {
+                    const float2 v = s2[c];
+                    if (v.x > best) { best = v.x; bi = 2 * c; }
+                    if (v.y > best) { best = v.y; bi = 2 * c + 1; }
+                }
+        }
         label[rowbase + x] = bi;
         if (prob) {
             // softmax statistics of the pixel; the normalised row is written by the cooperative pass below
@@ -360,13 +417,14 @@ k_up8_heads(const float* __restrict__ lr /*[B,h,w,4C]*/, const float* __restrict
 // score channels are staged once (k_up8_heads re-stages two rows for every output row); per output row, thread =
 // (cell, class pair) blends vertically in registers, emits the cell's 8 pixels into a shared score row, and thread =
 // pixel takes the arg-max (lowest index on ties).  Same operation sequence as k_up8_heads (heads_common.cuh): identical
-// labels.  CT = compile-time class count (even).
+// labels.  CT = compile-time class count (even), CPT = channels per thread as in k_up8_heads: at CPT = 1 (C odd) the staged rows
+// are [3][w][C] scalars and a thread blends (cell, class).
 // ---------------------------------------------------------------------------------------------
 // 512 threads: the kernel is latency-bound (shared-memory chains between two barriers per output row); with 77 KB of shared
 // memory per CTA only two CTAs fit an SM, so the warps have to come from the CTA itself
 constexpr int kLabelThreads = 512;
 
-template <int CT>
+template <int CT, int CPT>
 __global__ void __launch_bounds__(kLabelThreads)
 k_up8_label(const float* __restrict__ lr /*[B,h,w,4C]*/, const float* __restrict__ bias_s /*[C]*/, int h, int w, int C_rt,
             int* __restrict__ label /*[B,8h,8w]*/)
@@ -377,11 +435,21 @@ k_up8_label(const float* __restrict__ lr /*[B,h,w,4C]*/, const float* __restrict
     float2* rows = reinterpret_cast<float2*>(smem_f);              // [3][w][C2]: low-resolution rows my - 1, my, my + 1 (score channels)
     float* sc = smem_f + (size_t)3 * w * C;                        // [W][C] scores of one output row
     const int my = blockIdx.x, n = blockIdx.y, t = threadIdx.x;
-    for (int i = t; i < 3 * w * C2; i += kLabelThreads) {
-        const int r = i / (w * C2), j = i - r * (w * C2);
-        const int cell = j / C2, c2 = j - cell * C2;
-        const int iy = min(max(my - 1 + r, 0), h - 1);             // clamped like k_up8_heads; out-of-range rows get weight 0
-        rows[i] = __ldg(reinterpret_cast<const float2*>(lr + (((size_t)n * h + iy) * w + cell) * No) + c2);
+    float* rows1 = smem_f;                                         // CPT = 1: [3][w][C]
+    if constexpr (CPT == 1) {
+        for (int i = t; i < 3 * w * C; i += kLabelThreads) {
+            const int r = i / (w * C), j = i - r * (w * C);
+            const int cell = j / C, c = j - cell * C;
+            const int iy = min(max(my - 1 + r, 0), h - 1);
+            rows1[i] = __ldg(lr + (((size_t)n * h + iy) * w + cell) * No + c);
+        }
+    } else {
+        for (int i = t; i < 3 * w * C2; i += kLabelThreads) {
+            const int r = i / (w * C2), j = i - r * (w * C2);
+            const int cell = j / C2, c2 = j - cell * C2;
+            const int iy = min(max(my - 1 + r, 0), h - 1);         // clamped like k_up8_heads; out-of-range rows get weight 0
+            rows[i] = __ldg(reinterpret_cast<const float2*>(lr + (((size_t)n * h + iy) * w + cell) * No) + c2);
+        }
     }
     __syncthreads();
     const float2 zero = make_float2(0.f, 0.f);
@@ -392,38 +460,66 @@ k_up8_label(const float* __restrict__ lr /*[B,h,w,4C]*/, const float* __restrict
         const float wy1 = (iy1 >= 0 && iy1 < h) ? deconv_w(y - 8 * iy1 + 4, 16) : 0.f;
         const float2* r0 = rows + (size_t)(iy0 - (my - 1)) * w * C2;     // staged slot of row iy0 (slot 0..2); clamping is
         const float2* r1 = rows + (size_t)(iy1 - (my - 1)) * w * C2;     // irrelevant where the weight is 0, identical otherwise
-        for (int i = t; i < w * C2; i += kLabelThreads) {
-            const int mx = i / C2, c2 = i - mx * C2;
-            const float2 bb = make_float2(__ldg(bias_s + 2 * c2), __ldg(bias_s + 2 * c2 + 1));
-            auto vb = [&](int cell) -> float2 {
-                const float2 a = r0[cell * C2 + c2], b = r1[cell * C2 + c2];
-                return make_float2(up8_vblend(wy0, a.x, wy1, b.x), up8_vblend(wy0, a.y, wy1, b.y));
-            };
-            const float2 vl = mx > 0 ? vb(mx - 1) : zero;
-            const float2 vc = vb(mx);
-            const float2 vr = mx + 1 < w ? vb(mx + 1) : zero;
-            float* sp = sc + (size_t)8 * mx * C + 2 * c2;
+        if constexpr (CPT == 1) {
+            const float* q0 = rows1 + (size_t)(iy0 - (my - 1)) * w * C;
+            const float* q1 = rows1 + (size_t)(iy1 - (my - 1)) * w * C;
+            for (int i = t; i < w * C; i += kLabelThreads) {
+                const int mx = i / C, c = i - mx * C;
+                const float bb = __ldg(bias_s + c);
+                auto vb = [&](int cell) -> float { return up8_vblend(wy0, q0[cell * C + c], wy1, q1[cell * C + c]); };
+                const float vl = mx > 0 ? vb(mx - 1) : 0.f;
+                const float vc = vb(mx);
+                const float vr = mx + 1 < w ? vb(mx + 1) : 0.f;
+                float* sp = sc + (size_t)8 * mx * C + c;
 #pragma unroll
-            for (int tx = 0; tx < 8; tx++) {
-                const float wa = deconv_w(tx < 4 ? tx + 12 : tx + 4, 16), wb = deconv_w(tx < 4 ? tx + 4 : tx - 4, 16);
-                const float2 a = tx < 4 ? vl : vc, b = tx < 4 ? vc : vr;
-                const float v0 = fmaxf(up8_hblend(wa, a.x, wb, b.x, bb.x), 0.f);      // `score` has a ReLU
-                const float v1 = fmaxf(up8_hblend(wa, a.y, wb, b.y, bb.y), 0.f);
-                *reinterpret_cast<float2*>(sp + tx * C) = make_float2(v0, v1);
+                for (int tx = 0; tx < 8; tx++) {
+                    const float wa = deconv_w(tx < 4 ? tx + 12 : tx + 4, 16), wb = deconv_w(tx < 4 ? tx + 4 : tx - 4, 16);
+                    sp[tx * C] = fmaxf(up8_hblend(wa, tx < 4 ? vl : vc, wb, tx < 4 ? vc : vr, bb), 0.f);   // `score` has a ReLU
+                }
+            }
+        } else {
+            for (int i = t; i < w * C2; i += kLabelThreads) {
+                const int mx = i / C2, c2 = i - mx * C2;
+                const float2 bb = make_float2(__ldg(bias_s + 2 * c2), __ldg(bias_s + 2 * c2 + 1));
+                auto vb = [&](int cell) -> float2 {
+                    const float2 a = r0[cell * C2 + c2], b = r1[cell * C2 + c2];
+                    return make_float2(up8_vblend(wy0, a.x, wy1, b.x), up8_vblend(wy0, a.y, wy1, b.y));
+                };
+                const float2 vl = mx > 0 ? vb(mx - 1) : zero;
+                const float2 vc = vb(mx);
+                const float2 vr = mx + 1 < w ? vb(mx + 1) : zero;
+                float* sp = sc + (size_t)8 * mx * C + 2 * c2;
+#pragma unroll
+                for (int tx = 0; tx < 8; tx++) {
+                    const float wa = deconv_w(tx < 4 ? tx + 12 : tx + 4, 16), wb = deconv_w(tx < 4 ? tx + 4 : tx - 4, 16);
+                    const float2 a = tx < 4 ? vl : vc, b = tx < 4 ? vc : vr;
+                    const float v0 = fmaxf(up8_hblend(wa, a.x, wb, b.x, bb.x), 0.f);      // `score` has a ReLU
+                    const float v1 = fmaxf(up8_hblend(wa, a.y, wb, b.y, bb.y), 0.f);
+                    *reinterpret_cast<float2*>(sp + tx * C) = make_float2(v0, v1);
+                }
             }
         }
         __syncthreads();
         for (int x = t; x < W; x += kLabelThreads) {
-            const float2* s2 = reinterpret_cast<const float2*>(sc + (size_t)x * C);
-            float best = s2[0].x;
-            int bi = 0;
-            if (s2[0].y > best) { best = s2[0].y; bi = 1; }
-            for (int c = 1; c < C2; c++) {
-                const float2 v = s2[c];
-                if (v.x > best) { best = v.x; bi = 2 * c; }
-                if (v.y > best) { best = v.y; bi = 2 * c + 1; }
+            if constexpr (CPT == 1) {
+                const float* s1 = sc + (size_t)x * C;
+                float best = s1[0];
+                int bi = 0;
+                for (int c = 1; c < C; c++)
+                    if (s1[c] > best) { best = s1[c]; bi = c; }
+                label[((size_t)n * 8 * h + y) * W + x] = bi;
+            } else {
+                const float2* s2 = reinterpret_cast<const float2*>(sc + (size_t)x * C);
+                float best = s2[0].x;
+                int bi = 0;
+                if (s2[0].y > best) { best = s2[0].y; bi = 1; }
+                for (int c = 1; c < C2; c++) {
+                    const float2 v = s2[c];
+                    if (v.x > best) { best = v.x; bi = 2 * c; }
+                    if (v.y > best) { best = v.y; bi = 2 * c + 1; }
+                }
+                label[((size_t)n * 8 * h + y) * W + x] = bi;
             }
-            label[((size_t)n * 8 * h + y) * W + x] = bi;
         }
         __syncthreads();
     }
@@ -489,20 +585,24 @@ extern "C" int pcnn_up8_heads(const float* lowres, const float* bias_score, cons
 {
     // vertex == NULL: label-only mode (label_2d / prob / score; the dense vertex_pred is not produced)
     PCNN_REQUIRE(lowres && bias_score && label && (bias_vertex || !vertex), "up8_heads: NULL tensor pointer");
-    PCNN_REQUIRE(C >= 1 && B >= 1 && h >= 1 && w >= 1, "up8_heads: bad shape");
+    PCNN_REQUIRE(C >= 2 && C <= 128, "up8_heads: num_classes must be in 2..128 (got %d)", C);
+    PCNN_REQUIRE(B >= 1 && h >= 1 && w >= 1, "up8_heads: bad shape");
     PCNN_REQUIRE(8 * h <= 65535 * 1 && B <= 65535, "up8_heads: image too tall for the launch grid");
-    PCNN_REQUIRE(C % 2 == 0 && 2 * C <= 256, "up8_heads: num_classes must be even and <= 128 (got %d)", C);
+    const bool odd = C % 2 != 0;   // odd C: the one-channel-per-thread forms (CPT = 1)
     if (!vertex && !prob && !score) {
         // label-only fast path: one CTA per low-resolution row (8 output rows), three staged rows + one score row in smem
         const size_t smem_l = sizeof(float) * ((size_t)3 * w * C + (size_t)8 * w * C);
         if (smem_l <= 200 * 1024 && h <= 65535) {
             dim3 grid_l(h, B);
             if (C == 22) {
-                PCNN_SMEM_OPTIN(k_up8_label<22>, 200 * 1024, "up8_label<22>");
-                k_up8_label<22><<<grid_l, kLabelThreads, smem_l, (cudaStream_t)stream>>>(lowres, bias_score, h, w, C, label);
+                PCNN_SMEM_OPTIN((k_up8_label<22, 2>), 200 * 1024, "up8_label<22>");
+                k_up8_label<22, 2><<<grid_l, kLabelThreads, smem_l, (cudaStream_t)stream>>>(lowres, bias_score, h, w, C, label);
+            } else if (odd) {
+                PCNN_SMEM_OPTIN((k_up8_label<0, 1>), 200 * 1024, "up8_label<0, odd>");
+                k_up8_label<0, 1><<<grid_l, kLabelThreads, smem_l, (cudaStream_t)stream>>>(lowres, bias_score, h, w, C, label);
             } else {
-                PCNN_SMEM_OPTIN(k_up8_label<0>, 200 * 1024, "up8_label<0>");
-                k_up8_label<0><<<grid_l, kLabelThreads, smem_l, (cudaStream_t)stream>>>(lowres, bias_score, h, w, C, label);
+                PCNN_SMEM_OPTIN((k_up8_label<0, 2>), 200 * 1024, "up8_label<0>");
+                k_up8_label<0, 2><<<grid_l, kLabelThreads, smem_l, (cudaStream_t)stream>>>(lowres, bias_score, h, w, C, label);
             }
             return check_launch("up8_label");
         }
@@ -511,14 +611,18 @@ extern "C" int pcnn_up8_heads(const float* lowres, const float* bias_score, cons
     size_t smem = sizeof(float) * ((size_t)(seg_cells + 2) * 4 * C + (size_t)8 * seg_cells * C + (size_t)16 * seg_cells);
     PCNN_REQUIRE(smem <= 200 * 1024, "up8_heads: segment does not fit shared memory (C = %d)", C);
     dim3 grid(8 * h, B, (w + seg_cells - 1) / seg_cells);
-    PCNN_SMEM_OPTIN(k_up8_heads<0>, 200 * 1024, "up8_heads<0>");
-    PCNN_SMEM_OPTIN(k_up8_heads<22>, 200 * 1024, "up8_heads<22>");
+    PCNN_SMEM_OPTIN((k_up8_heads<0, 2>), 200 * 1024, "up8_heads<0>");
+    PCNN_SMEM_OPTIN((k_up8_heads<22, 2>), 200 * 1024, "up8_heads<22>");
+    PCNN_SMEM_OPTIN((k_up8_heads<0, 1>), 200 * 1024, "up8_heads<0, odd>");
     if (C == 22)   // the YCB / LOV class count (lov_color_2d.yml:14): compile-time strides
-        k_up8_heads<22><<<grid, 256, smem, (cudaStream_t)stream>>>(lowres, bias_score, bias_vertex, h, w, C, seg_cells, label, vertex,
-                                                                   prob, score);
+        k_up8_heads<22, 2><<<grid, 256, smem, (cudaStream_t)stream>>>(lowres, bias_score, bias_vertex, h, w, C, seg_cells, label, vertex,
+                                                                      prob, score);
+    else if (odd)  // e.g. the multi-object LINEMOD model (linemod_color_2d.yml: 9 classes)
+        k_up8_heads<0, 1><<<grid, 256, smem, (cudaStream_t)stream>>>(lowres, bias_score, bias_vertex, h, w, C, seg_cells, label, vertex,
+                                                                     prob, score);
     else
-        k_up8_heads<0><<<grid, 256, smem, (cudaStream_t)stream>>>(lowres, bias_score, bias_vertex, h, w, C, seg_cells, label, vertex,
-                                                                  prob, score);
+        k_up8_heads<0, 2><<<grid, 256, smem, (cudaStream_t)stream>>>(lowres, bias_score, bias_vertex, h, w, C, seg_cells, label, vertex,
+                                                                     prob, score);
     return check_launch("up8_heads");
 }
 

@@ -17,6 +17,8 @@
 #include <cuda_fp16.h>
 #include <float.h>
 
+#include <type_traits>
+
 #include "common.cuh"
 #include "heads_common.cuh"
 
@@ -144,6 +146,9 @@ k_pack_lowres(const __nv_bfloat16* __restrict__ sc, int Cs, const __nv_bfloat16*
 // Strip width SC: 4 cells for C >= 6 (40 columns x C / 2 pairs = 120 .. 1000 threads).  At C = 2 a column is one thread, so a 4-cell
 // strip would be a 40-thread CTA; the two-class kernel takes 16 cells (136 threads), which also cuts the halo.
 // Redundant reads: (8 SC + 8) / (8 SC) x (8 rb + 8) / (8 rb) = 1.25 x 1.07 at SC = 4, 1.06 x 1.07 at SC = 16 (rb = 16).
+// CPT = channels per thread: 2 (C even, the pairs above) or 1 (C = 9: a pixel's score / prob row is not 8-byte aligned, so a thread
+// owns (output column, channel), kSCols * C threads with one running (lo, hi, bias) triple and 32-bit loads; the CTA still reads
+// one contiguous run of (8 SC + 8) * C floats per output row).
 // ---------------------------------------------------------------------------------------------
 constexpr int kStrip = 4;                           // strip width (cells) of the C >= 6 kernels
 constexpr int kStrip2 = 16;                         // strip width (cells) of the C = 2 kernel
@@ -152,9 +157,11 @@ constexpr int kStrip2 = 16;                         // strip width (cells) of th
 // extents (coord_scale / coord_target, heads_common.cuh) instead of the 2-D centre direction + log z.  The per-class (a_k, b_k) sit in
 // shared memory after the per-class listed flags (where the 2-D mode keeps log z: 6 C more floats), and the vertex-role thread loads
 // a pixel's three vertmap floats one row ahead, together with the label it already prefetches, and only for weighted pixels.
-// C = 2: 6 resident CTAs per SM caps the kernel at 64 registers without spills (-Xptxas -v); 8 would spill
-template <int CT, int SC, bool kCoord = false>
-__global__ void __launch_bounds__(CT ? (8 * SC + 8) * (CT / 2) : 1024, CT == 2 ? 6 : (CT ? 2 : 1))
+// C = 2: 6 resident CTAs per SM caps the kernel at 64 registers without spills (-Xptxas -v); 8 would spill.
+// CPT = 1 runs at C = 9 only (kSCols * 9 = 360 threads): bounding it at 360 x 2 CTAs instead of 1024 lifts the register cap from 64,
+// where the coordinate form spills, to 80
+template <int CT, int SC, bool kCoord, int CPT>
+__global__ void __launch_bounds__(CT ? (8 * SC + 8) * (CT / 2) : (CPT == 1 ? (8 * SC + 8) * 9 : 1024), CT == 2 ? 6 : (CT || CPT == 1 ? 2 : 1))
 k_up8_bwd_strip(const float* __restrict__ prob, const float* __restrict__ score, const int* __restrict__ gt, const float* __restrict__ cls_out,
                 float up_cls, float threshold, const float* __restrict__ vpred, const float* __restrict__ lowres,
                 const float* __restrict__ bias_v, const float* __restrict__ centers,
@@ -162,11 +169,12 @@ k_up8_bwd_strip(const float* __restrict__ prob, const float* __restrict__ score,
                 __nv_bfloat16* __restrict__ d_sc, __nv_bfloat16* __restrict__ d_vt, float* __restrict__ dbias_partial /*[ctas][4C]*/,
                 const float* __restrict__ vertmap, const float* __restrict__ extents)
 {
-    // C == 2 or C even in 6..50: thread = (output column, channel pair), kSCols * C / 2 threads; threads t < kSCols also own the
-    // vertex channels of output column t (at C = 2 that is every thread)
+    // C == 2 or C even in 6..50: thread = (output column, channel pair), kSCols * C / 2 threads; C = 9: (output column, channel),
+    // kSCols * C threads.  Threads t < kSCols also own the vertex channels of output column t (at C = 2 that is every thread)
+    using V = std::conditional_t<CPT == 2, float2, float>;
     constexpr int kSC = SC, kSCols = 8 * SC + 8;
     const int C = CT ? CT : C_rt;
-    const int CP = C / 2, No = 4 * C, VC = 3 * C, NT = kSCols * CP;
+    const int CP = C / CPT, No = 4 * C, VC = 3 * C, NT = kSCols * CP;
     const int H = 8 * h, W = 8 * w;
     const int c_lo = blockIdx.x * kSC, c_hi = min(c_lo + kSC, w);
     const int m_lo = blockIdx.y * rb, m_hi = min(m_lo + rb, h);
@@ -211,9 +219,9 @@ k_up8_bwd_strip(const float* __restrict__ prob, const float* __restrict__ score,
     const int xs = xin ? x : 0;                      // a thread outside the strip / image never loads (labels stay -1)
     const int* gt_c = gt + img + xs;
     const float* pr0_c = prob + (img + xs) * C;
-    const float2* sc2_c = reinterpret_cast<const float2*>(score) + (img + xs) * CP + j;
-    const float2* pr2_c = reinterpret_cast<const float2*>(prob) + (img + xs) * CP + j;
-    const int j2 = 2 * j;
+    const V* sc2_c = reinterpret_cast<const V*>(score) + (img + xs) * CP + j;
+    const V* pr2_c = reinterpret_cast<const V*>(prob) + (img + xs) * CP + j;
+    const int j2 = CPT * j;
     const int own_lo = 8 * m_lo, own_hi = 8 * m_hi;
     // vertex role (threads t < kSCols): column xB, labels prefetched two rows ahead
     const int xB = 8 * c_lo - 4 + t;
@@ -225,8 +233,8 @@ k_up8_bwd_strip(const float* __restrict__ prob, const float* __restrict__ score,
     const size_t r0 = (size_t)y_first * W;
     const int* gp2 = gt_c + r0 + 2 * (size_t)W;
     const float* qp2 = pr0_c + (r0 + 2 * (size_t)W) * C;
-    const float2* sp1 = sc2_c + (r0 + W) * CP;
-    const float2* pp1 = pr2_c + (r0 + W) * CP;
+    const V* sp1 = sc2_c + (r0 + W) * CP;
+    const V* pp1 = pr2_c + (r0 + W) * CP;
     const int* gpB2 = gtB_c + r0 + 2 * (size_t)W;
     const size_t stepQ = (size_t)W * C, stepS = (size_t)W * CP;
     int gB0 = -1, gB1 = -1;
@@ -244,7 +252,7 @@ k_up8_bwd_strip(const float* __restrict__ prob, const float* __restrict__ score,
     }
     int g0 = -1, g1 = -1, g2;
     float q0 = 0.f, q1 = 0.f, q2;
-    float2 sv0 = make_float2(0.f, 0.f), pv0 = sv0, sv1 = sv0, pv1 = sv0;
+    V sv0 = V{}, pv0 = sv0, sv1 = sv0, pv1 = sv0;
     if (xin) {
         if (y_first <= y_last) { g0 = __ldg(gt_c + r0); q0 = __ldg(pr0_c + r0 * C); }
         if (y_first + 1 <= y_last) { g1 = __ldg(gt_c + r0 + W); q1 = __ldg(pr0_c + (r0 + W) * C); }
@@ -259,7 +267,14 @@ k_up8_bwd_strip(const float* __restrict__ prob, const float* __restrict__ score,
         const bool s1 = (unsigned)g1 < (unsigned)C && (g1 > 0 || q1 < threshold);
         if (s1) { sv1 = __ldg(sp1); pv1 = __ldg(pp1); }
         gp2 += W; qp2 += stepQ; sp1 += stepS; pp1 += stepS;
-        if (s0) {
+        if constexpr (CPT == 1) {
+            if (s0) {
+                const float d0 = sv0 > 0.f ? s_cls * (pv0 - (j == g0 ? 1.f : 0.f)) : 0.f;
+                lo0 = fmaf(w_lo, d0, lo0);
+                hi0 = fmaf(w_hi, d0, hi0);
+                if (own_x && y >= own_lo && y < own_hi) b0 += d0;
+            }
+        } else if (s0) {
             const float d0 = sv0.x > 0.f ? s_cls * (pv0.x - (j2 == g0 ? 1.f : 0.f)) : 0.f;
             const float d1 = sv0.y > 0.f ? s_cls * (pv0.y - (j2 + 1 == g0 ? 1.f : 0.f)) : 0.f;
             lo0 = fmaf(w_lo, d0, lo0); lo1 = fmaf(w_lo, d1, lo1);
@@ -319,7 +334,8 @@ k_up8_bwd_strip(const float* __restrict__ prob, const float* __restrict__ score,
             // the older row m_old = ((y + 4) >> 3) - 1 has seen its last tap (15)
             const int m_old = ((y + 4) >> 3) - 1;
             if (m_old >= m_lo) {                      // block-uniform (m_old < m_hi by the loop bounds)
-                v_s[col * C + 2 * j] = lo0; v_s[col * C + 2 * j + 1] = lo1;
+                if constexpr (CPT == 1) v_s[col * C + j] = lo0;
+                else { v_s[col * C + 2 * j] = lo0; v_s[col * C + 2 * j + 1] = lo1; }
             }
             __syncthreads();                          // every thread's updates of vacc for this row are done (also when the row is discarded)
             if (m_old >= m_lo) {
@@ -351,7 +367,8 @@ k_up8_bwd_strip(const float* __restrict__ prob, const float* __restrict__ score,
             slot_lo ^= 1;
         }
     }
-    bs[col * C + 2 * j] = b0; bs[col * C + 2 * j + 1] = b1;
+    if constexpr (CPT == 1) bs[col * C + j] = b0;
+    else { bs[col * C + 2 * j] = b0; bs[col * C + 2 * j + 1] = b1; }
     __syncthreads();
     const size_t cta = ((size_t)blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
     for (int ch = t; ch < No; ch += NT) {
@@ -511,7 +528,8 @@ static int up8_heads_bwd(const char* what, const float* prob, const float* score
                      d_vt_bf16 && dbias && workspace && (!kCoord || (vertmap && extents)),
                  "%s: NULL tensor pointer", what);
     PCNN_REQUIRE(Cs >= C && Cv >= 3 * C && h <= 65535 && B <= 65535, "%s: bad shape", what);
-    PCNN_REQUIRE(C == 2 || (C % 2 == 0 && C >= 6 && C <= 50), "%s: C must be even and 2 or in 6..50 (C = %d)", what, C);
+    // class counts of the reference's configurations: 2 (single object), 22 (YCB), 9 (multi-object LINEMOD), and the even range
+    PCNN_REQUIRE(C == 2 || C == 9 || (C % 2 == 0 && C >= 6 && C <= 50), "%s: C must be even and 2 or in 6..50, or 9 (C = %d)", what, C);
     // coalesced strip kernel (see k_up8_bwd_strip); partial bias sums: one row of 4C floats per CTA
     const int sc = C == 2 ? kStrip2 : kStrip, cols = 8 * sc + 8;
     const int rb = 16, bands = (h + rb - 1) / rb, strips = (w + sc - 1) / sc;
@@ -522,18 +540,23 @@ static int up8_heads_bwd(const char* what, const float* prob, const float* score
     const size_t smem = sizeof(float) * ((size_t)cols * 11 * C + C + (kCoord ? 6 * C : 0));
     const dim3 grid(strips, bands, B);
     if (C == 22)
-        k_up8_bwd_strip<22, kStrip, kCoord><<<grid, cols * 11, smem, st>>>(prob, score, gt, cls_loss_out, upstream_cls, threshold, vertex_pred, lowres,
+        k_up8_bwd_strip<22, kStrip, kCoord, 2><<<grid, cols * 11, smem, st>>>(prob, score, gt, cls_loss_out, upstream_cls, threshold, vertex_pred, lowres,
                                                                           bias_vertex, centers, vertex_loss_out, upstream_vertex, w_inside,
                                                                           sigma * sigma, h, w, rb, C, Cs, Cv, (__nv_bfloat16*)d_sc_bf16,
                                                                           (__nv_bfloat16*)d_vt_bf16, (float*)workspace, vertmap, extents);
     else if (C == 2)
-        k_up8_bwd_strip<2, kStrip2, kCoord><<<grid, cols, smem, st>>>(prob, score, gt, cls_loss_out, upstream_cls, threshold, vertex_pred, lowres,
+        k_up8_bwd_strip<2, kStrip2, kCoord, 2><<<grid, cols, smem, st>>>(prob, score, gt, cls_loss_out, upstream_cls, threshold, vertex_pred, lowres,
                                                                      bias_vertex, centers, vertex_loss_out, upstream_vertex, w_inside, sigma * sigma, h,
                                                                      w, rb, C, Cs, Cv, (__nv_bfloat16*)d_sc_bf16, (__nv_bfloat16*)d_vt_bf16,
                                                                      (float*)workspace, vertmap, extents);
+    else if (C % 2)   // C = 9: one channel per thread (at 40 x 9 threads the strip's shared memory is 16 KB: no opt-in)
+        k_up8_bwd_strip<0, kStrip, kCoord, 1><<<grid, cols * C, smem, st>>>(prob, score, gt, cls_loss_out, upstream_cls, threshold, vertex_pred,
+                                                                           lowres, bias_vertex, centers, vertex_loss_out, upstream_vertex, w_inside,
+                                                                           sigma * sigma, h, w, rb, C, Cs, Cv, (__nv_bfloat16*)d_sc_bf16,
+                                                                           (__nv_bfloat16*)d_vt_bf16, (float*)workspace, vertmap, extents);
     else {
-        PCNN_SMEM_OPTIN((k_up8_bwd_strip<0, kStrip, kCoord>), 100 * 1024, kCoord ? "up8_bwd_strip<0, coord>" : "up8_bwd_strip<0>");
-        k_up8_bwd_strip<0, kStrip, kCoord><<<grid, cols * (C / 2), smem, st>>>(prob, score, gt, cls_loss_out, upstream_cls, threshold, vertex_pred,
+        PCNN_SMEM_OPTIN((k_up8_bwd_strip<0, kStrip, kCoord, 2>), 100 * 1024, kCoord ? "up8_bwd_strip<0, coord>" : "up8_bwd_strip<0>");
+        k_up8_bwd_strip<0, kStrip, kCoord, 2><<<grid, cols * (C / 2), smem, st>>>(prob, score, gt, cls_loss_out, upstream_cls, threshold, vertex_pred,
                                                                               lowres, bias_vertex, centers, vertex_loss_out, upstream_vertex, w_inside,
                                                                               sigma * sigma, h, w, rb, C, Cs, Cv, (__nv_bfloat16*)d_sc_bf16,
                                                                               (__nv_bfloat16*)d_vt_bf16, (float*)workspace, vertmap, extents);

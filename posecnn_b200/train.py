@@ -10,7 +10,8 @@ This is the keep_prob = 1.0 graph (the reference trains with dropout 0.5; random
 A network built with pose_reg=False (the linemod_{benchvise,camera,iron,lamp,phone}.yml models) trains
     loss = loss_cls + VERTEX_W * loss_vertex + l2 regularisation (train.py:517, vgg16_convs.py:128-163):
 no Hough voting, RoiPool or fc6-fc8 in the step, and no fc6-fc8 parameters in it.
-Every class count the kernels take trains: C = 2 (the single-object LINEMOD / YCB models) and even C in 6..50.
+Every class count the kernels take trains: C = 2 (the single-object LINEMOD / YCB models), even C in 6..50, and C = 9 (the
+multi-object LINEMOD model linemod_color_2d.yml, eight objects plus background, pose_reg=False).
 A network built with vertex_reg_2d=False, vertex_reg_3d=True (the object-coordinate models linemod_*_3d.yml, lov_color_3d.yml) trains
 its vertex head on 3-D targets (minibatch.py:595-600, 605-616): a labelled pixel of a listed class regresses its object coordinate
 vertmap [B,H,W,3] scaled into [0, 1] by the class's extents.  Its graph has no pose head whatever pose_reg says (vgg16_convs.py:165-200

@@ -1,0 +1,397 @@
+"""Odd class counts on the GPU: the one-channel-per-thread forms of k_up8_heads, k_up8_label and k_up8_bwd_strip bit for bit
+against the float64 references of tests/heads_ref.py (C = 3, 9, 21, 127 forward; C = 9 adjoint, both target modes), the
+class-count generic kernels on the C = 9 network path, the training step at C = 9 against torch autograd, and inference at
+480 x 640 with C = 9 (the multi-object LINEMOD model, linemod_color_2d.yml: eight objects plus background)."""
+
+import numpy as np
+import pytest
+import torch
+
+from posecnn_b200 import synth
+from tests import heads_ref as R
+from tests import ref_network as RN
+from tests import vertex_loss_ref as V
+from tests.train_ref import bits, compare_grads, limits, make_inputs, reference_grads, rel_l2, synthetic_pose_targets
+from tests.util import to_np
+
+pytestmark = pytest.mark.gpu
+torch.backends.cudnn.allow_tf32 = False
+torch.backends.cuda.matmul.allow_tf32 = False
+MEANS = (102.9801, 115.9465, 122.7717)
+
+
+def assert_same(got, want, what):
+    bad = got != want
+    assert not bool(bad.any()), (f"{what}: {int(bad.sum())} of {bad.numel()} values differ; first at {bad.nonzero()[0].tolist()}: "
+                                 f"{got[tuple(bad.nonzero()[0])].item()} != {want[tuple(bad.nonzero()[0])].item()}")
+
+
+def bf16(ref):
+    return ref.float().to(torch.bfloat16)
+
+
+def odd_heads_roles(C, label_only):
+    """k_up8_heads<0, 1>: cell phases gv and the roles of one CTA (one channel each: 3C vertex + C score per phase, score only in
+    label-only mode), looped over the 256 threads."""
+    gv = max(256 // (4 * C), 1) if not label_only else 256 // C
+    roles = gv * (C if label_only else 4 * C)
+    return dict(phases=gv, roles=roles, role_loops=-(-roles // 256))
+
+
+def odd_bwd_plan(B, h, w, C):
+    """pcnn_up8_heads_bwd_ex / _coord at odd C: the 4-cell strips of heads_ref.up8_bwd_plan, one channel per thread:
+    (8 SC + 8) C threads."""
+    plan = dict(R.up8_bwd_plan(B, h, w, C))
+    plan.update(kernel="<0, odd>", threads=(8 * plan["strip"] + 8) * C)
+    return plan
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# 1. forward heads (k_up8_heads<0, 1>, k_up8_label<0, 1>)
+# ---------------------------------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("h,w", [(60, 80), (37, 27)])
+@pytest.mark.parametrize("C", [3, 9, 21, 127])
+def test_up8_heads_odd_exact(cuda, C, h, w):
+    """pcnn_up8_heads at 480 x 640 and 296 x 216 (w = 27: a ragged last segment of 7 cells), B = 2: vertex and score exact, label
+    the first-index arg-max (ties from coarse scores and all-zero ReLU pixels), prob within the softmax bound; the label-only
+    call gives the same labels (k_up8_label, or at C = 127, w = 80, where 11 w C floats exceed 200 KB, k_up8_heads)."""
+    from posecnn_b200._lib import check, lib, ptr, stream
+    B = 2
+    H, W = 8 * h, 8 * w
+    full, lab = R.up8_heads_plan(B, h, w, C), R.up8_heads_plan(B, h, w, C, label_only=True)
+    rf, rl = odd_heads_roles(C, False), odd_heads_roles(C, True)
+    print(f"C={C} {H}x{W}: {full['kernel']} grid {full['grid']} ({full['segments']} segments, ragged last {full['ragged_segment']}), "
+          f"{rf['phases']} cell phases, {rf['roles']} roles in {rf['role_loops']} loop(s); label-only: {lab['kernel']} grid {lab['grid']}, "
+          f"{lab['smem']} B of shared memory" + (f", {rl['roles']} roles in {rl['role_loops']} loop(s)" if lab["kernel"] == "k_up8_heads" else ""))
+    assert full["ragged_segment"] == (w == 27)
+    assert lab["kernel"] == ("k_up8_heads" if (C, w) == (127, 80) else "k_up8_label")
+    assert (rf["role_loops"] == 2) == (C == 127)
+    g = torch.Generator().manual_seed(500 + C + w)
+    lowres = R.dyadic((B, h, w, 4 * C), -1, 1, 0.125, g)
+    lowres[..., :C] = R.dyadic((B, h, w, C), -1, 1, 0.5, g)                # coarse scores: exact ties between classes
+    for y0, x0 in ((8, 8), (h // 2, w // 2), (h - 3, w - 3)):
+        lowres[:, y0:y0 + 3, x0:x0 + 3, :C] = -1.0                          # every class negative: ReLU zeros tie across classes
+    bs = R.dyadic((C,), -0.25, 0.25, 0.125, g) * (torch.arange(C) % 2)
+    bv = R.dyadic((3 * C,), -1, 1, 0.125, g)
+    lowres, bs, bv = lowres.to(cuda), bs.to(cuda), bv.to(cuda)
+    label = torch.full((B, H, W), -7, dtype=torch.int32, device=cuda)
+    vertex = torch.empty((B, H, W, 3 * C), device=cuda)
+    prob = torch.empty((B, H, W, C), device=cuda)
+    score = torch.empty((B, H, W, C), device=cuda)
+    check(lib().pcnn_up8_heads(ptr(lowres), ptr(bs), ptr(bv), B, h, w, C, ptr(label), ptr(vertex), ptr(prob), ptr(score), stream()))
+    label2 = torch.full((B, H, W), -7, dtype=torch.int32, device=cuda)
+    check(lib().pcnn_up8_heads(ptr(lowres), ptr(bs), ptr(bv), B, h, w, C, ptr(label2), ptr(None), ptr(None), ptr(None), stream()))
+    ref = R.up8_heads(lowres, bs, bv, C, 0.125)
+    print(f"  bit budget {ref['budget']:.0f} of 2^24")
+    assert_same(vertex, ref["vertex"].float(), "vertex")
+    assert_same(score, ref["score"].float(), "score")
+    del vertex
+    top2 = ref["score"].topk(2, -1).values
+    ties, zeros = (top2[..., 0] == top2[..., 1]) & (top2[..., 0] > 0), (top2[..., 0] == 0)
+    print(f"  {int(ties.sum())} pixels with tied positive maxima, {int(zeros.sum())} all-zero pixels")
+    assert bool(ties.any()) and bool(zeros.any())
+    assert_same(label, ref["label"].int(), "label")
+    assert torch.equal(label2, label), "label-only labels differ from the full mode's"
+    err = (prob.double() - ref["prob"]).abs()
+    bound = R.softmax_bound(ref["prob"], C)
+    print(f"  prob: max |err| / bound = {float((err / bound).max()):.3f}")
+    assert bool((err <= bound).all()), f"prob outside the softmax bound at {int((err > bound).sum())} values"
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# 2. the up-sampling adjoint (k_up8_bwd_strip<0, 4, ., 1>)
+# ---------------------------------------------------------------------------------------------------------------------
+def _up8_bwd(P, sigma, thr, dense, Cv):
+    from posecnn_b200._lib import check, lib, ptr, stream
+    B, h, w, C = P["B"], P["h"], P["w"], P["C"]
+    dev = P["prob"].device
+    d_sc = torch.full((B, h, w, 64), 7.0, dtype=torch.bfloat16, device=dev)          # padding channels must be written as 0
+    d_vt = torch.full((B, h, w, Cv), 7.0, dtype=torch.bfloat16, device=dev)
+    dbias = torch.full((4 * C,), 7.0, device=dev)
+    cls_out = torch.tensor([0.5, P["count"]], device=dev)
+    vtx_out = torch.tensor([0.25, P["sumw"]], device=dev)
+    ws = torch.empty(odd_bwd_plan(B, h, w, C)["workspace"], dtype=torch.uint8, device=dev)
+    vpred = P["pv"].float().contiguous() if dense else None
+    head = (ptr(P["prob"]), ptr(P["score"]), ptr(P["gt"]), ptr(cls_out), P["up_cls"], thr, ptr(vpred),
+            ptr(None if dense else P["lowres"]), ptr(None if dense else P["bias_v"]))
+    tail = (ptr(vtx_out), P["up_vtx"], P["w_inside"], sigma, B, h, w, C, 64, Cv, ptr(d_sc), ptr(d_vt), ptr(dbias), ptr(ws), ws.numel(),
+            stream())
+    if P["coord"]:
+        check(lib().pcnn_up8_heads_bwd_coord(*head, ptr(P["vertmap"]), ptr(P["centers"]), ptr(P["extents"]), *tail))
+    else:
+        check(lib().pcnn_up8_heads_bwd_ex(*head, ptr(P["centers"]), *tail))
+    return d_sc, d_vt, dbias
+
+
+@pytest.mark.parametrize("coord", [False, True], ids=["2d", "3d"])
+@pytest.mark.parametrize("h,w", [(60, 80), (37, 27)])
+def test_up8_bwd_nine_classes_exact(cuda, h, w, coord):
+    """test_heads_exact_gpu.py::test_up8_bwd_exact at C = 9: d_sc, d_vt and d bias exact after one bf16 / fp32 rounding,
+    padding channels 0, dense and low-resolution vertex sources bit-identical, two launches bit-identical."""
+    B, C, Cv = 2, 9, 128
+    plan = odd_bwd_plan(B, h, w, C)
+    print(f"C={C} {h}x{w} {'3d' if coord else '2d'}: kernel {plan['kernel']} strip {plan['strip']}: {plan['strips']} strips x "
+          f"{plan['bands']} bands x {B} images = {plan['ctas']} CTAs of {plan['threads']} threads; last strip {plan['last_strip_cells']} "
+          f"cells, last band {plan['last_band_rows']} rows")
+    assert plan["threads"] == 360 and plan["last_band_rows"] < 16 and plan["strips"] >= 2 and plan["bands"] >= 3
+    if (h, w) == (37, 27):
+        assert plan["last_strip_cells"] < plan["strip"]
+    g = torch.Generator().manual_seed(9000 + h + 2 * coord)
+    P = R.up8_bwd_problem(B, h, w, C, coord, g, device=cuda)
+    gt, p0 = P["gt"], P["prob"][..., 0]
+    assert bool((gt == -1).any() and (gt >= C).any() and (gt < -1).any() and (P["score"] == 0).any())
+    for sigma, thr in ((1.0, 1.0), (2.0, 0.5)):
+        bg = gt == 0
+        assert bool((bg & (p0 < thr)).any() and (bg & (p0 == thr)).any() and (bg & (p0 == thr - 0.125)).any())
+        ref = R.up8_bwd(P, sigma, thr, 2.0 ** -10)
+        print(f"  sigma={sigma} threshold={thr}: bit budget {ref['budget']:.0f} of 2^24")
+        d_sc, d_vt, dbias = _up8_bwd(P, sigma, thr, True, Cv)
+        e_sc, e_vt, ebias = _up8_bwd(P, sigma, thr, False, Cv)
+        again = _up8_bwd(P, sigma, thr, False, Cv)
+        torch.cuda.synchronize()
+        for a, b, name in zip((d_sc, d_vt, dbias), (e_sc, e_vt, ebias), ("d_sc", "d_vt", "dbias")):
+            assert torch.equal(bits(a), bits(b)), f"{name}: dense and low-resolution vertex sources differ"
+        for a, b in zip((e_sc, e_vt, ebias), again):
+            assert torch.equal(bits(a), bits(b)), "two launches differ"
+        assert_same(e_sc[..., :C], bf16(ref["d_sc"]), "d_sc")
+        assert_same(e_vt[..., :3 * C], bf16(ref["d_vt"]), "d_vt")
+        assert_same(ebias, ref["dbias"].float(), "dbias")
+        assert not bool(e_sc[..., C:].float().ne(0).any()) and not bool(e_vt[..., 3 * C:].float().ne(0).any()), "padding channels"
+        assert bool(ref["d_vt"].ne(0).any()) and bool(ref["dbias"][C:].ne(0).any())
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# 3. the class-count generic kernels on the C = 9 network path
+# ---------------------------------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("folded", [False, True], ids=["unfolded", "folded"])
+@pytest.mark.parametrize("h,w", [(60, 80), (62, 82)])
+def test_lowres_heads_nine_classes_exact(cuda, h, w, folded):
+    """pcnn_lowres_heads at C = 9 (27 vertex columns: no full pass, one tail pass with split columns) exact."""
+    from posecnn_b200._lib import check, lib, ptr, stream
+    C, Cs, Cv = 9, 64, 128
+    B = 15 if folded else (4 if (h, w) == (60, 80) else 5)
+    plan = R.lowres_heads_plan(B, h, w, C, Cs, Cv, folded)
+    print(f"C={C} {'folded' if folded else 'unfolded'} {h}x{w} B={B}: {plan['groups']} groups on {plan['warps']} warps, up to "
+          f"{plan['groups_per_warp']} per warp; {plan['full_passes']} full + {plan['tail_passes']} tail passes, ragged last group "
+          f"{plan['ragged_group']}")
+    assert plan["groups_per_warp"] >= 2
+    g = torch.Generator().manual_seed(90 + h + folded)
+    s4, s5 = R.dyadic((B, h, w, Cs), -3, 3, 1, g), R.dyadic((B, h // 2, w // 2, Cs), -3, 3, 1, g)
+    v4, v5 = R.dyadic((B, h, w, Cv), -3, 3, 1, g), R.dyadic((B, h // 2, w // 2, Cv), -3, 3, 1, g)
+    Ws = R.dyadic((Cs, C), -2, 2, 0.125, g).to(cuda)
+    Wv = None if folded else R.dyadic((Cv, 3 * C), -2, 2, 0.125, g).to(cuda)
+    s4, s5, v4, v5 = (t.to(cuda).bfloat16() for t in (s4, s5, v4, v5))
+    out = torch.full((B, h, w, 4 * C), 7.0, device=cuda)
+    check(lib().pcnn_lowres_heads(ptr(s4), ptr(s5), ptr(v4), ptr(v5), ptr(Ws), ptr(Wv), B, h, w, Cs, Cv, C, ptr(out), stream()))
+    ref, budget = R.lowres_heads(s4, s5, v4, v5, Ws, Wv, C, 1.0, 0.125)
+    print(f"  bit budget {budget:.0f} of 2^24")
+    assert_same(out, ref.float(), "lowres_heads")
+
+
+@pytest.mark.parametrize("thr", [0.5, 1.0])
+def test_loss_cls_nine_classes(cuda, thr):
+    """train_ops.loss_cls at C = 9, 2 x 480 x 640: count exact, loss within heads_ref.loss_cls_hard_raw's bound."""
+    from posecnn_b200.train_ops import loss_cls
+    B, H, W, C = 2, 480, 640, 9
+    g = torch.Generator().manual_seed(309)
+    score = R.dyadic((B, H, W, C), -8, 8, 0.125, g).to(cuda)
+    prob = R.dyadic((B, H, W, C), 0, 1, 0.125, g).to(cuda)
+    gt = R.int_operands((B, H, W), -2, C, g).to(torch.int32).to(cuda)
+    a = loss_cls(score, prob, gt, thr)
+    loss, n, bound, _ = R.loss_cls_hard_raw(score, prob, gt, thr)
+    print(f"threshold {thr}: loss {a[0].item():.9f} ref {loss:.9f} |err| {abs(a[0].item() - loss):.3e} bound {bound:.3e}; count {n}")
+    assert a[1].item() == n and abs(a[0].item() - loss) <= bound
+
+
+@pytest.mark.parametrize("sigma", [1.0, 2.5])
+def test_loss_vertex_nine_classes_exact(cuda, sigma):
+    """The fused 2-D vertex loss (pcnn_vertex_loss_fused_lowres_fwd) at C = 9, 2 x 480 x 640: loss and weight sum equal
+    vertex_loss_ref.reference's exact sum / weights."""
+    from posecnn_b200 import train_ops
+    B, H, W, C = 2, 480, 640, 9
+    g = torch.Generator().manual_seed(4090 + 2 * int(sigma))
+    P = V.loss_problem(B, H, W, C, False, sigma, g)
+    ref = V.reference(P)
+    print(f"C=9 sigma={sigma}: foreground {ref['count']}, {ref['n_terms']} terms, {ref['boundary']} at |diff| == 1/sigma^2; "
+          f"loss {ref['out0']!r}, sum w {ref['out1']!r}")
+    assert ref["boundary"] > 0
+    T = lambda a: a.contiguous().to(cuda) if isinstance(a, torch.Tensor) else torch.as_tensor(np.ascontiguousarray(a)).to(cuda)
+    out = train_ops.loss_vertex(T(P["lowres"]), T(P["bias_v"]), T(P["label"]), T(P["centers"]), P["w_inside"], P["sigma"]).cpu().numpy()
+    assert out[1] == ref["out1"], f"weight sum {out[1]!r} != {ref['out1']!r}"
+    assert out[0] == ref["out0"], f"loss {out[0]!r} != {ref['out0']!r}"
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# 4. the training step at C = 9
+# ---------------------------------------------------------------------------------------------------------------------
+def make_net9(cuda, pose_reg):
+    """tests/train_ref.make_net at C = 9 with pose_reg as an argument."""
+    from posecnn_b200.networks.vgg16_convs import vgg16_convs
+    net = vgg16_convs(num_classes=9, device=cuda, is_train=True, fold_vertex_head=False, pose_reg=pose_reg).init_random(seed=0, bias_std=0.02)
+    net.params["score/weights"] *= 0.02
+    net.params["vertex_pred/weights"] *= 0.02
+    net.params["fc8/weights"] *= 0.01
+    net.prepare()
+    return net
+
+
+@pytest.mark.parametrize("pose_reg", [False, True], ids=["no_pose_reg", "pose_reg"])
+def test_training_step_nine_classes(cuda, pose_reg):
+    """Trainer at C = 9, B = 2, 64 x 96: every gradient against the 16-bit-rounded and the pure fp32 autograd graph within
+    train_ref.limits(), the limits that hold at C = 6.  pose_reg=False is linemod_color_2d.yml (the restatement's pose term is
+    held at exactly 0, as in test_single_class_gpu.py::test_pose_reg_false_step); pose_reg=True puts fc8 at 36 columns."""
+    from posecnn_b200.train import Trainer
+    C, vw_, wi, margin = 9, 2.0, 10.0, 0.01
+    args, _, _ = make_inputs(cuda, C=C)
+    data, gt, centers, meta, ext, gtp, pts, sym = args
+    net = make_net9(cuda, pose_reg)
+    tr = Trainer(net, lr=0.01, weight_decay=1e-4, vertex_w=vw_, vertex_w_inside=wi, margin=margin)
+    assert tr.master["score/w"].shape[0] >= C
+    A = tr.forward(*args)
+    if pose_reg:
+        assert tr.master["fc8/w"].shape == (128, 4096) and A["poses_tanh"].shape[1] == 4 * C
+        print(f"rows {A['rows']}, num_rois {A['num_rois'].item()}")
+        assert A["rows"] >= 1
+        tw, wt = synthetic_pose_targets(A, pts, sym, margin)
+        Z, m = A, margin
+    else:
+        assert not any(k.startswith(("fc6", "fc7", "fc8")) for k in tr.master)
+        n = 1
+        Z = dict(rois=torch.zeros((n, 7), device=cuda), a5=torch.zeros((n, 7, 7, 512), dtype=torch.int32, device=cuda),
+                 a4=torch.zeros((n, 7, 7, 512), dtype=torch.int32, device=cuda))
+        tw, wt = torch.zeros((n, 4 * C), device=cuda), torch.zeros((n, 4 * C), device=cuda)
+        tw[:, 4], wt[:, 4:8] = 1.0, 1.0
+        m = 1e9
+    grads = tr.backward(A, gt, centers)
+    torch.cuda.synchronize()
+    P, ref = reference_grads(net, Z, args, tw, wt, True, vw_, wi, m)
+    Pf, reff = reference_grads(net, Z, args, tw, wt, False, vw_, wi, m)
+    es, ev = rel_l2(A["score"].permute(0, 3, 1, 2), ref["score"]), rel_l2(tr.dense_vertex_pred(A).permute(0, 3, 1, 2), ref["vertex"])
+    print(f"forward: score rel-L2 {es:.2e}, vertex_pred rel-L2 {ev:.2e}")
+    assert es < 5e-3 and ev < 5e-3
+    for r_ in (ref, reff):
+        assert abs(A["cls_out"][0].item() - r_["loss_cls"]) < 3e-2 * max(1.0, abs(r_["loss_cls"]))
+        assert abs(vw_ * A["vtx_out"][0].item() - r_["loss_vertex"]) < 3e-2 * max(1.0, abs(r_["loss_vertex"]))
+        if pose_reg:
+            assert abs(A["loss_pose"].item() - r_["loss_pose"]) < 3e-2 * max(1e-3, abs(r_["loss_pose"]))
+        else:
+            assert r_["loss_pose"] == 0.0
+    assert set(grads) == set(tr.master)
+    compare_grads(tr, grads, P, Pf, sorted(grads), limits)
+    out = tr.step(*args)
+    assert torch.isfinite(out["loss"]).all()
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# 5. inference at 480 x 640
+# ---------------------------------------------------------------------------------------------------------------------
+@pytest.fixture(scope="module")
+def full9(cuda):
+    from posecnn_b200.networks.vgg16_convs import vgg16_convs
+    B, H, W, C = 2, 480, 640, 9
+    net = vgg16_convs(num_classes=C, device=cuda).init_random(seed=0)
+    rgb, _ = synth.make_images(B, H, W, seed=3)
+    data = torch.from_numpy(rgb).to(cuda)
+    meta = torch.from_numpy(np.stack([synth.make_meta(synth.intrinsics(H, W))] * B)).to(cuda)
+    ext = torch.from_numpy(synth.extents_for(C)).to(cuda)
+    net.calibrate_background(data, meta, ext, 0.75)
+    out = dict(net.forward(data, meta, ext, want_prob=True, want_score=True, sync_rois=False))
+    lowres = net._last_lowres.clone()
+    torch.cuda.synchronize()
+    return net, data, meta, ext, out, lowres
+
+
+def test_inference_nine_classes_480x640(full9):
+    """Trunk, labels (pixels whose fp32 logit margin is > 5 %), vertex_pred and the pose head's quaternions (fc8: 36 columns)
+    against the fp32 restatement, with the limits of test_single_class_gpu.py::test_inference_two_classes_480x640."""
+    from oracle import oracle
+    from posecnn_b200 import pose_head
+    C = 9
+    net, data, meta, ext, out, _ = full9
+    x = (data.float() - torch.tensor(MEANS, device=data.device)).permute(0, 3, 1, 2)
+    with torch.no_grad():
+        feats = RN.trunk(net.params, x)
+        for name in ("conv4_3", "conv5_3"):
+            assert rel_l2(out[name].float().permute(0, 3, 1, 2), feats[name]) < 2e-2, name
+        score, label, prob, vertex = RN.heads(net.params, feats["conv4_3"], feats["conv5_3"], C)
+    ev = rel_l2(out["vertex_pred"].permute(0, 3, 1, 2), vertex)
+    top2 = torch.topk(score, 2, dim=1).values
+    decided = (top2[:, 0] - top2[:, 1]) / top2[:, 0].abs().clamp(min=1e-6) > 0.05
+    frac = decided.float().mean().item()
+    flips = (out["label_2d"][decided] != label[decided]).float().mean().item()
+    print(f"C = 9: vertex rel-L2 {ev:.2e}; {frac:.3f} decided by > 5 %, flip rate there {flips:.2e}; classes present "
+          f"{torch.unique(out['label_2d']).tolist()}")
+    assert ev < 2e-2 and frac > 0.2 and flips < 1e-3
+    assert torch.allclose(out["prob_normalized"].sum(3), torch.ones_like(out["prob_normalized"][..., 0]), atol=1e-5)
+    n = int(out["num_rois"].item())
+    rois = to_np(out["rois_capacity"][:n])
+    assert n >= 1
+    p5, _ = oracle.roi_pool(to_np(out["conv5_3"].float()), rois, 7, 7, 1.0 / 16.0)
+    p4, _ = oracle.roi_pool(to_np(out["conv4_3"].float()), rois, 7, 7, 1.0 / 8.0)
+    x0 = torch.from_numpy(p5 + p4).reshape(n, -1).to(data.device)
+    P, T = net.params, net._tc
+    h7 = torch.relu(torch.relu(x0 @ P["fc6/weights"] + P["fc6/biases"]) @ P["fc7/weights"] + P["fc7/biases"])
+    pre = h7 @ P["fc8/weights"] + P["fc8/biases"]
+    e_pre = rel_l2(pose_head.fc(out["fc7"][:n].contiguous(), T["fc8/weights"], P["fc8/biases"], "none", torch.float32), pre)
+    print(f"  {n} rois; fc8 pre-activation rel-L2 {e_pre:.2e}")
+    assert out["poses_tanh"].shape[1] == 4 * C
+    assert e_pre < 1.5e-3
+    assert rel_l2(out["poses_tanh"][:n], torch.tanh(pre)) < 1.5e-3
+
+
+def test_hough_from_lowres_nine_classes(full9):
+    """Hough voting sampling its vertex values from lowres (stride 4C = 36, vertex channels from offset 9) equals Hough on the
+    dense vertex_pred, row for row."""
+    from posecnn_b200.hough_voting_gpu_layer import hough_voting_gpu_op as op
+    net, data, meta, ext, out, lowres = full9
+    P = net.params
+    a = op.hough_voting_gpu_capacity(out["label_2d"], out["vertex_pred"], ext, meta, None, 0, net.vote_threshold, net.vote_percentage,
+                                     net.skip_pixels)
+    b = op.hough_voting_gpu_capacity(out["label_2d"], None, ext, meta, None, 0, net.vote_threshold, net.vote_percentage, net.skip_pixels,
+                                     lowres=lowres, bias_vertex=P["vertex_pred/biases"])
+    n = int(a[5].item())
+    print(f"{n} rois from the dense and the low-resolution vertex source")
+    assert n >= 1 and int(b[5].item()) == n
+    for x, y in zip(a[:2], b[:2]):
+        assert torch.equal(bits(x[:n]), bits(y[:n]))
+
+
+def test_inference_nine_classes_records(full9):
+    """dense_vertex=False gives the dense run's ROIs and poses; two image shards give the whole batch's records; the CUDA graph
+    replays the eager pass bit for bit; Evaluator(num_classes=9) scores the records."""
+    from posecnn_b200 import parallel
+    from posecnn_b200.evaluate import Evaluator
+    from posecnn_b200.networks.vgg16_convs import GraphedForward
+    net, data, meta, ext, _, _ = full9
+    B, C = data.shape[0], 9
+    dense = net.forward(data, meta, ext, sync_rois=False)
+    lean = net.forward(data, meta, ext, sync_rois=False, dense_vertex=False)
+    n = int(dense["num_rois"].item())
+    assert n >= 1 and int(lean["num_rois"].item()) == n
+    for k in ("rois_capacity", "poses_tanh", "detections_rois", "detections_poses"):
+        assert torch.equal(bits(dense[k]), bits(lean[k])), k
+    whole = parallel.compact_records(parallel.pack_detections(lean))
+    parts = []
+    for r in range(2):
+        o, m = parallel.shard_range(B, r, 2)
+        parts.append(parallel.pack_detections(net.forward(data[o:o + m], meta[o:o + m], ext, sync_rois=False, dense_vertex=False,
+                                                          batch_global=B, batch_offset=o)))
+    assert torch.equal(parallel.compact_records(torch.cat(parts)), whole)
+    g = GraphedForward(net, data, meta, ext, pack_records=True, dense_vertex=False)
+    assert torch.equal(parallel.compact_records(g(data)["records"]), whole)
+    assert torch.equal(parallel.compact_records(g(data)["records"]), whole)
+    # one gt row per image on a class the network detected: the evaluator runs over C = 9 tables
+    cls = int(to_np(lean["detections_rois"])[0, 1])
+    gt_rows = np.zeros((B, 14), np.float32)
+    for b in range(B):
+        RT = np.zeros((3, 4), np.float32)
+        RT[:, :3], RT[:, 3] = np.eye(3), (0.0, 0.0, 1.0)
+        gt_rows[b] = np.r_[b, cls, RT.reshape(-1)]
+    ev = Evaluator(C, synth.make_model_points(C, 500), ext.cpu().numpy(), np.zeros(C, np.float32), device=data.device)
+    res = ev.add_poses(torch.from_numpy(gt_rows).to(data.device), lean["detections_rois"], {"poses": lean["detections_poses"]},
+                       lean["num_detections"], meta)
+    ev.add_labels(lean["label_2d"], lean["label_2d"])
+    s = ev.summary()
+    print(f"records: {n} rois, {int(res['num_pairs'].item())} scored pairs; mean IoU {s['mean_iu']:.3f}")
+    assert int(ev.hist.sum()) == data.shape[0] * data.shape[1] * data.shape[2]
+    assert s["overall_accuracy"] == 1.0
