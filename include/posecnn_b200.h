@@ -524,6 +524,29 @@ int pcnn_eval_pose_errors(const float* gt_rows, int num_gt, const float* rois, i
                           int32_t* flags, int32_t* num_pairs, int64_t* counts, int64_t* status, void* stream);
 int pcnn_eval_gt_rows_from_blob(const float* pose_blob, int n, float* gt_rows, void* stream);
 
+/* ---------------------------------------------------------------------------------------
+ * Image scale (csrc/rescale.cu, DESIGN.md 15): cv2.resize(x, None, None, fx=fx, fy=fx, interpolation) of the SCALES_BASE != 1
+ * configurations (the LINEMOD *_3d.yml models use 1.5), batched NHWC, with OpenCV's generic (non-SIMD) arithmetic bit for bit:
+ *   LINEAR   coordinate f = float((d + 0.5) / fx - 0.5) in double, s = floor(f), a = f - s; columns clamp s to [0, W - 1] with
+ *            a = 0 there, rows clamp only the two row indices; two float32 lerps with every product and sum rounded (no FMA).
+ *   NEAREST  s = min(floor(d * (1 / fx)), n - 1) in double.
+ * The destination [B,Ho,Wo,...] must be Ho = round(H * fx), Wo = round(W * fx) (half to even, as cv2 sizes it), else
+ * PCNN_E_INVALID; so must a row whose W * C or Wo * C elements overflow int (the kernels' in-row index).  B <= 65535.
+ *  pcnn_resize_color_u8     the test-time colour blob (fcn/test.py:49-65): frames [B,H,W,3] u8 BGR -> blob [B,Ho,Wo,3] f32, the
+ *      source value f32(f64(u8) - mean3_host[c]) (numpy's float64 PIXEL_MEANS), resized LINEAR.
+ *  pcnn_resize_linear_f32   LINEAR on [B,H,W,C] f32, C = 1 or 3: the training colour blob after augmentation and PIXEL_MEANS
+ *      (gt_synthesize_layer/minibatch.py:179-183) and the object-coordinate vertmap (minibatch.py:416).
+ *  pcnn_resize_depth        LINEAR on the raw depth [B,H,W] (fcn/test.py:1335, 1384): u16 (depth_is_u16) or f32 holding integer
+ *      sensor units; the result, of the input's type, is rounded half to even and saturated to [0, 65535] as cv2's uint16 output.
+ *  pcnn_resize_nearest_i32  NEAREST on label maps [B,H,W] int32: the training label image (minibatch.py:352) and the predicted
+ *      labels back to the frame with fx = 1 / s (fcn/test.py:1421).
+ * One CTA per output row; no allocation, no host synchronisation; CUDA-graph capturable. */
+int pcnn_resize_color_u8(const uint8_t* frames, int B, int H, int W, double fx, int Ho, int Wo, const double* mean3_host, float* blob,
+                         void* stream);
+int pcnn_resize_linear_f32(const float* src, int B, int H, int W, int C, double fx, int Ho, int Wo, float* dst, void* stream);
+int pcnn_resize_depth(const void* depth, int depth_is_u16, int B, int H, int W, double fx, int Ho, int Wo, void* dst, void* stream);
+int pcnn_resize_nearest_i32(const int32_t* label, int B, int H, int W, double fx, int Ho, int Wo, int32_t* dst, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
