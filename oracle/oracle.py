@@ -151,6 +151,18 @@ def project_grad(top_diff, depth, meta, grid_size, kernel_size, threshold, retur
     return (out, amb.astype(bool)) if return_ambig else out
 
 
+def voxel_window(depth, meta, grid_size, kernel_size, threshold):
+    """The windows of Backproject / ProjectGrad: per voxel [B,G,G,G] the hit count (int32) and whether the image border
+    clips the window (bool)."""
+    depth = _f32(depth); meta = _f32(meta)
+    B, H, W = depth.shape[0], depth.shape[1], depth.shape[2]
+    G = grid_size
+    count = np.zeros((B, G, G, G), np.int32); clipped = np.zeros((B, G, G, G), np.uint8)
+    lib().pcnn_oracle_voxel_window(_p(depth), _p(meta), B, H, W, meta.shape[-1], G, int(kernel_size),
+                                   ctypes.c_float(threshold), _p(count, ctypes.c_int), _p(clipped, ctypes.c_ubyte))
+    return count, clipped.astype(bool)
+
+
 def average_distance_loss(pred, target, weight, point, symmetry, margin):
     pred = _f32(pred); target = _f32(target); weight = _f32(weight); point = _f32(point); symmetry = _f32(symmetry)
     N = pred.shape[0]

@@ -571,6 +571,30 @@ int pcnn_oracle_voxel_average(const float* data, const float* label, const float
     return 0;
 }
 
+/* the windows of the window average, for test coverage: per voxel the hit count and whether the image border clips the
+ * (2 ks + 1)^2 window */
+int pcnn_oracle_voxel_window(const float* depth, const float* meta, int B, int H, int W, int num_meta, int G, int ks,
+                             float threshold, int* count, unsigned char* clipped)
+{
+#pragma omp parallel for collapse(2)
+    for (int n = 0; n < B; n++)
+        for (int d = 0; d < G; d++)
+            for (int h = 0; h < G; h++)
+                for (int w = 0; w < G; w++) {
+                    size_t v = (((size_t)n * G + d) * G + h) * G + w;
+                    int px, py, cnt = 0;
+                    float Z1;
+                    voxel_to_pixel(meta + (size_t)n * num_meta, d, h, w, &px, &py, &Z1, NULL);
+                    for (int x = px - ks; x <= px + ks; x++)
+                        for (int y = py - ks; y <= py + ks; y++)
+                            if (x >= 0 && x < W && y >= 0 && y < H && fabsf(depth[((size_t)n * H + y) * W + x] - Z1) < threshold)
+                                cnt++;
+                    count[v] = cnt;
+                    clipped[v] = (unsigned char)(px - ks < 0 || px + ks > W - 1 || py - ks < 0 || py + ks > H - 1);
+                }
+    return 0;
+}
+
 /* ------------------------------------------------------------------------- */
 /* Averagedistance — average_distance_loss/average_distance_loss_op_gpu.cu.cc:34-252 */
 /* ------------------------------------------------------------------------- */

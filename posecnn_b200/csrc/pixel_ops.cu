@@ -688,7 +688,9 @@ k_backproject_fused(const float* __restrict__ data, const float* __restrict__ la
         }
     }
     // ---- top_label: C floats per voxel; the slab's nvox * C floats are contiguous (float4 path when the slab is 16-byte
-    // aligned and whole: kBpVox * C * 4 bytes is a multiple of 16 for every C)
+    // aligned and whole: kBpVox * C * 4 bytes is a multiple of 16 for every C).  The float4 path decides per group of 4
+    // elements from the voxels of its first and last element, which are all the voxels the group touches only for C >= 2;
+    // with C = 1 the group spans four voxels, so C = 1 takes the per-element path.
     {
         float* ol = top_label + vbase * C;
         const float* l3 = label_3d + vbase * C;
@@ -710,7 +712,7 @@ k_backproject_fused(const float* __restrict__ data, const float* __restrict__ la
                 }
             return __fdiv_rn(acc, (float)cnt);
         };
-        if ((total & 3) == 0 && ((reinterpret_cast<uintptr_t>(ol) | reinterpret_cast<uintptr_t>(l3)) & 15) == 0) {
+        if (C > 1 && (total & 3) == 0 && ((reinterpret_cast<uintptr_t>(ol) | reinterpret_cast<uintptr_t>(l3)) & 15) == 0) {
             for (int i4 = t; i4 < total / 4; i4 += 256) {
                 const int i = 4 * i4;
                 const int va = i / C, vb = (i + 3) / C;

@@ -42,8 +42,8 @@ def test_first_max_route_reference():
 def test_coverage_helpers(native_lib):
     B, p = util.conv_batch_for_coverage(480, 640, 64, 64, 3, sms=132)                 # conv1_2: RESB row mode, 5 segments
     assert (B, p["kernel"], p["items"], p["per_cta"]) == (1, "row_resb", 1200, 9)
-    B, p = util.conv_batch_for_coverage(240, 320, 64, 128, 3, sms=132)                # conv2_1: two N tiles, ragged segment
-    assert (B, p["kernel"], p["items"], p["per_cta"]) == (1, "row", 720, 5)
+    B, p = util.conv_batch_for_coverage(240, 320, 64, 128, 3, sms=132)                # conv2_1: 256-pixel tile, BN = 128
+    assert (B, p["kernel"], p["items"], p["per_cta"]) == (2, "tile256", 600, 4)
     B, p = util.conv_batch_for_coverage(30, 40, 512, 512, 3, sms=132)                 # conv5: 16 x 8 tiles
     assert (B, p["tile"], p["bn"], p["per_cta"]) == (20, (16, 8), 256, 3)
     B, p = util.conv_batch_for_coverage(120, 160, 256, 256, 3, pool=True, sms=132)    # fused pool: always 8 x 16
@@ -56,3 +56,22 @@ def test_coverage_helpers(native_lib):
     assert p["min_ktiles"] >= 8 and rows % 64 == 1
     assert util.fc_plan(600, 4096, 25088, native_lib)["splits"] == 1
     assert util.fc_plan(600, 128, 4096, native_lib)["splits"] == 16
+
+
+def test_conv_plan_follows_the_dispatcher():
+    """conv_bf16_tc_impl (csrc/conv_tc.cu) runs the 3x3, Cin <= 128 layers with Cout = 128 on the 256-pixel tile (16 x 16,
+    BN = 128) and only Cout = 64 in row mode.  At 132 SMs every conv2 case of test_conv_exact_at_network_shapes therefore needs
+    batch 2 for three work items per CTA; the 720 x 960 shapes of test_rescale_gpu.py get there at batch 1."""
+    from tests.test_conv_gpu import _network_conv_cases
+    for H, W, want_B in ((480, 640, 2), (720, 960, 1)):
+        cases = {c[0]: c for c in _network_conv_cases(H, W)}
+        for name in ("conv2_1", "conv2_2", "conv2_2+pool"):
+            _, h, w, ci, co, k, pool, _ = cases[name]
+            B, p = util.conv_batch_for_coverage(h, w, ci, co, k, pool=pool, sms=132)
+            assert (p["kernel"], p["tile"], p["bn"]) == ("tile256", (16, 16), 128), (name, p)
+            assert p["items"] == B * -(-h // 16) * -(-w // 16) and p["grid"] == 132, (name, p)
+            assert (B, p["per_cta"] >= 3) == (want_B, True), (name, H, B, p)
+        for name in ("conv1_2", "conv1_2+pool", "conv2_1_dgrad"):                    # Cout = 64: row mode
+            _, h, w, ci, co, k, pool, _ = cases[name]
+            assert util.conv_plan(1, h, w, ci, co, k, pool=pool, sms=132)["kernel"] in ("row", "row_resb"), name
+        assert util.conv_plan(1, 240, 320, 64, 128, 3, block_n=128, sms=132)["tile"] == (8, 16)   # explicit N tile: 128 pixels

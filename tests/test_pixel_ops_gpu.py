@@ -1,4 +1,4 @@
-"""GPU parity of RoiPool, Hardlabel, Backproject, Project, Averagedistance (C ABI) vs the CPU oracle."""
+"""GPU parity of RoiPool, Hardlabel, Averagedistance (C ABI) vs the CPU oracle (Backproject / Project: test_project_exact_gpu.py)."""
 import numpy as np
 import pytest
 import torch
@@ -55,40 +55,6 @@ def test_hard_label(cuda, C):
         np.testing.assert_array_equal(to_np(out), oracle.hard_label(prob, gt, thr))
     gp, gg = op.hard_label_grad(T(prob, cuda), T(gt, cuda), out)
     assert gp.shape == (2, 37, 53, C) and gg.shape == (2, 37, 53) and not gp.any() and not gg.any()
-
-
-@pytest.mark.parametrize("Cf,C,G", [(64, 22, 32), (6, 3, 16), (8, 3, 128)])   # G = 128: the SURVEY 8(d) primary grid
-def test_project_backproject(cuda, Cf, C, G):
-    from posecnn_b200.backprojecting_layer import backprojecting_op as bop
-    from posecnn_b200.projecting_layer import projecting_op as pop
-    case = synth.make_projection_case(2, 48, 64, Cf, C, G, seed=5)
-    d = {k: T(v, cuda) for k, v in case.items()}
-    ks, thr = 3, 0.02
-    # Project forward (gather); pixels whose pre-round coordinate is within 1e-3 of a half integer are excluded
-    want, amb = oracle.project(case["vox"], case["depth"], case["meta"], return_ambig=True)
-    got = to_np(pop.project(d["vox"], d["depth"], d["meta"], ks, thr))
-    assert amb.mean() < 0.02
-    np.testing.assert_array_equal(got[~amb], want[~amb])
-    assert (np.abs(want).sum(-1) > 0).mean() > 0.5
-    # Backproject forward
-    td_w, tl_w, tf_w, amb3 = oracle.backproject(case["data"], case["label"], case["depth"], case["meta"], case["label_3d"],
-                                                G, ks, thr, return_ambig=True)
-    td, tl, tf = bop.backproject(d["data"], d["label"], d["depth"], d["meta"], d["label_3d"], G, ks, thr)
-    ok = ~amb3
-    assert ok.mean() > 0.9 and tf_w[..., 0].mean() > 0.001
-    np.testing.assert_array_equal(to_np(tf)[ok], tf_w[ok])
-    np.testing.assert_allclose(to_np(td)[ok], td_w[ok], rtol=1e-6, atol=1e-6)
-    np.testing.assert_allclose(to_np(tl)[ok], tl_w[ok], rtol=1e-6, atol=1e-6)
-    # gradients: BackprojectGrad = gather of top_diff; ProjectGrad = window average of top_diff
-    rng = np.random.default_rng(6)
-    g3 = rng.standard_normal((2, G, G, G, Cf)).astype(np.float32)
-    gb_w, amb2 = oracle.backproject_grad(g3, case["depth"], case["meta"], return_ambig=True)
-    gb = to_np(bop.backproject_grad(d["data"], d["depth"], d["meta"], T(g3, cuda), G))
-    np.testing.assert_array_equal(gb[~amb2], gb_w[~amb2])
-    g2 = rng.standard_normal((2, 48, 64, Cf)).astype(np.float32)
-    gp_w, amb4 = oracle.project_grad(g2, case["depth"], case["meta"], G, ks, thr, return_ambig=True)
-    gp = to_np(pop.project_grad(d["vox"], d["depth"], d["meta"], T(g2, cuda), ks, thr))
-    np.testing.assert_allclose(gp[~amb4], gp_w[~amb4], rtol=1e-6, atol=1e-6)
 
 
 @pytest.mark.parametrize("P,N", [(2620, 18), (300, 5)])

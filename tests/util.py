@@ -92,16 +92,16 @@ def num_sms(sms=None):
 # shrink a case back to one work item per CTA.
 # ---------------------------------------------------------------------------------------------------------------------
 def conv_plan(B, H, W, Cin, Cout, k, block_n=0, pool=False, sms=None):
-    """Work items and grid of one pcnn_conv_bf16_tc / pcnn_conv_pool_bf16_tc call (default row-mode switch)."""
+    """Work items and grid of one pcnn_conv_bf16_tc / pcnn_conv_pool_bf16_tc call (default N tile, block_n = 0): the 3x3 layers
+    with Cin <= 128 run Cout = 128 on the 256-pixel (16 x 16) tile at BN = 128, and Cout = 64 in row mode (two rows x 128 px)."""
     sms = num_sms(sms)
-    if block_n == 0 and k == 3 and Cin <= 128 and Cout <= 128 and H % 2 == 0 and W >= 128:
-        resb = Cin == 64 and Cout == 64
-        n_tiles = Cout // 64
-        items = B * (H // 2) * math.ceil(W / 128) * n_tiles
-        grid = min(items, sms)
-        if resb:
-            grid = grid // n_tiles * n_tiles
-        return dict(kernel="row_resb" if resb else "row", bn=64, tile=(2, 128), items=items, grid=grid)
+    if block_n == 0 and k == 3 and Cin <= 128 and Cout == 64 and H % 2 == 0 and W >= 128:
+        resb = Cin == 64
+        items = B * (H // 2) * math.ceil(W / 128)
+        return dict(kernel="row_resb" if resb else "row", bn=64, tile=(2, 128), items=items, grid=min(items, sms))
+    if block_n == 0 and k == 3 and Cin <= 128 and Cout == 128:
+        items = B * math.ceil(H / 16) * math.ceil(W / 16)
+        return dict(kernel="tile256", bn=128, tile=(16, 16), items=items, grid=min(items, sms))
     bn = block_n or (256 if Cout % 256 == 0 and k * k * Cin >= 2304 else (128 if Cout % 128 == 0 else 64))
     th, tw = 8, 16
     if not pool and math.ceil(H / 16) * math.ceil(W / 8) < math.ceil(H / 8) * math.ceil(W / 16):
