@@ -547,6 +547,37 @@ int pcnn_resize_linear_f32(const float* src, int B, int H, int W, int C, double 
 int pcnn_resize_depth(const void* depth, int depth_is_u16, int B, int H, int W, double fx, int Ho, int Wo, void* dst, void* stream);
 int pcnn_resize_nearest_i32(const int32_t* label, int B, int H, int W, double fx, int Ho, int Wo, int32_t* dst, void* stream);
 
+/* ---------------------------------------------------------------------------------------
+ * Detection network at test time (csrc/det.cu, DESIGN.md 16): networks/vgg16_det.py:94-137, from conv_rpn to the fc6 operand.
+ *  pcnn_rpn_heads_fwd   conv_rpn [npix,512] bf16 x weights [6A][512] bf16 (rows 0..2A-1 rpn_cls_score, 2A..6A-1 rpn_bbox_pred;
+ *      output-major) + bias [6A] f32, fp32 accumulation on the tensor cores; both 1x1 convolutions keep Network.conv's ReLU
+ *      (network.py:160).  -> cls_prob [npix,2A] f32 = the pair softmax of reshape_score (channel a against channel A + a,
+ *      network.py:700-710; foreground = channels A..2A-1), bbox_pred [npix,4A] f32 (ReLU'd deltas, anchor-major).  1 <= A <= 64.
+ *  pcnn_rpn_proposals_fwd   rpn_layer/proposal_layer.py for each of B images: cls_prob [B,h,w,2A], bbox_pred [B,h,w,4A], anchors
+ *      [h*w*A,4] f32 (snippets.py:generate_anchors_pre, order (h, w, a)); bbox_transform_inv + clip_boxes to [0, im_w - 1] x
+ *      [0, im_h - 1] in fp32 with numpy's operation order (no FMA); the K = min(pre_top_n, h*w*A) best anchors in the canonical
+ *      order (descending foreground probability, ties by ascending anchor index; the reference's unstable argsort leaves ties
+ *      unordered); greedy NMS with nms_kernel.cu's devIoU (+1 areas, fp32, no FMA), suppressing IoU > nms_thresh; the first
+ *      post_top_n kept boxes.  -> rois [B*post_top_n,5] (b, x1, y1, x2, y2), scores [B*post_top_n] and num_rois [B] int32;
+ *      rows past num_rois[b] are (b, 0, 0, 0, 0) with score 0.  pre_boxes [B*K,5] (nullable): the sorted, decoded, clipped
+ *      candidates (x1, y1, x2, y2, score) NMS ran on.  1 <= A <= 64, 1 <= pre_top_n <= 16384, post_top_n >= 1.  workspace:
+ *      pcnn_rpn_proposals_workspace_bytes (B * K * (20 + 8 * ceil(K / 64)) bytes, the NMS bitmask).
+ *  pcnn_crop_pool_f16   network.py:791-809: each ROI (b, x1, y1, x2, y2) of rois [N, roi_stride] divided by ((H-1) * feat_stride,
+ *      (W-1) * feat_stride), tf.image.crop_and_resize (TF 1.x bilinear: in_y = y1 * (H-1) + y * (y2-y1) * (H-1) / 13, samples
+ *      outside [0, H-1] x [0, W-1] are 0) to 14 x 14 on feat [B,H,W,C] bf16, then max_pool2d 2 x 2 / 2 -> out [N, 7*7*C] fp16
+ *      (h, w, c), saturated to +-65504.  fp32, every product and sum rounded.  A batch index outside [0, B) crops zeros.  C % 8 == 0.
+ *  pcnn_softmax_rows_f32   out[r] = softmax(in[r]) over cols (cls_prob = softmax(cls_score)).
+ * No allocation, no host synchronisation; CUDA-graph capturable. */
+int pcnn_rpn_heads_fwd(const void* conv_rpn_bf16, const void* weights_bf16, const float* bias, int npix, int A, float* cls_prob,
+                       float* bbox_pred, void* stream);
+int pcnn_rpn_proposals_workspace_bytes(int B, int h, int w, int A, int pre_top_n, size_t* bytes);
+int pcnn_rpn_proposals_fwd(const float* cls_prob, const float* bbox_pred, const float* anchors, int B, int h, int w, int A, float im_h,
+                           float im_w, int pre_top_n, int post_top_n, float nms_thresh, float* rois, float* scores, int32_t* num_rois,
+                           float* pre_boxes, void* workspace, size_t workspace_bytes, void* stream);
+int pcnn_crop_pool_f16(const void* feat_bf16, int B, int H, int W, int C, const float* rois, int num_rois, int roi_stride,
+                       float feat_stride, void* out_f16, void* stream);
+int pcnn_softmax_rows_f32(const float* in, int rows, int cols, float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -25,13 +25,7 @@ from .._lib import check, lib, ptr, stream
 from ..hough_voting_gpu_layer import hough_voting_gpu_op
 from ..roi_pooling_layer import roi_pooling_op
 from ..utils import nms as dev_nms
-
-PIXEL_MEANS = (102.9801, 115.9465, 122.7717)  # lib/fcn/config.py:242 (BGR)
-
-VGG_CFG = [("conv1_1", 3, 64), ("conv1_2", 64, 64), "pool1", ("conv2_1", 64, 128), ("conv2_2", 128, 128), "pool2",
-           ("conv3_1", 128, 256), ("conv3_2", 256, 256), ("conv3_3", 256, 256), "pool3", ("conv4_1", 256, 512),
-           ("conv4_2", 512, 512), ("conv4_3", 512, 512), "pool4", ("conv5_1", 512, 512), ("conv5_2", 512, 512),
-           ("conv5_3", 512, 512)]
+from .trunk import PIXEL_MEANS, VGG_CFG, conv_weights_to_tc, run_trunk, trunk_shapes  # noqa: F401
 
 
 class vgg16_convs:
@@ -71,11 +65,7 @@ class vgg16_convs:
         shapes = {}
         trunks = [""] + (["_p"] if self.input_format == "RGBD" else [])
         for sfx in trunks:
-            for item in VGG_CFG:
-                if isinstance(item, tuple):
-                    name, ci, co = item
-                    shapes[f"{name}{sfx}/weights"] = (3, 3, ci, co)
-                    shapes[f"{name}{sfx}/biases"] = (co,)
+            shapes.update(trunk_shapes(sfx))
         cin_head = 1024 if self.input_format == "RGBD" else 512
         for name, co in (("score_conv5", U), ("score_conv4", U), ("score_conv5_vertex", 128), ("score_conv4_vertex", 128)):
             shapes[f"{name}/weights"] = (1, 1, cin_head if not name.endswith("vertex") else 512, co)
@@ -155,11 +145,7 @@ class vgg16_convs:
         for name, shp in self.param_shapes().items():
             if not name.endswith("weights") or name.startswith("fc") or name in ("score/weights", "vertex_pred/weights", "domain_score/weights"):
                 continue
-            w = P[name]
-            if w.shape[2] == 3:  # conv1_1: im2col K order
-                T[name] = conv.conv1_1_weights_to_tc(w)
-            else:
-                T[name] = conv.hwio_to_tc(w)
+            T[name] = conv_weights_to_tc(P[name])
         for name in ("fc6", "fc7", "fc8"):
             T[f"{name}/weights"] = pose_head.fc_weights_to_tc(P[f"{name}/weights"])   # [out (padded to x128), in] fp16
         if self.domain_branch:
@@ -180,35 +166,8 @@ class vgg16_convs:
 
     # ------------------------------------------------------------------ graph pieces
     def _trunk(self, data, sfx=""):
-        """13 x (conv3x3 + bias + ReLU), 4 x max-pool (vgg16_convs.py:80-97).  data: [B,H,W,3] u8 (BGR, mean
-        subtracted on the fly) or f32 (already pre-processed), or [B,H,W] f32 = a RAW depth image (sensor units) whose
-        blob clip(d / 2000, 0, 1) * 255 x3 - PIXEL_MEANS (lib/fcn/test.py:70-76) is formed in the conv1_1 loader."""
-        P, T = self.params, self._tc
-        if data.dim() == 3:
-            x = conv.conv1_depth_fused(data, T[f"conv1_1{sfx}/weights"], P[f"conv1_1{sfx}/biases"], PIXEL_MEANS, True)
-        else:
-            mean = PIXEL_MEANS if data.dtype == torch.uint8 else None
-            x = conv.conv1_fused(data, T[f"conv1_1{sfx}/weights"], P[f"conv1_1{sfx}/biases"], mean, True)
-        feats = {}
-        cfg = VGG_CFG[1:]
-        i = 0
-        while i < len(cfg):
-            item = cfg[i]
-            if isinstance(item, str):
-                x = conv.maxpool2x2(x)
-                i += 1
-                continue
-            name = item[0]
-            fuse_pool = i + 1 < len(cfg) and isinstance(cfg[i + 1], str) and name not in ("conv4_3", "conv5_3")
-            if fuse_pool:   # conv + ReLU + max-pool in one kernel (the un-pooled tensor is not needed downstream)
-                x = conv.conv_pool_bf16(x, T[f"{name}{sfx}/weights"], P[f"{name}{sfx}/biases"], 3, True)
-                i += 2
-                continue
-            x = conv.conv_bf16(x, T[f"{name}{sfx}/weights"], P[f"{name}{sfx}/biases"], 3, True)
-            if name in ("conv4_3", "conv5_3"):
-                feats[name] = x
-            i += 1
-        return feats
+        """13 x (conv3x3 + bias + ReLU), 4 x max-pool (vgg16_convs.py:80-97): trunk.run_trunk on this network's weights."""
+        return run_trunk(self.params, self._tc, data, sfx)
 
     def forward(self, data, meta_data, extents, poses=None, data_p=None, want_prob=False, sync_rois=True, want_score=False,
                 dense_vertex=True, batch_global=None, batch_offset=0, depth=None, refine_depth=None, refine_points=None,

@@ -34,6 +34,26 @@ def roi_pool_pair(f5: torch.Tensor, f4: torch.Tensor, rois: torch.Tensor, pooled
     return out
 
 
+def crop_pool(feat: torch.Tensor, rois: torch.Tensor, feat_stride: float = 16.0) -> torch.Tensor:
+    """crop_pool of the detection network (network.py:791-809): [N, 7 * 7 * C] fp16 = max_pool2d 2x2 of crop_and_resize to 14 x 14
+    of feat [B,H,W,C] bf16 at the boxes rois [N,5] (b, x1, y1, x2, y2) in image pixels, flattened (h, w, c)."""
+    assert feat.is_cuda and feat.dtype == torch.bfloat16 and feat.is_contiguous() and feat.dim() == 4
+    assert rois.is_cuda and rois.dtype == torch.float32 and rois.is_contiguous() and rois.dim() == 2
+    B, H, W, C = feat.shape
+    n = rois.shape[0]
+    out = torch.empty((n, 7 * 7 * C), dtype=torch.float16, device=feat.device)
+    check(lib().pcnn_crop_pool_f16(ptr(feat), B, H, W, C, ptr(rois), n, rois.shape[1], float(feat_stride), ptr(out), stream()))
+    return out
+
+
+def softmax_rows(x: torch.Tensor) -> torch.Tensor:
+    """softmax over the last dimension of x [rows, cols] f32 (cls_prob = softmax(cls_score))."""
+    assert x.is_cuda and x.dtype == torch.float32 and x.is_contiguous() and x.dim() == 2
+    out = torch.empty_like(x)
+    check(lib().pcnn_softmax_rows_f32(ptr(x), x.shape[0], x.shape[1], ptr(out), stream()))
+    return out
+
+
 def fc(a: torch.Tensor, w_tc: torch.Tensor, bias: torch.Tensor, act: str = "relu", out_dtype=torch.float16) -> torch.Tensor:
     """act(a @ w^T + bias).  a [M, K] fp16, w_tc = fc_weights_to_tc(W) [Npad, K] fp16, bias [n_valid] f32.
     out_dtype fp16 -> [M, Npad] (the next layer's operand; padding columns are zero), f32 -> [M, n_valid]."""
