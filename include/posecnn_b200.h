@@ -567,6 +567,17 @@ int pcnn_resize_nearest_i32(const int32_t* label, int B, int H, int W, double fx
  *      outside [0, H-1] x [0, W-1] are 0) to 14 x 14 on feat [B,H,W,C] bf16, then max_pool2d 2 x 2 / 2 -> out [N, 7*7*C] fp16
  *      (h, w, c), saturated to +-65504.  fp32, every product and sum rounded.  A batch index outside [0, B) crops zeros.  C % 8 == 0.
  *  pcnn_softmax_rows_f32   out[r] = softmax(in[r]) over cols (cls_prob = softmax(cls_score)).
+ *  pcnn_det_records_fwd   the test loop's records (fcn/test.py:1589-1616, 1639-1691, 1731-1746) for B images of `rows` proposal
+ *      rows each: cls_prob [B*rows,C], bbox_pred [B*rows,4C] (normalised deltas), poses_tanh [B*rows,4C], rois [B*rows,5]
+ *      (b, x1, y1, x2, y2), num_rois [B] int32 (rows r < num_rois[b] count).  For each class j = 1..C-1 of image b, slot
+ *      b*(C-1) + j-1: the row with the top cls_prob[:, j] > 0.02f (ties: the lowest row; NaN never), its box de-normalised
+ *      (f32(f64(d) * (0.1, 0.1, 0.2, 0.2))), bbox_transform_inv'd and clipped to [0, im_w-1] x [0, im_h-1] in fp32 without FMA,
+ *      and the depth z of compute_translations' Nelder-Mead fit (scipy 1.18.1 at N = 1, x0 = 0.5, at most 200 evaluations) of
+ *      the projected points [C,P,3] of class j (R = quat2mat(q) in fp64 rounded to fp32, fp32 camera coordinates, K =
+ *      f64(meta[b, 0:9]) in fp64) to the box's width and height.  -> dets [B*(C-1),7] (b, j, x1, y1, x2, y2, score), poses
+ *      [B*(C-1),7] (q raw, f32(rx z), f32(ry z), f32(z)), trace [B*(C-1),2] int32 (iterations, evaluations), num_dets [B] int32
+ *      (zeroed here, then counted).  An empty slot is (b, 0, 0, 0, 0, 0, 0) with a zero pose and trace.  2 <= C <= 128,
+ *      1 <= P <= 4096, 1 <= B <= 65535, num_meta >= 9.
  * No allocation, no host synchronisation; CUDA-graph capturable. */
 int pcnn_rpn_heads_fwd(const void* conv_rpn_bf16, const void* weights_bf16, const float* bias, int npix, int A, float* cls_prob,
                        float* bbox_pred, void* stream);
@@ -577,6 +588,9 @@ int pcnn_rpn_proposals_fwd(const float* cls_prob, const float* bbox_pred, const 
 int pcnn_crop_pool_f16(const void* feat_bf16, int B, int H, int W, int C, const float* rois, int num_rois, int roi_stride,
                        float feat_stride, void* out_f16, void* stream);
 int pcnn_softmax_rows_f32(const float* in, int rows, int cols, float* out, void* stream);
+int pcnn_det_records_fwd(const float* cls_prob, const float* bbox_pred, const float* poses_tanh, const float* rois,
+                         const int32_t* num_rois, int B, int rows, int C, int im_h, int im_w, const float* meta, int num_meta,
+                         const float* points, int P, float* dets, float* poses, int32_t* num_dets, int32_t* trace, void* stream);
 
 #ifdef __cplusplus
 }

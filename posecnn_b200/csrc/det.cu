@@ -16,6 +16,7 @@
 #include <cuda_runtime.h>
 
 #include "common.cuh"
+#include "pose_common.cuh"
 
 namespace pcnn {
 namespace det {
@@ -111,6 +112,17 @@ __device__ __forceinline__ float fg_score(const float* cls_prob, size_t img_base
     return cls_prob[img_base + (size_t)pix * 2 * A + A + a];
 }
 
+// bbox_transform.py:bbox_transform_inv of one box and its deltas (dx, dy, dw, dh), fp32 with every product and sum rounded
+__device__ __forceinline__ float4 bbox_transform_inv(const float4 an, const float4 d)
+{
+    const float wd = __fadd_rn(__fsub_rn(an.z, an.x), 1.f), ht = __fadd_rn(__fsub_rn(an.w, an.y), 1.f);
+    const float cx = __fadd_rn(an.x, __fmul_rn(0.5f, wd)), cy = __fadd_rn(an.y, __fmul_rn(0.5f, ht));
+    const float pcx = __fadd_rn(__fmul_rn(d.x, wd), cx), pcy = __fadd_rn(__fmul_rn(d.y, ht), cy);
+    const float pw = __fmul_rn(expf(d.z), wd), ph = __fmul_rn(expf(d.w), ht);
+    const float hw = __fmul_rn(0.5f, pw), hh = __fmul_rn(0.5f, ph);
+    return make_float4(__fsub_rn(pcx, hw), __fsub_rn(pcy, hh), __fadd_rn(pcx, hw), __fadd_rn(pcy, hh));
+}
+
 // one CTA per image: radix-select the K-th largest key, gather the K keys above it, bitonic-sort them in shared memory,
 // decode + clip the sorted boxes (bbox_transform.py:bbox_transform_inv, clip_boxes)
 __global__ void __launch_bounds__(kSelThreads)
@@ -176,16 +188,11 @@ k_rpn_select(const float* __restrict__ cls_prob, const float* __restrict__ bbox_
         const int i = (int)(~(uint32_t)skeys[r]);
         const float4 an = reinterpret_cast<const float4*>(anchors)[i];
         const float4 d = reinterpret_cast<const float4*>(bbox_pred)[(size_t)b * n + i];
-        const float wd = __fadd_rn(__fsub_rn(an.z, an.x), 1.f), ht = __fadd_rn(__fsub_rn(an.w, an.y), 1.f);
-        const float cx = __fadd_rn(an.x, __fmul_rn(0.5f, wd)), cy = __fadd_rn(an.y, __fmul_rn(0.5f, ht));
-        const float pcx = __fadd_rn(__fmul_rn(d.x, wd), cx), pcy = __fadd_rn(__fmul_rn(d.y, ht), cy);
-        const float pw = __fmul_rn(expf(d.z), wd), ph = __fmul_rn(expf(d.w), ht);
-        const float hw = __fmul_rn(0.5f, pw), hh = __fmul_rn(0.5f, ph);
-        float4 o;
-        o.x = fmaxf(fminf(__fsub_rn(pcx, hw), xmax), 0.f);
-        o.y = fmaxf(fminf(__fsub_rn(pcy, hh), ymax), 0.f);
-        o.z = fmaxf(fminf(__fadd_rn(pcx, hw), xmax), 0.f);
-        o.w = fmaxf(fminf(__fadd_rn(pcy, hh), ymax), 0.f);
+        float4 o = bbox_transform_inv(an, d);
+        o.x = fmaxf(fminf(o.x, xmax), 0.f);
+        o.y = fmaxf(fminf(o.y, ymax), 0.f);
+        o.z = fmaxf(fminf(o.z, xmax), 0.f);
+        o.w = fmaxf(fminf(o.w, ymax), 0.f);
         const float score = fg_score(cls_prob, img_base, A, i);
         boxes[(size_t)b * K + r] = o;
         sorted_scores[(size_t)b * K + r] = score;
@@ -356,6 +363,229 @@ k_softmax_rows(const float* __restrict__ in, int rows, int cols, float* __restri
     for (int j = lane; j < cols; j += 32) out[(size_t)row * cols + j] = expf(x[j] - m) / s;
 }
 
+// ---------------------------------------------------------------------------------------------------- detection records
+// lib/fcn/test.py's post-processing of the detection network (1589-1616, 1639-1691, 1731-1746) for one (image, class j >= 1) slot
+// per CTA: the argmax of cls_prob[:, j] over the kept proposals above 0.02, its de-normalised and clipped class-j box, and the
+// depth z of compute_translations' Nelder-Mead fit (scipy 1.18.1 _minimize_neldermead at N = 1).  Every thread runs the same
+// scalar Nelder-Mead decisions on the objective values the block computes together, so control flow stays uniform.
+constexpr int kRecThreads = 256;
+constexpr int kRecMaxPoints = 4096;
+constexpr int kRecMaxClasses = 128;
+constexpr int kNmMaxFun = 200;   // maxiter = maxfun = 200 * N
+
+// np.minimum / np.maximum: NaN propagates (fminf / fmaxf would drop it)
+__device__ __forceinline__ double nan_min(double a, double b) { return (a < b || a != a) ? a : b; }
+__device__ __forceinline__ double nan_max(double a, double b) { return (a > b || a != a) ? a : b; }
+// clip_boxes: np.maximum(np.minimum(v, hi), 0) with numpy's scalar rules (NaN kept, ties keep the first operand)
+__device__ __forceinline__ float clip_f(float v, float hi)
+{
+    const float m = (v <= hi || v != v) ? v : hi;
+    return (m >= 0.f || m != m) ? m : 0.f;
+}
+
+// np.argsort of two values (insertion sort: stable, NaN last): true when the second sorts before the first
+__device__ __forceinline__ bool nm_swap(double f0, double f1) { return f1 < f0 || (f0 != f0 && f1 == f1); }
+
+struct RecObjective {
+    const float* pts;   // [P,3] of the slot's class, in shared memory
+    int P;
+    float R[9];
+    double K[9], rx, ry, width, height;
+    double (*red)[kRecThreads / 32][4];   // [2][warps][xmin, xmax, ymin, ymax]
+};
+
+// distance_objective(z): fp32 camera coordinates ((r0 px + r1 py) + r2 pz) + t with t = f32(rx z, ry z, z), the K row products
+// and the division in fp64, NaN-propagating extents, (w - width)^2 + (h - height)^2.  Called by every thread of the block.
+__device__ __forceinline__ double rec_objective(const RecObjective& o, double z, int& parity)
+{
+    const float t[3] = {(float)__dmul_rn(o.rx, z), (float)__dmul_rn(o.ry, z), (float)z};
+    double x1 = INFINITY, x2 = -INFINITY, y1 = INFINITY, y2 = -INFINITY;
+    for (int p = threadIdx.x; p < o.P; p += kRecThreads) {
+        const float px = o.pts[3 * p], py = o.pts[3 * p + 1], pz = o.pts[3 * p + 2];
+        double c[3];
+#pragma unroll
+        for (int r = 0; r < 3; r++)
+            c[r] = (double)__fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(o.R[3 * r], px), __fmul_rn(o.R[3 * r + 1], py)),
+                                               __fmul_rn(o.R[3 * r + 2], pz)), t[r]);
+        double q[3];
+#pragma unroll
+        for (int r = 0; r < 3; r++)
+            q[r] = __dadd_rn(__dadd_rn(__dmul_rn(o.K[3 * r], c[0]), __dmul_rn(o.K[3 * r + 1], c[1])), __dmul_rn(o.K[3 * r + 2], c[2]));
+        const double u = __ddiv_rn(q[0], q[2]), v = __ddiv_rn(q[1], q[2]);
+        x1 = nan_min(x1, u); x2 = nan_max(x2, u); y1 = nan_min(y1, v); y2 = nan_max(y2, v);
+    }
+    for (int off = 16; off; off >>= 1) {
+        x1 = nan_min(x1, __shfl_xor_sync(0xffffffffu, x1, off)); x2 = nan_max(x2, __shfl_xor_sync(0xffffffffu, x2, off));
+        y1 = nan_min(y1, __shfl_xor_sync(0xffffffffu, y1, off)); y2 = nan_max(y2, __shfl_xor_sync(0xffffffffu, y2, off));
+    }
+    double (*red)[4] = o.red[parity];
+    parity ^= 1;   // alternate buffers: one barrier per evaluation
+    if ((threadIdx.x & 31) == 0) {
+        double* r = red[threadIdx.x >> 5];
+        r[0] = x1; r[1] = x2; r[2] = y1; r[3] = y2;
+    }
+    __syncthreads();
+    x1 = red[0][0]; x2 = red[0][1]; y1 = red[0][2]; y2 = red[0][3];
+    for (int w = 1; w < kRecThreads / 32; w++) {
+        x1 = nan_min(x1, red[w][0]); x2 = nan_max(x2, red[w][1]); y1 = nan_min(y1, red[w][2]); y2 = nan_max(y2, red[w][3]);
+    }
+    const double dw = __dsub_rn(__dsub_rn(x2, x1), o.width), dh = __dsub_rn(__dsub_rn(y2, y1), o.height);
+    return __dadd_rn(__dmul_rn(dw, dw), __dmul_rn(dh, dh));
+}
+
+// _wrap_scalar_function_maxfun_validation: the 201st call raises _MaxFuncCallError instead of evaluating
+__device__ __forceinline__ bool nm_call(const RecObjective& o, double x, double& fx, int& nfev, int& parity)
+{
+    if (nfev >= kNmMaxFun) return false;
+    nfev++;
+    fx = rec_objective(o, x, parity);
+    return true;
+}
+
+// scipy.optimize._optimize._minimize_neldermead at N = 1, x0 = 0.5, defaults (rho 1, chi 2, psi 0.5, sigma 0.5, xatol = fatol =
+// 1e-4, maxiter = maxfun = 200), with its expression shapes.  For N = 1 xbar = sim[0] and fsim[-2] = fsim[0], so the
+// reflection's `fxr < fsim[-2]` branch can never be taken after `fxr < fsim[0]` failed.  Returns sim[0].
+__device__ __forceinline__ double nelder_mead(const RecObjective& o, int& nit, int& nfev)
+{
+    int parity = 0;
+    nfev = 0;
+    double s0 = 0.5, s1 = __dmul_rn(__dadd_rn(1.0, 0.05), 0.5), f0, f1;   // sim[1] = (1 + nonzdelt) * x0
+    nm_call(o, s0, f0, nfev, parity);
+    nm_call(o, s1, f1, nfev, parity);
+    if (nm_swap(f0, f1)) { const double ts = s0, tf = f0; s0 = s1; f0 = f1; s1 = ts; f1 = tf; }
+    int it = 1;
+    while (nfev < kNmMaxFun && it < kNmMaxFun) {
+        if (fabs(__dsub_rn(s1, s0)) <= 1e-4 && fabs(__dsub_rn(f0, f1)) <= 1e-4) break;
+        do {   // `break` below is scipy's `except _MaxFuncCallError: pass`
+            const double xbar = s0;
+            const double xr = __dsub_rn(__dmul_rn(2.0, xbar), __dmul_rn(1.0, s1));
+            double fxr;
+            if (!nm_call(o, xr, fxr, nfev, parity)) break;
+            if (fxr < f0) {
+                const double xe = __dsub_rn(__dmul_rn(3.0, xbar), __dmul_rn(2.0, s1));
+                double fxe;
+                if (!nm_call(o, xe, fxe, nfev, parity)) break;
+                if (fxe < fxr) { s1 = xe; f1 = fxe; } else { s1 = xr; f1 = fxr; }
+            } else {
+                bool shrink = false;
+                if (fxr < f1) {
+                    const double xc = __dsub_rn(__dmul_rn(1.5, xbar), __dmul_rn(0.5, s1));
+                    double fxc;
+                    if (!nm_call(o, xc, fxc, nfev, parity)) break;
+                    if (fxc <= fxr) { s1 = xc; f1 = fxc; } else shrink = true;
+                } else {
+                    const double xcc = __dadd_rn(__dmul_rn(0.5, xbar), __dmul_rn(0.5, s1));
+                    double fxcc;
+                    if (!nm_call(o, xcc, fxcc, nfev, parity)) break;
+                    if (fxcc < f1) { s1 = xcc; f1 = fxcc; } else shrink = true;
+                }
+                if (shrink) {
+                    s1 = __dadd_rn(s0, __dmul_rn(0.5, __dsub_rn(s1, s0)));
+                    double fs;
+                    if (!nm_call(o, s1, fs, nfev, parity)) break;
+                    f1 = fs;
+                }
+            }
+            it++;
+        } while (false);
+        if (nm_swap(f0, f1)) { const double ts = s0, tf = f0; s0 = s1; f0 = f1; s1 = ts; f1 = tf; }
+    }
+    nit = it;
+    return s0;
+}
+
+struct RecArgs {
+    const float *cls_prob, *bbox_pred, *poses_tanh, *rois;
+    const int32_t* num_rois;
+    int rows, C, P, num_meta;
+    float xmax, ymax;
+    const float *meta, *points;
+    float *dets, *poses;
+    int32_t *num_dets, *trace;
+};
+
+__global__ void __launch_bounds__(kRecThreads) k_det_records(RecArgs a)
+{
+    extern __shared__ float s_pts[];   // [P,3]
+    __shared__ double s_red[2][kRecThreads / 32][4];
+    __shared__ unsigned long long s_best[kRecThreads / 32];
+    const int j = blockIdx.x + 1, b = blockIdx.y, C = a.C, t = threadIdx.x, lane = t & 31;
+    const size_t slot = (size_t)b * (C - 1) + (j - 1);
+    const int nr = min(max(a.num_rois[b], 0), a.rows);
+    // argmax over rows r < nr with score > 0.02f; key = (score bits, ~r): the largest key is the top score at the lowest row.
+    // Scores above 0.02 are positive, so their bit patterns order as the values; NaN fails the comparison.
+    unsigned long long best = 0;
+    for (int r = t; r < nr; r += kRecThreads) {
+        const float s = a.cls_prob[((size_t)b * a.rows + r) * C + j];
+        if (s > 0.02f) {
+            const unsigned long long key = ((unsigned long long)__float_as_uint(s) << 32) | (uint32_t)~(uint32_t)r;
+            best = key > best ? key : best;
+        }
+    }
+    for (int off = 16; off; off >>= 1) {
+        const unsigned long long o = __shfl_xor_sync(0xffffffffu, best, off);
+        best = o > best ? o : best;
+    }
+    if (lane == 0) s_best[t >> 5] = best;
+    for (int p = t; p < a.P * 3; p += kRecThreads) s_pts[p] = a.points[(size_t)j * a.P * 3 + p];
+    __syncthreads();
+    best = s_best[0];
+    for (int w = 1; w < kRecThreads / 32; w++) best = s_best[w] > best ? s_best[w] : best;
+    float* det = a.dets + slot * 7;
+    float* pose = a.poses + slot * 7;
+    int32_t* tr = a.trace + slot * 2;
+    if (best == 0) {   // nothing above the threshold: an empty slot
+        if (t < 7) { det[t] = t == 0 ? (float)b : 0.f; pose[t] = 0.f; }
+        if (t < 2) tr[t] = 0;
+        return;
+    }
+    const int r = (int)~(uint32_t)best;
+    const size_t row = (size_t)b * a.rows + r;
+    const float* q = a.poses_tanh + row * 4 * C + 4 * j;
+    __shared__ float s_box[4], s_R[9];
+    __shared__ double s_ray[4];   // rx, ry, width, height
+    if (t == 0) {
+        // test.py:1731-1743: bbox_pred *= stds (float64, stored back to float32), += means (0); boxes = rois[:, 1:5] / im_scale (1)
+        const float* dp = a.bbox_pred + row * 4 * C + 4 * j;
+        const double stds[4] = {0.1, 0.1, 0.2, 0.2};
+        float dn[4];
+#pragma unroll
+        for (int k = 0; k < 4; k++) dn[k] = (float)__dadd_rn((double)(float)__dmul_rn((double)dp[k], stds[k]), 0.0);
+        const float* roi = a.rois + row * 5;
+        float4 box = bbox_transform_inv(make_float4(roi[1], roi[2], roi[3], roi[4]), make_float4(dn[0], dn[1], dn[2], dn[3]));
+        box.x = clip_f(box.x, a.xmax); box.y = clip_f(box.y, a.ymax); box.z = clip_f(box.z, a.xmax); box.w = clip_f(box.w, a.ymax);
+        s_box[0] = box.x; s_box[1] = box.y; s_box[2] = box.z; s_box[3] = box.w;
+        // compute_translations (test.py:1646-1653): centre and size in float32 (x * 0.5f is x / 2 exactly), the ray in float64
+        const float* m = a.meta + (size_t)b * a.num_meta;
+        const float cxf = __fmul_rn(__fadd_rn(box.x, box.z), 0.5f), cyf = __fmul_rn(__fadd_rn(box.y, box.w), 0.5f);
+        s_ray[0] = __ddiv_rn(__dsub_rn((double)cxf, (double)m[2]), (double)m[0]);
+        s_ray[1] = __ddiv_rn(__dsub_rn((double)cyf, (double)m[5]), (double)m[4]);
+        s_ray[2] = (double)__fsub_rn(box.z, box.x);
+        s_ray[3] = (double)__fsub_rn(box.w, box.y);
+        quat2mat_f32(q[0], q[1], q[2], q[3], s_R);
+    }
+    __syncthreads();
+    RecObjective o;
+    o.pts = s_pts;
+    o.P = a.P;
+    o.red = s_red;
+    const float* m = a.meta + (size_t)b * a.num_meta;
+#pragma unroll
+    for (int k = 0; k < 9; k++) { o.K[k] = (double)m[k]; o.R[k] = s_R[k]; }
+    o.rx = s_ray[0]; o.ry = s_ray[1]; o.width = s_ray[2]; o.height = s_ray[3];
+    int nit, nfev;
+    const double z = nelder_mead(o, nit, nfev);
+    if (t == 0) {
+        const float d[7] = {(float)b, (float)j, s_box[0], s_box[1], s_box[2], s_box[3], __uint_as_float((uint32_t)(best >> 32))};
+        const float p[7] = {q[0], q[1], q[2], q[3], (float)__dmul_rn(o.rx, z), (float)__dmul_rn(o.ry, z), (float)z};
+#pragma unroll
+        for (int k = 0; k < 7; k++) { det[k] = d[k]; pose[k] = p[k]; }
+        tr[0] = nit;
+        tr[1] = nfev;
+        atomicAdd(a.num_dets + b, 1);
+    }
+}
+
 struct PropLayout {
     int K, sortN, col_blocks;
     size_t boxes, scores, mask, total;
@@ -468,4 +698,30 @@ extern "C" int pcnn_softmax_rows_f32(const float* in, int rows, int cols, float*
     PCNN_REQUIRE(rows >= 1 && cols >= 1, "softmax_rows: non-positive size (%d x %d)", rows, cols);
     k_softmax_rows<<<(rows + 7) / 8, 256, 0, (cudaStream_t)stream>>>(in, rows, cols, out);
     return check_launch("softmax_rows");
+}
+
+extern "C" int pcnn_det_records_fwd(const float* cls_prob, const float* bbox_pred, const float* poses_tanh, const float* rois,
+                                    const int32_t* num_rois, int B, int rows, int C, int im_h, int im_w, const float* meta,
+                                    int num_meta, const float* points, int P, float* dets, float* poses, int32_t* num_dets,
+                                    int32_t* trace, void* stream)
+{
+    PCNN_REQUIRE(cls_prob && bbox_pred && poses_tanh && rois && num_rois && meta && points && dets && poses && num_dets && trace,
+                 "det_records: NULL tensor pointer");
+    PCNN_REQUIRE(C >= 2 && C <= kRecMaxClasses, "det_records: C = %d classes (2 <= C <= %d)", C, kRecMaxClasses);
+    PCNN_REQUIRE(P >= 1 && P <= kRecMaxPoints, "det_records: P = %d points per class (1 <= P <= %d)", P, kRecMaxPoints);
+    PCNN_REQUIRE(B >= 1 && B <= 65535, "det_records: B = %d images (1 <= B <= 65535)", B);
+    PCNN_REQUIRE(rows >= 1 && (long long)B * rows * 4 * C <= 0x7fffffffLL, "det_records: %d rows per image", rows);
+    PCNN_REQUIRE(im_h >= 1 && im_w >= 1, "det_records: image size %d x %d", im_h, im_w);
+    PCNN_REQUIRE(num_meta >= 9, "det_records: num_meta = %d (K is meta[b, 0:9])", num_meta);
+    cudaStream_t st = (cudaStream_t)stream;
+    const cudaError_t e = cudaMemsetAsync(num_dets, 0, sizeof(int32_t) * B, st);
+    if (e != cudaSuccess) {
+        set_error("det_records: %s", cudaGetErrorString(e));
+        return PCNN_E_CUDA;
+    }
+    RecArgs a{cls_prob, bbox_pred, poses_tanh, rois, num_rois, rows, C, P, num_meta, (float)(im_w - 1), (float)(im_h - 1), meta, points,
+              dets, poses, num_dets, trace};
+    PCNN_SMEM_OPTIN(k_det_records, sizeof(float) * 3 * kRecMaxPoints, "det_records");
+    k_det_records<<<dim3(C - 1, B), kRecThreads, sizeof(float) * 3 * P, st>>>(a);
+    return check_launch("det_records");
 }

@@ -1,5 +1,6 @@
-// pose_common.cuh — rotation helpers shared by the kernels that write quaternion pose rows (train_targets.cu: the pose
-// blob; coord_pose.cu: the VERTEX_REG_3D detection records).
+// pose_common.cuh — rotation helpers shared by the kernels that read or write quaternion pose rows (train_targets.cu: the
+// pose blob; coord_pose.cu: the VERTEX_REG_3D detection records; evaluate.cu: the scored estimates; det.cu: the box-fitted
+// translations of the detection records).
 #pragma once
 #include "common.cuh"
 
@@ -51,5 +52,24 @@ __device__ inline void mat2quat_d(const float* __restrict__ rt /*3x4 row-major*/
     q[0] = (float)w; q[1] = (float)x; q[2] = (float)y; q[3] = (float)z;
 }
 
+// transforms3d.quaternions.quat2mat (transforms3d 0.3.1, quaternions.py): normalise by |q|^2, identity below float64 eps
+// (_FLOAT_EPS = np.finfo(np.float64).eps).  Evaluated in fp64 in the published operation order with the rounding intrinsics
+// (never contracted into FMAs), then rounded to fp32 like the reference's float32 RT (lov.py:586-588).
+__device__ __forceinline__ void quat2mat_f32(double w, double x, double y, double z, float* R)
+{
+    const double Nq = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(w, w), __dmul_rn(x, x)), __dmul_rn(y, y)), __dmul_rn(z, z));
+    if (Nq < 2.220446049250313e-16) {   // `if Nq < _FLOAT_EPS: return np.eye(3)`
+        for (int i = 0; i < 9; i++) R[i] = (i % 4 == 0) ? 1.f : 0.f;
+        return;
+    }
+    const double s = __ddiv_rn(2.0, Nq);
+    const double X = __dmul_rn(x, s), Y = __dmul_rn(y, s), Z = __dmul_rn(z, s);
+    const double wX = __dmul_rn(w, X), wY = __dmul_rn(w, Y), wZ = __dmul_rn(w, Z);
+    const double xX = __dmul_rn(x, X), xY = __dmul_rn(x, Y), xZ = __dmul_rn(x, Z);
+    const double yY = __dmul_rn(y, Y), yZ = __dmul_rn(y, Z), zZ = __dmul_rn(z, Z);
+    R[0] = (float)__dsub_rn(1.0, __dadd_rn(yY, zZ)); R[1] = (float)__dsub_rn(xY, wZ); R[2] = (float)__dadd_rn(xZ, wY);
+    R[3] = (float)__dadd_rn(xY, wZ); R[4] = (float)__dsub_rn(1.0, __dadd_rn(xX, zZ)); R[5] = (float)__dsub_rn(yZ, wX);
+    R[6] = (float)__dsub_rn(xZ, wY); R[7] = (float)__dadd_rn(yZ, wX); R[8] = (float)__dsub_rn(1.0, __dadd_rn(xX, yY));
+}
 
 }  // namespace pcnn

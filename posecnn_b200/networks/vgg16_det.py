@@ -11,6 +11,8 @@ checkpoint maps one to one.  The graph of vgg16_det.setup() up to the five tenso
     crop_pool (crop_and_resize 14x14, max 2x2)     fp16 fc6 operand                           csrc/det.cu
     fc6, fc7 (ReLU), cls_score (ReLU) -> softmax,  split-K wgmma GEMMs                        csrc/fc_tc.cu, csrc/det.cu
       bbox_pred, poses_pred_unnormalized -> tanh
+    with meta_data: the test loop's records        det_records.detection_records              csrc/det.cu
+      (top box per class, box-fitted translation)
 
 Dropout is the identity (keep_prob 1).  Proposals are per image (the reference runs one image; rois[:,0] is the image index
 here), and every output is capacity-shaped with a device row count per image, so the whole forward needs no host
@@ -24,6 +26,7 @@ import numpy as np
 import torch
 
 from .. import conv, pose_head
+from ..det_records import detection_records
 from ..rpn_layer.proposal_layer import proposal_layer, rpn_heads
 from ..rpn_layer.snippets import generate_anchors_pre
 from .trunk import conv_weights_to_tc, run_trunk, trunk_shapes
@@ -48,6 +51,7 @@ class vgg16_det:
         self._tc: dict[str, torch.Tensor] = {}
         self._anchors: dict[tuple, torch.Tensor] = {}
         self.layers: dict[str, torch.Tensor] = {}
+        self.points: torch.Tensor | None = None
 
     # ------------------------------------------------------------------ parameters
     def param_shapes(self):
@@ -109,14 +113,29 @@ class vgg16_det:
             self._anchors[key] = torch.from_numpy(a).to(self.device)
         return self._anchors[key]
 
+    def set_points(self, points):
+        """The object-point table [C,P,3] compute_translations projects (the imdb's _points_all, lov.py:141-158: every class
+        truncated to the smallest point count), P <= 4096."""
+        pts = torch.as_tensor(points, dtype=torch.float32).to(self.device).contiguous()
+        if pts.dim() != 3 or pts.shape[0] != self.num_classes or pts.shape[2] != 3:
+            raise ValueError(f"points must be [C,P,3] with C = {self.num_classes}")
+        self.points = pts
+        return self
+
     # ------------------------------------------------------------------ forward
-    def forward(self, data, sync_rois=True):
+    def forward(self, data, sync_rois=True, meta_data=None):
         """Test-time forward.  data [B,H,W,3] u8 BGR (PIXEL_MEANS subtracted in conv1_1's loader) or pre-processed f32, H and W
         multiples of 16; im_info is (H, W) of this blob.  Returns self.layers: conv5_3, conv_rpn, rpn_cls_prob [B,h,w,2A],
         rpn_bbox_pred [B,h,w,4A], rois [B*N,5], rpn_scores [B*N,1], num_rois [B] int32, cls_prob [B*N,C], bbox_pred [B*N,4C],
         poses_tanh [B*N,4C] with N = 300 proposals per image (TEST.RPN_POST_NMS_TOP_N); rows past num_rois[b] are zero boxes
         carrying b, and their head outputs are those of that box.  sync_rois=True reads num_rois back and keeps only the
-        proposals each image has (at B = 1: the reference's shapes)."""
+        proposals each image has (at B = 1: the reference's shapes).
+
+        meta_data [B,>=9] f32 on the device (K = meta_data[b, 0:9]) adds the records of the reference's test loop
+        (det_records.detection_records, points from set_points): dets [B*(C-1),7] (b, class, x1, y1, x2, y2, score), poses
+        [B*(C-1),7] (quaternion, translation), num_dets [B] int32 and det_trace [B*(C-1),2] (Nelder-Mead iterations,
+        evaluations), one slot per (image, class >= 1).  sync_rois=True drops the empty slots: the records of each image in
+        ascending class order, whose columns 1: are the reference's `rois` [n,6] at B = 1."""
         if self.is_train:
             raise NotImplementedError("vgg16_det runs at test time only (is_train=False)")
         P, T = self.params, self._tc
@@ -146,34 +165,49 @@ class vgg16_det:
         L["cls_prob"] = pose_head.softmax_rows(out["cls_score"])
         L["bbox_pred"] = out["bbox_pred"]
         L["poses_tanh"] = out["poses_pred_unnormalized"]
+        if meta_data is not None:
+            if self.points is None:
+                raise ValueError("the records need the object-point table: call set_points first")
+            L["dets"], L["poses"], L["num_dets"], L["det_trace"] = detection_records(
+                L["cls_prob"], L["bbox_pred"], L["poses_tanh"], rois, num, (H, W), meta_data, self.points)
         if sync_rois:
             counts = num.tolist()   # the one host read the reference's data-dependent shapes require
             per = rois.shape[0] // B
             idx = torch.cat([torch.arange(b * per, b * per + n, device=rois.device) for b, n in enumerate(counts)])
             for k in ("rois", "rpn_scores", "cls_score", "cls_prob", "bbox_pred", "poses_tanh"):
                 L[k] = L[k].index_select(0, idx)
+            if meta_data is not None:
+                filled = (L["dets"][:, 1] > 0).nonzero().squeeze(1)
+                for k in ("dets", "poses", "det_trace"):
+                    L[k] = L[k].index_select(0, filled)
         return L
 
 
 class GraphedForward:
     """vgg16_det.forward captured once into a CUDA graph (every shape is static: proposals are capacity buffers with a device
-    count per image).  __call__(data) copies the batch into the captured input and replays."""
+    count per image, records fixed slots per (image, class)).  With meta_data the graph includes the records stage.
+    __call__(data, meta_data) copies the batch (and its meta data) into the captured inputs and replays."""
 
-    def __init__(self, net: vgg16_det, data: torch.Tensor, warmup: int = 2):
+    def __init__(self, net: vgg16_det, data: torch.Tensor, warmup: int = 2, meta_data: torch.Tensor | None = None):
         self.net = net
         self.s_data = data.clone()
+        self.s_meta = None if meta_data is None else meta_data.clone()
         side = torch.cuda.Stream(device=data.device)
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):
             for _ in range(warmup):
-                net.forward(self.s_data, sync_rois=False)
+                net.forward(self.s_data, sync_rois=False, meta_data=self.s_meta)
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
         self.graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(self.graph):
-            self.layers = dict(net.forward(self.s_data, sync_rois=False))
+            self.layers = dict(net.forward(self.s_data, sync_rois=False, meta_data=self.s_meta))
 
-    def __call__(self, data: torch.Tensor):
+    def __call__(self, data: torch.Tensor, meta_data: torch.Tensor | None = None):
         self.s_data.copy_(data, non_blocking=True)
+        if meta_data is not None:
+            if self.s_meta is None:
+                raise ValueError("this graph was captured without meta_data")
+            self.s_meta.copy_(meta_data, non_blocking=True)
         self.graph.replay()
         return self.layers
