@@ -48,10 +48,13 @@ def _i32(a):
 
 
 def hough_voting_gpu(label, vertex, extents, meta, gt, is_train=0, threshold_vote=-1.0, threshold_percentage=0.02,
-                     skip_pixels=10, inlier_threshold=0.9, label_threshold=500, debug=False):
+                     skip_pixels=10, inlier_threshold=0.9, label_threshold=500, debug=False, slack=False):
     """Canonical-order restatement of Houghvotinggpu.  Returns the five op outputs
     (with the >=1 dummy-row rule of hough_voting_gpu_op.cc:379-383) and, if debug,
-    a dict with the raw row count, vote planes and ambiguity counts."""
+    a dict with the raw row count, vote planes and ambiguity counts; with slack=True (implies debug) also the
+    exactness analysis of the interval scan: `slack` [B,C,H,W] int32 (irregular (sample, row) pairs whose window row
+    holds the cell) and `pairs` [B,C,2] int64 ((sample, row) pairs inside a window, irregular ones)."""
+    debug = debug or slack
     label = _i32(label); vertex = _f32(vertex); extents = _f32(extents); meta = _f32(meta)
     gt = np.zeros((0, 13), np.float32) if gt is None else _f32(gt).reshape(-1, 13)
     B, H, W = label.shape
@@ -63,18 +66,40 @@ def hough_voting_gpu(label, vertex, extents, meta, gt, is_train=0, threshold_vot
     nrois = ctypes.c_int(0)
     votes = np.zeros((B, C, H, W), np.float32) if debug else None
     ambig = np.zeros((B, C, H, W), np.int32) if debug else None
+    slk = np.zeros((B, C, H, W), np.int32) if slack else None
+    pairs = np.zeros((B, C, 2), np.int64) if slack else None
     gt_arg = gt if gt.size else np.zeros((1, 13), np.float32)
     rc = lib().pcnn_oracle_hough(
         _p(label, ctypes.c_int), _p(vertex), _p(extents), _p(meta), _p(gt_arg), B, H, W, C, gt.shape[0], num_meta,
         int(is_train), ctypes.c_float(inlier_threshold), int(label_threshold), ctypes.c_float(threshold_vote),
         ctypes.c_float(threshold_percentage), int(skip_pixels), _p(box), _p(pose), _p(target), _p(weight),
-        _p(domain, ctypes.c_int), ctypes.byref(nrois), _p(votes), _p(ambig, ctypes.c_int))
+        _p(domain, ctypes.c_int), ctypes.byref(nrois), _p(votes), _p(ambig, ctypes.c_int), _p(slk, ctypes.c_int),
+        _p(pairs, ctypes.c_longlong))
     assert rc == 0
     n = max(1, nrois.value)
     outs = (box[:n].copy(), pose[:n].copy(), target[:n].copy(), weight[:n].copy(), domain[:n].copy())
     if debug:
-        return outs, dict(num_rois=nrois.value, votes=votes, ambig=ambig)
+        dbg = dict(num_rois=nrois.value, votes=votes, ambig=ambig)
+        if slack:
+            dbg.update(slack=slk, pairs=pairs)
+        return outs, dbg
     return outs
+
+
+def project_box(extents, meta, cls, distance, factor=0.6):
+    """project_box (.cu.cc:84-120) of one image's meta record: the half-size of a sample's vote window at depth distance."""
+    f = lib().pcnn_oracle_project_box
+    f.restype = ctypes.c_float
+    return f(int(cls), _p(_f32(extents)), _p(_f32(meta).reshape(-1)), ctypes.c_float(distance), ctypes.c_float(factor))
+
+
+def hough_row_exact(passes, wmin, x, own_row):
+    """The exactness criterion of one (sample, row) pair (pcnn_oracle_hough_row_exact): `passes` = the reference
+    predicate on the window row's cells wmin .. wmin + len - 1; True when the set is empty or one interval (on the
+    pixel's own row: empty or one whole side of the window)."""
+    p = np.ascontiguousarray(passes, dtype=np.uint8)
+    return bool(lib().pcnn_oracle_hough_row_exact(_p(p, ctypes.c_ubyte), int(wmin), int(wmin) + p.size - 1, int(x),
+                                                  int(bool(own_row))))
 
 
 def roi_pool(data, rois, pooled_height, pooled_width, spatial_scale, pool_channel=0):

@@ -87,6 +87,11 @@ static float project_box_f(int cls, const float* extents, const float* meta, flo
     return fmaxf(width, height) * factor;
 }
 
+float pcnn_oracle_project_box(int cls, const float* extents, const float* meta, float distance, float factor)
+{
+    return project_box_f(cls, extents, meta, distance, factor);
+}
+
 /* IoU, .cu.cc:73-82 */
 static float iou_f(const float* a, const float* b)
 {
@@ -172,6 +177,60 @@ static void vote_plane(const sample_t* S, int ns, int H, int W, float inlier, fl
             if (ambig) ambig[cy * W + cx] = amb;
         }
     }
+}
+
+/* Exactness criterion of the interval scan (DESIGN.md §3.3).  The device op represents the vote set of one (sample,
+ * row) pair as one interval of cells, the pixel's own row as one whole side of its window.  `pass[i]` is the
+ * reference predicate at cell wmin + i of the window row; the pair is exact when its set has that form (or is empty),
+ * irregular otherwise (the fp32 predicate is not monotone along the row there). */
+int pcnn_oracle_hough_row_exact(const unsigned char* pass, int wmin, int wmax, int x, int own_row)
+{
+    int n = wmax - wmin + 1, first = -1, last = -1, count = 0;
+    for (int i = 0; i < n; i++)
+        if (pass[i]) {
+            if (first < 0) first = i;
+            last = i;
+            count++;
+        }
+    if (count == 0) return 1;
+    if (count != last - first + 1) return 0;
+    if (!own_row) return 1;
+    /* own row: exactly the cells x+1 .. wmax or wmin .. x-1 */
+    return (wmin + first == x + 1 && wmin + last == wmax) || (wmin + first == wmin && wmin + last == x - 1);
+}
+
+/* slack[H*W]: for each cell, the number of irregular (sample, row) pairs whose window row contains it; pairs[0] =
+ * (sample, row) pairs inside a window, pairs[1] = irregular ones.  Same predicate and window test as vote_plane. */
+static void slack_plane(const sample_t* S, int ns, int H, int W, float inlier, int* slack, long long* pairs)
+{
+    long long np = 0, nirr = 0;
+#pragma omp parallel reduction(+ : np, nirr)
+    {
+        unsigned char* pass = (unsigned char*)malloc((size_t)W);
+#pragma omp for schedule(dynamic, 4)
+        for (int cy = 0; cy < H; cy++) {
+            int* srow = slack + (size_t)cy * W;
+            memset(srow, 0, sizeof(int) * (size_t)W);
+            for (int i = 0; i < ns; i++) {
+                const sample_t* s = &S[i];
+                if (!(fabsf((float)(s->y - cy)) < s->thr)) continue;
+                int wmin = s->x, wmax = s->x;
+                if (!(0.f < s->thr)) continue;
+                while (wmin > 0 && fabsf((float)(s->x - (wmin - 1))) < s->thr) wmin--;
+                while (wmax < W - 1 && fabsf((float)(s->x - (wmax + 1))) < s->thr) wmax++;
+                for (int cx = wmin; cx <= wmax; cx++)
+                    pass[cx - wmin] = angle_distance_f(cx, cy, s->x, s->y, s->u, s->v, s->n1) > inlier;
+                np++;
+                if (!pcnn_oracle_hough_row_exact(pass, wmin, wmax, s->x, cy == s->y)) {
+                    nirr++;
+                    for (int cx = wmin; cx <= wmax; cx++) srow[cx]++;
+                }
+            }
+        }
+        free(pass);
+    }
+    pairs[0] = np;
+    pairs[1] = nirr;
 }
 
 /* hough_data for one cell, .cu.cc:296-331.  dist accumulated sequentially in the
@@ -267,13 +326,13 @@ static void emit_rows(int roi_index, int is_train, int batch_index, int cls, int
  * and are zero-filled here (reset_outputs, .cu.cc:579-588).  *num_rois receives the
  * emitted row count (the op then reports max(1, num_rois) rows, .cc:379-383).
  * votes_dbg / ambig_dbg: optional [B][C][H][W] planes (zero for classes not voted).
- * maxima_dbg: optional [B*C*4] ints: per image up to C entries of (cls, x, y, valid).
+ * slack_dbg / pairs_dbg: optional [B][C][H][W] slack planes and [B][C][2] pair counts of slack_plane (both or neither).
  */
 int pcnn_oracle_hough(const int* label, const float* vertex, const float* extents, const float* meta_all,
                       const float* gt, int B, int H, int W, int C, int num_gt, int num_meta, int is_train,
                       float inlier, int label_thr, float vote_thr, float per_thr, int skip, float* top_box,
                       float* top_pose, float* top_target, float* top_weight, int* top_domain, int* num_rois,
-                      float* votes_dbg, int* ambig_dbg)
+                      float* votes_dbg, int* ambig_dbg, int* slack_dbg, long long* pairs_dbg)
 {
     const int cap_rows = MAX_ROI * 9;
     memset(top_box, 0, sizeof(float) * cap_rows * 7);
@@ -283,6 +342,8 @@ int pcnn_oracle_hough(const int* label, const float* vertex, const float* extent
     memset(top_domain, 0, sizeof(int) * cap_rows);
     if (votes_dbg) memset(votes_dbg, 0, sizeof(float) * (size_t)B * C * H * W);
     if (ambig_dbg) memset(ambig_dbg, 0, sizeof(int) * (size_t)B * C * H * W);
+    if (slack_dbg) memset(slack_dbg, 0, sizeof(int) * (size_t)B * C * H * W);
+    if (pairs_dbg) memset(pairs_dbg, 0, sizeof(long long) * (size_t)B * C * 2);
     int nrois = 0;
     int index_size = B > 0 ? MAX_ROI / B : 0; /* .cu.cc:733 */
     int HW = H * W;
@@ -326,6 +387,8 @@ int pcnn_oracle_hough(const int* label, const float* vertex, const float* extent
             vote_plane(S, ns, H, W, inlier, votes, amb);
             if (votes_dbg) memcpy(votes_dbg + ((size_t)n * C + c) * HW, votes, sizeof(float) * HW);
             if (ambig_dbg) memcpy(ambig_dbg + ((size_t)n * C + c) * HW, amb, sizeof(int) * HW);
+            if (slack_dbg)
+                slack_plane(S, ns, H, W, inlier, slack_dbg + ((size_t)n * C + c) * HW, pairs_dbg + ((size_t)n * C + c) * 2);
             if (vote_thr > 0) {
                 /* compute_max_indexes_kernel, .cu.cc:335-383 (canonical: ascending flat index) */
                 for (int p = 0; p < HW && nmax < index_size; p++) {

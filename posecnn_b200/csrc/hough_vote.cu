@@ -362,22 +362,47 @@ k_emit(const int* __restrict__ label, const VertexSrc vsrc, const float* __restr
                 z = up8_value(vsrc.lowres, b, vsrc.h, vsrc.w, 4 * C, ch + 2, y, x, __ldg(vsrc.bias + 3 * cls + 2));
             }
             float d = expf(z);
-            float n1 = __fsqrt_rn(__fmaf_rn(u, u, __fmul_rn(v, v)));
+            const float s2 = __fmaf_rn(u, u, __fmul_rn(v, v));
+            float n1 = __fsqrt_rn(s2);
             float thr = project_box(cls, extents, meta, d, 0.6f);
+            // (u, v) != 0 but u*u + v*v underflows to n1 = 0: the reference's dot / (n1 * n2) is +-inf, so the pixel
+            // votes for every cell of its window with dot > 0, a half-plane
+            const bool half = n1 == 0.f && (u != 0.f || v != 0.f);
             int m = -1;
-            if (thr == thr && n1 > 0.f && n1 < INFINITY) {
+            if (thr == thr && (n1 > 0.f || half) && n1 < INFINITY) {
                 float mf = fminf(fmaxf(ceilf(thr) - 1.f, -1.f), (float)kMaxM);
                 m = (int)mf;
             }
             // boundary rays of the cone: axis rotated by +-acos(inlier)
             float inv = 1.f / n1, uh = u * inv, vh = v * inv;
-            float ca = inlier, sa = sqrtf(fmaxf(1.f - ca * ca, 0.f));
+            float ca = inlier;
+            // u*u + v*v subnormal: n1 = sqrt(s2) carries the rounding of a subnormal (up to ~50% near the bottom of the
+            // range, ~1% at |(u, v)| = 1e-22), so the reference's cone is cos > inlier * n1 / |(u, v)|.  The rays are
+            // built from that threshold and the direction normalised in scaled arithmetic (2^64: exact, and |(u, v)| >=
+            // 2^-75 here), and flag 256 has k_vote re-check every end point of the sample with the reference predicate.
+            const bool sub = s2 > 0.f && s2 < FLT_MIN;
+            if (sub) {
+                const float us = u * 0x1p64f, vs = v * 0x1p64f, ns = sqrtf(us * us + vs * vs);
+                uh = us / ns;
+                vh = vs / ns;
+                ca = fminf(inlier * (n1 * 0x1p64f) / ns, 1.f);
+            }
+            float sa = sqrtf(fmaxf(1.f - ca * ca, 0.f));
             float r1x = ca * uh - sa * vh, r1y = ca * vh + sa * uh;
             float r2x = ca * uh + sa * vh, r2y = ca * vh - sa * uh;
             float k1 = r1x / r1y, k2 = r2x / r2y;
             int flags = (r1y > 0.f ? 1 : 0) | (r1y < 0.f ? 2 : 0) | (r2y > 0.f ? 4 : 0) | (r2y < 0.f ? 8 : 0) |
                         ((r2x - r2y * k1) > 0.f ? 16 : 0) | ((r1x - r1y * k2) > 0.f ? 32 : 0) |
-                        (pred_exact(u, v, n1, 1.f, 0.f, inlier) ? 64 : 0) | (pred_exact(u, v, n1, -1.f, 0.f, inlier) ? 128 : 0);
+                        (pred_exact(u, v, n1, 1.f, 0.f, inlier) ? 64 : 0) | (pred_exact(u, v, n1, -1.f, 0.f, inlier) ? 128 : 0) |
+                        (sub ? 256 : 0);
+            if (half) {
+                // one boundary line dot = 0, dx = dy * (-v / u), for rows above and below; the voted cells lie on the
+                // side u points to.  u == 0: dot = v * dy, whole rows on the side v points to (k1 = -inf there puts
+                // the line's crossing at -infinity, so the single-ray case below opens the interval over the row).
+                // The own-row flags are already the reference's (dot = u * dx).
+                k1 = k2 = u != 0.f ? -v / u : (v > 0.f ? -INFINITY : INFINITY);
+                flags = (flags & (64 | 128)) | (u != 0.f ? 1 | 2 : (v > 0.f ? 1 : 2)) | (u >= 0.f ? 16 : 0);
+            }
             Sample rec;
             rec.xy = x | (y << 16);
             rec.u = u; rec.v = v; rec.n1 = n1; rec.k1 = k1; rec.k2 = k2;
@@ -560,7 +585,8 @@ k_vote(int H, int W, int C, int R, int nbands, float inlier, float tau0, const i
             const bool reach = scur < ns && m >= 0 && row_lo <= row_hi;
             if (!__any_sync(0xffffffffu, reach)) continue;
             const int wmin = max(x - m, 0), wmax = min(x + m, W - 1);
-            const float fm2 = (float)(m * m);
+            // flag 256: every end point of this sample is re-checked (the m^2 term then puts tau far above 1)
+            const float fm2 = (fl & 256) ? 1e12f : (float)(m * m);
 #pragma unroll 1
             for (int k = 0; k < R; k++) {
                 const int rl = (lane + k) & (R - 1);
@@ -602,9 +628,12 @@ k_vote(int H, int W, int C, int R, int nbands, float inlier, float tau0, const i
                                 const float ma = (float)(a - x) - lo, me = hi - (float)(e - x);
                                 const bool va = a >= wmin && (ma < tau || ma > 1.f - tau);
                                 const bool ve = e <= wmax && (me < tau || me > 1.f - tau);
+                                const int chk = (va || ve) ? 1 : 0;
                                 a = max(a, wmin);
                                 e = min(e, wmax);
-                                if (a <= e) { act = (va || ve) ? 2 : 1; mode = (va ? 1 : 0) | (ve ? 2 : 0); }
+                                // a == e + 1 with a checked end point: the estimate starts (ends) within rounding distance of
+                                // the window edge, just outside it; the exact check grows it back over the edge cell
+                                if (a <= e + chk) { act = 1 + chk; mode = (va ? 1 : 0) | (ve ? 2 : 0); }
                             }
                         }
                     }
@@ -796,7 +825,7 @@ k_celldata(int B, int H, int W, int C, int num_meta, float inlier, int cand_cap,
                     const int x = q.xy & 0xffff, y = q.xy >> 16;
                     const float dx = fabsf((float)(x - cx)), dy = fabsf((float)(y - cy));
                     if (!(dx < thr2 && dy < thr2)) continue;
-                    if (q.n1 > 0.f && pred_exact(q.u, q.v, q.n1, (float)(cx - x), (float)(cy - y), inlier)) {
+                    if (pred_exact(q.u, q.v, q.n1, (float)(cx - x), (float)(cy - y), inlier)) {
                         bbw = fmaxf(bbw, dx);
                         bbh = fmaxf(bbh, dy);
                     }
@@ -1023,8 +1052,8 @@ static int run_front(const Layout& L, char* ws, const int32_t* label, const Vert
     size_t smem = sizeof(int) * (size_t)L.R * (W + 3);
     PCNN_SMEM_OPTIN(k_vote, 110 * 1024, "hough k_vote");
     // end points closer than tau0 (+ a term growing with the distance) to a cell centre are re-checked with the reference
-    // predicate; the estimate's own error is ~1e-4 cells (DESIGN.md §3.3), the default keeps a 40x margin (sweep 0.03 .. 0.002: all parity
-    // tests identical, 0.438 -> 0.393 ms at batch 32, profiles/r02_hough_tau_sweep.txt)
+    // predicate; the estimate's own error is ~1e-4 cells (DESIGN.md §3.3), the default keeps a 40x margin (0.438 -> 0.393 ms at batch 32
+    // against 0.03, profiles/r02_hough_tau_sweep.txt); tests/test_hough_exact_gpu.py holds the planes to §3.3's exactness criterion
     static const float tau0 = getenv("PCNN_HOUGH_TAU0") ? (float)atof(getenv("PCNN_HOUGH_TAU0")) : 0.004f;
     k_vote<<<4 * kNumSMs, kThreads, smem, st>>>(H, W, C, L.R, L.nbands, inlier, tau0, slot_cls, cls_nsamp, cls_soff, bbox,
                                                 samples, L.samp_cap, work, work_ctr, band_res, votes_out);
