@@ -227,12 +227,15 @@ int pcnn_add_to_bf16(const void* a_bf16, const void* b_bf16, const float* b_f32,
  * losses lib/fcn/train.py:455-465, 564-573, optimizer tf.train.MomentumOptimizer (train.py:633):
  *  pcnn_add_up2_bf16 / pcnn_up2_bwd_bf16   add = a4 + up2(a5) (fixed bilinear conv2d_transpose 4x4 / 2) and its adjoint (+ ReLU mask of a5)
  *  pcnn_pack_lowres       [score C | vertex 3C] f32 head tensor from the two bf16 1x1-convolution outputs (row strides Cs, Cv)
- *  pcnn_up8_heads_bwd_ex  gradient of loss_cls (Hardlabel-selected cross entropy through log-softmax and the ReLU of `score`) and of
+ *  pcnn_up8_heads_bwd     gradient of loss_cls (Hardlabel-selected cross entropy through log-softmax and the ReLU of `score`) and of
  *                         loss_vertex (smooth L1 on the labelled pixels' own class) w.r.t. the low-resolution head tensor, formed from
  *                         the loss structure on the fly: d_sc [B,h,w,Cs], d_vt [B,h,w,Cv] bf16 (padding channels zero), dbias [4C]
- *                         (C = 2, C even in 6..50, or C = 9); the labelled pixels' vertex values come from vertex_pred [B,H,W,3C], or
- *                         with vertex_pred == NULL from the low-resolution head tensor `lowres` [B,h,w,4C] + bias_vertex [3C];
- *                         workspace >= 16 C B ceil(h / 16) ceil(w / S) bytes, S = 16 cells at C = 2 and 4 otherwise (4 C floats per CTA)
+ *                         (C = 2, C even in 6..50, or C = 9); the labelled pixels' vertex values come from the low-resolution head
+ *                         tensor `lowres` [B,h,w,4C] + bias_vertex [3C].  Vertex target: vertmap == extents == NULL, the 2-D centre
+ *                         direction + log z; both given, the VERTEX_REG_3D object coordinate (a weighted pixel, label c in 1..C-1 with
+ *                         centers[b, c, 2] > 0, has target vertmap [B,8h,8w,3] f32 scaled by extents [C,3] f32, as
+ *                         pcnn_vertex_targets_3d_fwd); one of the two alone is rejected.
+ *                         workspace: pcnn_up8_heads_bwd_workspace_bytes(B, h, w, C) (4 C floats per CTA)
  *  pcnn_pose_chain_bwd    Averagedistance's bottom_diff through l2_normalize, * poses_weight and tanh -> d fc8 pre-activation (fp16)
  *  pcnn_sgd_momentum      accum = mu * accum + (gscale * grad + wd * w); w -= lr * accum; refreshed 16-bit tensor-core copy (kind 0 bf16, 1 fp16)
  *  pcnn_transpose16 / pcnn_half_to_float   layout / precision glue of the fully connected backward GEMMs
@@ -240,19 +243,12 @@ int pcnn_add_to_bf16(const void* a_bf16, const void* b_bf16, const float* b_f32,
 int pcnn_add_up2_bf16(const void* a4_bf16, const void* a5_bf16, int B, int h, int w, int C, void* out_bf16, void* stream);
 int pcnn_up2_bwd_bf16(const void* dadd_bf16, const void* y5_bf16, int B, int h, int w, int C, void* d5_bf16, void* stream);
 int pcnn_pack_lowres(const void* sc_bf16, int Cs, const void* vt_bf16, int Cv, int B, int h, int w, int C, float* lowres, void* stream);
-int pcnn_up8_heads_bwd_ex(const float* prob, const float* score, const int32_t* gt, const float* cls_loss_out, float upstream_cls,
-                          float threshold, const float* vertex_pred, const float* lowres, const float* bias_vertex, const float* centers,
-                          const float* vertex_loss_out, float upstream_vertex, float w_inside, float sigma, int B, int h, int w, int C,
-                          int Cs, int Cv, void* d_sc_bf16, void* d_vt_bf16, float* dbias, void* workspace, size_t workspace_bytes,
-                          void* stream);
-/* pcnn_up8_heads_bwd_coord  the same adjoint for the VERTEX_REG_3D networks: the vertex target of a weighted pixel (label c in 1..C-1,
- *      centers[b, c, 2] > 0) is its object coordinate vertmap [B,8h,8w,3] f32 scaled by extents [C,3] f32 (as
- *      pcnn_vertex_targets_3d_fwd); every other argument, check, output and the workspace are those of pcnn_up8_heads_bwd_ex. */
-int pcnn_up8_heads_bwd_coord(const float* prob, const float* score, const int32_t* gt, const float* cls_loss_out, float upstream_cls,
-                             float threshold, const float* vertex_pred, const float* lowres, const float* bias_vertex, const float* vertmap,
-                             const float* centers, const float* extents, const float* vertex_loss_out, float upstream_vertex, float w_inside,
-                             float sigma, int B, int h, int w, int C, int Cs, int Cv, void* d_sc_bf16, void* d_vt_bf16, float* dbias,
-                             void* workspace, size_t workspace_bytes, void* stream);
+int pcnn_up8_heads_bwd_workspace_bytes(int B, int h, int w, int C, size_t* bytes);
+int pcnn_up8_heads_bwd(const float* prob, const float* score, const int32_t* gt, const float* cls_loss_out, float upstream_cls,
+                       float threshold, const float* lowres, const float* bias_vertex, const float* centers, const float* vertmap,
+                       const float* extents, const float* vertex_loss_out, float upstream_vertex, float w_inside, float sigma, int B, int h,
+                       int w, int C, int Cs, int Cv, void* d_sc_bf16, void* d_vt_bf16, float* dbias, void* workspace,
+                       size_t workspace_bytes, void* stream);
 int pcnn_pose_chain_bwd(const float* bottom_diff, const float* poses_tanh, const float* poses_weight, int N, int D, float upstream,
                         void* dpre_f16, int ld, void* stream);
 int pcnn_sgd_momentum(float* w, float* accum, const float* grad, size_t n, float lr, float mu, float wd, float gscale, void* copy16,
@@ -357,11 +353,11 @@ int pcnn_nms_pose_fwd(const float* rois, const float* poses_init, const float* p
  *      branch): label [B,H,W] int32, centers [B,C,3] = (cx, cy, z) of each class's projected centre (z <= 0: class
  *      absent from the image) -> vertex_targets / vertex_weights [B,H,W,3C] f32 (zero elsewhere); float64 arithmetic
  *      rounded to float32 like numpy's (float32 centre - int64 pixel grid).
- * The losses (their gradients are the up-sampling adjoint's, pcnn_up8_heads_bwd_ex / _coord):
+ * The losses (their gradients are the up-sampling adjoint's, pcnn_up8_heads_bwd):
  *  pcnn_loss_cls_hard_raw_fwd  loss_cls, lib/fcn/train.py:455-465 over the Hardlabel selection (hard_label_op_gpu.cu.cc:16-29) on
  *      the raw `score` [B,H,W,C]: loss_out[0] = -sum_{selected p} log_softmax(score[p])[gt_p] / (count + 1e-10),
  *      loss_out[1] = count; neither the log-softmax nor the mask is materialised (declared above, with the backward kernels).
- *  pcnn_vertex_loss_fused_lowres_fwd / pcnn_vertex_loss_coord_lowres_fwd (below)   loss_vertex, lib/fcn/train.py:564-573
+ *  pcnn_vertex_loss_fwd (below)   loss_vertex, lib/fcn/train.py:564-573
  *      (smooth_l1_loss_vertex) on the 2-D or the 3-D targets: loss_out[0] = sum(in_loss) / (sum(weights) + 1e-10),
  *      loss_out[1] = sum(weights).
  * Each reduces per-CTA partial sums (double) in index order: run-to-run deterministic.  workspace: zero-filled
@@ -383,25 +379,22 @@ int pcnn_pack_pose_meta_fwd(const float* poses, const int32_t* cls, const float*
 int pcnn_train_loss_workspace_bytes(size_t* bytes);
 int pcnn_vertex_targets_fwd(const int32_t* label, const float* centers, int B, int H, int W, int C, float w_inside,
                             float* targets, float* weights, void* stream);
-/* the vertex loss on the targets / weights of pcnn_vertex_targets_fwd(label, centers, w_inside) WITHOUT materialising them
- * (5.2 GB at batch 32), with the vertex head given as the 1/8-resolution head tensor `lowres` [B,H/8,W/8,4C] + the vertex_pred
- * bias [3C] (values formed on demand with k_up8_heads' operation sequence: bit-identical to the dense tensor); H, W % 8 == 0 */
-int pcnn_vertex_loss_fused_lowres_fwd(const float* lowres, const float* bias_vertex, const int32_t* label, const float* centers, int B,
-                                      int H, int W, int C, float w_inside, float sigma, float* loss_out, void* workspace,
-                                      size_t workspace_bytes, void* stream);
 /* VERTEX_REG_3D targets (the 3-D branch of _generate_vertex_targets, minibatch.py:595-600, and _scale_vertmap, :605-616):
  *  pcnn_vertex_targets_3d_fwd   label [B,H,W] int32, vertmap [B,H,W,3] f32 (the object coordinate of each pixel, metres in the model
  *      frame), centers [B,C,3] (only z > 0 is read: the class is listed in the frame), extents [C,3] f32 -> vertex_targets /
  *      vertex_weights [B,H,W,3C] f32: for a pixel labelled c in 1..C-1 with a listed class, channel 3c+k = a_k * v_k + b_k with
  *      vmin = -e_k / 2, vmax = e_k / 2, a_k = 1 / (vmax - vmin), b_k = -vmin / (vmax - vmin) (a_k = b_k = 0 where vmax - vmin <= 0),
  *      all in float32 with the product rounded before the sum; weight w_inside on those channels; zero elsewhere.
- *  pcnn_vertex_loss_coord_lowres_fwd   pcnn_vertex_loss_fused_lowres_fwd on that target, without materialising it (same
- *      outputs and workspace). */
+ *  pcnn_vertex_loss_fwd   the vertex loss on the targets / weights of pcnn_vertex_targets_fwd(label, centers, w_inside) (vertmap ==
+ *      extents == NULL) or of pcnn_vertex_targets_3d_fwd(label, vertmap, centers, extents, w_inside) (both given; one alone is rejected)
+ *      WITHOUT materialising them (5.2 GB at batch 32), with the vertex head given as the 1/8-resolution head tensor `lowres`
+ *      [B,H/8,W/8,4C] + the vertex_pred bias [3C] (values formed on demand with k_up8_heads' operation sequence: bit-identical to the
+ *      dense tensor); H, W % 8 == 0. */
 int pcnn_vertex_targets_3d_fwd(const int32_t* label, const float* vertmap, const float* centers, const float* extents, int B, int H, int W,
                                int C, float w_inside, float* targets, float* weights, void* stream);
-int pcnn_vertex_loss_coord_lowres_fwd(const float* lowres, const float* bias_vertex, const int32_t* label, const float* vertmap,
-                                      const float* centers, const float* extents, int B, int H, int W, int C, float w_inside, float sigma,
-                                      float* loss_out, void* workspace, size_t workspace_bytes, void* stream);
+int pcnn_vertex_loss_fwd(const float* lowres, const float* bias_vertex, const int32_t* label, const float* centers, const float* vertmap,
+                         const float* extents, int B, int H, int W, int C, float w_inside, float sigma, float* loss_out, void* workspace,
+                         size_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * Training image blobs (csrc/augment.cu): the image side of the synthetic-data loader, lib/gt_synthesize_layer/minibatch.py:147-200

@@ -152,18 +152,20 @@ k_pack_lowres(const __nv_bfloat16* __restrict__ sc, int Cs, const __nv_bfloat16*
 // ---------------------------------------------------------------------------------------------
 constexpr int kStrip = 4;                           // strip width (cells) of the C >= 6 kernels
 constexpr int kStrip2 = 16;                         // strip width (cells) of the C = 2 kernel
+constexpr int kBand = 16;                           // band height (low-resolution rows) of every CTA
 
 // Target mode kCoord (VERTEX_REG_3D): the vertex target is the pixel's object coordinate vertmap [B,H,W,3] scaled by its class's
 // extents (coord_scale / coord_target, heads_common.cuh) instead of the 2-D centre direction + log z.  The per-class (a_k, b_k) sit in
 // shared memory after the per-class listed flags (where the 2-D mode keeps log z: 6 C more floats), and the vertex-role thread loads
 // a pixel's three vertmap floats one row ahead, together with the label it already prefetches, and only for weighted pixels.
-// C = 2: 6 resident CTAs per SM caps the kernel at 64 registers without spills (-Xptxas -v); 8 would spill.
+// C = 2: 6 resident CTAs per SM caps the kernel at 64 registers without spills in the 2-D mode (-Xptxas -v; the 3-D mode spills a few
+// bytes, DESIGN §10); 8 would spill.
 // CPT = 1 runs at C = 9 only (kSCols * 9 = 360 threads): bounding it at 360 x 2 CTAs instead of 1024 lifts the register cap from 64,
 // where the coordinate form spills, to 80
 template <int CT, int SC, bool kCoord, int CPT>
 __global__ void __launch_bounds__(CT ? (8 * SC + 8) * (CT / 2) : (CPT == 1 ? (8 * SC + 8) * 9 : 1024), CT == 2 ? 6 : (CT || CPT == 1 ? 2 : 1))
 k_up8_bwd_strip(const float* __restrict__ prob, const float* __restrict__ score, const int* __restrict__ gt, const float* __restrict__ cls_out,
-                float up_cls, float threshold, const float* __restrict__ vpred, const float* __restrict__ lowres,
+                float up_cls, float threshold, const float* __restrict__ lowres,
                 const float* __restrict__ bias_v, const float* __restrict__ centers,
                 const float* __restrict__ vtx_out, float up_vtx, float w_inside, float sigma2, int h, int w, int rb, int C_rt, int Cs, int Cv,
                 __nv_bfloat16* __restrict__ d_sc, __nv_bfloat16* __restrict__ d_vt, float* __restrict__ dbias_partial /*[ctas][4C]*/,
@@ -301,14 +303,12 @@ k_up8_bwd_strip(const float* __restrict__ prob, const float* __restrict__ score,
                         const double nrm = sqrt(dx * dx + dy * dy) + 1e-10;
                         tg[0] = (float)(dx / nrm); tg[1] = (float)(dy / nrm); tg[2] = logz[gB];
                     }
-                    const size_t pB = img + (size_t)y * W + xB;
                     float* a_lo = vacc + ((size_t)slot_lo * kSCols + t) * VC + 3 * gB;
                     float* a_hi = vacc + ((size_t)(slot_lo ^ 1) * kSCols + t) * VC + 3 * gB;
 #pragma unroll
                     for (int k = 0; k < 3; k++) {
-                        // vpred == NULL: the value is formed from the low-resolution head tensor (bit-identical, heads_common.cuh)
-                        const float pv = vpred ? __ldg(vpred + pB * VC + 3 * gB + k)
-                                               : up8_value(lowres, n, h, w, No, C + 3 * gB + k, y, xB, __ldg(bias_v + 3 * gB + k));
+                        // vertex_pred's value, formed from the low-resolution head tensor with k_up8_heads' operation sequence
+                        const float pv = up8_value(lowres, n, h, w, No, C + 3 * gB + k, y, xB, __ldg(bias_v + 3 * gB + k));
                         const float diff = w_inside * (pv - tg[k]);
                         const float ad = fabsf(diff);
                         const float dt = ad < 1.f / sigma2 ? diff * sigma2 : (diff > 0.f ? 1.f : (diff < 0.f ? -1.f : 0.f));
@@ -516,77 +516,68 @@ extern "C" int pcnn_pack_lowres(const void* sc, int Cs, const void* vt, int Cv, 
     return check_launch("pack_lowres");
 }
 
-// the adjoint in either target mode (kCoord: vertmap + extents give the vertex target); `what` names the entry point in messages
-template <bool kCoord>
-static int up8_heads_bwd(const char* what, const float* prob, const float* score, const int32_t* gt, const float* cls_loss_out,
-                         float upstream_cls, float threshold, const float* vertex_pred, const float* lowres, const float* bias_vertex,
-                         const float* vertmap, const float* centers, const float* extents, const float* vertex_loss_out, float upstream_vertex,
-                         float w_inside, float sigma, int B, int h, int w, int C, int Cs, int Cv, void* d_sc_bf16, void* d_vt_bf16, float* dbias,
-                         void* workspace, size_t workspace_bytes, void* stream)
+extern "C" int pcnn_up8_heads_bwd_workspace_bytes(int B, int h, int w, int C, size_t* bytes)
 {
-    PCNN_REQUIRE(prob && score && gt && cls_loss_out && (vertex_pred || (lowres && bias_vertex)) && centers && vertex_loss_out && d_sc_bf16 &&
-                     d_vt_bf16 && dbias && workspace && (!kCoord || (vertmap && extents)),
-                 "%s: NULL tensor pointer", what);
-    PCNN_REQUIRE(Cs >= C && Cv >= 3 * C && h <= 65535 && B <= 65535, "%s: bad shape", what);
+    PCNN_REQUIRE(bytes && B >= 1 && h >= 1 && w >= 1 && C >= 1, "up8_heads_bwd_workspace_bytes: bad arguments");
+    // partial bias sums of k_up8_bwd_strip: one row of 4C floats per CTA = (image, strip of cells, band of kBand rows)
+    const int sc = C == 2 ? kStrip2 : kStrip;
+    *bytes = sizeof(float) * (size_t)B * ((w + sc - 1) / sc) * ((h + kBand - 1) / kBand) * 4 * C;
+    return PCNN_OK;
+}
+
+// every instantiation of the strip kernel has this signature; the entry point picks one by class count and target mode
+using UpBwdKernel = decltype(&k_up8_bwd_strip<2, kStrip2, false, 2>);
+template <int CT, int SC, int CPT>
+static UpBwdKernel up8_bwd_kernel(bool coord) { return coord ? k_up8_bwd_strip<CT, SC, true, CPT> : k_up8_bwd_strip<CT, SC, false, CPT>; }
+
+// the target mode follows vertmap / extents: both NULL = 2-D centre direction, both given = 3-D object coordinate (VERTEX_REG_3D:
+// vertmap [B,8h,8w,3] f32 and extents [C,3] f32; centers stays the presence table, a class's pixels are weighted iff
+// centers[b, c, 2] > 0)
+extern "C" int pcnn_up8_heads_bwd(const float* prob, const float* score, const int32_t* gt, const float* cls_loss_out, float upstream_cls,
+                                  float threshold, const float* lowres, const float* bias_vertex, const float* centers, const float* vertmap,
+                                  const float* extents, const float* vertex_loss_out, float upstream_vertex, float w_inside, float sigma, int B,
+                                  int h, int w, int C, int Cs, int Cv, void* d_sc_bf16, void* d_vt_bf16, float* dbias, void* workspace,
+                                  size_t workspace_bytes, void* stream)
+{
+    PCNN_REQUIRE(prob && score && gt && cls_loss_out && lowres && bias_vertex && centers && vertex_loss_out && d_sc_bf16 && d_vt_bf16 &&
+                     dbias && workspace,
+                 "up8_heads_bwd: NULL tensor pointer");
+    PCNN_REQUIRE(!vertmap == !extents, "up8_heads_bwd: vertmap and extents must both be given (3-D target) or both be NULL (2-D target)");
+    PCNN_REQUIRE(Cs >= C && Cv >= 3 * C && h <= 65535 && B <= 65535, "up8_heads_bwd: bad shape");
     // class counts of the reference's configurations: 2 (single object), 22 (YCB), 9 (multi-object LINEMOD), and the even range
-    PCNN_REQUIRE(C == 2 || C == 9 || (C % 2 == 0 && C >= 6 && C <= 50), "%s: C must be even and 2 or in 6..50, or 9 (C = %d)", what, C);
-    // coalesced strip kernel (see k_up8_bwd_strip); partial bias sums: one row of 4C floats per CTA
+    PCNN_REQUIRE(C == 2 || C == 9 || (C % 2 == 0 && C >= 6 && C <= 50), "up8_heads_bwd: C must be even and 2 or in 6..50, or 9 (C = %d)", C);
+    size_t need = 0;
+    PCNN_REQUIRE(pcnn_up8_heads_bwd_workspace_bytes(B, h, w, C, &need) == PCNN_OK, "up8_heads_bwd: bad shape");
+    PCNN_REQUIRE(workspace_bytes >= need, "up8_heads_bwd: workspace too small (%zu < %zu)", workspace_bytes, need);
+    // coalesced strip kernel (see k_up8_bwd_strip)
+    const bool coord = vertmap != nullptr;
     const int sc = C == 2 ? kStrip2 : kStrip, cols = 8 * sc + 8;
-    const int rb = 16, bands = (h + rb - 1) / rb, strips = (w + sc - 1) / sc;
-    const size_t need = sizeof(float) * (size_t)B * strips * bands * 4 * C;
-    PCNN_REQUIRE(workspace_bytes >= need, "%s: workspace too small (%zu < %zu)", what, workspace_bytes, need);
-    PCNN_REQUIRE(bands <= 65535, "%s: bad shape", what);
-    cudaStream_t st = (cudaStream_t)stream;
-    const size_t smem = sizeof(float) * ((size_t)cols * 11 * C + C + (kCoord ? 6 * C : 0));
-    const dim3 grid(strips, bands, B);
-    if (C == 22)
-        k_up8_bwd_strip<22, kStrip, kCoord, 2><<<grid, cols * 11, smem, st>>>(prob, score, gt, cls_loss_out, upstream_cls, threshold, vertex_pred, lowres,
-                                                                          bias_vertex, centers, vertex_loss_out, upstream_vertex, w_inside,
-                                                                          sigma * sigma, h, w, rb, C, Cs, Cv, (__nv_bfloat16*)d_sc_bf16,
-                                                                          (__nv_bfloat16*)d_vt_bf16, (float*)workspace, vertmap, extents);
-    else if (C == 2)
-        k_up8_bwd_strip<2, kStrip2, kCoord, 2><<<grid, cols, smem, st>>>(prob, score, gt, cls_loss_out, upstream_cls, threshold, vertex_pred, lowres,
-                                                                     bias_vertex, centers, vertex_loss_out, upstream_vertex, w_inside, sigma * sigma, h,
-                                                                     w, rb, C, Cs, Cv, (__nv_bfloat16*)d_sc_bf16, (__nv_bfloat16*)d_vt_bf16,
-                                                                     (float*)workspace, vertmap, extents);
-    else if (C % 2)   // C = 9: one channel per thread (at 40 x 9 threads the strip's shared memory is 16 KB: no opt-in)
-        k_up8_bwd_strip<0, kStrip, kCoord, 1><<<grid, cols * C, smem, st>>>(prob, score, gt, cls_loss_out, upstream_cls, threshold, vertex_pred,
-                                                                           lowres, bias_vertex, centers, vertex_loss_out, upstream_vertex, w_inside,
-                                                                           sigma * sigma, h, w, rb, C, Cs, Cv, (__nv_bfloat16*)d_sc_bf16,
-                                                                           (__nv_bfloat16*)d_vt_bf16, (float*)workspace, vertmap, extents);
-    else {
-        PCNN_SMEM_OPTIN((k_up8_bwd_strip<0, kStrip, kCoord, 2>), 100 * 1024, kCoord ? "up8_bwd_strip<0, coord>" : "up8_bwd_strip<0>");
-        k_up8_bwd_strip<0, kStrip, kCoord, 2><<<grid, cols * (C / 2), smem, st>>>(prob, score, gt, cls_loss_out, upstream_cls, threshold, vertex_pred,
-                                                                              lowres, bias_vertex, centers, vertex_loss_out, upstream_vertex, w_inside,
-                                                                              sigma * sigma, h, w, rb, C, Cs, Cv, (__nv_bfloat16*)d_sc_bf16,
-                                                                              (__nv_bfloat16*)d_vt_bf16, (float*)workspace, vertmap, extents);
+    const int bands = (h + kBand - 1) / kBand, strips = (w + sc - 1) / sc;
+    PCNN_REQUIRE(bands <= 65535, "up8_heads_bwd: bad shape");
+    UpBwdKernel kernel;
+    int threads;
+    if (C == 22) {
+        kernel = up8_bwd_kernel<22, kStrip, 2>(coord);
+        threads = cols * 11;
+    } else if (C == 2) {
+        kernel = up8_bwd_kernel<2, kStrip2, 2>(coord);
+        threads = cols;
+    } else if (C % 2) {   // C = 9: one channel per thread (at 40 x 9 threads the strip's shared memory is 16 KB: no opt-in)
+        kernel = up8_bwd_kernel<0, kStrip, 1>(coord);
+        threads = cols * C;
+    } else {
+        kernel = up8_bwd_kernel<0, kStrip, 2>(coord);
+        threads = cols * (C / 2);
+        PCNN_SMEM_OPTIN(kernel, 100 * 1024, coord ? "up8_bwd_strip<0, coord>" : "up8_bwd_strip<0>");
     }
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t smem = sizeof(float) * ((size_t)cols * 11 * C + C + (coord ? 6 * C : 0));
+    kernel<<<dim3(strips, bands, B), threads, smem, st>>>(prob, score, gt, cls_loss_out, upstream_cls, threshold, lowres, bias_vertex, centers,
+                                                          vertex_loss_out, upstream_vertex, w_inside, sigma * sigma, h, w, kBand, C, Cs, Cv,
+                                                          (__nv_bfloat16*)d_sc_bf16, (__nv_bfloat16*)d_vt_bf16, (float*)workspace, vertmap,
+                                                          extents);
     k_sum_partials<<<(4 * C + 31) / 32, 256, 0, st>>>((const float*)workspace, B * strips * bands, 4 * C, 1.f, nullptr, 0.f, dbias);
-    return check_launch(what);
-}
-
-extern "C" int pcnn_up8_heads_bwd_ex(const float* prob, const float* score, const int32_t* gt, const float* cls_loss_out, float upstream_cls,
-                                     float threshold, const float* vertex_pred, const float* lowres, const float* bias_vertex, const float* centers,
-                                     const float* vertex_loss_out, float upstream_vertex, float w_inside, float sigma, int B, int h, int w, int C,
-                                     int Cs, int Cv, void* d_sc_bf16, void* d_vt_bf16, float* dbias, void* workspace, size_t workspace_bytes,
-                                     void* stream)
-{
-    return up8_heads_bwd<false>("up8_heads_bwd", prob, score, gt, cls_loss_out, upstream_cls, threshold, vertex_pred, lowres, bias_vertex, nullptr,
-                                centers, nullptr, vertex_loss_out, upstream_vertex, w_inside, sigma, B, h, w, C, Cs, Cv, d_sc_bf16, d_vt_bf16, dbias,
-                                workspace, workspace_bytes, stream);
-}
-
-// VERTEX_REG_3D: the same adjoint with the object-coordinate target (vertmap [B,8h,8w,3] f32, extents [C,3] f32); centers stays the
-// presence table (a class's pixels are weighted iff centers[b, c, 2] > 0)
-extern "C" int pcnn_up8_heads_bwd_coord(const float* prob, const float* score, const int32_t* gt, const float* cls_loss_out, float upstream_cls,
-                                        float threshold, const float* vertex_pred, const float* lowres, const float* bias_vertex, const float* vertmap,
-                                        const float* centers, const float* extents, const float* vertex_loss_out, float upstream_vertex,
-                                        float w_inside, float sigma, int B, int h, int w, int C, int Cs, int Cv, void* d_sc_bf16, void* d_vt_bf16,
-                                        float* dbias, void* workspace, size_t workspace_bytes, void* stream)
-{
-    return up8_heads_bwd<true>("up8_heads_bwd_coord", prob, score, gt, cls_loss_out, upstream_cls, threshold, vertex_pred, lowres, bias_vertex,
-                               vertmap, centers, extents, vertex_loss_out, upstream_vertex, w_inside, sigma, B, h, w, C, Cs, Cv, d_sc_bf16, d_vt_bf16,
-                               dbias, workspace, workspace_bytes, stream);
+    return check_launch("up8_heads_bwd");
 }
 
 extern "C" int pcnn_pose_chain_bwd(const float* bottom_diff, const float* poses_tanh, const float* poses_weight, int N, int D, float upstream,

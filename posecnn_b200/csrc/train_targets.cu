@@ -7,8 +7,8 @@
 //                                      :605-616): the pixel's object coordinate scaled into [0, 1] by its class's extents
 //   pcnn_loss_cls_hard_raw_fwd         lib/fcn/train.py:455-465 (loss_cross_entropy_single_frame) on log_softmax(score) over the
 //                                      Hardlabel selection (hard_label_op_gpu.cu.cc:16-29), neither tensor materialised
-//   pcnn_vertex_loss_fused_lowres_fwd  lib/fcn/train.py:564-573 (smooth_l1_loss_vertex) on the targets of either branch, vertex
-//   pcnn_vertex_loss_coord_lowres_fwd  values from the 1/8-resolution head tensor, targets / weights never materialised
+//   pcnn_vertex_loss_fwd               lib/fcn/train.py:564-573 (smooth_l1_loss_vertex) on the targets of either branch, vertex
+//                                      values from the 1/8-resolution head tensor, targets / weights never materialised
 // Losses: fixed 592-CTA grid, per-CTA partial sums in double, last CTA to finish reduces them in index order
 // (run-to-run deterministic).  Their gradients are the up-sampling adjoint's (train_bwd.cu).
 #include <cuda_runtime.h>
@@ -299,44 +299,26 @@ k_vertex_loss_fused(const float* __restrict__ lowres, const float* __restrict__ 
 
 using namespace pcnn;
 
-// the fused vertex loss of either target mode on `lowres` + `bias_vertex`; `what` names the entry point in error messages
-template <bool kCoord>
-static int vertex_loss_fused(const char* what, const float* lowres, const float* bias_vertex, const int32_t* label, const float* vertmap,
-                             const float* centers, const float* extents, int B, int H, int W, int C, float w_inside, float sigma,
-                             float* loss_out, void* workspace, size_t workspace_bytes, void* stream)
+// the vertex head given as the 1/8-resolution head tensor `lowres` [B,H/8,W/8,4C] (channels C.. = vertex) + the vertex_pred bias
+// [3C]: no dense vertex_pred tensor is needed anywhere in the training step.  vertmap and extents both NULL: the 2-D target; both
+// given: the VERTEX_REG_3D scaled object-coordinate target (pixel_targets_3d)
+extern "C" int pcnn_vertex_loss_fwd(const float* lowres, const float* bias_vertex, const int32_t* label, const float* centers,
+                                    const float* vertmap, const float* extents, int B, int H, int W, int C, float w_inside, float sigma,
+                                    float* loss_out, void* workspace, size_t workspace_bytes, void* stream)
 {
-    PCNN_REQUIRE(lowres && bias_vertex && label && centers && loss_out && workspace && (!kCoord || (vertmap && extents)),
-                 "%s: NULL tensor pointer", what);
-    PCNN_REQUIRE(sigma > 0.f && B >= 1 && H >= 8 && W >= 8 && H % 8 == 0 && W % 8 == 0 && C >= 1, "%s: bad arguments", what);
-    PCNN_REQUIRE((unsigned long long)B * H * W < 0xffffffffULL, "%s: too many pixels", what);
+    PCNN_REQUIRE(lowres && bias_vertex && label && centers && loss_out && workspace, "vertex_loss: NULL tensor pointer");
+    PCNN_REQUIRE(!vertmap == !extents, "vertex_loss: vertmap and extents must both be given (3-D target) or both be NULL (2-D target)");
+    PCNN_REQUIRE(sigma > 0.f && B >= 1 && H >= 8 && W >= 8 && H % 8 == 0 && W % 8 == 0 && C >= 1, "vertex_loss: bad arguments");
+    PCNN_REQUIRE((unsigned long long)B * H * W < 0xffffffffULL, "vertex_loss: too many pixels");
     size_t need = 0;
     pcnn_train_loss_workspace_bytes(&need);
-    PCNN_REQUIRE(workspace_bytes >= need, "%s: workspace too small (%zu < %zu)", what, workspace_bytes, need);
+    PCNN_REQUIRE(workspace_bytes >= need, "vertex_loss: workspace too small (%zu < %zu)", workspace_bytes, need);
     double* partial = (double*)workspace;
     unsigned* ticket = (unsigned*)(partial + 2 * kLossBlocks);
-    k_vertex_loss_fused<kCoord><<<kLossBlocks, kLossThreads, 0, (cudaStream_t)stream>>>(lowres, bias_vertex, label, centers, (unsigned)B * H * W,
-                                                                                         H * W, W, C, w_inside, sigma * sigma, partial, ticket,
-                                                                                         loss_out, vertmap, extents);
-    return check_launch(what);
-}
-
-// the vertex head given as the 1/8-resolution head tensor `lowres` [B,H/8,W/8,4C] (channels C.. = vertex) + the vertex_pred bias
-// [3C]: no dense vertex_pred tensor is needed anywhere in the training step
-extern "C" int pcnn_vertex_loss_fused_lowres_fwd(const float* lowres, const float* bias_vertex, const int32_t* label, const float* centers, int B,
-                                                 int H, int W, int C, float w_inside, float sigma, float* loss_out, void* workspace,
-                                                 size_t workspace_bytes, void* stream)
-{
-    return vertex_loss_fused<false>("vertex_loss_fused_lowres", lowres, bias_vertex, label, nullptr, centers, nullptr, B, H, W, C, w_inside,
-                                    sigma, loss_out, workspace, workspace_bytes, stream);
-}
-
-// VERTEX_REG_3D: the same loss on the scaled object-coordinate target (pixel_targets_3d)
-extern "C" int pcnn_vertex_loss_coord_lowres_fwd(const float* lowres, const float* bias_vertex, const int32_t* label, const float* vertmap,
-                                                 const float* centers, const float* extents, int B, int H, int W, int C, float w_inside,
-                                                 float sigma, float* loss_out, void* workspace, size_t workspace_bytes, void* stream)
-{
-    return vertex_loss_fused<true>("vertex_loss_coord_lowres", lowres, bias_vertex, label, vertmap, centers, extents, B, H, W, C, w_inside,
-                                   sigma, loss_out, workspace, workspace_bytes, stream);
+    (vertmap ? k_vertex_loss_fused<true> : k_vertex_loss_fused<false>)<<<kLossBlocks, kLossThreads, 0, (cudaStream_t)stream>>>(
+        lowres, bias_vertex, label, centers, (unsigned)B * H * W, H * W, W, C, w_inside, sigma * sigma, partial, ticket, loss_out, vertmap,
+        extents);
+    return check_launch("vertex_loss");
 }
 
 extern "C" int pcnn_train_loss_workspace_bytes(size_t* bytes)

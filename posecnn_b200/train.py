@@ -381,19 +381,14 @@ class Trainer:
         d_sc = torch.empty((B, h, w, 64), dtype=torch.bfloat16, device=dev)
         d_vt = torch.empty((B, h, w, 128), dtype=torch.bfloat16, device=dev)
         dbias = torch.empty((4 * C,), dtype=torch.float32, device=dev)
-        # 4C floats per CTA of >= 4 columns x 16 rows: covers every strip width; the entry point checks its own requirement
-        ws = workspace("up8_bwd", 4 * B * ((w + 3) // 4) * ((h + 15) // 16) * 4 * C, dev)
-        if self.coord:
-            vm = self._require_vertmap(vertmap, data)
-            check(lib().pcnn_up8_heads_bwd_coord(ptr(A["prob_normalized"]), ptr(A["score"]), ptr(gt_label_2d), ptr(A["cls_out"]), 1.0,
-                                                 net.threshold_label, ptr(None), ptr(A["lowres"]), ptr(M["vertex_pred/b"]), ptr(vm),
-                                                 ptr(centers), ptr(A["extents"]), ptr(A["vtx_out"]), self.vertex_w, self.w_inside, 1.0, B,
-                                                 h, w, C, 64, 128, ptr(d_sc), ptr(d_vt), ptr(dbias), ptr(ws), ws.numel(), stream()))
-        else:
-            check(lib().pcnn_up8_heads_bwd_ex(ptr(A["prob_normalized"]), ptr(A["score"]), ptr(gt_label_2d), ptr(A["cls_out"]), 1.0,
-                                              net.threshold_label, ptr(None), ptr(A["lowres"]), ptr(M["vertex_pred/b"]), ptr(centers),
-                                              ptr(A["vtx_out"]), self.vertex_w, self.w_inside, 1.0, B, h, w, C, 64, 128, ptr(d_sc),
-                                              ptr(d_vt), ptr(dbias), ptr(ws), ws.numel(), stream()))
+        nbytes = ctypes.c_size_t(0)
+        check(lib().pcnn_up8_heads_bwd_workspace_bytes(B, h, w, C, ctypes.byref(nbytes)))
+        ws = workspace("up8_bwd", nbytes.value, dev)
+        vm, ext = (self._require_vertmap(vertmap, data), A["extents"]) if self.coord else (None, None)
+        check(lib().pcnn_up8_heads_bwd(ptr(A["prob_normalized"]), ptr(A["score"]), ptr(gt_label_2d), ptr(A["cls_out"]), 1.0,
+                                       net.threshold_label, ptr(A["lowres"]), ptr(M["vertex_pred/b"]), ptr(centers), ptr(vm), ptr(ext),
+                                       ptr(A["vtx_out"]), self.vertex_w, self.w_inside, 1.0, B, h, w, C, 64, 128, ptr(d_sc), ptr(d_vt),
+                                       ptr(dbias), ptr(ws), ws.numel(), stream()))
         self._emit(grads, "score/b", dbias[:C].contiguous())
         self._emit(grads, "vertex_pred/b", dbias[C:].contiguous())
         self._emit(grads, "score/w", bw.conv_wgrad(A["add_s"], d_sc, 1))

@@ -128,11 +128,9 @@ def loss_vertex(lowres, bias_vertex, im_label, centers, w_inside, sigma=1.0, ver
         raise ValueError("lowres must be [B,H/8,W/8,4C] with a [3C] bias, and centers [B,C,3]")
     out = torch.empty((2,), dtype=torch.float32, device=lr.device)
     ws = _workspace(lr.device)
-    if vertmap is None:
-        check(lib().pcnn_vertex_loss_fused_lowres_fwd(ptr(lr), ptr(bv), ptr(lab), ptr(cen), B, H, W, C, w_inside, sigma, ptr(out), ptr(ws),
-                                                      ws.numel(), stream()))
-    else:
+    vm = ext = None
+    if vertmap is not None:
         lab, vm, cen, ext = _coord_inputs(lab, vertmap, cen, extents)
-        check(lib().pcnn_vertex_loss_coord_lowres_fwd(ptr(lr), ptr(bv), ptr(lab), ptr(vm), ptr(cen), ptr(ext), B, H, W, C, w_inside, sigma,
-                                                      ptr(out), ptr(ws), ws.numel(), stream()))
+    check(lib().pcnn_vertex_loss_fwd(ptr(lr), ptr(bv), ptr(lab), ptr(cen), ptr(vm), ptr(ext), B, H, W, C, w_inside, sigma, ptr(out), ptr(ws),
+                                     ws.numel(), stream()))
     return out

@@ -173,7 +173,7 @@ def coord_scale(extents):
 
 
 def up8_bwd(P, sigma, thr, pv_unit, prob_unit=0.125):
-    """Reference of pcnn_up8_heads_bwd_ex (P["coord"] False) / pcnn_up8_heads_bwd_coord (True) on problem P
+    """Reference of pcnn_up8_heads_bwd with the 2-D (P["coord"] False) or the 3-D target (True) on problem P
     (up8_bwd_problem).  pv_unit: grid of the predicted vertex values and (2-D log z / 3-D) targets.
 
     d up, score channel c: s_cls * sel_p * (prob[p, c] - [c == gt_p]) * [score[p, c] > 0], s_cls = up_cls / (count + 1e-10f),
@@ -396,7 +396,7 @@ def up8_heads_plan(B, h, w, C, label_only=False):
 
 
 def up8_bwd_plan(B, h, w, C):
-    """pcnn_up8_heads_bwd_ex / _coord: CTAs of strips (4 cells, 16 at C = 2) x bands of 16 low-resolution rows x images,
+    """pcnn_up8_heads_bwd: CTAs of strips (4 cells, 16 at C = 2) x bands of 16 low-resolution rows x images,
     (8 SC + 8) C / 2 threads, instantiation <22>, <2> or the generic <0>; 4C partial bias floats per CTA.  smem is the 2-D
     mode's (the 3-D mode adds 6C floats)."""
     sc = 16 if C == 2 else 4

@@ -94,8 +94,8 @@ def test_plain_scalars_reach_c(native_lib):
     buf = ctypes.create_string_buffer(64)                      # any non-NULL host address: the checks fail before it is read
 
     def up8(C, h, w, ws):
-        return native_lib.pcnn_up8_heads_bwd_ex(buf, buf, buf, buf, 1.0, 0.7, buf, None, None, buf, buf, 2.0, 10.0, 1.0, 1, h, w, C,
-                                                64, 160, buf, buf, buf, buf, ws, None)
+        return native_lib.pcnn_up8_heads_bwd(buf, buf, buf, buf, 1.0, 0.7, buf, buf, buf, None, None, buf, 2.0, 10.0, 1.0, 1, h, w, C,
+                                             64, 160, buf, buf, buf, buf, ws, None)
     assert up8(7, 8, 8, 1 << 20) == -1 and b"(C = 7)" in native_lib.pcnn_last_error()                       # int
     assert up8(2, 60, 80, 16) == -1 and b"workspace too small (16 < 640)" in native_lib.pcnn_last_error()   # size_t
     assert native_lib.pcnn_average_distance_fwd(None, None, None, None, None, 1, 22, 100, -0.25, None, None, None, 0, None) == -1

@@ -57,14 +57,14 @@ def test_host_planning_without_gpu(native_lib):
         assert 1 <= splits <= 2 * 132                                                              # at most two waves of work items on 132 SMs
     assert native_lib.pcnn_conv_wgrad_workspace_bytes(1, 8, 8, 48, 64, 3, ctypes.byref(nbytes)) == -1  # Cin % 64
     f1 = 1.0
-    assert native_lib.pcnn_up8_heads_bwd_ex(None, None, None, None, f1, f1, None, None, None, None, None, f1, f1, f1, 1, 8, 8, 22, 64, 128,
-                                            None, None, None, None, 0, None) == -1
+    assert native_lib.pcnn_up8_heads_bwd(None, None, None, None, f1, f1, None, None, None, None, None, None, f1, f1, f1, 1, 8, 8, 22, 64,
+                                         128, None, None, None, None, 0, None) == -1
     buf = ctypes.create_string_buffer(64)                      # any non-NULL host address: the checks fail before it is read
     for C in (4, 7, 23, 52):                                   # the strip kernel's class counts: even, 6..50
-        assert native_lib.pcnn_up8_heads_bwd_ex(buf, buf, buf, buf, f1, f1, buf, None, None, buf, buf, f1, f1, f1, 1, 8, 8, C, 64, 160,
-                                                buf, buf, buf, buf, 1 << 20, None) == -1, C
+        assert native_lib.pcnn_up8_heads_bwd(buf, buf, buf, buf, f1, f1, buf, buf, buf, None, None, buf, f1, f1, f1, 1, 8, 8, C, 64, 160,
+                                             buf, buf, buf, buf, 1 << 20, None) == -1, C
         assert b"C must be even" in native_lib.pcnn_last_error()
-    assert native_lib.pcnn_vertex_loss_fused_lowres_fwd(None, None, None, None, 1, 64, 96, 22, 1.0, 1.0, None, None, 0, None) == -1
+    assert native_lib.pcnn_vertex_loss_fwd(None, None, None, None, None, None, 1, 64, 96, 22, 1.0, 1.0, None, None, 0, None) == -1
 
 
 def test_ops_refuse_cpu_tensors(native_lib):

@@ -167,8 +167,8 @@ def test_coverage_helpers(native_lib):
     # the workspace the entry point asks for (its "workspace too small (have < need)" check runs before any launch)
     buf = ctypes.create_string_buffer(64)
     for B, h, w, C in ((2, 60, 80, 50), (2, 37, 27, 2), (2, 37, 27, 12)):
-        rc = native_lib.pcnn_up8_heads_bwd_ex(buf, buf, buf, buf, 1.0, 1.0, buf, None, None, buf, buf, 1.0, 1.0, 1.0, B, h, w, C, 64,
-                                              R.vertex_stride(C), buf, buf, buf, buf, 16, None)
+        rc = native_lib.pcnn_up8_heads_bwd(buf, buf, buf, buf, 1.0, 1.0, buf, buf, buf, None, None, buf, 1.0, 1.0, 1.0, B, h, w, C, 64,
+                                           R.vertex_stride(C), buf, buf, buf, buf, 16, None)
         assert rc == -1
         need = re.search(rb"workspace too small \(16 < (\d+)\)", native_lib.pcnn_last_error())
         assert need and int(need.group(1)) == R.up8_bwd_plan(B, h, w, C)["workspace"], native_lib.pcnn_last_error()
@@ -184,3 +184,19 @@ def test_coverage_helpers(native_lib):
     assert R.up8_heads_plan(2, 60, 80, 58, label_only=True)["kernel"] == "k_up8_label"
     assert R.up8_heads_plan(2, 60, 80, 64, label_only=True)["kernel"] == "k_up8_heads"     # 11 w C floats > 200 KB
     assert R.up8_heads_plan(2, 60, 80, 22)["segments"] == 4
+
+
+@pytest.mark.parametrize("C", [2, 6, 9, 22, 50])
+def test_up8_bwd_workspace_query(native_lib, C):
+    """pcnn_up8_heads_bwd_workspace_bytes is the size heads_ref.up8_bwd_plan restates (4C floats per CTA of its strips and 16-row
+    bands) at 480 x 640, at 296 x 216 (partial last strip and band) and on an odd batch, and the size the entry point checks."""
+    nbytes = ctypes.c_size_t(0)
+    buf = ctypes.create_string_buffer(64)
+    for B, h, w in ((2, 60, 80), (2, 37, 27), (5, 37, 27)):
+        assert native_lib.pcnn_up8_heads_bwd_workspace_bytes(B, h, w, C, ctypes.byref(nbytes)) == 0
+        assert nbytes.value == R.up8_bwd_plan(B, h, w, C)["workspace"], (B, h, w)
+        rc = native_lib.pcnn_up8_heads_bwd(buf, buf, buf, buf, 1.0, 1.0, buf, buf, buf, None, None, buf, 1.0, 1.0, 1.0, B, h, w, C, 64,
+                                           R.vertex_stride(C), buf, buf, buf, buf, nbytes.value - 1, None)
+        assert rc == -1 and f"workspace too small ({nbytes.value - 1} < {nbytes.value})".encode() in native_lib.pcnn_last_error()
+    assert native_lib.pcnn_up8_heads_bwd_workspace_bytes(2, 60, 80, C, None) == -1
+    assert native_lib.pcnn_up8_heads_bwd_workspace_bytes(0, 60, 80, C, ctypes.byref(nbytes)) == -1

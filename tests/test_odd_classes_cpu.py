@@ -6,16 +6,16 @@ import ctypes
 import pytest
 
 
-def _bwd_ex(native_lib, buf, C, ws_bytes):
+def _bwd_ex(native_lib, buf, C, ws_bytes):                     # 2-D target: no vertmap / extents
     f1 = 1.0
-    return native_lib.pcnn_up8_heads_bwd_ex(buf, buf, buf, buf, f1, f1, buf, None, None, buf, buf, f1, f1, f1, 1, 60, 80, C, 64, 128,
-                                            buf, buf, buf, buf, ws_bytes, None)
+    return native_lib.pcnn_up8_heads_bwd(buf, buf, buf, buf, f1, f1, buf, buf, buf, None, None, buf, f1, f1, f1, 1, 60, 80, C, 64, 128,
+                                         buf, buf, buf, buf, ws_bytes, None)
 
 
-def _bwd_coord(native_lib, buf, C, ws_bytes):
+def _bwd_coord(native_lib, buf, C, ws_bytes):                  # 3-D target: vertmap and extents given
     f1 = 1.0
-    return native_lib.pcnn_up8_heads_bwd_coord(buf, buf, buf, buf, f1, f1, buf, None, None, buf, buf, buf, buf, f1, f1, f1, 1, 60, 80, C,
-                                               64, 128, buf, buf, buf, buf, ws_bytes, None)
+    return native_lib.pcnn_up8_heads_bwd(buf, buf, buf, buf, f1, f1, buf, buf, buf, buf, buf, buf, f1, f1, f1, 1, 60, 80, C, 64, 128,
+                                         buf, buf, buf, buf, ws_bytes, None)
 
 
 @pytest.mark.parametrize("entry", [_bwd_ex, _bwd_coord], ids=["2d", "coord"])

@@ -2,6 +2,7 @@
 against the float64 references of tests/heads_ref.py (C = 3, 9, 21, 127 forward; C = 9 adjoint, both target modes), the
 class-count generic kernels on the C = 9 network path, the training step at C = 9 against torch autograd, and inference at
 480 x 640 with C = 9 (the multi-object LINEMOD model, linemod_color_2d.yml: eight objects plus background)."""
+import ctypes
 
 import numpy as np
 import pytest
@@ -39,7 +40,7 @@ def odd_heads_roles(C, label_only):
 
 
 def odd_bwd_plan(B, h, w, C):
-    """pcnn_up8_heads_bwd_ex / _coord at odd C: the 4-cell strips of heads_ref.up8_bwd_plan, one channel per thread:
+    """pcnn_up8_heads_bwd at odd C: the 4-cell strips of heads_ref.up8_bwd_plan, one channel per thread:
     (8 SC + 8) C threads."""
     plan = dict(R.up8_bwd_plan(B, h, w, C))
     plan.update(kernel="<0, odd>", threads=(8 * plan["strip"] + 8) * C)
@@ -101,7 +102,7 @@ def test_up8_heads_odd_exact(cuda, C, h, w):
 # ---------------------------------------------------------------------------------------------------------------------
 # 2. the up-sampling adjoint (k_up8_bwd_strip<0, 4, ., 1>)
 # ---------------------------------------------------------------------------------------------------------------------
-def _up8_bwd(P, sigma, thr, dense, Cv):
+def _up8_bwd(P, sigma, thr, Cv):
     from posecnn_b200._lib import check, lib, ptr, stream
     B, h, w, C = P["B"], P["h"], P["w"], P["C"]
     dev = P["prob"].device
@@ -110,16 +111,13 @@ def _up8_bwd(P, sigma, thr, dense, Cv):
     dbias = torch.full((4 * C,), 7.0, device=dev)
     cls_out = torch.tensor([0.5, P["count"]], device=dev)
     vtx_out = torch.tensor([0.25, P["sumw"]], device=dev)
-    ws = torch.empty(odd_bwd_plan(B, h, w, C)["workspace"], dtype=torch.uint8, device=dev)
-    vpred = P["pv"].float().contiguous() if dense else None
-    head = (ptr(P["prob"]), ptr(P["score"]), ptr(P["gt"]), ptr(cls_out), P["up_cls"], thr, ptr(vpred),
-            ptr(None if dense else P["lowres"]), ptr(None if dense else P["bias_v"]))
-    tail = (ptr(vtx_out), P["up_vtx"], P["w_inside"], sigma, B, h, w, C, 64, Cv, ptr(d_sc), ptr(d_vt), ptr(dbias), ptr(ws), ws.numel(),
-            stream())
-    if P["coord"]:
-        check(lib().pcnn_up8_heads_bwd_coord(*head, ptr(P["vertmap"]), ptr(P["centers"]), ptr(P["extents"]), *tail))
-    else:
-        check(lib().pcnn_up8_heads_bwd_ex(*head, ptr(P["centers"]), *tail))
+    nbytes = ctypes.c_size_t(0)
+    check(lib().pcnn_up8_heads_bwd_workspace_bytes(B, h, w, C, ctypes.byref(nbytes)))
+    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+    vm, ext = (P["vertmap"], P["extents"]) if P["coord"] else (None, None)
+    check(lib().pcnn_up8_heads_bwd(ptr(P["prob"]), ptr(P["score"]), ptr(P["gt"]), ptr(cls_out), P["up_cls"], thr, ptr(P["lowres"]),
+                                   ptr(P["bias_v"]), ptr(P["centers"]), ptr(vm), ptr(ext), ptr(vtx_out), P["up_vtx"], P["w_inside"], sigma, B,
+                                   h, w, C, 64, Cv, ptr(d_sc), ptr(d_vt), ptr(dbias), ptr(ws), ws.numel(), stream()))
     return d_sc, d_vt, dbias
 
 
@@ -127,7 +125,7 @@ def _up8_bwd(P, sigma, thr, dense, Cv):
 @pytest.mark.parametrize("h,w", [(60, 80), (37, 27)])
 def test_up8_bwd_nine_classes_exact(cuda, h, w, coord):
     """test_heads_exact_gpu.py::test_up8_bwd_exact at C = 9: d_sc, d_vt and d bias exact after one bf16 / fp32 rounding,
-    padding channels 0, dense and low-resolution vertex sources bit-identical, two launches bit-identical."""
+    padding channels 0, two launches bit-identical."""
     B, C, Cv = 2, 9, 128
     plan = odd_bwd_plan(B, h, w, C)
     print(f"C={C} {h}x{w} {'3d' if coord else '2d'}: kernel {plan['kernel']} strip {plan['strip']}: {plan['strips']} strips x "
@@ -145,12 +143,9 @@ def test_up8_bwd_nine_classes_exact(cuda, h, w, coord):
         assert bool((bg & (p0 < thr)).any() and (bg & (p0 == thr)).any() and (bg & (p0 == thr - 0.125)).any())
         ref = R.up8_bwd(P, sigma, thr, 2.0 ** -10)
         print(f"  sigma={sigma} threshold={thr}: bit budget {ref['budget']:.0f} of 2^24")
-        d_sc, d_vt, dbias = _up8_bwd(P, sigma, thr, True, Cv)
-        e_sc, e_vt, ebias = _up8_bwd(P, sigma, thr, False, Cv)
-        again = _up8_bwd(P, sigma, thr, False, Cv)
+        e_sc, e_vt, ebias = _up8_bwd(P, sigma, thr, Cv)
+        again = _up8_bwd(P, sigma, thr, Cv)
         torch.cuda.synchronize()
-        for a, b, name in zip((d_sc, d_vt, dbias), (e_sc, e_vt, ebias), ("d_sc", "d_vt", "dbias")):
-            assert torch.equal(bits(a), bits(b)), f"{name}: dense and low-resolution vertex sources differ"
         for a, b in zip((e_sc, e_vt, ebias), again):
             assert torch.equal(bits(a), bits(b)), "two launches differ"
         assert_same(e_sc[..., :C], bf16(ref["d_sc"]), "d_sc")
@@ -205,7 +200,7 @@ def test_loss_cls_nine_classes(cuda, thr):
 
 @pytest.mark.parametrize("sigma", [1.0, 2.5])
 def test_loss_vertex_nine_classes_exact(cuda, sigma):
-    """The fused 2-D vertex loss (pcnn_vertex_loss_fused_lowres_fwd) at C = 9, 2 x 480 x 640: loss and weight sum equal
+    """The fused vertex loss (pcnn_vertex_loss_fwd, 2-D target) at C = 9, 2 x 480 x 640: loss and weight sum equal
     vertex_loss_ref.reference's exact sum / weights."""
     from posecnn_b200 import train_ops
     B, H, W, C = 2, 480, 640, 9

@@ -2,6 +2,7 @@
 two-class kernel, the network's forward at 480 x 640, Hough voting in train mode, the training step with and without pose_reg,
 the domain branch and two ranks.  Every comparison is against the same references and within the same stated limits as the
 C = 6 / 22 tests (tests/train_ref.py, oracle/ref_network.py, the C oracle); every measured error is printed."""
+import ctypes
 
 import numpy as np
 import pytest
@@ -68,7 +69,7 @@ def _up8_problem(cuda, B, h, w, seed):
     return dict(lowres=lowres, bv=bv, vertex=vertex, prob=prob, score=score, gt=gt.to(cuda), centers=centers.to(cuda), B=B, h=h, w=w)
 
 
-def _up8_bwd(P, dense, thr, up_vtx=2.0, w_in=10.0, count=937.0, sumw=411.0):
+def _up8_bwd(P, thr, up_vtx=2.0, w_in=10.0, count=937.0, sumw=411.0):
     from posecnn_b200._lib import check, lib, ptr, stream
     B, h, w = P["B"], P["h"], P["w"]
     dev = P["lowres"].device
@@ -76,11 +77,12 @@ def _up8_bwd(P, dense, thr, up_vtx=2.0, w_in=10.0, count=937.0, sumw=411.0):
     d_vt = torch.full((B, h, w, 128), 7.0, dtype=torch.bfloat16, device=dev)
     dbias = torch.empty((4 * C,), device=dev)
     cls_out, vtx_out = torch.tensor([0.5, count], device=dev), torch.tensor([0.25, sumw], device=dev)
-    ws = torch.empty(4 * B * ((w + 15) // 16) * ((h + 15) // 16) * 4 * C, dtype=torch.uint8, device=dev)    # 16-cell strips
-    check(lib().pcnn_up8_heads_bwd_ex(ptr(P["prob"]), ptr(P["score"]), ptr(P["gt"]), ptr(cls_out), 1.0, thr,
-                                      ptr(P["vertex"] if dense else None), ptr(None if dense else P["lowres"]), ptr(None if dense else P["bv"]),
-                                      ptr(P["centers"]), ptr(vtx_out), up_vtx, w_in, 1.0, B, h, w, C, 64, 128, ptr(d_sc), ptr(d_vt),
-                                      ptr(dbias), ptr(ws), ws.numel(), stream()))
+    nbytes = ctypes.c_size_t(0)
+    check(lib().pcnn_up8_heads_bwd_workspace_bytes(B, h, w, C, ctypes.byref(nbytes)))
+    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+    check(lib().pcnn_up8_heads_bwd(ptr(P["prob"]), ptr(P["score"]), ptr(P["gt"]), ptr(cls_out), 1.0, thr, ptr(P["lowres"]), ptr(P["bv"]),
+                                   ptr(P["centers"]), ptr(None), ptr(None), ptr(vtx_out), up_vtx, w_in, 1.0, B, h, w, C, 64, 128, ptr(d_sc),
+                                   ptr(d_vt), ptr(dbias), ptr(ws), ws.numel(), stream()))
     return d_sc, d_vt, dbias
 
 
@@ -91,15 +93,11 @@ def test_up8_backward_two_classes_against_torch(cuda, h, w, thr):
     lib/fcn/train.py:455-465, 564-573 in torch, pushed through the adjoint of the bilinear x8 transposed convolution."""
     B, up_vtx, w_in, count, sumw = 2, 2.0, 10.0, 937.0, 411.0
     P = _up8_problem(cuda, B, h, w, seed=h * 100 + w)
-    d_sc, d_vt, dbias = _up8_bwd(P, True, thr)
-    e_sc, e_vt, ebias = _up8_bwd(P, False, thr)
-    again = _up8_bwd(P, False, thr)
+    d_sc, d_vt, dbias = _up8_bwd(P, thr)
+    again = _up8_bwd(P, thr)
     torch.cuda.synchronize()
-    for a, b in zip((e_sc, e_vt, ebias), again):
+    for a, b in zip((d_sc, d_vt, dbias), again):
         assert torch.equal(bits(a), bits(b))                                                  # two launches: bit-identical
-    print("dense vs low-resolution vertex source: max |d_vt diff| %.3e, max |dbias diff| %.3e" % (
-        (d_vt.float() - e_vt.float()).abs().max().item(), (dbias - ebias).abs().max().item()))
-    assert torch.equal(d_sc, e_sc)
     H, W = 8 * h, 8 * w
     gt = P["gt"].long()
     prob, score, vertex = P["prob"], P["score"], P["vertex"]
@@ -127,12 +125,11 @@ def test_up8_backward_two_classes_against_torch(cuda, h, w, thr):
     e = rel_l2(d_sc[..., :C].float(), want[..., :C])
     print(f"h, w = {h}, {w}, threshold {thr}: d_sc rel-L2 {e:.2e}")
     assert e < 4e-3
-    for vt_, b_ in ((d_vt, dbias), (e_vt, ebias)):
-        ev = rel_l2(vt_[..., :3 * C].float(), want[..., C:])
-        print(f"  d_vt rel-L2 {ev:.2e}")
-        assert ev < 4e-3
-        assert (vt_[..., 3 * C:].float() == 0).all()
-        assert torch.allclose(b_, d_up.sum((0, 2, 3)), rtol=2e-4, atol=1e-7)
+    ev = rel_l2(d_vt[..., :3 * C].float(), want[..., C:])
+    print(f"  d_vt rel-L2 {ev:.2e}")
+    assert ev < 4e-3
+    assert (d_vt[..., 3 * C:].float() == 0).all()
+    assert torch.allclose(dbias, d_up.sum((0, 2, 3)), rtol=2e-4, atol=1e-7)
     assert (d_sc[..., C:].float() == 0).all()
 
 

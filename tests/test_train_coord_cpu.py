@@ -43,31 +43,31 @@ def test_coord_target_and_loss_entries_check_arguments(native_lib):
     assert b"vertex_targets_3d: bad shape" in native_lib.pcnn_last_error()
     assert native_lib.pcnn_vertex_targets_3d_fwd(buf, buf, buf, buf, 65536, 256, 256, 6, f1, buf, buf, None) == -1
     assert b"too many pixels" in native_lib.pcnn_last_error()
-    # fused loss: vertmap and extents are required on top of the 2-D twin's tensors; sigma > 0; H, W % 8 == 0; workspace size
-    assert native_lib.pcnn_vertex_loss_coord_lowres_fwd(buf, None, buf, buf, buf, buf, 1, 64, 96, 22, f1, f1, buf, buf, ws, None) == -1
-    assert b"vertex_loss_coord_lowres: NULL tensor pointer" in native_lib.pcnn_last_error()
-    assert native_lib.pcnn_vertex_loss_coord_lowres_fwd(buf, buf, buf, None, buf, buf, 1, 64, 96, 22, f1, f1, buf, buf, ws, None) == -1
-    assert b"vertex_loss_coord_lowres: NULL tensor pointer" in native_lib.pcnn_last_error()
-    assert native_lib.pcnn_vertex_loss_coord_lowres_fwd(buf, buf, buf, buf, buf, None, 1, 64, 96, 22, f1, f1, buf, buf, ws, None) == -1
-    assert b"vertex_loss_coord_lowres: NULL tensor pointer" in native_lib.pcnn_last_error()
-    assert native_lib.pcnn_vertex_loss_coord_lowres_fwd(buf, buf, buf, buf, buf, buf, 1, 64, 96, 22, f1, 0.0, buf, buf, ws, None) == -1
-    assert b"vertex_loss_coord_lowres: bad arguments" in native_lib.pcnn_last_error()
-    assert native_lib.pcnn_vertex_loss_coord_lowres_fwd(buf, buf, buf, buf, buf, buf, 1, 64, 96, 22, f1, f1, buf, buf, 16, None) == -1
-    assert b"vertex_loss_coord_lowres: workspace too small" in native_lib.pcnn_last_error()
-    assert native_lib.pcnn_vertex_loss_coord_lowres_fwd(buf, buf, buf, buf, buf, buf, 1, 60, 96, 22, f1, f1, buf, buf, ws, None) == -1
-    assert b"vertex_loss_coord_lowres: bad arguments" in native_lib.pcnn_last_error()
+    # fused loss: the head tensor and its bias are required; vertmap and extents go together; sigma > 0; H, W % 8 == 0; workspace size
+    def loss(lowres, bias, vertmap, extents, H=64, sigma=f1, ws=ws):
+        return native_lib.pcnn_vertex_loss_fwd(lowres, bias, buf, buf, vertmap, extents, 1, H, 96, 22, f1, sigma, buf, buf, ws, None)
+    assert loss(buf, None, buf, buf) == -1 and b"vertex_loss: NULL tensor pointer" in native_lib.pcnn_last_error()
+    assert loss(None, buf, buf, buf) == -1 and b"vertex_loss: NULL tensor pointer" in native_lib.pcnn_last_error()
+    assert loss(buf, buf, None, buf) == -1 and b"vertex_loss: vertmap and extents" in native_lib.pcnn_last_error()
+    assert loss(buf, buf, buf, None) == -1 and b"vertex_loss: vertmap and extents" in native_lib.pcnn_last_error()
+    assert loss(buf, buf, buf, buf, sigma=0.0) == -1 and b"vertex_loss: bad arguments" in native_lib.pcnn_last_error()
+    assert loss(buf, buf, buf, buf, ws=16) == -1 and b"vertex_loss: workspace too small" in native_lib.pcnn_last_error()
+    assert loss(buf, buf, buf, buf, H=60) == -1 and b"vertex_loss: bad arguments" in native_lib.pcnn_last_error()
+    assert loss(buf, buf, None, None, H=60) == -1 and b"vertex_loss: bad arguments" in native_lib.pcnn_last_error()   # 2-D target
 
 
 def test_coord_adjoint_checks_arguments(native_lib):
     f1 = 1.0
     buf = ctypes.create_string_buffer(64)
 
-    def call(vertmap, extents, C, h=8, w=8, ws=1 << 20):
-        return native_lib.pcnn_up8_heads_bwd_coord(buf, buf, buf, buf, f1, f1, buf, None, None, vertmap, buf, extents, buf, f1, f1, f1, 1, h,
-                                                   w, C, 64, 160, buf, buf, buf, buf, ws, None)
-    assert call(None, buf, 22) == -1 and b"up8_heads_bwd_coord: NULL tensor pointer" in native_lib.pcnn_last_error()
-    assert call(buf, None, 22) == -1 and b"up8_heads_bwd_coord: NULL tensor pointer" in native_lib.pcnn_last_error()
-    for C in (4, 7, 23, 52):                                   # the class counts of the 2-D entry, no others
+    def call(vertmap, extents, C, h=8, w=8, ws=1 << 20, lowres=buf):
+        return native_lib.pcnn_up8_heads_bwd(buf, buf, buf, buf, f1, f1, lowres, buf, buf, vertmap, extents, buf, f1, f1, f1, 1, h, w, C, 64,
+                                             160, buf, buf, buf, buf, ws, None)
+    assert call(None, buf, 22) == -1 and b"up8_heads_bwd: vertmap and extents" in native_lib.pcnn_last_error()
+    assert call(buf, None, 22) == -1 and b"up8_heads_bwd: vertmap and extents" in native_lib.pcnn_last_error()
+    for vm in (None, buf):                                     # the low-resolution head tensor is required in both target modes
+        assert call(vm, vm, 22, lowres=None) == -1 and b"up8_heads_bwd: NULL tensor pointer" in native_lib.pcnn_last_error()
+    for C in (4, 7, 23, 52):                                   # the class counts of the 2-D target, no others
         assert call(buf, buf, C) == -1, C
         assert b"C must be even" in native_lib.pcnn_last_error()
     # C = 2 (16-cell strips: 5 x 4 CTAs x 8 floats at 60 x 80) passes the class-count check and stops at the workspace check

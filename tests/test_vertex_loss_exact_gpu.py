@@ -1,7 +1,7 @@
 """The training step's vertex loss and the targets it is built from, bit for bit against the float64 references of
 tests/vertex_loss_ref.py at training shapes.
 
-- loss_vertex (pcnn_vertex_loss_fused_lowres_fwd / _coord_lowres_fwd) at 2 x 480 x 640, C = 22 and 2, sigma 1 and 2.5, both
+- loss_vertex (pcnn_vertex_loss_fwd) at 2 x 480 x 640, C = 22 and 2, sigma 1 and 2.5, both
   target modes: out[0] is the fp32 rounding of the exact term sum over the weight sum (an order-independent check that
   raises Straddle where the kernel's double accumulation could round either way), out[1] the exact weight sum.  Checked on
   a fresh workspace, after loss_cls on the same workspace and on a repeated call (both read the ticket the previous launch
@@ -44,13 +44,8 @@ def _loss_abi(P, D, ws, label=None):
     lab = D["label"] if label is None else label
     out = torch.full((2,), float("nan"), device=ws.device)
     B, H, W, C = P["B"], P["H"], P["W"], P["C"]
-    if P["coord"]:
-        check(lib().pcnn_vertex_loss_coord_lowres_fwd(ptr(D["lowres"]), ptr(D["bias_v"]), ptr(lab), ptr(D["vertmap"]), ptr(D["centers"]),
-                                                      ptr(D["extents"]), B, H, W, C, P["w_inside"], P["sigma"], ptr(out), ptr(ws),
-                                                      ws.numel(), stream()))
-    else:
-        check(lib().pcnn_vertex_loss_fused_lowres_fwd(ptr(D["lowres"]), ptr(D["bias_v"]), ptr(lab), ptr(D["centers"]), B, H, W, C,
-                                                      P["w_inside"], P["sigma"], ptr(out), ptr(ws), ws.numel(), stream()))
+    check(lib().pcnn_vertex_loss_fwd(ptr(D["lowres"]), ptr(D["bias_v"]), ptr(lab), ptr(D["centers"]), ptr(D.get("vertmap")),
+                                     ptr(D.get("extents")), B, H, W, C, P["w_inside"], P["sigma"], ptr(out), ptr(ws), ws.numel(), stream()))
     return out
 
 

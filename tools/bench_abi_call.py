@@ -1,5 +1,5 @@
-"""Host cost of one call into libposecnn_b200.so through ctypes: the widest call of the training step, pcnn_up8_heads_bwd_ex
-(26 arguments), on a path its argument check rejects before any CUDA work (C = 7), so it runs on a machine without a GPU.
+"""Host cost of one call into libposecnn_b200.so through ctypes: the training step's loss-gradient adjoint, pcnn_up8_heads_bwd
+(27 arguments), on a path its argument check rejects before any CUDA work (C = 7), so it runs on a machine without a GPU.
 
   typed    the package's binding: argtypes from include/posecnn_b200.h, ptr(t) as a plain int, plain Python scalars
   untyped  a second handle of the same library without argtypes, every argument wrapped in Python (c_void_p / c_float /
@@ -44,16 +44,16 @@ def main():
         return ctypes.c_float(float(x))
 
     def call_typed():
-        return lib().pcnn_up8_heads_bwd_ex(ptr(t["prob"]), ptr(t["score"]), ptr(t["gt"]), ptr(t["cls"]), 1.0, 0.7, ptr(None),
-                                           ptr(t["lowres"]), ptr(t["bv"]), ptr(t["centers"]), ptr(t["vtx"]), 2.0, 10.0, 1.0, B, h, w, C, 64,
-                                           160, ptr(t["d_sc"]), ptr(t["d_vt"]), ptr(t["dbias"]), ptr(t["ws"]), t["ws"].numel(), 0)
+        return lib().pcnn_up8_heads_bwd(ptr(t["prob"]), ptr(t["score"]), ptr(t["gt"]), ptr(t["cls"]), 1.0, 0.7, ptr(t["lowres"]),
+                                        ptr(t["bv"]), ptr(t["centers"]), ptr(None), ptr(None), ptr(t["vtx"]), 2.0, 10.0, 1.0, B, h, w, C, 64,
+                                        160, ptr(t["d_sc"]), ptr(t["d_vt"]), ptr(t["dbias"]), ptr(t["ws"]), t["ws"].numel(), 0)
 
     def call_untyped():
         p, f = old_ptr, old_f32
-        return plain.pcnn_up8_heads_bwd_ex(p(t["prob"]), p(t["score"]), p(t["gt"]), p(t["cls"]), f(1.0), f(0.7), p(None), p(t["lowres"]),
-                                           p(t["bv"]), p(t["centers"]), p(t["vtx"]), f(2.0), f(10.0), f(1.0), B, h, w, C, 64, 160,
-                                           p(t["d_sc"]), p(t["d_vt"]), p(t["dbias"]), p(t["ws"]), ctypes.c_size_t(t["ws"].numel()),
-                                           ctypes.c_void_p(0))
+        return plain.pcnn_up8_heads_bwd(p(t["prob"]), p(t["score"]), p(t["gt"]), p(t["cls"]), f(1.0), f(0.7), p(t["lowres"]), p(t["bv"]),
+                                        p(t["centers"]), p(None), p(None), p(t["vtx"]), f(2.0), f(10.0), f(1.0), B, h, w, C, 64, 160,
+                                        p(t["d_sc"]), p(t["d_vt"]), p(t["dbias"]), p(t["ws"]), ctypes.c_size_t(t["ws"].numel()),
+                                        ctypes.c_void_p(0))
 
     res = {"typed": [], "untyped": []}
     for _ in range(a.repeats):
@@ -63,7 +63,7 @@ def main():
             for _ in range(a.calls):
                 fn()
             res[name].append((time.perf_counter() - t0) / a.calls * 1e6)
-    out = dict(metric="host microseconds per pcnn_up8_heads_bwd_ex call (26 arguments, rejected before CUDA work)",
+    out = dict(metric="host microseconds per pcnn_up8_heads_bwd call (27 arguments, rejected before CUDA work)",
                cpu=platform.processor() or platform.machine(), python=platform.python_version(), calls=a.calls, repeats=a.repeats)
     out.update({f"{k}_us": statistics.median(v) for k, v in res.items()})
     out["typed_over_untyped"] = out["typed_us"] / out["untyped_us"]

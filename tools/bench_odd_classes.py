@@ -5,7 +5,7 @@ Inputs: a seeded synthetic 640x480 scene with C classes per arm (synth.make_scen
 scene), random low-resolution head tensors for the kernel arms.  Reported, median of the runs with every run listed:
   up8_heads       ms per launch of pcnn_up8_heads at batch --infer-batch (32): full mode (label, vertex_pred, prob, score) and the
                   pipeline's label-only mode (k_up8_label)
-  up8_bwd         ms per launch of pcnn_up8_heads_bwd_ex alone at batch --batch (64)
+  up8_bwd         ms per launch of pcnn_up8_heads_bwd alone at batch --batch (64)
   infer           ms per forward of the inference network as one CUDA graph (GraphedForward, dense_vertex=False) at batch 32
   train           ms per step of the training step (pose_reg False: linemod_color_2d.yml) at batch --batch, CUDA events
 The card name and power limit are read in the same run with a read-only nvidia-smi query.
@@ -13,6 +13,7 @@ The card name and power limit are read in the same run with a read-only nvidia-s
     python tools/bench_odd_classes.py [--batch 64] [--infer-batch 32] [--steps 10] [--warmup 3] [--runs 3]
 """
 import argparse
+import ctypes
 import json
 import os
 import statistics
@@ -79,7 +80,7 @@ def heads_arms(dev, B, C):
 
 
 def bwd_arm(dev, B, C, gt):
-    """pcnn_up8_heads_bwd_ex on the heads of a random low-resolution tensor and the scene's labels."""
+    """pcnn_up8_heads_bwd on the heads of a random low-resolution tensor and the scene's labels."""
     h, w = H // 8, W // 8
     g = torch.Generator().manual_seed(100 + C)
     lowres = (torch.randn(B, h, w, 4 * C, generator=g) * 0.7).to(dev)
@@ -93,12 +94,14 @@ def bwd_arm(dev, B, C, gt):
     d_sc = torch.empty((B, h, w, 64), dtype=torch.bfloat16, device=dev)
     d_vt = torch.empty((B, h, w, 128), dtype=torch.bfloat16, device=dev)
     dbias = torch.empty((4 * C,), device=dev)
-    ws = torch.empty(4 * B * ((w + 3) // 4) * ((h + 15) // 16) * 4 * C, dtype=torch.uint8, device=dev)
+    nbytes = ctypes.c_size_t(0)
+    check(lib().pcnn_up8_heads_bwd_workspace_bytes(B, h, w, C, ctypes.byref(nbytes)))
+    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
 
     def run():
-        check(lib().pcnn_up8_heads_bwd_ex(ptr(prob), ptr(score), ptr(gt), ptr(cls_out), 1.0, 0.7, ptr(None), ptr(lowres), ptr(bv),
-                                          ptr(centers), ptr(vtx_out), 1.0, 10.0, 1.0, B, h, w, C, 64, 128, ptr(d_sc), ptr(d_vt),
-                                          ptr(dbias), ptr(ws), ws.numel(), stream()))
+        check(lib().pcnn_up8_heads_bwd(ptr(prob), ptr(score), ptr(gt), ptr(cls_out), 1.0, 0.7, ptr(lowres), ptr(bv), ptr(centers),
+                                       ptr(None), ptr(None), ptr(vtx_out), 1.0, 10.0, 1.0, B, h, w, C, 64, 128, ptr(d_sc), ptr(d_vt),
+                                       ptr(dbias), ptr(ws), ws.numel(), stream()))
     return run
 
 

@@ -7,13 +7,14 @@ reference's loader forms it for a LINEMOD / per-object YCB model.  Reported:
           (pose_reg False, the linemod_{benchvise,camera,iron,lamp,phone}.yml models); --runs runs of --warmup + --steps steps
           each, the three arms in turn, CUDA events
   infer   ms per forward of the C = 2 inference network as one CUDA graph (GraphedForward, dense_vertex=False) at batch 32 and 1
-  up8_bwd ms per launch of pcnn_up8_heads_bwd_ex alone (the loss-gradient up-sampling adjoint) at C = 2 and C = 22, batch --batch,
+  up8_bwd ms per launch of pcnn_up8_heads_bwd alone (the loss-gradient up-sampling adjoint) at C = 2 and C = 22, batch --batch,
           60 x 80 low-resolution cells, the two class counts alternating
 The card name and power limit are read in the same run with a read-only nvidia-smi query.
 
     python tools/bench_single_class.py [--batch 64] [--steps 10] [--warmup 3] [--runs 3]
 """
 import argparse
+import ctypes
 import json
 import os
 import statistics
@@ -88,12 +89,14 @@ def up8_problem(dev, B, C, gt):
     d_sc = torch.empty((B, h, w, 64), dtype=torch.bfloat16, device=dev)
     d_vt = torch.empty((B, h, w, 128), dtype=torch.bfloat16, device=dev)
     dbias = torch.empty((4 * C,), device=dev)
-    ws = torch.empty(4 * B * ((w + 3) // 4) * ((h + 15) // 16) * 4 * C, dtype=torch.uint8, device=dev)
+    nbytes = ctypes.c_size_t(0)
+    check(lib().pcnn_up8_heads_bwd_workspace_bytes(B, h, w, C, ctypes.byref(nbytes)))
+    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
 
     def run():
-        check(lib().pcnn_up8_heads_bwd_ex(ptr(prob), ptr(score), ptr(lab), ptr(cls_out), 1.0, 0.7, ptr(None), ptr(lowres), ptr(bv),
-                                          ptr(centers), ptr(vtx_out), 1.0, 10.0, 1.0, B, h, w, C, 64, 128, ptr(d_sc), ptr(d_vt),
-                                          ptr(dbias), ptr(ws), ws.numel(), stream()))
+        check(lib().pcnn_up8_heads_bwd(ptr(prob), ptr(score), ptr(lab), ptr(cls_out), 1.0, 0.7, ptr(lowres), ptr(bv), ptr(centers),
+                                       ptr(None), ptr(None), ptr(vtx_out), 1.0, 10.0, 1.0, B, h, w, C, 64, 128, ptr(d_sc), ptr(d_vt),
+                                       ptr(dbias), ptr(ws), ws.numel(), stream()))
     return run
 
 

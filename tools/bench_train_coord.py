@@ -5,13 +5,14 @@ its single-class view (tools/bench_single_class.py two_class_inputs), and a seed
 in +-0.1 m; the cost does not depend on the values).  Both arms of a class count train the same labels and presence table; the 2-D
 arm is vgg16_convs(pose_reg=False), the 3-D arm vgg16_convs(vertex_reg_2d=False, vertex_reg_3d=True).  Reported per C in (2, 22):
   train    ms per step at --batch (64), --runs runs of --warmup + --steps steps, the two arms in turn, CUDA events
-  up8_bwd  ms per launch of the up-sampling adjoint alone, pcnn_up8_heads_bwd_ex (2-D target) and pcnn_up8_heads_bwd_coord (3-D
-           target) on the same heads, labels and presence table, alternating
+  up8_bwd  ms per launch of the up-sampling adjoint alone, pcnn_up8_heads_bwd with the 2-D and with the 3-D target (vertmap and
+           extents given) on the same heads, labels and presence table, alternating
 The card name and power limit are read in the same run with a read-only nvidia-smi query.
 
     python tools/bench_train_coord.py [--batch 64] [--steps 10] [--warmup 3] [--runs 3]
 """
 import argparse
+import ctypes
 import json
 import os
 import statistics
@@ -59,17 +60,15 @@ def up8_problem(dev, B, C, gt, centers, vertmap, ext):
     d_sc = torch.empty((B, h, w, 64), dtype=torch.bfloat16, device=dev)
     d_vt = torch.empty((B, h, w, 128), dtype=torch.bfloat16, device=dev)
     dbias = torch.empty((4 * C,), device=dev)
-    ws = torch.empty(4 * B * ((w + 3) // 4) * ((h + 15) // 16) * 4 * C, dtype=torch.uint8, device=dev)
-    head = lambda: (ptr(prob), ptr(score), ptr(gt), ptr(cls_out), 1.0, 0.7, ptr(None), ptr(lowres), ptr(bv))
-    tail = lambda: (ptr(vtx_out), 1.0, 10.0, 1.0, B, h, w, C, 64, 128, ptr(d_sc), ptr(d_vt), ptr(dbias), ptr(ws),
-                    ws.numel(), stream())
+    nbytes = ctypes.c_size_t(0)
+    check(lib().pcnn_up8_heads_bwd_workspace_bytes(B, h, w, C, ctypes.byref(nbytes)))
+    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
 
-    def run_2d():
-        check(lib().pcnn_up8_heads_bwd_ex(*head(), ptr(centers), *tail()))
-
-    def run_3d():
-        check(lib().pcnn_up8_heads_bwd_coord(*head(), ptr(vertmap), ptr(centers), ptr(ext), *tail()))
-    return run_2d, run_3d
+    def run(vm, ex):                                   # vertmap / extents NULL: the 2-D target
+        check(lib().pcnn_up8_heads_bwd(ptr(prob), ptr(score), ptr(gt), ptr(cls_out), 1.0, 0.7, ptr(lowres), ptr(bv), ptr(centers), ptr(vm),
+                                       ptr(ex), ptr(vtx_out), 1.0, 10.0, 1.0, B, h, w, C, 64, 128, ptr(d_sc), ptr(d_vt), ptr(dbias), ptr(ws),
+                                       ws.numel(), stream()))
+    return (lambda: run(None, None)), (lambda: run(vertmap, ext))
 
 
 def main():
