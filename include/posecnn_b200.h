@@ -327,8 +327,6 @@ int pcnn_lowres_heads(const void* score4, const void* score5, const void* vert4,
  * consumer) */
 int pcnn_up8_heads(const float* lowres, const float* bias_score, const float* bias_vertex, int B, int h, int w,
                    int C, int32_t* label, float* vertex, float* prob, float* score, void* stream);
-/* depthwise bilinear conv2d_transpose (k x k, stride s, SAME) on f32 NHWC — un-fused reference path */
-int pcnn_deconv_bilinear(const float* in, float* out, int B, int h, int w, int C, int k, int s, void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * Test-time post-processing on the device (SURVEY.md 8(f) rank 1) — replaces lib/utils/nms.py:3-32

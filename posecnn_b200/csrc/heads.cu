@@ -525,33 +525,6 @@ k_up8_label(const float* __restrict__ lr /*[B,h,w,4C]*/, const float* __restrict
     }
 }
 
-// generic bilinear transposed convolution (depthwise, diagonal filter): out[B,s*h,s*w,C] f32 from in[B,h,w,C] f32.
-// Only used by tests / the un-fused reference path.
-__global__ void __launch_bounds__(256)
-k_deconv_bilinear(const float* __restrict__ in, float* __restrict__ out, int B, int h, int w, int C, int k, int s)
-{
-    const int H = h * s, W = w * s, pad = (k - s) / 2;
-    const size_t total = (size_t)B * H * W * C;
-    for (size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
-        const int c = (int)(idx % C);
-        size_t r = idx / C;
-        const int x = (int)(r % W); r /= W;
-        const int y = (int)(r % H);
-        const size_t n = r / H;
-        float acc = 0.f;
-        for (int iy = 0; iy < h; iy++) {
-            int ky = y - s * iy + pad;
-            if (ky < 0 || ky >= k) continue;
-            for (int ix = 0; ix < w; ix++) {
-                int kx = x - s * ix + pad;
-                if (kx < 0 || kx >= k) continue;
-                acc += deconv_w(ky, k) * deconv_w(kx, k) * in[((n * h + iy) * w + ix) * C + c];
-            }
-        }
-        out[idx] = acc;
-    }
-}
-
 }  // namespace pcnn
 
 using namespace pcnn;
@@ -626,11 +599,3 @@ extern "C" int pcnn_up8_heads(const float* lowres, const float* bias_score, cons
     return check_launch("up8_heads");
 }
 
-extern "C" int pcnn_deconv_bilinear(const float* in, float* out, int B, int h, int w, int C, int k, int s, void* stream)
-{
-    PCNN_REQUIRE(in && out && k >= s && (k - s) % 2 == 0, "deconv_bilinear: bad arguments");
-    size_t total = (size_t)B * h * s * w * s * C;
-    int blocks = (int)std::min<size_t>((total + 255) / 256, (size_t)kNumSMs * 16);
-    k_deconv_bilinear<<<blocks, 256, 0, (cudaStream_t)stream>>>(in, out, B, h, w, C, k, s);
-    return check_launch("deconv_bilinear");
-}

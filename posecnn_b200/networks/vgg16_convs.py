@@ -20,8 +20,7 @@ import math
 import numpy as np
 import torch
 
-from .. import conv, pose_head
-from .._lib import check, lib, ptr, stream
+from .. import conv, heads, pose_head
 from ..hough_voting_gpu_layer import hough_voting_gpu_op
 from ..roi_pooling_layer import roi_pooling_op
 from ..utils import nms as dev_nms
@@ -101,16 +100,15 @@ class vgg16_convs:
         self.forward(data, meta_data, extents, want_prob=False, sync_rois=False, **forward_kwargs)
         C = self.num_classes
         B, H, W, _ = data.shape
-        lab = torch.empty((B, H, W), dtype=torch.int32, device=data.device)
-        vert = torch.empty((B, H, W, 3 * C), dtype=torch.float32, device=data.device)
+        bufs = (torch.empty((B, H, W), dtype=torch.int32, device=data.device),
+                torch.empty((B, H, W, 3 * C), dtype=torch.float32, device=data.device), None, None)
         lowres = self._last_lowres
         bias = self.params["score/biases"]
         base = float(bias[0])
 
         def fg_fraction(b0):
             bias[0] = b0
-            check(lib().pcnn_up8_heads(ptr(lowres), ptr(bias), ptr(self.params["vertex_pred/biases"]), B, H // 8, W // 8, C,
-                                       ptr(lab), ptr(vert), ptr(None), ptr(None), stream()))
+            lab = heads.up8_heads(lowres, bias, self.params["vertex_pred/biases"], out=bufs)[0]
             return float((lab > 0).float().mean())
 
         scale = float(lowres[..., :C].abs().max()) + 1.0
@@ -232,17 +230,10 @@ class vgg16_convs:
             v4 = conv.conv_bf16(c4, T["score_conv4_vertex/weights"], P["score_conv4_vertex/biases"], 1, False)
             L["score_conv4_vertex"], L["score_conv5_vertex"] = v4, v5
             w_vertex = T["vertex_pred/w"]
-        h, w = H // 8, W // 8
-        lowres = torch.empty((B, h, w, 4 * C), dtype=torch.float32, device=data.device)
-        check(lib().pcnn_lowres_heads(ptr(s4), ptr(s5), ptr(v4), ptr(v5), ptr(T["score/w"]), ptr(w_vertex), B, h, w,
-                                      self.num_units, 128, C, ptr(lowres), stream()))
+        lowres = heads.lowres_heads(s4, s5, v4, v5, T["score/w"], w_vertex, C)
         self._last_lowres = lowres
-        label = torch.empty((B, H, W), dtype=torch.int32, device=data.device)
-        vertex = torch.empty((B, H, W, 3 * C), dtype=torch.float32, device=data.device) if dense_vertex else None
-        prob = torch.empty((B, H, W, C), dtype=torch.float32, device=data.device) if want_prob else None
-        score = torch.empty((B, H, W, C), dtype=torch.float32, device=data.device) if want_score else None
-        check(lib().pcnn_up8_heads(ptr(lowres), ptr(P["score/biases"]), ptr(P["vertex_pred/biases"]), B, h, w, C, ptr(label),
-                                   ptr(vertex), ptr(prob), ptr(score), stream()))
+        label, vertex, prob, score = heads.up8_heads(lowres, P["score/biases"], P["vertex_pred/biases"], vertex=dense_vertex,
+                                                     prob=want_prob, score=want_score)
         L["label_2d"] = label
         if dense_vertex:
             L["vertex_pred"] = vertex

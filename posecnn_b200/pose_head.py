@@ -1,6 +1,7 @@
 """Host-side bindings of the pose-regression head kernels (include/posecnn_b200.h, csrc/fc_tc.cu):
 RoiPool x2 + add (-> fp16 fc6 operand), and the fully connected layers as split-K wgmma GEMMs with fused
-bias / ReLU / tanh (lib/networks/vgg16_convs.py:177-197, lib/networks/network.py:392-422)."""
+bias / ReLU / tanh (lib/networks/vgg16_convs.py:177-197, lib/networks/network.py:392-422); the training step's backward of
+those layers (input and weight gradients, the pose-loss chain into fc8, and their layout / precision glue)."""
 from __future__ import annotations
 
 import ctypes
@@ -73,6 +74,57 @@ def fc(a: torch.Tensor, w_tc: torch.Tensor, bias: torch.Tensor, act: str = "relu
     else:
         out = torch.empty((M, nv), dtype=torch.float32, device=a.device)
         check(lib().pcnn_fc_f16_tc(ptr(a), ptr(w_tc), ptr(bias), M, N, K, nv, code, ptr(None), 0, ptr(out), ptr(ws), ws.numel(), stream()))
+    return out
+
+
+def fc_dgrad(dy: torch.Tensor, w_t: torch.Tensor, relu_mask: torch.Tensor | None) -> torch.Tensor:
+    """Input gradient of a fully connected layer (pcnn_fc_dgrad_f16_tc): [M, N] fp16 = (dy [M, K] @ w_t^T) * [relu_mask > 0].
+    w_t [N][K] fp16 = the layer's [in][out padded] weights (transpose16 of its fc_weights_to_tc copy); relu_mask [M, N] fp16 = the
+    stored output of the ReLU layer below, or None."""
+    M, K = dy.shape
+    N = w_t.shape[0]
+    out = torch.empty((M, N), dtype=torch.float16, device=dy.device)
+    nbytes = ctypes.c_size_t(0)
+    check(lib().pcnn_fc_workspace_bytes(M, N, K, ctypes.byref(nbytes)))
+    ws = workspace("fc", nbytes.value, dy.device)
+    check(lib().pcnn_fc_dgrad_f16_tc(ptr(dy), ptr(w_t), M, N, K, ptr(relu_mask), ptr(out), N, ptr(ws), ws.numel(), stream()))
+    return out
+
+
+def fc_wgrad(x: torch.Tensor, dy: torch.Tensor, scale: float = 1.0) -> torch.Tensor:
+    """Weight gradient of a fully connected layer (pcnn_fc_wgrad_f16_tc): [Cout][Cin] f32 = scale * dy^T @ x, x [rows, Cin] and
+    dy [rows, Cout] fp16."""
+    rows, Cin = x.shape
+    Cout = dy.shape[1]
+    out = torch.empty((Cout, Cin), dtype=torch.float32, device=x.device)
+    nbytes = ctypes.c_size_t(0)
+    check(lib().pcnn_conv_wgrad_workspace_bytes(1, 1, rows, Cin, Cout, 1, ctypes.byref(nbytes)))
+    ws = workspace("wgrad", nbytes.value, x.device)
+    check(lib().pcnn_fc_wgrad_f16_tc(ptr(x), ptr(dy), rows, Cin, Cout, scale, ptr(None), 0.0, ptr(out), ptr(ws), ws.numel(), stream()))
+    return out
+
+
+def pose_chain_bwd(bottom_diff: torch.Tensor, poses_tanh: torch.Tensor, poses_weight: torch.Tensor, upstream: float,
+                   out: torch.Tensor) -> torch.Tensor:
+    """pcnn_pose_chain_bwd: Averagedistance's bottom_diff [N, D] f32 through l2_normalize, * poses_weight and tanh, times upstream,
+    written to out [N, ld] fp16 (fc8's d pre-activation; ld = fc8's padded output count, columns D.. written as 0).  Returns out."""
+    N, D = bottom_diff.shape
+    check(lib().pcnn_pose_chain_bwd(ptr(bottom_diff), ptr(poses_tanh), ptr(poses_weight), N, D, upstream, ptr(out), out.shape[1], stream()))
+    return out
+
+
+def transpose16(x: torch.Tensor) -> torch.Tensor:
+    """pcnn_transpose16: x [rows, cols] (any 16-bit dtype) -> [cols, rows]."""
+    rows, cols = x.shape
+    out = torch.empty((cols, rows), dtype=x.dtype, device=x.device)
+    check(lib().pcnn_transpose16(ptr(x), rows, cols, ptr(out), stream()))
+    return out
+
+
+def half_to_float(x: torch.Tensor, scale: float) -> torch.Tensor:
+    """pcnn_half_to_float: scale * x in f32, x fp16 of any shape (contiguous)."""
+    out = torch.empty(x.shape, dtype=torch.float32, device=x.device)
+    check(lib().pcnn_half_to_float(ptr(x), x.numel(), scale, ptr(out), stream()))
     return out
 
 

@@ -38,15 +38,14 @@ PyTorch supplies device memory, streams, NCCL plumbing and a few tiny glue ops o
 """
 from __future__ import annotations
 
-import ctypes
 from typing import Callable, NamedTuple
 
 import torch
 import torch.distributed as dist
 
 from . import backward as bw
-from . import conv, pose_head, train_ops
-from ._lib import check, lib, ptr, stream, workspace
+from . import conv, heads, pose_head, train_ops
+from ._lib import check, lib, ptr, stream
 from .average_distance_loss import average_distance_loss_op
 from .hough_voting_gpu_layer import hough_voting_gpu_op
 from .networks.vgg16_convs import PIXEL_MEANS, VGG_CFG
@@ -101,13 +100,14 @@ def trains_coords(net) -> bool:
 
 def param_layout(net) -> dict:
     """{master name: (TF parameter name, kind, master rows)} for every parameter the training step updates.  score / vertex_pred
-    keep C / 3C rows zero-padded to 64 / 128: the channel counts of their 1x1 GEMMs, which pcnn_pack_lowres and the up8
-    backward read.  A pose_reg=False network has no fc6-fc8: the reference creates those variables only under POSE_REG
-    (vgg16_convs.py:175-200), so they are neither trained, decayed nor exported.  Neither has an object-coordinate network, whose
+    keep C / 3C rows zero-padded to heads.SCORE_ROWS / heads.vertex_rows(C): the channel counts of their 1x1 GEMMs, which
+    heads.pack_lowres and heads.up8_heads_bwd read.  A pose_reg=False network has no fc6-fc8: the reference creates those
+    variables only under POSE_REG (vgg16_convs.py:175-200), so they are neither trained, decayed nor exported.  Neither has an object-coordinate network, whose
     pose head sits under vertex_reg_2d in the reference graph."""
     trunks = ("", "_p") if net.input_format == "RGBD" else ("",)
     weights = [(layer + sfx, "conv1_1" if layer == "conv1_1" else "conv", None) for sfx in trunks for layer in CONV_NAMES]
-    weights += [(name, "conv", None) for name in SCORE_HEADS] + [("score", "conv", 64), ("vertex_pred", "conv", 128)]
+    weights += [(name, "conv", None) for name in SCORE_HEADS] + [("score", "conv", heads.SCORE_ROWS),
+                                                               ("vertex_pred", "conv", heads.vertex_rows(net.num_classes))]
     fc = (("fc6", "fc7", "fc8") if net.pose_reg and not trains_coords(net) else ()) + (("fc9",) if net.domain_branch else ())
     weights += [(name, "fc", None) for name in fc]
     if net.domain_branch:
@@ -160,7 +160,7 @@ class Trainer:
         self.conv1_tc = conv.conv1_1_weights_to_tc(P["conv1_1/weights"])
         self.conv1_tc_p = conv.conv1_1_weights_to_tc(P["conv1_1_p/weights"]) if self.rgbd else None
         self._refresh_derived()
-        self.zero_bias = {n: torch.zeros(n, device=dev) for n in (64, 128, 256, 512)}
+        self.zero_bias = {n: torch.zeros(n, device=dev) for n in (64, 128, 256, 512, heads.vertex_rows(self.C))}
 
     # ------------------------------------------------------------------ derived weight copies
     def _refresh_derived(self):
@@ -180,10 +180,7 @@ class Trainer:
                 self.dg[name], self.dg[name + "_p"] = d[:512], d[512:]
         self.fc_t = {}
         for name in self.fc_names:
-            w = self.tc[name + "/w"]
-            t = torch.empty((w.shape[1], w.shape[0]), dtype=torch.float16, device=w.device)
-            check(lib().pcnn_transpose16(ptr(w), w.shape[0], w.shape[1], ptr(t), stream()))
-            self.fc_t[name] = t
+            self.fc_t[name] = pose_head.transpose16(self.tc[name + "/w"])
         self.conv1_tc.zero_()
         self.conv1_tc[:, :27] = self.master["conv1_1/w"].to(torch.bfloat16)
         if self.rgbd:
@@ -257,22 +254,14 @@ class Trainer:
         s5 = conv.conv_bf16(h5, T["score_conv5/w"], M["score_conv5/b"], 1, True)
         v4 = conv.conv_bf16(c4, T["score_conv4_vertex/w"], M["score_conv4_vertex/b"], 1, False)
         v5 = conv.conv_bf16(c5, T["score_conv5_vertex/w"], M["score_conv5_vertex/b"], 1, False)
-        h, w = H // 8, W // 8
-        add_s, add_v = torch.empty_like(s4), torch.empty_like(v4)
-        check(lib().pcnn_add_up2_bf16(ptr(s4), ptr(s5), B, h, w, s4.shape[3], ptr(add_s), stream()))
-        check(lib().pcnn_add_up2_bf16(ptr(v4), ptr(v5), B, h, w, v4.shape[3], ptr(add_v), stream()))
-        lr_s = conv.conv_bf16(add_s, T["score/w"], self.zero_bias[64], 1, False)               # bias added after the up-sampling
-        lr_v = conv.conv_bf16(add_v, T["vertex_pred/w"], self.zero_bias[128], 1, False)
-        lowres = torch.empty((B, h, w, 4 * C), dtype=torch.float32, device=data.device)
-        check(lib().pcnn_pack_lowres(ptr(lr_s), 64, ptr(lr_v), 128, B, h, w, C, ptr(lowres), stream()))
-        label = torch.empty((B, H, W), dtype=torch.int32, device=data.device)
-        prob = torch.empty((B, H, W, C), dtype=torch.float32, device=data.device)
-        score = torch.empty((B, H, W, C), dtype=torch.float32, device=data.device)
+        add_s, add_v = heads.add_up2(s4, s5), heads.add_up2(v4, v5)
+        lr_s = conv.conv_bf16(add_s, T["score/w"], self.zero_bias[heads.SCORE_ROWS], 1, False)   # bias added after the up-sampling
+        lr_v = conv.conv_bf16(add_v, T["vertex_pred/w"], self.zero_bias[heads.vertex_rows(C)], 1, False)
+        lowres = heads.pack_lowres(lr_s, lr_v, C)
         # The dense vertex_pred [B,H,W,3C] (81 MB / frame) is never written: its only consumers — the vertex loss, its gradient and the
         # Hough sampler — read three values per labelled / sampled pixel and form them on demand from `lowres` with k_up8_heads' own
         # operation sequence (heads_common.cuh: bit-identical).  dense_vertex_pred(A) materialises it for inspection.
-        check(lib().pcnn_up8_heads(ptr(lowres), ptr(M["score/b"]), ptr(M["vertex_pred/b"]), B, h, w, C, ptr(label), ptr(None), ptr(prob),
-                                   ptr(score), stream()))
+        label, _, prob, score = heads.up8_heads(lowres, M["score/b"], M["vertex_pred/b"], prob=True, score=True)
         A.update(s4=s4, s5=s5, v4=v4, v5=v5, add_s=add_s, add_v=add_v, label_2d=label, lowres=lowres, prob_normalized=prob, score=score)
         # losses on the dense heads (fused kernels; the masks / targets are never materialised)
         cls_out = train_ops.loss_cls(score, prob, gt_label_2d, net.threshold_label)
@@ -317,14 +306,7 @@ class Trainer:
 
     def dense_vertex_pred(self, A):
         """The dense vertex_pred [B,H,W,3C] of a forward pass (the training step itself never materialises it)."""
-        lowres = A["lowres"]
-        B, h, w, _ = lowres.shape
-        C, M = self.C, self.master
-        label = torch.empty((B, 8 * h, 8 * w), dtype=torch.int32, device=lowres.device)
-        vertex = torch.empty((B, 8 * h, 8 * w, 3 * C), dtype=torch.float32, device=lowres.device)
-        check(lib().pcnn_up8_heads(ptr(lowres), ptr(M["score/b"]), ptr(M["vertex_pred/b"]), B, h, w, C, ptr(label), ptr(vertex), ptr(None),
-                                   ptr(None), stream()))
-        return vertex
+        return heads.up8_heads(A["lowres"], self.master["score/b"], self.master["vertex_pred/b"], vertex=True)[1]
 
     # ------------------------------------------------------------------ gradient plumbing
     def _emit(self, grads, name, g):
@@ -335,35 +317,12 @@ class Trainer:
             with torch.cuda.stream(self.comm):
                 dist.all_reduce(g, op=dist.ReduceOp.SUM)
 
-    def _fc_dgrad(self, dy, name, mask):
-        wt = self.fc_t[name]                                    # [in][out_pad] fp16
-        M_, K = dy.shape
-        N = wt.shape[0]
-        out = torch.empty((M_, N), dtype=torch.float16, device=dy.device)
-        nbytes = ctypes.c_size_t(0)
-        check(lib().pcnn_fc_workspace_bytes(M_, N, K, ctypes.byref(nbytes)))
-        ws = workspace("fc", nbytes.value, dy.device)
-        check(lib().pcnn_fc_dgrad_f16_tc(ptr(dy), ptr(wt), M_, N, K, ptr(mask), ptr(out), N, ptr(ws), ws.numel(), stream()))
-        return out
-
-    def _fc_wgrad(self, x, dy, scale=1.0):
-        rows, Cin = x.shape
-        Cout = dy.shape[1]
-        out = torch.empty((Cout, Cin), dtype=torch.float32, device=x.device)
-        nbytes = ctypes.c_size_t(0)
-        check(lib().pcnn_conv_wgrad_workspace_bytes(1, 1, rows, Cin, Cout, 1, ctypes.byref(nbytes)))
-        ws = workspace("wgrad", nbytes.value, x.device)
-        check(lib().pcnn_fc_wgrad_f16_tc(ptr(x), ptr(dy), rows, Cin, Cout, scale, ptr(None), 0.0, ptr(out), ptr(ws), ws.numel(), stream()))
-        return out
-
     def backward(self, A, gt_label_2d, centers, vertmap=None):
         """All parameter gradients of loss = loss_cls + vertex_w * loss_vertex + loss_pose (weight decay is applied in the update);
         without pose_reg, of loss_cls + vertex_w * loss_vertex.  Loss normalisers (selected-pixel count, vertex weight sum, ROI rows)
         are GLOBAL over the ranks.  An object-coordinate network needs the forward's vertmap= again (its extents are kept in A)."""
         net, C, M, T = self.net, self.C, self.master, self.tc
         data = A["data"]
-        B, H, W, _ = data.shape
-        h, w = H // 8, W // 8
         dev = data.device
         grads = {}
         # ---- global loss normalisers: one all-reduce of [count_cls, sum_w_vertex(, rows)]
@@ -378,17 +337,10 @@ class Trainer:
         if self.pose_reg:
             g5_roi, g4_roi = self._pose_bwd(grads, A, norm)
         # ---- FCN heads
-        d_sc = torch.empty((B, h, w, 64), dtype=torch.bfloat16, device=dev)
-        d_vt = torch.empty((B, h, w, 128), dtype=torch.bfloat16, device=dev)
-        dbias = torch.empty((4 * C,), dtype=torch.float32, device=dev)
-        nbytes = ctypes.c_size_t(0)
-        check(lib().pcnn_up8_heads_bwd_workspace_bytes(B, h, w, C, ctypes.byref(nbytes)))
-        ws = workspace("up8_bwd", nbytes.value, dev)
         vm, ext = (self._require_vertmap(vertmap, data), A["extents"]) if self.coord else (None, None)
-        check(lib().pcnn_up8_heads_bwd(ptr(A["prob_normalized"]), ptr(A["score"]), ptr(gt_label_2d), ptr(A["cls_out"]), 1.0,
-                                       net.threshold_label, ptr(A["lowres"]), ptr(M["vertex_pred/b"]), ptr(centers), ptr(vm), ptr(ext),
-                                       ptr(A["vtx_out"]), self.vertex_w, self.w_inside, 1.0, B, h, w, C, 64, 128, ptr(d_sc), ptr(d_vt),
-                                       ptr(dbias), ptr(ws), ws.numel(), stream()))
+        d_sc, d_vt, dbias = heads.up8_heads_bwd(A["prob_normalized"], A["score"], gt_label_2d, A["cls_out"], 1.0, net.threshold_label,
+                                                A["lowres"], M["vertex_pred/b"], centers, A["vtx_out"], self.vertex_w, self.w_inside, 1.0,
+                                                vertmap=vm, extents=ext)
         self._emit(grads, "score/b", dbias[:C].contiguous())
         self._emit(grads, "vertex_pred/b", dbias[C:].contiguous())
         self._emit(grads, "score/w", bw.conv_wgrad(A["add_s"], d_sc, 1))
@@ -397,12 +349,10 @@ class Trainer:
         d_add_v = conv.conv_bf16(d_vt, self.dg["vertex_pred"], self.zero_bias[128], 1, False)
         d_s4, db = bw.relu_bwd(d_add_s, A["s4"], True, want_bias=True)
         self._emit(grads, "score_conv4/b", db)
-        d_s5 = torch.empty_like(A["s5"])
-        check(lib().pcnn_up2_bwd_bf16(ptr(d_add_s), ptr(A["s5"]), B, h, w, 64, ptr(d_s5), stream()))
+        d_s5 = heads.up2_bwd(d_add_s, A["s5"])
         self._emit(grads, "score_conv5/b", bw.relu_bwd(d_s5, None, False, want_bias=True, want_dz=False)[1])
         self._emit(grads, "score_conv4_vertex/b", bw.relu_bwd(d_add_v, None, False, want_bias=True, want_dz=False)[1])
-        d_v5 = torch.empty_like(A["v5"])
-        check(lib().pcnn_up2_bwd_bf16(ptr(d_add_v), ptr(None), B, h, w, 128, ptr(d_v5), stream()))
+        d_v5 = heads.up2_bwd(d_add_v)
         self._emit(grads, "score_conv5_vertex/b", bw.relu_bwd(d_v5, None, False, want_bias=True, want_dz=False)[1])
         c4, c5 = A["conv4_3"], A["conv5_3"]
         # RGB-D: score_conv4/5 read the 1024-channel concat, so their weight gradient is one wgrad on it
@@ -448,8 +398,7 @@ class Trainer:
         # dpre's row stride is fc8's output count padded to a multiple of 128 (its fp16 weight copy's rows): 128 up to C = 32, 256 above
         D, ld = 4 * C, self.tc["fc8/w"].shape[0]
         dpre = torch.empty((rows, ld), dtype=torch.float16, device=dev)
-        check(lib().pcnn_pose_chain_bwd(ptr(A["pose_diff"]), ptr(A["poses_tanh"]), ptr(A["poses_weight"]), rows, D, pose_scale, ptr(dpre), ld,
-                                        stream()))
+        pose_head.pose_chain_bwd(A["pose_diff"], A["poses_tanh"], A["poses_weight"], pose_scale, dpre)
         # dynamic loss scale: a power of two that puts the largest element of the chain's entry point at ~2^11 (one host read; the
         # un-scaled pass above is only used for its maximum, which fp16 represents well enough even when the small elements underflow)
         amax = torch.stack([dpre.float().abs().max()] + ([dom["amax"][0]] if self.adapt else []))
@@ -466,26 +415,24 @@ class Trainer:
             A["loss_domain"] = dom["loss"]
             self._emit(grads, "domain_score/w", dom["dw10"])
             self._emit(grads, "domain_score/b", dom["db10"])
-            self._emit(grads, "fc9/w", self._fc_wgrad(A["pool"], dom["dpre9"], 1.0 / S_d))
+            self._emit(grads, "fc9/w", pose_head.fc_wgrad(A["pool"], dom["dpre9"], 1.0 / S_d))
             self._emit(grads, "fc9/b", dom["db9"])
-            d9 = self._fc_dgrad(dom["dpre9"], "fc9", None)                                    # [rows, 25088], scaled by S_d
-        check(lib().pcnn_pose_chain_bwd(ptr(A["pose_diff"]), ptr(A["poses_tanh"]), ptr(A["poses_weight"]), rows, D, pose_scale * S, ptr(dpre), ld,
-                                        stream()))
-        self._emit(grads, "fc8/w", self._fc_wgrad(A["fc7"], dpre, 1.0 / S))
+            d9 = pose_head.fc_dgrad(dom["dpre9"], self.fc_t["fc9"], None)                     # [rows, 25088], scaled by S_d
+        pose_head.pose_chain_bwd(A["pose_diff"], A["poses_tanh"], A["poses_weight"], pose_scale * S, dpre)
+        self._emit(grads, "fc8/w", pose_head.fc_wgrad(A["fc7"], dpre, 1.0 / S))
         self._emit(grads, "fc8/b", dpre[:, :D].float().sum(0) / S)
-        d7 = self._fc_dgrad(dpre, "fc8", A["fc7"])
-        self._emit(grads, "fc7/w", self._fc_wgrad(A["fc6"], d7, 1.0 / S))
+        d7 = pose_head.fc_dgrad(dpre, self.fc_t["fc8"], A["fc7"])
+        self._emit(grads, "fc7/w", pose_head.fc_wgrad(A["fc6"], d7, 1.0 / S))
         self._emit(grads, "fc7/b", d7.float().sum(0) / S)
-        d6 = self._fc_dgrad(d7, "fc7", A["fc6"])
-        self._emit(grads, "fc6/w", self._fc_wgrad(A["pool"], d6, 1.0 / S))
+        d6 = pose_head.fc_dgrad(d7, self.fc_t["fc7"], A["fc6"])
+        self._emit(grads, "fc6/w", pose_head.fc_wgrad(A["pool"], d6, 1.0 / S))
         self._emit(grads, "fc6/b", d6.float().sum(0) / S)
-        dpool16 = self._fc_dgrad(d6, "fc6", None)                                              # [rows, 25088]
+        dpool16 = pose_head.fc_dgrad(d6, self.fc_t["fc6"], None)                               # [rows, 25088]
         if self.adapt:
             # pool_score's gradient from both branches in one pass; gradient_reversal is the factor -lambda of the domain term
             dpool = pose_head.domain_grad_merge(dpool16, 1.0 / S, d9, -GRL_LAMBDA / S_d, (rows, 7, 7, 512))
         else:
-            dpool = torch.empty((rows, 7, 7, 512), dtype=torch.float32, device=dev)
-            check(lib().pcnn_half_to_float(ptr(dpool16), dpool16.numel(), 1.0 / S, ptr(dpool), stream()))
+            dpool = pose_head.half_to_float(dpool16, 1.0 / S).view(rows, 7, 7, 512)
         A["dpool"] = dpool                                                                      # d loss / d pool_score (kept for inspection)
         g5_roi = roi_pooling_op.roi_pool_grad(A["conv5_3"], A["rois"], A["a5"], dpool, 7, 7, 1.0 / 16.0, 0)       # fp32 dense
         g4_roi = roi_pooling_op.roi_pool_grad(A["conv4_3"], A["rois"], A["a4"], dpool, 7, 7, 1.0 / 8.0, 0)

@@ -310,6 +310,21 @@ def up8_bwd_problem(B, h, w, C, coord, gen, device="cpu", w_inside=4.0, up_cls=1
     return P
 
 
+def run_up8_bwd(P, sigma, thr, Cv):
+    """The adjoint (posecnn_b200.heads.up8_heads_bwd) on problem P on the GPU, into outputs pre-filled with 7 so that padding
+    channels must be written as 0; d_vt has channel stride Cv.  Returns (d_sc, d_vt, dbias)."""
+    from posecnn_b200 import heads
+    B, h, w, C = P["B"], P["h"], P["w"], P["C"]
+    dev = P["prob"].device
+    out = (torch.full((B, h, w, 64), 7.0, dtype=torch.bfloat16, device=dev), torch.full((B, h, w, Cv), 7.0, dtype=torch.bfloat16, device=dev),
+           torch.full((4 * C,), 7.0, device=dev))
+    cls_out = torch.tensor([0.5, P["count"]], device=dev)
+    vtx_out = torch.tensor([0.25, P["sumw"]], device=dev)
+    vm, ext = (P["vertmap"], P["extents"]) if P["coord"] else (None, None)
+    return heads.up8_heads_bwd(P["prob"], P["score"], P["gt"], cls_out, P["up_cls"], thr, P["lowres"], P["bias_v"], P["centers"], vtx_out,
+                               P["up_vtx"], P["w_inside"], sigma, vertmap=vm, extents=ext, out=out)
+
+
 # ---------------------------------------------------------------------------------------------------------------------
 # The classification loss of the training step (k_loss_cls_hard_raw): Hardlabel-selected cross entropy from raw scores
 # ---------------------------------------------------------------------------------------------------------------------

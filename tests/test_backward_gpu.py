@@ -2,8 +2,6 @@
 operands: weight gradients on wgmma (MN-major operands, split-K), ReLU-mask / max-pool routing, bias gradients, and the
 input gradient through the forward kernel on flipped weights.  Reference semantics: TensorFlow's gradients of
 Network.conv / max_pool (lib/networks/network.py:159-188, 303-310) as driven by lib/fcn/train.py:206-260."""
-import ctypes
-
 import pytest
 import torch
 import torch.nn.functional as F
@@ -105,31 +103,21 @@ def test_conv_dgrad_through_forward_kernel(cuda, Cin, Cout, k):
 
 def test_fc_dgrad_wgrad_and_pose_chain(cuda):
     """Fully connected backward GEMMs (fp16 operands) and the pose-loss chain against torch on the same operands."""
-    import ctypes
     from posecnn_b200 import pose_head
-    from posecnn_b200._lib import check, lib, ptr, stream, workspace
     g = torch.Generator().manual_seed(11)
     rows, Kin, Nout = 45, 4096, 256
     x = torch.relu(torch.randn(rows, Kin, generator=g)).to(torch.float16).to(cuda)          # stored output of the layer below (ReLU)
     w = (torch.randn(Kin, Nout, generator=g) / Kin ** 0.5).to(cuda)                           # TF layout [in, out]
     dy = (torch.randn(rows, Nout, generator=g) * 0.3).to(torch.float16).to(cuda)
     w_tc = pose_head.fc_weights_to_tc(w)                                                       # [out][in] fp16
-    w_t = torch.empty((Kin, Nout), dtype=torch.float16, device=cuda)
-    check(lib().pcnn_transpose16(ptr(w_tc), Nout, Kin, ptr(w_t), stream()))
+    w_t = pose_head.transpose16(w_tc)
     assert torch.equal(w_t, w_tc.t().contiguous())
     # input gradient with the ReLU mask of the layer below
-    out = torch.empty((rows, Kin), dtype=torch.float16, device=cuda)
-    nbytes = ctypes.c_size_t(0)
-    check(lib().pcnn_fc_workspace_bytes(rows, Kin, Nout, ctypes.byref(nbytes)))
-    ws = workspace("fc", nbytes.value, cuda)
-    check(lib().pcnn_fc_dgrad_f16_tc(ptr(dy), ptr(w_t), rows, Kin, Nout, ptr(x), ptr(out), Kin, ptr(ws), ws.numel(), stream()))
+    out = pose_head.fc_dgrad(dy, w_t, x)
     want = (dy.float() @ w_tc.float()) * (x.float() > 0)
     assert rel_l2(out.float(), want) < 2e-3
     # weight gradient [out][in] with a scale
-    dw = torch.empty((Nout, Kin), dtype=torch.float32, device=cuda)
-    check(lib().pcnn_conv_wgrad_workspace_bytes(1, 1, rows, Kin, Nout, 1, ctypes.byref(nbytes)))
-    ws2 = workspace("wgrad", nbytes.value, cuda)
-    check(lib().pcnn_fc_wgrad_f16_tc(ptr(x), ptr(dy), rows, Kin, Nout, 0.25, ptr(None), 0.0, ptr(dw), ptr(ws2), ws2.numel(), stream()))
+    dw = pose_head.fc_wgrad(x, dy, 0.25)
     assert rel_l2(dw, 0.25 * dy.float().t() @ x.float()) < 1e-4
     # pose chain: d pre-activation of fc8 from d loss / d poses_pred, poses_pred = l2_normalize(tanh(pre) * weight)
     N, D = 19, 24
@@ -140,24 +128,19 @@ def test_fc_dgrad_wgrad_and_pose_chain(cuda):
     mul = th * wt
     pred = mul / mul.pow(2).sum(1, keepdim=True).clamp(min=1e-12).sqrt()
     (pred * gup).sum().backward()
-    dpre = torch.empty((N, 128), dtype=torch.float16, device=cuda)
-    check(lib().pcnn_pose_chain_bwd(ptr(gup), ptr(th.detach().contiguous()), ptr(wt), N, D, 1.0, ptr(dpre), 128, stream()))
+    dpre = pose_head.pose_chain_bwd(gup, th.detach().contiguous(), wt, 1.0, torch.empty((N, 128), dtype=torch.float16, device=cuda))
     assert rel_l2(dpre[:, :D].float(), pre.grad) < 2e-3 and float(dpre[:, D:].float().abs().max()) == 0.0
 
 
 def _up8_problem(cuda, B, h, w, C, seed):
     """A low-resolution head tensor, its dense up-sampling (pcnn_up8_heads), ground-truth labels with ignore / background /
     foreground pixels, centres with one listed and one unlisted class."""
-    import ctypes
-    from posecnn_b200._lib import check, lib, ptr, stream
+    from posecnn_b200 import heads
     g = torch.Generator().manual_seed(seed)
     H, W = 8 * h, 8 * w
     lowres = (torch.randn(B, h, w, 4 * C, generator=g) * 0.7).to(cuda)
     bs, bv = (torch.randn(C, generator=g) * 0.1).to(cuda), (torch.randn(3 * C, generator=g) * 0.1).to(cuda)
-    label = torch.empty((B, H, W), dtype=torch.int32, device=cuda)
-    vertex = torch.empty((B, H, W, 3 * C), device=cuda)
-    prob, score = torch.empty((B, H, W, C), device=cuda), torch.empty((B, H, W, C), device=cuda)
-    check(lib().pcnn_up8_heads(ptr(lowres), ptr(bs), ptr(bv), B, h, w, C, ptr(label), ptr(vertex), ptr(prob), ptr(score), stream()))
+    _, vertex, prob, score = heads.up8_heads(lowres, bs, bv, vertex=True, prob=True, score=True)
     gt = torch.randint(-1, C, (B, H, W), generator=g).to(torch.int32)
     gt[:, : H // 3] = 0                                                      # a background region (Hardlabel: selected only if uncertain)
     gt[:, H // 3: H // 2, : W // 2] = 3                                      # a coherent object
@@ -170,20 +153,14 @@ def _up8_problem(cuda, B, h, w, C, seed):
 
 
 def _up8_bwd(P, thr=0.7, up_cls=1.0, up_vtx=2.0, w_in=10.0, sigma=1.0, count=937.0, sumw=411.0):
-    from posecnn_b200._lib import check, lib, ptr, stream
+    from posecnn_b200 import heads
     B, h, w, C = P["B"], P["h"], P["w"], P["C"]
     dev = P["lowres"].device
-    d_sc = torch.full((B, h, w, 64), 7.0, dtype=torch.bfloat16, device=dev)
-    d_vt = torch.full((B, h, w, 128), 7.0, dtype=torch.bfloat16, device=dev)
-    dbias = torch.empty((4 * C,), device=dev)
+    out = (torch.full((B, h, w, 64), 7.0, dtype=torch.bfloat16, device=dev), torch.full((B, h, w, 128), 7.0, dtype=torch.bfloat16, device=dev),
+           torch.empty((4 * C,), device=dev))
     cls_out, vtx_out = torch.tensor([0.5, count], device=dev), torch.tensor([0.25, sumw], device=dev)
-    nbytes = ctypes.c_size_t(0)
-    check(lib().pcnn_up8_heads_bwd_workspace_bytes(B, h, w, C, ctypes.byref(nbytes)))
-    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
-    check(lib().pcnn_up8_heads_bwd(ptr(P["prob"]), ptr(P["score"]), ptr(P["gt"]), ptr(cls_out), up_cls, thr, ptr(P["lowres"]), ptr(P["bv"]),
-                                   ptr(P["centers"]), ptr(None), ptr(None), ptr(vtx_out), up_vtx, w_in, sigma, B, h, w, C, 64, 128, ptr(d_sc),
-                                   ptr(d_vt), ptr(dbias), ptr(ws), ws.numel(), stream()))
-    return d_sc, d_vt, dbias
+    return heads.up8_heads_bwd(P["prob"], P["score"], P["gt"], cls_out, up_cls, thr, P["lowres"], P["bv"], P["centers"], vtx_out, up_vtx, w_in,
+                               sigma, out=out)
 
 
 @pytest.mark.parametrize("C,h,w", [(22, 8, 12), (6, 18, 10), (22, 60, 80)])
@@ -230,23 +207,21 @@ def test_up8_heads_backward_against_torch(cuda, C, h, w):
 
 def test_add_up2_and_adjoint(cuda):
     """add = a4 + up2(a5) (fixed bilinear conv2d_transpose 4x4 / 2, vgg16_convs.py:134-138) and the adjoint with the ReLU mask."""
-    from posecnn_b200._lib import check, lib, ptr, stream
+    from posecnn_b200 import heads
     g = torch.Generator().manual_seed(5)
     B, h, w, C = 2, 12, 16, 64
     a4 = torch.randn(B, h, w, C, generator=g).to(torch.bfloat16).to(cuda)
     a5 = torch.randn(B, h // 2, w // 2, C, generator=g).to(torch.bfloat16).to(cuda)
-    out = torch.empty_like(a4)
-    check(lib().pcnn_add_up2_bf16(ptr(a4), ptr(a5), B, h, w, C, ptr(out), stream()))
+    out = heads.add_up2(a4, a5)
     k1 = torch.tensor([1.0 - abs(i / 2.0 - 0.75) for i in range(4)], device=cuda)
     filt = (k1[:, None] * k1[None, :])[None, None].expand(C, 1, 4, 4).contiguous()
     up = F.conv_transpose2d(a5.float().permute(0, 3, 1, 2), filt, stride=2, padding=1, groups=C).permute(0, 2, 3, 1)
     assert rel_l2(out.float(), a4.float() + up) < 3e-3
     dadd = torch.randn(B, h, w, C, generator=g).to(torch.bfloat16).to(cuda)
-    d5 = torch.empty_like(a5)
-    check(lib().pcnn_up2_bwd_bf16(ptr(dadd), ptr(a5), B, h, w, C, ptr(d5), stream()))
+    d5 = heads.up2_bwd(dadd, a5)
     want = F.conv2d(dadd.float().permute(0, 3, 1, 2), filt, stride=2, padding=1, groups=C).permute(0, 2, 3, 1) * (a5.float() > 0)
     assert rel_l2(d5.float(), want) < 3e-3
-    check(lib().pcnn_up2_bwd_bf16(ptr(dadd), ptr(None), B, h, w, C, ptr(d5), stream()))
+    d5 = heads.up2_bwd(dadd)
     assert rel_l2(d5.float(), F.conv2d(dadd.float().permute(0, 3, 1, 2), filt, stride=2, padding=1, groups=C).permute(0, 2, 3, 1)) < 3e-3
 
 
@@ -335,8 +310,7 @@ def test_conv_wgrad_exact_at_training_shapes(cuda, name, H, W, Cin, Cout, k):
 def test_fc_wgrad_exact(cuda, name, Cin, Cout, rows):
     """pcnn_fc_wgrad_f16_tc at the fc6 / fc7 shapes with 600 ROI rows (direct mode, ten 64-row K tiles, the last ragged) and
     at Cin = 192 / 384 (one / two 64-channel B blocks), with a power-of-two scale: exact against the float64 product."""
-    import ctypes
-    from posecnn_b200._lib import check, lib, ptr, stream, workspace
+    from posecnn_b200 import pose_head
     from tests.util import int_operands, wgrad_batch_for_coverage, wgrad_plan
     if rows == 0:
         rows, plan = wgrad_batch_for_coverage(1, 1, Cin, Cout, 1)
@@ -348,11 +322,7 @@ def test_fc_wgrad_exact(cuda, name, Cin, Cout, rows):
     g = torch.Generator().manual_seed(Cin + rows)
     x = int_operands((rows, Cin), -1, 1, g).to(torch.float16).to(cuda)
     dy = int_operands((rows, Cout), -1, 1, g).to(torch.float16).to(cuda)
-    dw = torch.empty((Cout, Cin), dtype=torch.float32, device=cuda)
-    nbytes = ctypes.c_size_t(0)
-    check(lib().pcnn_conv_wgrad_workspace_bytes(1, 1, rows, Cin, Cout, 1, ctypes.byref(nbytes)))
-    ws = workspace("wgrad", nbytes.value, cuda)
-    check(lib().pcnn_fc_wgrad_f16_tc(ptr(x), ptr(dy), rows, Cin, Cout, 0.25, ptr(None), 0.0, ptr(dw), ptr(ws), ws.numel(), stream()))
+    dw = pose_head.fc_wgrad(x, dy, 0.25)
     want = (dy.double().t() @ x.double()).float() * 0.25
     torch.cuda.synchronize()
     bad = dw != want

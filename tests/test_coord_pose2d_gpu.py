@@ -119,7 +119,7 @@ def test_per_hypothesis_counts_against_oracle(cuda):
 
 
 def test_lowres_source_bit_identical_to_dense(cuda):
-    from posecnn_b200._lib import check, lib, ptr, stream
+    from posecnn_b200 import heads
     B, C = 2, 22
     sc = scene(B, C, 13)
     h, w = 60, 80
@@ -128,10 +128,7 @@ def test_lowres_source_bit_identical_to_dense(cuda):
     lr = torch.from_numpy(lowres).to(cuda)
     bv = torch.full((3 * C,), 0.01, device=cuda)
     bs = torch.zeros(C, device=cuda)
-    dense = torch.empty((B, 480, 640, 3 * C), device=cuda)
-    lab, prob, score = (torch.empty((B, 480, 640), dtype=torch.int32, device=cuda), torch.empty((B, 480, 640, C), device=cuda),
-                        torch.empty((B, 480, 640, C), device=cuda))
-    check(lib().pcnn_up8_heads(ptr(lr), ptr(bs), ptr(bv), B, h, w, C, ptr(lab), ptr(dense), ptr(prob), ptr(score), stream()))
+    dense = heads.up8_heads(lr, bs, bv, vertex=True, prob=True, score=True)[1]
     a = run(sc, cuda, KEYS, trace=True, src=dict(vertex=dense))
     b = run(sc, cuda, KEYS, trace=True, src=dict(lowres=lr, bias_vertex=bv))
     for k in a:

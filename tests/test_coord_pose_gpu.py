@@ -6,8 +6,7 @@ import numpy as np
 import pytest
 import torch
 
-from posecnn_b200 import synth
-from posecnn_b200._lib import check, lib, ptr, stream
+from posecnn_b200 import heads, synth
 from posecnn_b200.coord_pose import CoordPoseEstimator, estimate_poses_3d
 from tests import coord_pose_ref as ref
 from tests.test_coord_pose_cpu import PLANTED_ROT_DEG, PLANTED_TRANS_M, rot_err_deg
@@ -86,10 +85,7 @@ def test_lowres_source_bit_identical_to_dense(cuda):
     lr = torch.from_numpy(lowres).to(cuda)
     bv = torch.full((3 * C,), 0.01, device=cuda)
     bs = torch.zeros(C, device=cuda)
-    dense = torch.empty((B, 480, 640, 3 * C), device=cuda)
-    lab, prob, score = (torch.empty((B, 480, 640), dtype=torch.int32, device=cuda), torch.empty((B, 480, 640, C), device=cuda),
-                        torch.empty((B, 480, 640, C), device=cuda))
-    check(lib().pcnn_up8_heads(ptr(lr), ptr(bs), ptr(bv), B, h, w, C, ptr(lab), ptr(dense), ptr(prob), ptr(score), stream()))
+    dense = heads.up8_heads(lr, bs, bv, vertex=True, prob=True, score=True)[1]
     a = run(sc, cuda, KEYS, trace=True, src=dict(vertex=dense))
     b = run(sc, cuda, KEYS, trace=True, src=dict(lowres=lr, bias_vertex=bv))
     for k in a:

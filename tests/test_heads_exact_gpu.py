@@ -8,8 +8,6 @@ errors.  Kernel-vs-reference comparisons are by value (+0 == -0); kernel-vs-kern
 pattern.  Each test prints the launch plan it covered and asserts that coverage.
 The rel-L2 tests of the same kernels (test_backward_gpu.py, test_network_gpu.py, ...) stay: they cover random-float
 rounding, a different question."""
-import ctypes
-
 import pytest
 import torch
 
@@ -35,25 +33,6 @@ def bf16(ref):
 # ---------------------------------------------------------------------------------------------------------------------
 # 1. the up-sampling adjoint of both losses (k_up8_bwd_strip + k_sum_partials)
 # ---------------------------------------------------------------------------------------------------------------------
-def _up8_bwd(P, sigma, thr, Cv):
-    from posecnn_b200._lib import check, lib, ptr, stream
-    B, h, w, C = P["B"], P["h"], P["w"], P["C"]
-    dev = P["prob"].device
-    d_sc = torch.full((B, h, w, 64), 7.0, dtype=torch.bfloat16, device=dev)          # padding channels must be written as 0
-    d_vt = torch.full((B, h, w, Cv), 7.0, dtype=torch.bfloat16, device=dev)
-    dbias = torch.full((4 * C,), 7.0, device=dev)
-    cls_out = torch.tensor([0.5, P["count"]], device=dev)
-    vtx_out = torch.tensor([0.25, P["sumw"]], device=dev)
-    nbytes = ctypes.c_size_t(0)
-    check(lib().pcnn_up8_heads_bwd_workspace_bytes(B, h, w, C, ctypes.byref(nbytes)))
-    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
-    vm, ext = (P["vertmap"], P["extents"]) if P["coord"] else (None, None)
-    check(lib().pcnn_up8_heads_bwd(ptr(P["prob"]), ptr(P["score"]), ptr(P["gt"]), ptr(cls_out), P["up_cls"], thr, ptr(P["lowres"]),
-                                   ptr(P["bias_v"]), ptr(P["centers"]), ptr(vm), ptr(ext), ptr(vtx_out), P["up_vtx"], P["w_inside"], sigma, B,
-                                   h, w, C, 64, Cv, ptr(d_sc), ptr(d_vt), ptr(dbias), ptr(ws), ws.numel(), stream()))
-    return d_sc, d_vt, dbias
-
-
 @pytest.mark.parametrize("coord", [False, True], ids=["2d", "3d"])
 @pytest.mark.parametrize("h,w", [(60, 80), (37, 27)])
 @pytest.mark.parametrize("C", [2, 6, 12, 22, 50])
@@ -78,8 +57,8 @@ def test_up8_bwd_exact(cuda, C, h, w, coord):
         assert bool((bg & (p0 < thr)).any() and (bg & (p0 == thr)).any() and (bg & (p0 == thr - 0.125)).any())
         ref = R.up8_bwd(P, sigma, thr, 2.0 ** -10)
         print(f"  sigma={sigma} threshold={thr}: bit budget {ref['budget']:.0f} of 2^24")
-        e_sc, e_vt, ebias = _up8_bwd(P, sigma, thr, Cv)
-        again = _up8_bwd(P, sigma, thr, Cv)
+        e_sc, e_vt, ebias = R.run_up8_bwd(P, sigma, thr, Cv)
+        again = R.run_up8_bwd(P, sigma, thr, Cv)
         torch.cuda.synchronize()
         for a, b in zip((e_sc, e_vt, ebias), again):
             assert torch.equal(bits(a), bits(b)), "two launches differ"
@@ -98,7 +77,7 @@ def test_up8_bwd_exact(cuda, C, h, w, coord):
 def test_add_up2_and_adjoint_exact(cuda, C, h, w):
     """pcnn_add_up2_bf16 / pcnn_up2_bwd_bf16 at conv4 60 x 80 (conv5 30 x 40) and 62 x 82 (odd conv5 grid 31 x 41) on small
     integers, batches chosen so that the grid-stride loop runs at least twice; masks with exact zeros (the test is y5 > 0)."""
-    from posecnn_b200._lib import check, lib, ptr, stream
+    from posecnn_b200 import heads
     g = torch.Generator().manual_seed(C + h)
     Bf, pf = R.ew_batch_for_coverage(h * w * C // 8)
     Bb, pb = R.ew_batch_for_coverage((h // 2) * (w // 2) * C // 8)
@@ -108,16 +87,14 @@ def test_add_up2_and_adjoint_exact(cuda, C, h, w):
     # operands stay referenced while the kernels run: a temporary's block could be handed to the next allocation
     a4 = R.dyadic((Bf, h, w, C), -3, 3, 1, g).to(cuda).bfloat16()
     a5 = R.dyadic((Bf, h // 2, w // 2, C), -3, 3, 1, g).to(cuda).bfloat16()
-    out = torch.empty((Bf, h, w, C), dtype=torch.bfloat16, device=cuda)
-    check(lib().pcnn_add_up2_bf16(ptr(a4), ptr(a5), Bf, h, w, C, ptr(out), stream()))
+    out = heads.add_up2(a4, a5)
     ref, budget = R.add_up2(a4, a5, 1.0)
     assert_same(out, bf16(ref), "add_up2")
     dadd = R.dyadic((Bb, h, w, C), -3, 3, 1, g).to(cuda).bfloat16()
     y5 = R.dyadic((Bb, h // 2, w // 2, C), -1, 1, 1, g).to(cuda).bfloat16()
     assert bool((y5 == 0).any())
-    d5 = torch.empty((Bb, h // 2, w // 2, C), dtype=torch.bfloat16, device=cuda)
     for mask in (y5, None):
-        check(lib().pcnn_up2_bwd_bf16(ptr(dadd), ptr(mask), Bb, h, w, C, ptr(d5), stream()))
+        d5 = heads.up2_bwd(dadd, mask)
         ref5, b5 = R.up2_bwd(dadd, mask, 1.0)
         assert_same(d5, bf16(ref5), "up2_bwd" + (" (masked)" if mask is not None else ""))
     print(f"  bit budgets {budget:.0f}, {b5:.0f} of 2^24")
@@ -126,7 +103,7 @@ def test_add_up2_and_adjoint_exact(cuda, C, h, w):
 @pytest.mark.parametrize("C", [2, 22, 50])
 def test_pack_lowres_exact(cuda, C):
     """pcnn_pack_lowres: an exact copy of the first C score channels (stride 64) and 3C vertex channels (stride Cv)."""
-    from posecnn_b200._lib import check, lib, ptr, stream
+    from posecnn_b200 import heads
     h, w, Cs, Cv = 60, 80, 64, R.vertex_stride(C)
     B, plan = R.ew_batch_for_coverage(h * w * 4 * C)
     print(f"C={C} Cv={Cv}: B={B}, {plan['total']} floats on {plan['blocks']} blocks, {plan['iters']} grid-stride iterations")
@@ -134,8 +111,7 @@ def test_pack_lowres_exact(cuda, C):
     g = torch.Generator().manual_seed(C)
     sc = torch.randn(B, h, w, Cs, generator=g).to(torch.bfloat16).to(cuda)
     vt = torch.randn(B, h, w, Cv, generator=g).to(torch.bfloat16).to(cuda)
-    out = torch.full((B, h, w, 4 * C), 7.0, device=cuda)
-    check(lib().pcnn_pack_lowres(ptr(sc), Cs, ptr(vt), Cv, B, h, w, C, ptr(out), stream()))
+    out = heads.pack_lowres(sc, vt, C)
     assert torch.equal(bits(out), bits(R.pack_lowres(sc, vt, C).float()))
 
 
@@ -151,7 +127,7 @@ def test_lowres_heads_exact(cuda, C, folded, h, w):
     """pcnn_lowres_heads at 60 x 80 and 62 x 82 (B h w not a multiple of 8), batches chosen so that warps take at least two
     8-pixel groups (block caps kNumSMs x 2 unfolded, x 8 folded).  Unfolded C = 50 runs four full vertex passes and three
     tail passes.  Folded mode needs 3C <= Cv = 128, so its largest class count is 42."""
-    from posecnn_b200._lib import check, lib, ptr, stream
+    from posecnn_b200 import heads
     Cs, Cv = 64, 128
     B = 15 if folded else (4 if (h, w) == (60, 80) else 5)
     plan = R.lowres_heads_plan(B, h, w, C, Cs, Cv, folded)
@@ -166,8 +142,7 @@ def test_lowres_heads_exact(cuda, C, folded, h, w):
     Ws = R.dyadic((Cs, C), -2, 2, 0.125, g).to(cuda)
     Wv = None if folded else R.dyadic((Cv, 3 * C), -2, 2, 0.125, g).to(cuda)
     s4, s5, v4, v5 = (t.to(cuda).bfloat16() for t in (s4, s5, v4, v5))
-    out = torch.full((B, h, w, 4 * C), 7.0, device=cuda)
-    check(lib().pcnn_lowres_heads(ptr(s4), ptr(s5), ptr(v4), ptr(v5), ptr(Ws), ptr(Wv), B, h, w, Cs, Cv, C, ptr(out), stream()))
+    out = heads.lowres_heads(s4, s5, v4, v5, Ws, Wv, C)
     ref, budget = R.lowres_heads(s4, s5, v4, v5, Ws, Wv, C, 1.0, 0.125)
     print(f"  bit budget {budget:.0f} of 2^24")
     assert_same(out, ref.float(), "lowres_heads")
@@ -181,7 +156,7 @@ def test_up8_heads_exact(cuda, C):
     """pcnn_up8_heads at 480 x 640, B = 2: vertex and score exact, label the first-index arg-max (exact ties from coarse
     scores and all-class ties from ReLU zeros), prob within the softmax bound; the label-only call (k_up8_label, or at
     C = 64, where 11 w C floats exceed its shared memory, k_up8_heads without outputs) gives the same labels."""
-    from posecnn_b200._lib import check, lib, ptr, stream
+    from posecnn_b200 import heads
     B, h, w = 2, 60, 80
     H, W = 8 * h, 8 * w
     full, lab = R.up8_heads_plan(B, h, w, C), R.up8_heads_plan(B, h, w, C, label_only=True)
@@ -197,12 +172,9 @@ def test_up8_heads_exact(cuda, C):
     bv = R.dyadic((3 * C,), -1, 1, 0.125, g)
     lowres, bs, bv = lowres.to(cuda), bs.to(cuda), bv.to(cuda)
     label = torch.full((B, H, W), -7, dtype=torch.int32, device=cuda)
-    vertex = torch.empty((B, H, W, 3 * C), device=cuda)
-    prob = torch.empty((B, H, W, C), device=cuda)
-    score = torch.empty((B, H, W, C), device=cuda)
-    check(lib().pcnn_up8_heads(ptr(lowres), ptr(bs), ptr(bv), B, h, w, C, ptr(label), ptr(vertex), ptr(prob), ptr(score), stream()))
-    label2 = torch.full((B, H, W), -7, dtype=torch.int32, device=cuda)
-    check(lib().pcnn_up8_heads(ptr(lowres), ptr(bs), ptr(bv), B, h, w, C, ptr(label2), ptr(None), ptr(None), ptr(None), stream()))
+    _, vertex, prob, score = heads.up8_heads(lowres, bs, bv, out=(label, torch.empty((B, H, W, 3 * C), device=cuda),
+                                                                  torch.empty((B, H, W, C), device=cuda), torch.empty((B, H, W, C), device=cuda)))
+    label2 = heads.up8_heads(lowres, bs, bv, out=(torch.full((B, H, W), -7, dtype=torch.int32, device=cuda), None, None, None))[0]
     ref = R.up8_heads(lowres, bs, bv, C, 0.125)
     print(f"  bit budget {ref['budget']:.0f} of 2^24")
     assert_same(vertex, ref["vertex"].float(), "vertex")

@@ -168,7 +168,7 @@ def _lowres_from_scenes(sc, B, C, seed=11):
 
 
 def test_lowres_source_batch32(cuda):
-    from posecnn_b200._lib import check, lib, ptr, stream
+    from posecnn_b200 import heads
     op = _op()
     sc = HR.bench_scenes()
     B, C = 32, 22
@@ -179,12 +179,8 @@ def test_lowres_source_batch32(cuda):
     lab = torch.from_numpy(sc32["label"]).to(cuda)
     ext = torch.from_numpy(sc32["extents"]).to(cuda)
     meta = torch.from_numpy(np.ascontiguousarray(sc32["meta"])).to(cuda)
-    scratch = torch.empty((B, H, W), dtype=torch.int32, device=cuda)
-    dense = torch.empty((B, H, W, 3 * C), device=cuda)
     zero_bias = torch.zeros(C, device=cuda)
-    check(lib().pcnn_up8_heads(ptr(lowres), ptr(zero_bias), ptr(bias), B, H // 8, W // 8, C, ptr(scratch), ptr(dense), ptr(None),
-                               ptr(None), stream()))
-    del scratch
+    dense = heads.up8_heads(lowres, zero_bias, bias, vertex=True)[1]
     full = op.hough_voting_gpu_capacity(lab, dense, ext, meta, None, 0, -1.0, 0.02, 10)
     low = op.hough_voting_gpu_capacity(lab, None, ext, meta, None, 0, -1.0, 0.02, 10, lowres=lowres, bias_vertex=bias)
     names = ("box", "pose", "target", "weight", "domain", "num_rois", "status")

@@ -130,7 +130,7 @@ def test_rgbd_two_trunk_network(cuda):
 def test_lowres_heads_kernel(cuda, C):
     """pcnn_lowres_heads alone (register-tiled column map: full vertex passes, then score columns next to split
     left-over vertex columns) against torch fp32: add = conv4 branch + up2(conv5 branch), then the two 1x1 matrices."""
-    from posecnn_b200._lib import lib, check, ptr, stream
+    from posecnn_b200 import heads
     g = torch.Generator(device="cpu").manual_seed(C)
     B, h, w, Cs, Cv = 2, 6, 10, 64, 128      # 120 pixels: 15 groups of 8; also run a ragged count below
     for (hh, ww) in ((h, w), (2, 6)):         # 24 px = 3 groups; B*hh*ww not a multiple of 8 when B = 1
@@ -139,8 +139,7 @@ def test_lowres_heads_kernel(cuda, C):
             s4, s5 = mk(Bn, hh, ww, Cs).bfloat16(), mk(Bn, hh // 2, ww // 2, Cs).bfloat16()
             v4, v5 = mk(Bn, hh, ww, Cv).bfloat16(), mk(Bn, hh // 2, ww // 2, Cv).bfloat16()
             Ws, Wv = mk(Cs, C) * 0.1, mk(Cv, 3 * C) * 0.1
-            out = torch.empty((Bn, hh, ww, 4 * C), dtype=torch.float32, device=cuda)
-            check(lib().pcnn_lowres_heads(ptr(s4), ptr(s5), ptr(v4), ptr(v5), ptr(Ws), ptr(Wv), Bn, hh, ww, Cs, Cv, C, ptr(out), stream()))
+            out = heads.lowres_heads(s4, s5, v4, v5, Ws, Wv, C)
             nchw = lambda t: t.float().permute(0, 3, 1, 2)
             add_s = nchw(s4) + R.deconv(nchw(s5), 4, 2)
             add_v = nchw(v4) + R.deconv(nchw(v5), 4, 2)
@@ -178,17 +177,12 @@ def test_folded_vertex_head(cuda, C):
 def test_up8_heads_kernel(cuda, C):
     """pcnn_up8_heads alone (C = 22 is the compile-time-stride specialisation) against the dense transposed
     convolution of the reference graph: bilinear x8 of the low-resolution maps, + bias, ReLU / arg-max / softmax."""
-    from posecnn_b200._lib import lib, check, ptr, stream
+    from posecnn_b200 import heads
     g = torch.Generator(device="cpu").manual_seed(100 + C)
     B, h, w = 2, 5, 23                           # 23 cells: one full 20-cell segment + a ragged one
     lowres = torch.randn(B, h, w, 4 * C, generator=g).to(cuda)
     bs, bv = torch.randn(C, generator=g).to(cuda), torch.randn(3 * C, generator=g).to(cuda)
-    H, W = 8 * h, 8 * w
-    label = torch.empty((B, H, W), dtype=torch.int32, device=cuda)
-    vertex = torch.empty((B, H, W, 3 * C), dtype=torch.float32, device=cuda)
-    prob = torch.empty((B, H, W, C), dtype=torch.float32, device=cuda)
-    score = torch.empty((B, H, W, C), dtype=torch.float32, device=cuda)
-    check(lib().pcnn_up8_heads(ptr(lowres), ptr(bs), ptr(bv), B, h, w, C, ptr(label), ptr(vertex), ptr(prob), ptr(score), stream()))
+    label, vertex, prob, score = heads.up8_heads(lowres, bs, bv, vertex=True, prob=True, score=True)
     up = R.deconv(lowres.permute(0, 3, 1, 2), 16, 8).permute(0, 2, 3, 1)
     want_s = torch.relu(up[..., :C] + bs)
     want_v = up[..., C:] + bv

@@ -96,11 +96,11 @@ def test_average_distance_realistic_bound(cuda):
 # 3. the pose chain
 # ---------------------------------------------------------------------------------------------------------------------
 def _chain(P, upstream, cuda, ld):
-    from posecnn_b200._lib import check, lib, ptr, stream
-    N, D = P["g"].shape
+    from posecnn_b200 import pose_head
+    N = P["g"].shape[0]
     g, t, w = (P[k].to(cuda).contiguous() for k in ("g", "tanh", "w"))
     out = torch.full((N, ld), 7.0, dtype=torch.float16, device=cuda)          # padding columns must be written as 0
-    check(lib().pcnn_pose_chain_bwd(ptr(g), ptr(t), ptr(w), N, D, upstream, ptr(out), ld, stream()))
+    pose_head.pose_chain_bwd(g, t, w, upstream, out)
     torch.cuda.synchronize()
     return out.cpu()
 

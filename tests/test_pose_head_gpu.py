@@ -199,8 +199,7 @@ def test_fc_exact_at_head_shapes(cuda, layer, K, N, M):
 def test_fc_dgrad_exact_at_fc6(cuda, M):
     """pcnn_fc_dgrad_f16_tc at fc6 (N = 25,088 input features, K = 4096) with the ReLU mask of the stored pooled features:
     out = (dy @ W^T) * [mask > 0], exact against the float64 product."""
-    import ctypes
-    from posecnn_b200._lib import check, lib, ptr, stream, workspace
+    from posecnn_b200 import pose_head
     from tests.util import fc_plan, int_operands
     N, K = 25088, 4096
     g = torch.Generator().manual_seed(M + 1)
@@ -209,11 +208,7 @@ def test_fc_dgrad_exact_at_fc6(cuda, M):
     mask = int_operands((M, N), -1, 1, g).to(torch.float16).to(cuda)
     plan = fc_plan(M, N, K)
     print(f"fc6 dgrad M={M}: {plan['splits']} splits x {plan['chunks_per_split']} K chunks")
-    out = torch.empty((M, N), dtype=torch.float16, device=cuda)
-    nbytes = ctypes.c_size_t(0)
-    check(lib().pcnn_fc_workspace_bytes(M, N, K, ctypes.byref(nbytes)))
-    ws = workspace("fc", nbytes.value, cuda)
-    check(lib().pcnn_fc_dgrad_f16_tc(ptr(dy), ptr(wt), M, N, K, ptr(mask), ptr(out), N, ptr(ws), ws.numel(), stream()))
+    out = pose_head.fc_dgrad(dy, wt, mask)
     want = ((dy.double() @ wt.double().t()) * (mask > 0)).float().to(torch.float16)
     torch.cuda.synchronize()
     assert torch.equal(out, want), int((out != want).sum())

@@ -2,7 +2,6 @@
 two-class kernel, the network's forward at 480 x 640, Hough voting in train mode, the training step with and without pose_reg,
 the domain branch and two ranks.  Every comparison is against the same references and within the same stated limits as the
 C = 6 / 22 tests (tests/train_ref.py, oracle/ref_network.py, the C oracle); every measured error is printed."""
-import ctypes
 
 import numpy as np
 import pytest
@@ -52,15 +51,12 @@ def make_net2(cuda, pose_reg=True, adaptation=False, threshold_label=0.7, is_tra
 def _up8_problem(cuda, B, h, w, seed):
     """Low-resolution head tensor, its dense up-sampling, labels with ignore / background / object pixels; image 0 lists the
     object's centre, image 1 does not (z = 0)."""
-    from posecnn_b200._lib import check, lib, ptr, stream
+    from posecnn_b200 import heads
     g = torch.Generator().manual_seed(seed)
     H, W = 8 * h, 8 * w
     lowres = (torch.randn(B, h, w, 4 * C, generator=g) * 0.7).to(cuda)
     bs, bv = (torch.randn(C, generator=g) * 0.1).to(cuda), (torch.randn(3 * C, generator=g) * 0.1).to(cuda)
-    vertex = torch.empty((B, H, W, 3 * C), device=cuda)
-    label = torch.empty((B, H, W), dtype=torch.int32, device=cuda)
-    prob, score = torch.empty((B, H, W, C), device=cuda), torch.empty((B, H, W, C), device=cuda)
-    check(lib().pcnn_up8_heads(ptr(lowres), ptr(bs), ptr(bv), B, h, w, C, ptr(label), ptr(vertex), ptr(prob), ptr(score), stream()))
+    _, vertex, prob, score = heads.up8_heads(lowres, bs, bv, vertex=True, prob=True, score=True)
     gt = torch.randint(-1, C, (B, H, W), generator=g).to(torch.int32)
     gt[:, : H // 3] = 0
     gt[:, H // 3: H // 2, : W // 2] = 1
@@ -70,20 +66,14 @@ def _up8_problem(cuda, B, h, w, seed):
 
 
 def _up8_bwd(P, thr, up_vtx=2.0, w_in=10.0, count=937.0, sumw=411.0):
-    from posecnn_b200._lib import check, lib, ptr, stream
+    from posecnn_b200 import heads
     B, h, w = P["B"], P["h"], P["w"]
     dev = P["lowres"].device
-    d_sc = torch.full((B, h, w, 64), 7.0, dtype=torch.bfloat16, device=dev)             # padding channels must be written as 0
-    d_vt = torch.full((B, h, w, 128), 7.0, dtype=torch.bfloat16, device=dev)
-    dbias = torch.empty((4 * C,), device=dev)
+    out = (torch.full((B, h, w, 64), 7.0, dtype=torch.bfloat16, device=dev),             # padding channels must be written as 0
+           torch.full((B, h, w, 128), 7.0, dtype=torch.bfloat16, device=dev), torch.empty((4 * C,), device=dev))
     cls_out, vtx_out = torch.tensor([0.5, count], device=dev), torch.tensor([0.25, sumw], device=dev)
-    nbytes = ctypes.c_size_t(0)
-    check(lib().pcnn_up8_heads_bwd_workspace_bytes(B, h, w, C, ctypes.byref(nbytes)))
-    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
-    check(lib().pcnn_up8_heads_bwd(ptr(P["prob"]), ptr(P["score"]), ptr(P["gt"]), ptr(cls_out), 1.0, thr, ptr(P["lowres"]), ptr(P["bv"]),
-                                   ptr(P["centers"]), ptr(None), ptr(None), ptr(vtx_out), up_vtx, w_in, 1.0, B, h, w, C, 64, 128, ptr(d_sc),
-                                   ptr(d_vt), ptr(dbias), ptr(ws), ws.numel(), stream()))
-    return d_sc, d_vt, dbias
+    return heads.up8_heads_bwd(P["prob"], P["score"], P["gt"], cls_out, 1.0, thr, P["lowres"], P["bv"], P["centers"], vtx_out, up_vtx, w_in,
+                               1.0, out=out)
 
 
 @pytest.mark.parametrize("thr", [1.0, 0.7])

@@ -2,7 +2,6 @@
 the fused tail kernel, fc9's GEMMs at their shapes, the merge that applies the gradient reversal, the training step against torch
 fp32 autograd with the reversal restated as an autograd Function (identity forward, -lambda backward), invariants against the
 step without the branch, the dummy Hough row, inference and CUDA-graph capture, and two ranks."""
-import ctypes
 
 import numpy as np
 import pytest
@@ -108,7 +107,6 @@ def test_fc9_exact(cuda, M):
     K chunks; the input gradient's K = 256 is four 64-wide chunks, all of which every item runs; the weight gradient's items
     run >= 8 of its 64-row K tiles where the rows hold that many (M = 128 has 2)."""
     from posecnn_b200 import pose_head
-    from posecnn_b200._lib import check, lib, ptr, stream, workspace
     from tests.util import fc_plan, int_operands, wgrad_plan
     K, N = 25088, 256
     g = torch.Generator().manual_seed(M + 9)
@@ -132,18 +130,11 @@ def test_fc9_exact(cuda, M):
     # input gradient: dy [M,256] against the [25088][256] transposed copy, no mask (pool_score has none)
     dy = int_operands((M, N), -1, 1, g).to(torch.float16).to(cuda)
     wt = w_tc.t().contiguous()
-    dx = torch.empty((M, K), dtype=torch.float16, device=cuda)
-    nbytes = ctypes.c_size_t(0)
-    check(lib().pcnn_fc_workspace_bytes(M, K, N, ctypes.byref(nbytes)))
-    ws = workspace("fc", nbytes.value, cuda)
-    check(lib().pcnn_fc_dgrad_f16_tc(ptr(dy), ptr(wt), M, K, N, ptr(None), ptr(dx), K, ptr(ws), ws.numel(), stream()))
+    dx = pose_head.fc_dgrad(dy, wt, None)
     torch.cuda.synchronize()
     assert torch.equal(bits(dx), bits((dy.double() @ wt.double().t()).float().to(torch.float16)))
     # weight gradient [256][25088] with a power-of-two scale
-    dw = torch.empty((N, K), dtype=torch.float32, device=cuda)
-    check(lib().pcnn_conv_wgrad_workspace_bytes(1, 1, M, K, N, 1, ctypes.byref(nbytes)))
-    ws = workspace("wgrad", nbytes.value, cuda)
-    check(lib().pcnn_fc_wgrad_f16_tc(ptr(pool), ptr(dy), M, K, N, 0.25, ptr(None), 0.0, ptr(dw), ptr(ws), ws.numel(), stream()))
+    dw = pose_head.fc_wgrad(pool, dy, 0.25)
     torch.cuda.synchronize()
     want = (dy.double().t() @ pool.double()).float() * 0.25
     bad = dw != want
@@ -158,7 +149,6 @@ def test_domain_grad_merge_bit_exact(cuda, rows):
     """dst = (s_a * a) + (s_b * b) in float32, each product rounded: bit-exact against numpy; with b = 0 it is
     pcnn_half_to_float(a, s_a) bit for bit (signed zeros included)."""
     from posecnn_b200 import pose_head
-    from posecnn_b200._lib import check, lib, ptr, stream
     g = torch.Generator().manual_seed(rows)
     n = rows * 25088
     a = (torch.randn(n, generator=g) * torch.exp2(torch.randint(-20, 12, (n,), generator=g).float())).to(torch.float16)
@@ -174,8 +164,7 @@ def test_domain_grad_merge_bit_exact(cuda, rows):
     assert np.array_equal(got.cpu().numpy().reshape(-1).view(np.int32), want.view(np.int32))
     ad = a.to(cuda)
     zero = pose_head.domain_grad_merge(ad, sa, torch.zeros_like(ad), sb, (rows, 7, 7, 512))
-    h2f = torch.empty(n, dtype=torch.float32, device=cuda)
-    check(lib().pcnn_half_to_float(ptr(ad), n, sa, ptr(h2f), stream()))
+    h2f = pose_head.half_to_float(ad, sa)
     torch.cuda.synchronize()
     assert torch.equal(bits(zero.reshape(-1)), bits(h2f))
 

@@ -3,7 +3,6 @@ loss (1/8-resolution source) against the oracle's smooth_l1_loss_vertex on the 3
 against torch, the training step against the autograd graph, its contents, a short training run whose weights then estimate poses
 on an inference network, and two ranks.  Every measured error is printed."""
 
-import ctypes
 
 import numpy as np
 import pytest
@@ -84,16 +83,13 @@ def test_coord_loss_vertex_against_oracle(cuda, C):
     bit-identical, loss within 1e-6 relative.  That bound is the one the fused kernel was held to against smooth L1 on the
     materialised blobs: vertex values and targets are bit-identical, each term is the same fp32 expression, and the float64 sums
     differ only in order, so the quotient's fp32 rounding (2^-24 relative) dominates."""
-    from posecnn_b200 import train_ops
-    from posecnn_b200._lib import check, lib, ptr, stream
+    from posecnn_b200 import heads, train_ops
     B, H, W = 2, 240, 320
     sc, cen = coord_scene(B, H, W, C, seed=31)
     g = torch.Generator().manual_seed(C)
     lowres = (torch.randn(B, H // 8, W // 8, 4 * C, generator=g) * 0.5).to(cuda)
     bs, bv = torch.zeros(C, device=cuda), (torch.randn(3 * C, generator=g) * 0.1 + 0.5).to(cuda)
-    label = torch.empty((B, H, W), dtype=torch.int32, device=cuda)
-    vertex = torch.empty((B, H, W, 3 * C), device=cuda)
-    check(lib().pcnn_up8_heads(ptr(lowres), ptr(bs), ptr(bv), B, H // 8, W // 8, C, ptr(label), ptr(vertex), ptr(None), ptr(None), stream()))
+    vertex = heads.up8_heads(lowres, bs, bv, vertex=True)[1]
     vp = vertex.cpu().numpy()
     vt, vw = vertex_targets_3d(sc["label"], sc["coords"], cen, sc["extents"], 10.0)
     lab, vm, cn, ext = T(sc["label"], cuda), T(sc["coords"], cuda), T(cen, cuda), T(sc["extents"], cuda)
@@ -115,15 +111,12 @@ def test_coord_loss_vertex_against_oracle(cuda, C):
 # 3. the up-sampling adjoint's 3-D mode
 # ---------------------------------------------------------------------------------------------------------------------
 def _up8_problem(cuda, B, h, w, C, seed):
-    from posecnn_b200._lib import check, lib, ptr, stream
+    from posecnn_b200 import heads
     g = torch.Generator().manual_seed(seed)
     H, W = 8 * h, 8 * w
     lowres = (torch.randn(B, h, w, 4 * C, generator=g) * 0.7).to(cuda)
     bs, bv = (torch.randn(C, generator=g) * 0.1).to(cuda), (torch.randn(3 * C, generator=g) * 0.1 + 0.5).to(cuda)
-    vertex = torch.empty((B, H, W, 3 * C), device=cuda)
-    label = torch.empty((B, H, W), dtype=torch.int32, device=cuda)
-    prob, score = torch.empty((B, H, W, C), device=cuda), torch.empty((B, H, W, C), device=cuda)
-    check(lib().pcnn_up8_heads(ptr(lowres), ptr(bs), ptr(bv), B, h, w, C, ptr(label), ptr(vertex), ptr(prob), ptr(score), stream()))
+    _, vertex, prob, score = heads.up8_heads(lowres, bs, bv, vertex=True, prob=True, score=True)
     gt = torch.randint(-1, C, (B, H, W), generator=g).to(torch.int32)
     gt[:, : H // 4] = 0
     gt[:, H // 4: H // 2, : W // 2] = 1 if C == 2 else 2
@@ -139,21 +132,15 @@ def _up8_problem(cuda, B, h, w, C, seed):
 
 
 def _up8_bwd(P, coord, thr=0.7, up_vtx=2.0, w_in=10.0, count=937.0, sumw=411.0):
-    from posecnn_b200._lib import check, lib, ptr, stream
+    from posecnn_b200 import heads
     B, h, w, C = P["B"], P["h"], P["w"], P["C"]
     dev = P["lowres"].device
-    d_sc = torch.full((B, h, w, 64), 7.0, dtype=torch.bfloat16, device=dev)             # padding channels must be written as 0
-    d_vt = torch.full((B, h, w, 128), 7.0, dtype=torch.bfloat16, device=dev)
-    dbias = torch.empty((4 * C,), device=dev)
+    out = (torch.full((B, h, w, 64), 7.0, dtype=torch.bfloat16, device=dev),             # padding channels must be written as 0
+           torch.full((B, h, w, 128), 7.0, dtype=torch.bfloat16, device=dev), torch.empty((4 * C,), device=dev))
     cls_out, vtx_out = torch.tensor([0.5, count], device=dev), torch.tensor([0.25, sumw], device=dev)
-    nbytes = ctypes.c_size_t(0)
-    check(lib().pcnn_up8_heads_bwd_workspace_bytes(B, h, w, C, ctypes.byref(nbytes)))
-    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
     vm, ext = (P["vertmap"], P["ext"]) if coord else (None, None)
-    check(lib().pcnn_up8_heads_bwd(ptr(P["prob"]), ptr(P["score"]), ptr(P["gt"]), ptr(cls_out), 1.0, thr, ptr(P["lowres"]), ptr(P["bv"]),
-                                   ptr(P["centers"]), ptr(vm), ptr(ext), ptr(vtx_out), up_vtx, w_in, 1.0, B, h, w, C, 64, 128, ptr(d_sc),
-                                   ptr(d_vt), ptr(dbias), ptr(ws), ws.numel(), stream()))
-    return d_sc, d_vt, dbias
+    return heads.up8_heads_bwd(P["prob"], P["score"], P["gt"], cls_out, 1.0, thr, P["lowres"], P["bv"], P["centers"], vtx_out, up_vtx, w_in,
+                               1.0, vertmap=vm, extents=ext, out=out)
 
 
 @pytest.mark.parametrize("C", [2, 6, 22])

@@ -14,7 +14,7 @@ def _bits(t):
 
 def _explicit_master(name, w, C, U):
     """The master layouts, restated: [Cout][kh*kw*Cin] convolutions (conv1_1 [64][27]), score / vertex_pred zero-padded to 64 /
-    128 rows, fc [out padded to x128][in], domain_score [2][256], biases as they are."""
+    max(128, 3C rounded up to a multiple of 64) rows, fc [out padded to x128][in], domain_score [2][256], biases as they are."""
     layer, kind = name.split("/")
     if kind == "b":
         return w
@@ -25,7 +25,7 @@ def _explicit_master(name, w, C, U):
     if layer in ("score_conv4", "score_conv5", "score_conv4_vertex", "score_conv5_vertex"):
         return w.reshape(w.shape[2], w.shape[3]).t()
     if layer in ("score", "vertex_pred"):
-        rows, n = (64, C) if layer == "score" else (128, 3 * C)
+        rows, n = (64, C) if layer == "score" else (max(128, -(-3 * C // 64) * 64), 3 * C)
         out = torch.zeros((rows, w.shape[2]))
         out[:n] = w.reshape(w.shape[2], n).t()
         return out
@@ -36,11 +36,12 @@ def _explicit_master(name, w, C, U):
     return out
 
 
+@pytest.mark.parametrize("num_classes", [6, 44, 50])
 @pytest.mark.parametrize("fmt,adaptation", [("COLOR", False), ("RGBD", False), ("COLOR", True)])
-def test_param_layout_round_trips_bit_for_bit(fmt, adaptation):
+def test_param_layout_round_trips_bit_for_bit(fmt, adaptation, num_classes):
     from posecnn_b200.networks.vgg16_convs import vgg16_convs
     from posecnn_b200.train import KINDS, param_layout
-    net = vgg16_convs(input_format=fmt, num_classes=6, device="cpu", is_train=True, fold_vertex_head=False, adaptation=adaptation)
+    net = vgg16_convs(input_format=fmt, num_classes=num_classes, device="cpu", is_train=True, fold_vertex_head=False, adaptation=adaptation)
     shapes = net.param_shapes()
     layout = param_layout(net)
     assert sorted(tf for tf, _, _ in layout.values()) == sorted(shapes)

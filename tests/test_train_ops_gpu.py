@@ -126,8 +126,7 @@ def test_loss_vertex_full_frame(cuda, sigma):
     one the fused kernel was held to against smooth L1 on the materialised blobs: the vertex values are bit-identical to the dense
     tensor's, the targets are the oracle's to 1 ulp of log z, each term is the same fp32 expression, and the float64 sums differ
     only in order, so the quotient's fp32 rounding (2^-24 relative) dominates."""
-    from posecnn_b200 import synth, train_ops
-    from posecnn_b200._lib import check, lib, ptr, stream
+    from posecnn_b200 import heads, synth, train_ops
     B, H, W, C = 2, 480, 640, 22
     sc = synth.make_scene(batch=B, height=H, width=W, num_classes=C, seed=77)
     label = sc["label"]
@@ -137,8 +136,7 @@ def test_loss_vertex_full_frame(cuda, sigma):
     g = torch.Generator().manual_seed(9)
     lowres = (torch.randn(B, H // 8, W // 8, 4 * C, generator=g) * 0.5).to(cuda)
     bs, bv = torch.zeros(C, device=cuda), (torch.randn(3 * C, generator=g) * 0.1).to(cuda)
-    label_net, vertex = torch.empty((B, H, W), dtype=torch.int32, device=cuda), torch.empty((B, H, W, 3 * C), device=cuda)
-    check(lib().pcnn_up8_heads(ptr(lowres), ptr(bs), ptr(bv), B, H // 8, W // 8, C, ptr(label_net), ptr(vertex), ptr(None), ptr(None), stream()))
+    vertex = heads.up8_heads(lowres, bs, bv, vertex=True)[1]
     vp = to_np(vertex)
     vt, vw = oracle.generate_vertex_targets(label, centers, 10.0)
     assert (label[0] == c0).any() and not vw[0, ..., 3 * c0:3 * c0 + 3].any()

@@ -12,7 +12,6 @@ The card name and power limit are read in the same run with a read-only nvidia-s
     python tools/bench_train_coord.py [--batch 64] [--steps 10] [--warmup 3] [--runs 3]
 """
 import argparse
-import ctypes
 import json
 import os
 import statistics
@@ -25,7 +24,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from bench_single_class import timed, timed_steps, two_class_inputs   # noqa: E402
 from bench_train_rgbd import H, W, gpu_info, make_inputs           # noqa: E402
-from posecnn_b200._lib import check, lib, ptr, stream        # noqa: E402
+from posecnn_b200 import heads                                     # noqa: E402
 from posecnn_b200.networks.vgg16_convs import vgg16_convs         # noqa: E402
 from posecnn_b200.train import Trainer                             # noqa: E402
 
@@ -53,21 +52,12 @@ def up8_problem(dev, B, C, gt, centers, vertmap, ext):
     g = torch.Generator().manual_seed(C)
     lowres = (torch.randn(B, h, w, 4 * C, generator=g) * 0.7).to(dev)
     bs, bv = (torch.randn(C, generator=g) * 0.1).to(dev), (torch.randn(3 * C, generator=g) * 0.1).to(dev)
-    label = torch.empty((B, H, W), dtype=torch.int32, device=dev)
-    prob, score = torch.empty((B, H, W, C), device=dev), torch.empty((B, H, W, C), device=dev)
-    check(lib().pcnn_up8_heads(ptr(lowres), ptr(bs), ptr(bv), B, h, w, C, ptr(label), ptr(None), ptr(prob), ptr(score), stream()))
+    _, _, prob, score = heads.up8_heads(lowres, bs, bv, prob=True, score=True)
     cls_out, vtx_out = torch.tensor([0.5, 1e5], device=dev), torch.tensor([0.5, 1e5], device=dev)
-    d_sc = torch.empty((B, h, w, 64), dtype=torch.bfloat16, device=dev)
-    d_vt = torch.empty((B, h, w, 128), dtype=torch.bfloat16, device=dev)
-    dbias = torch.empty((4 * C,), device=dev)
-    nbytes = ctypes.c_size_t(0)
-    check(lib().pcnn_up8_heads_bwd_workspace_bytes(B, h, w, C, ctypes.byref(nbytes)))
-    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+    out = heads.up8_heads_bwd(prob, score, gt, cls_out, 1.0, 0.7, lowres, bv, centers, vtx_out, 1.0, 10.0, 1.0)
 
-    def run(vm, ex):                                   # vertmap / extents NULL: the 2-D target
-        check(lib().pcnn_up8_heads_bwd(ptr(prob), ptr(score), ptr(gt), ptr(cls_out), 1.0, 0.7, ptr(lowres), ptr(bv), ptr(centers), ptr(vm),
-                                       ptr(ex), ptr(vtx_out), 1.0, 10.0, 1.0, B, h, w, C, 64, 128, ptr(d_sc), ptr(d_vt), ptr(dbias), ptr(ws),
-                                       ws.numel(), stream()))
+    def run(vm, ex):                                   # vertmap / extents None: the 2-D target
+        heads.up8_heads_bwd(prob, score, gt, cls_out, 1.0, 0.7, lowres, bv, centers, vtx_out, 1.0, 10.0, 1.0, vertmap=vm, extents=ex, out=out)
     return (lambda: run(None, None)), (lambda: run(vertmap, ext))
 
 
