@@ -243,12 +243,25 @@ int pcnn_add_to_bf16(const void* a_bf16, const void* b_bf16, const float* b_f32,
 int pcnn_add_up2_bf16(const void* a4_bf16, const void* a5_bf16, int B, int h, int w, int C, void* out_bf16, void* stream);
 int pcnn_up2_bwd_bf16(const void* dadd_bf16, const void* y5_bf16, int B, int h, int w, int C, void* d5_bf16, void* stream);
 int pcnn_pack_lowres(const void* sc_bf16, int Cs, const void* vt_bf16, int Cv, int B, int h, int w, int C, float* lowres, void* stream);
+/* pcnn_pack_lowres with the head tensor's vertex width explicit: num_vertex = 3C is pcnn_pack_lowres; num_vertex = 0 is the segmentation
+ * network's score-only head tensor [B,h,w,C] f32 from the first C channels of sc (vt_bf16 must be NULL, Cv is ignored). */
+int pcnn_pack_lowres_nv(const void* sc_bf16, int Cs, const void* vt_bf16, int Cv, int B, int h, int w, int C, int num_vertex, float* lowres,
+                        void* stream);
 int pcnn_up8_heads_bwd_workspace_bytes(int B, int h, int w, int C, size_t* bytes);
 int pcnn_up8_heads_bwd(const float* prob, const float* score, const int32_t* gt, const float* cls_loss_out, float upstream_cls,
                        float threshold, const float* lowres, const float* bias_vertex, const float* centers, const float* vertmap,
                        const float* extents, const float* vertex_loss_out, float upstream_vertex, float w_inside, float sigma, int B, int h,
                        int w, int C, int Cs, int Cv, void* d_sc_bf16, void* d_vt_bf16, float* dbias, void* workspace,
                        size_t workspace_bytes, void* stream);
+/* Target mode "none" of pcnn_up8_heads_bwd, the segmentation network's training step (vertex_reg_2d and vertex_reg_3d both off,
+ * vgg16_convs.py:79-149, loss = loss_cls + l2, train.py:518-521): the gradient of upstream_cls * loss_cls w.r.t. the score-only head
+ * tensor [B,h,w,C], d_sc [B,h,w,Cs] bf16 (channels past C zero) and dbias [C]; nothing of the vertex head is read or written.  Same C
+ * set as pcnn_up8_heads_bwd; d_sc and dbias are bit-identical to its 2-D mode's d_sc and dbias[:C] at upstream_vertex = 0.
+ * workspace: pcnn_up8_scores_bwd_workspace_bytes(B, h, w, C) (C floats per CTA) */
+int pcnn_up8_scores_bwd_workspace_bytes(int B, int h, int w, int C, size_t* bytes);
+int pcnn_up8_scores_bwd(const float* prob, const float* score, const int32_t* gt, const float* cls_loss_out, float upstream_cls,
+                        float threshold, int B, int h, int w, int C, int Cs, void* d_sc_bf16, float* dbias, void* workspace,
+                        size_t workspace_bytes, void* stream);
 int pcnn_pose_chain_bwd(const float* bottom_diff, const float* poses_tanh, const float* poses_weight, int N, int D, float upstream,
                         void* dpre_f16, int ld, void* stream);
 int pcnn_sgd_momentum(float* w, float* accum, const float* grad, size_t n, float lr, float mu, float wd, float gscale, void* copy16,
@@ -327,6 +340,16 @@ int pcnn_lowres_heads(const void* score4, const void* score5, const void* vert4,
  * consumer) */
 int pcnn_up8_heads(const float* lowres, const float* bias_score, const float* bias_vertex, int B, int h, int w,
                    int C, int32_t* label, float* vertex, float* prob, float* score, void* stream);
+/* The two calls above with the head tensor's vertex width explicit: num_vertex = 3C is pcnn_lowres_heads / pcnn_up8_heads (row
+ * stride 4C); num_vertex = 0 is the segmentation network's score-only head tensor lowres [B,h,w,C] f32 (row stride C, no vertex
+ * head: vgg16_convs.py:79-149 with vertex_reg_2d and vertex_reg_3d both off).  With num_vertex = 0, vert4, vert5, w_vertex,
+ * bias_vertex and vertex must be NULL and Cv is ignored; label_2d, prob_normalized and score are bit-identical to those of the
+ * 4C-row head tensor that shares its score channels, in the label-only and in the full mode. */
+int pcnn_lowres_heads_nv(const void* score4, const void* score5, const void* vert4, const void* vert5,
+                         const float* w_score, const float* w_vertex, int B, int h, int w, int Cs, int Cv, int C,
+                         int num_vertex, float* lowres, void* stream);
+int pcnn_up8_heads_nv(const float* lowres, const float* bias_score, const float* bias_vertex, int B, int h, int w,
+                      int C, int num_vertex, int32_t* label, float* vertex, float* prob, float* score, void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * Test-time post-processing on the device (SURVEY.md 8(f) rank 1) — replaces lib/utils/nms.py:3-32

@@ -38,28 +38,31 @@ namespace pcnn {
 //            (K = Cs) next to the remaining vertex columns, each of those split over Cv/Cs lanes of Cs rows and
 //            summed by shuffle, so no lane idles behind a longer loop.
 // Requires Cs % 4 == 0, Cv % Cs == 0 (64 / 128 in the network).
+// kVertex = false: the segmentation network's score-only head tensor [B,h,w,C] (no vertex head, vgg16_convs.py:128-149 with the
+// vertex block skipped): v4 / v5 / Wv are not read, phase 1 stages the Cs score channels and phase 2 is the score-column tail pass.
 // ---------------------------------------------------------------------------------------------
 constexpr int kLrWarps = 8;
 constexpr int kLrPix = 8;
 
+template <bool kVertex>
 __global__ void __launch_bounds__(256)
 k_lowres_heads(const __nv_bfloat16* __restrict__ s4 /*[B,h,w,Cs]*/, const __nv_bfloat16* __restrict__ s5 /*[B,h/2,w/2,Cs]*/,
                const __nv_bfloat16* __restrict__ v4 /*[B,h,w,Cv]*/, const __nv_bfloat16* __restrict__ v5,
                const float* __restrict__ Ws /*[Cs][C]*/, const float* __restrict__ Wv /*[Cv][3C]*/, int B, int h, int w,
-               int Cs, int Cv, int C, float* __restrict__ out /*[B,h,w,4C]*/)
+               int Cs, int Cv, int C, float* __restrict__ out /*[B,h,w,4C], score-only [B,h,w,C]*/)
 {
     extern __shared__ __align__(16) float sm[];
     // folded mode (Wv == NULL): the vertex_pred matrix was multiplied into the two vertex 1x1 convolutions on the host
     // (both are linear, no ReLU between them), so v4 / v5 already hold the 3C vertex channels (row stride Cv) and the
     // vertex outputs are just v4 + up2(v5)
-    const bool folded = Wv == nullptr;
-    const int Ct = folded ? Cs : Cs + Cv;   // channels staged in shared memory
-    const int No = 4 * C;          // outputs per pixel
-    const int C3 = folded ? 0 : 3 * C;      // vertex columns of the matrix phase
+    const bool folded = kVertex && Wv == nullptr;
+    const int Ct = folded || !kVertex ? Cs : Cs + Cv;   // channels staged in shared memory
+    const int No = kVertex ? 4 * C : C;                 // outputs per pixel
+    const int C3 = folded || !kVertex ? 0 : 3 * C;      // vertex columns of the matrix phase
     float* sx_all = sm;                               // [kLrWarps][Ct][8]   (16-byte aligned rows)
     float* sW = sm + kLrWarps * Ct * kLrPix;          // [Cs*C + Cv*3C]
     for (int i = threadIdx.x; i < Cs * C; i += blockDim.x) sW[i] = Ws[i];
-    if (!folded)
+    if (kVertex && !folded)
         for (int i = threadIdx.x; i < Cv * C3; i += blockDim.x) sW[Cs * C + i] = Wv[i];
     __syncthreads();
     const float* sWv = sW + Cs * C;
@@ -72,7 +75,7 @@ k_lowres_heads(const __nv_bfloat16* __restrict__ s4 /*[B,h,w,Cs]*/, const __nv_b
     const int nquads = Ct / 4;
     // column map: n_full passes of 32 vertex columns (K = Cv); then "tail" passes whose lane jobs are the C score
     // columns (K = Cs) followed, from a split-aligned start, by split = Cv / Cs partial lanes per left-over vertex column
-    const int split = Cv / Cs;
+    const int split = kVertex ? Cv / Cs : 1;
     const int n_full = C3 / 32, v_left = C3 - 32 * n_full;
     const int tail_start = (C + split - 1) / split * split;
     const int n_pass = n_full + (tail_start + v_left * split + 31) / 32;
@@ -227,10 +230,11 @@ k_lowres_heads(const __nv_bfloat16* __restrict__ s4 /*[B,h,w,Cs]*/, const __nv_b
 // part of a low-resolution row are not 8-byte aligned: a role owns ONE channel (4-byte loads and stores, consecutive lanes still
 // on consecutive channels), so a cell phase takes 4C roles; at C >= 65 that exceeds the CTA and a thread loops over the roles
 // with stride 256.
+// kVertex = false: lr is the segmentation network's score-only head tensor [B,h,w,C] (row stride C instead of 4C); vertex is NULL.
 // ---------------------------------------------------------------------------------------------
-template <int CT, int CPT>
+template <int CT, int CPT, bool kVertex>
 __global__ void __launch_bounds__(256)
-k_up8_heads(const float* __restrict__ lr /*[B,h,w,4C]*/, const float* __restrict__ bias_s /*[C]*/,
+k_up8_heads(const float* __restrict__ lr /*[B,h,w,4C] or [B,h,w,C]*/, const float* __restrict__ bias_s /*[C]*/,
             const float* __restrict__ bias_v /*[3C]*/, int h, int w, int C_rt, int seg_cells, int* __restrict__ label /*[B,8h,8w]*/,
             float* __restrict__ vertex /*[B,8h,8w,3C]*/, float* __restrict__ prob /*[B,8h,8w,C] or null*/,
             float* __restrict__ score_out /*[B,8h,8w,C] or null*/)
@@ -238,7 +242,7 @@ k_up8_heads(const float* __restrict__ lr /*[B,h,w,4C]*/, const float* __restrict
     // CPT = 2, C even: every channel pair is one 8-byte vector (vertex rows are 3C floats = 8-byte aligned).
     extern __shared__ float smem_f[];
     const int C = CT ? CT : C_rt;
-    const int No = 4 * C, W = 8 * w, H = 8 * h, N2 = No / 2, C2 = C / 2, V2 = 3 * C2;
+    const int No = (kVertex ? 4 : 1) * C, W = 8 * w, H = 8 * h, N2 = No / 2, C2 = C / 2, V2 = 3 * C2;
     const int c_lo = blockIdx.z * seg_cells, c_hi = min(c_lo + seg_cells, w);   // cells [c_lo, c_hi)
     const int s_lo = max(c_lo - 1, 0), s_hi = min(c_hi + 1, w);                 // source cells incl. halo
     float2* rowi = reinterpret_cast<float2*>(smem_f) - (size_t)s_lo * N2;       // [s_lo, s_hi) x N2, indexed by absolute cell
@@ -418,20 +422,20 @@ k_up8_heads(const float* __restrict__ lr /*[B,h,w,4C]*/, const float* __restrict
 // (cell, class pair) blends vertically in registers, emits the cell's 8 pixels into a shared score row, and thread =
 // pixel takes the arg-max (lowest index on ties).  Same operation sequence as k_up8_heads (heads_common.cuh): identical
 // labels.  CT = compile-time class count (even), CPT = channels per thread as in k_up8_heads: at CPT = 1 (C odd) the staged rows
-// are [3][w][C] scalars and a thread blends (cell, class).
+// are [3][w][C] scalars and a thread blends (cell, class).  kVertex as in k_up8_heads (row stride 4C or C).
 // ---------------------------------------------------------------------------------------------
 // 512 threads: the kernel is latency-bound (shared-memory chains between two barriers per output row); with 77 KB of shared
 // memory per CTA only two CTAs fit an SM, so the warps have to come from the CTA itself
 constexpr int kLabelThreads = 512;
 
-template <int CT, int CPT>
+template <int CT, int CPT, bool kVertex>
 __global__ void __launch_bounds__(kLabelThreads)
-k_up8_label(const float* __restrict__ lr /*[B,h,w,4C]*/, const float* __restrict__ bias_s /*[C]*/, int h, int w, int C_rt,
+k_up8_label(const float* __restrict__ lr /*[B,h,w,4C] or [B,h,w,C]*/, const float* __restrict__ bias_s /*[C]*/, int h, int w, int C_rt,
             int* __restrict__ label /*[B,8h,8w]*/)
 {
     extern __shared__ float smem_f[];
     const int C = CT ? CT : C_rt;
-    const int No = 4 * C, C2 = C / 2, W = 8 * w;
+    const int No = (kVertex ? 4 : 1) * C, C2 = C / 2, W = 8 * w;
     float2* rows = reinterpret_cast<float2*>(smem_f);              // [3][w][C2]: low-resolution rows my - 1, my, my + 1 (score channels)
     float* sc = smem_f + (size_t)3 * w * C;                        // [W][C] scores of one output row
     const int my = blockIdx.x, n = blockIdx.y, t = threadIdx.x;
@@ -529,38 +533,50 @@ k_up8_label(const float* __restrict__ lr /*[B,h,w,4C]*/, const float* __restrict
 
 using namespace pcnn;
 
+extern "C" int pcnn_lowres_heads_nv(const void* score4, const void* score5, const void* vert4, const void* vert5,
+                                    const float* w_score, const float* w_vertex, int B, int h, int w, int Cs, int Cv, int C,
+                                    int num_vertex, float* out, void* stream)
+{
+    PCNN_REQUIRE(num_vertex == 3 * C || num_vertex == 0, "lowres_heads: num_vertex must be 3C or 0 (got %d, C = %d)", num_vertex, C);
+    const bool vtx = num_vertex != 0;
+    PCNN_REQUIRE(score4 && score5 && w_score && out && (!vtx || (vert4 && vert5)), "lowres_heads: NULL tensor pointer");
+    PCNN_REQUIRE(vtx || (!vert4 && !vert5 && !w_vertex), "lowres_heads: the score-only head tensor takes no vertex tensors");
+    const bool folded = vtx && w_vertex == nullptr;
+    PCNN_REQUIRE(!folded || (3 * C <= Cv && Cv % 4 == 0), "lowres_heads: folded vertex head needs 3C <= Cv (got C = %d, Cv = %d)", C, Cv);
+    PCNN_REQUIRE(h % 2 == 0 && w % 2 == 0, "lowres_heads: conv4 resolution must be even (got %d x %d)", h, w);
+    if (vtx)
+        PCNN_REQUIRE(Cs >= 4 && Cs % 4 == 0 && Cv % Cs == 0 && ((Cv / Cs) & (Cv / Cs - 1)) == 0,
+                     "lowres_heads: need Cs %% 4 == 0 and Cv = 2^k Cs (got %d, %d)", Cs, Cv);
+    else
+        PCNN_REQUIRE(Cs >= 4 && Cs % 4 == 0, "lowres_heads: need Cs %% 4 == 0 (got %d)", Cs);
+    PCNN_REQUIRE(C >= 1 && (!vtx || Cv / Cs <= 32), "lowres_heads: bad channel counts");
+    size_t smem = sizeof(float) * (!vtx || folded ? (size_t)Cs * C + (size_t)kLrWarps * kLrPix * Cs
+                                                  : (size_t)Cs * C + (size_t)Cv * 3 * C + (size_t)kLrWarps * kLrPix * (Cs + Cv));
+    PCNN_REQUIRE(smem <= 200 * 1024, "lowres_heads: weights do not fit shared memory");
+    auto kernel = vtx ? k_lowres_heads<true> : k_lowres_heads<false>;
+    PCNN_SMEM_OPTIN(kernel, 200 * 1024, "lowres_heads");
+    PCNN_REQUIRE((long long)B * h * w < 0x7fffffffLL, "lowres_heads: too many pixels");
+    size_t npix = (size_t)B * h * w;
+    int blocks = (int)std::min<size_t>((npix + kLrPix * kLrWarps - 1) / (kLrPix * kLrWarps), (size_t)kNumSMs * (vtx && !folded ? 2 : 8));
+    kernel<<<blocks, 256, smem, (cudaStream_t)stream>>>((const __nv_bfloat16*)score4, (const __nv_bfloat16*)score5,
+                                                        (const __nv_bfloat16*)vert4, (const __nv_bfloat16*)vert5, w_score, w_vertex, B, h,
+                                                        w, Cs, Cv, C, out);
+    return check_launch("lowres_heads");
+}
+
 extern "C" int pcnn_lowres_heads(const void* score4, const void* score5, const void* vert4, const void* vert5,
                                  const float* w_score, const float* w_vertex, int B, int h, int w, int Cs, int Cv, int C,
                                  float* out, void* stream)
 {
-    PCNN_REQUIRE(score4 && score5 && vert4 && vert5 && w_score && out, "lowres_heads: NULL tensor pointer");
-    const bool folded = w_vertex == nullptr;
-    PCNN_REQUIRE(!folded || (3 * C <= Cv && Cv % 4 == 0), "lowres_heads: folded vertex head needs 3C <= Cv (got C = %d, Cv = %d)", C, Cv);
-    PCNN_REQUIRE(h % 2 == 0 && w % 2 == 0, "lowres_heads: conv4 resolution must be even (got %d x %d)", h, w);
-    PCNN_REQUIRE(Cs >= 4 && Cs % 4 == 0 && Cv % Cs == 0 && ((Cv / Cs) & (Cv / Cs - 1)) == 0,
-                 "lowres_heads: need Cs %% 4 == 0 and Cv = 2^k Cs (got %d, %d)", Cs, Cv);
-    PCNN_REQUIRE(C >= 1 && Cv / Cs <= 32, "lowres_heads: bad channel counts");
-    size_t smem = sizeof(float) * (folded ? (size_t)Cs * C + (size_t)kLrWarps * kLrPix * Cs
-                                          : (size_t)Cs * C + (size_t)Cv * 3 * C + (size_t)kLrWarps * kLrPix * (Cs + Cv));
-    PCNN_REQUIRE(smem <= 200 * 1024, "lowres_heads: weights do not fit shared memory");
-    PCNN_SMEM_OPTIN(k_lowres_heads, 200 * 1024, "lowres_heads");
-    PCNN_REQUIRE((long long)B * h * w < 0x7fffffffLL, "lowres_heads: too many pixels");
-    size_t npix = (size_t)B * h * w;
-    int blocks = (int)std::min<size_t>((npix + kLrPix * kLrWarps - 1) / (kLrPix * kLrWarps), (size_t)kNumSMs * (folded ? 8 : 2));
-    k_lowres_heads<<<blocks, 256, smem, (cudaStream_t)stream>>>((const __nv_bfloat16*)score4, (const __nv_bfloat16*)score5,
-                                                               (const __nv_bfloat16*)vert4, (const __nv_bfloat16*)vert5, w_score,
-                                                               w_vertex, B, h, w, Cs, Cv, C, out);
-    return check_launch("lowres_heads");
+    PCNN_REQUIRE(vert4 && vert5, "lowres_heads: NULL tensor pointer");
+    return pcnn_lowres_heads_nv(score4, score5, vert4, vert5, w_score, w_vertex, B, h, w, Cs, Cv, C, 3 * C, out, stream);
 }
 
-extern "C" int pcnn_up8_heads(const float* lowres, const float* bias_score, const float* bias_vertex, int B, int h, int w, int C,
-                              int32_t* label, float* vertex, float* prob, float* score, void* stream)
+// the launches of pcnn_up8_heads_nv for a head tensor of row stride 4C (kVertex) or C
+template <bool kVertex>
+static int up8_heads_launch(const float* lowres, const float* bias_score, const float* bias_vertex, int B, int h, int w, int C,
+                            int32_t* label, float* vertex, float* prob, float* score, cudaStream_t stream)
 {
-    // vertex == NULL: label-only mode (label_2d / prob / score; the dense vertex_pred is not produced)
-    PCNN_REQUIRE(lowres && bias_score && label && (bias_vertex || !vertex), "up8_heads: NULL tensor pointer");
-    PCNN_REQUIRE(C >= 2 && C <= 128, "up8_heads: num_classes must be in 2..128 (got %d)", C);
-    PCNN_REQUIRE(B >= 1 && h >= 1 && w >= 1, "up8_heads: bad shape");
-    PCNN_REQUIRE(8 * h <= 65535 * 1 && B <= 65535, "up8_heads: image too tall for the launch grid");
     const bool odd = C % 2 != 0;   // odd C: the one-channel-per-thread forms (CPT = 1)
     if (!vertex && !prob && !score) {
         // label-only fast path: one CTA per low-resolution row (8 output rows), three staged rows + one score row in smem
@@ -568,34 +584,54 @@ extern "C" int pcnn_up8_heads(const float* lowres, const float* bias_score, cons
         if (smem_l <= 200 * 1024 && h <= 65535) {
             dim3 grid_l(h, B);
             if (C == 22) {
-                PCNN_SMEM_OPTIN((k_up8_label<22, 2>), 200 * 1024, "up8_label<22>");
-                k_up8_label<22, 2><<<grid_l, kLabelThreads, smem_l, (cudaStream_t)stream>>>(lowres, bias_score, h, w, C, label);
+                PCNN_SMEM_OPTIN((k_up8_label<22, 2, kVertex>), 200 * 1024, "up8_label<22>");
+                k_up8_label<22, 2, kVertex><<<grid_l, kLabelThreads, smem_l, stream>>>(lowres, bias_score, h, w, C, label);
             } else if (odd) {
-                PCNN_SMEM_OPTIN((k_up8_label<0, 1>), 200 * 1024, "up8_label<0, odd>");
-                k_up8_label<0, 1><<<grid_l, kLabelThreads, smem_l, (cudaStream_t)stream>>>(lowres, bias_score, h, w, C, label);
+                PCNN_SMEM_OPTIN((k_up8_label<0, 1, kVertex>), 200 * 1024, "up8_label<0, odd>");
+                k_up8_label<0, 1, kVertex><<<grid_l, kLabelThreads, smem_l, stream>>>(lowres, bias_score, h, w, C, label);
             } else {
-                PCNN_SMEM_OPTIN((k_up8_label<0, 2>), 200 * 1024, "up8_label<0>");
-                k_up8_label<0, 2><<<grid_l, kLabelThreads, smem_l, (cudaStream_t)stream>>>(lowres, bias_score, h, w, C, label);
+                PCNN_SMEM_OPTIN((k_up8_label<0, 2, kVertex>), 200 * 1024, "up8_label<0>");
+                k_up8_label<0, 2, kVertex><<<grid_l, kLabelThreads, smem_l, stream>>>(lowres, bias_score, h, w, C, label);
             }
             return check_launch("up8_label");
         }
     }
+    const int No = (kVertex ? 4 : 1) * C;
     int seg_cells = w <= 20 ? w : 20;  // 160 output pixels per CTA
-    size_t smem = sizeof(float) * ((size_t)(seg_cells + 2) * 4 * C + (size_t)8 * seg_cells * C + (size_t)16 * seg_cells);
+    size_t smem = sizeof(float) * ((size_t)(seg_cells + 2) * No + (size_t)8 * seg_cells * C + (size_t)16 * seg_cells);
     PCNN_REQUIRE(smem <= 200 * 1024, "up8_heads: segment does not fit shared memory (C = %d)", C);
     dim3 grid(8 * h, B, (w + seg_cells - 1) / seg_cells);
-    PCNN_SMEM_OPTIN((k_up8_heads<0, 2>), 200 * 1024, "up8_heads<0>");
-    PCNN_SMEM_OPTIN((k_up8_heads<22, 2>), 200 * 1024, "up8_heads<22>");
-    PCNN_SMEM_OPTIN((k_up8_heads<0, 1>), 200 * 1024, "up8_heads<0, odd>");
+    PCNN_SMEM_OPTIN((k_up8_heads<0, 2, kVertex>), 200 * 1024, "up8_heads<0>");
+    PCNN_SMEM_OPTIN((k_up8_heads<22, 2, kVertex>), 200 * 1024, "up8_heads<22>");
+    PCNN_SMEM_OPTIN((k_up8_heads<0, 1, kVertex>), 200 * 1024, "up8_heads<0, odd>");
     if (C == 22)   // the YCB / LOV class count (lov_color_2d.yml:14): compile-time strides
-        k_up8_heads<22, 2><<<grid, 256, smem, (cudaStream_t)stream>>>(lowres, bias_score, bias_vertex, h, w, C, seg_cells, label, vertex,
-                                                                      prob, score);
+        k_up8_heads<22, 2, kVertex><<<grid, 256, smem, stream>>>(lowres, bias_score, bias_vertex, h, w, C, seg_cells, label, vertex, prob,
+                                                                 score);
     else if (odd)  // e.g. the multi-object LINEMOD model (linemod_color_2d.yml: 9 classes)
-        k_up8_heads<0, 1><<<grid, 256, smem, (cudaStream_t)stream>>>(lowres, bias_score, bias_vertex, h, w, C, seg_cells, label, vertex,
-                                                                     prob, score);
+        k_up8_heads<0, 1, kVertex><<<grid, 256, smem, stream>>>(lowres, bias_score, bias_vertex, h, w, C, seg_cells, label, vertex, prob,
+                                                                score);
     else
-        k_up8_heads<0, 2><<<grid, 256, smem, (cudaStream_t)stream>>>(lowres, bias_score, bias_vertex, h, w, C, seg_cells, label, vertex,
-                                                                     prob, score);
+        k_up8_heads<0, 2, kVertex><<<grid, 256, smem, stream>>>(lowres, bias_score, bias_vertex, h, w, C, seg_cells, label, vertex, prob,
+                                                                score);
     return check_launch("up8_heads");
 }
 
+extern "C" int pcnn_up8_heads_nv(const float* lowres, const float* bias_score, const float* bias_vertex, int B, int h, int w, int C,
+                                 int num_vertex, int32_t* label, float* vertex, float* prob, float* score, void* stream)
+{
+    PCNN_REQUIRE(num_vertex == 3 * C || num_vertex == 0, "up8_heads: num_vertex must be 3C or 0 (got %d, C = %d)", num_vertex, C);
+    // vertex == NULL: label-only mode (label_2d / prob / score; the dense vertex_pred is not produced)
+    PCNN_REQUIRE(lowres && bias_score && label && (bias_vertex || !vertex), "up8_heads: NULL tensor pointer");
+    PCNN_REQUIRE(num_vertex || (!vertex && !bias_vertex), "up8_heads: the score-only head tensor has no vertex channels");
+    PCNN_REQUIRE(C >= 2 && C <= 128, "up8_heads: num_classes must be in 2..128 (got %d)", C);
+    PCNN_REQUIRE(B >= 1 && h >= 1 && w >= 1, "up8_heads: bad shape");
+    PCNN_REQUIRE(8 * h <= 65535 * 1 && B <= 65535, "up8_heads: image too tall for the launch grid");
+    return num_vertex ? up8_heads_launch<true>(lowres, bias_score, bias_vertex, B, h, w, C, label, vertex, prob, score, (cudaStream_t)stream)
+                      : up8_heads_launch<false>(lowres, bias_score, nullptr, B, h, w, C, label, nullptr, prob, score, (cudaStream_t)stream);
+}
+
+extern "C" int pcnn_up8_heads(const float* lowres, const float* bias_score, const float* bias_vertex, int B, int h, int w, int C,
+                              int32_t* label, float* vertex, float* prob, float* score, void* stream)
+{
+    return pcnn_up8_heads_nv(lowres, bias_score, bias_vertex, B, h, w, C, 3 * C, label, vertex, prob, score, stream);
+}

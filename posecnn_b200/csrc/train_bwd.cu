@@ -113,12 +113,14 @@ k_up2_bwd(const __nv_bfloat16* __restrict__ dadd /*[B,h,w,C]*/, const __nv_bfloa
     }
 }
 
-// lowres [B,h,w,4C] f32 = [score part (first C of sc, row stride Cs) | vertex part (first 3C of vt, row stride Cv)]
+// lowres [B,h,w,4C] f32 = [score part (first C of sc, row stride Cs) | vertex part (first 3C of vt, row stride Cv)];
+// kVertex = false: the segmentation network's score-only [B,h,w,C] (vt not read)
+template <bool kVertex>
 __global__ void __launch_bounds__(256)
 k_pack_lowres(const __nv_bfloat16* __restrict__ sc, int Cs, const __nv_bfloat16* __restrict__ vt, int Cv, size_t npix, int C,
               float* __restrict__ lowres)
 {
-    const int No = 4 * C;
+    const int No = kVertex ? 4 * C : C;
     const size_t total = npix * No;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
         const int ch = (int)(i % No);
@@ -162,13 +164,17 @@ constexpr int kBand = 16;                           // band height (low-resoluti
 // bytes, DESIGN §10); 8 would spill.
 // CPT = 1 runs at C = 9 only (kSCols * 9 = 360 threads): bounding it at 360 x 2 CTAs instead of 1024 lifts the register cap from 64,
 // where the coordinate form spills, to 80
-template <int CT, int SC, bool kCoord, int CPT>
+// kVertex = false: target mode "none", the segmentation network's adjoint of loss_cls alone (no vertex head): no vertex-role work and no
+// vacc / bv / logz / ab shared memory; vertex_loss_out, lowres, bias_v, centers, vertmap, extents and d_vt are not read, and a CTA's
+// dbias_partial row holds C floats instead of 4C.  The score channels' arithmetic is the vertex modes' own, so d_sc and the score
+// bias gradient equal theirs bit for bit.
+template <int CT, int SC, bool kCoord, int CPT, bool kVertex>
 __global__ void __launch_bounds__(CT ? (8 * SC + 8) * (CT / 2) : (CPT == 1 ? (8 * SC + 8) * 9 : 1024), CT == 2 ? 6 : (CT || CPT == 1 ? 2 : 1))
 k_up8_bwd_strip(const float* __restrict__ prob, const float* __restrict__ score, const int* __restrict__ gt, const float* __restrict__ cls_out,
                 float up_cls, float threshold, const float* __restrict__ lowres,
                 const float* __restrict__ bias_v, const float* __restrict__ centers,
                 const float* __restrict__ vtx_out, float up_vtx, float w_inside, float sigma2, int h, int w, int rb, int C_rt, int Cs, int Cv,
-                __nv_bfloat16* __restrict__ d_sc, __nv_bfloat16* __restrict__ d_vt, float* __restrict__ dbias_partial /*[ctas][4C]*/,
+                __nv_bfloat16* __restrict__ d_sc, __nv_bfloat16* __restrict__ d_vt, float* __restrict__ dbias_partial /*[ctas][4C or C]*/,
                 const float* __restrict__ vertmap, const float* __restrict__ extents)
 {
     // C == 2 or C even in 6..50: thread = (output column, channel pair), kSCols * C / 2 threads; C = 9: (output column, channel),
@@ -181,28 +187,30 @@ k_up8_bwd_strip(const float* __restrict__ prob, const float* __restrict__ score,
     const int c_lo = blockIdx.x * kSC, c_hi = min(c_lo + kSC, w);
     const int m_lo = blockIdx.y * rb, m_hi = min(m_lo + rb, h);
     const int n = blockIdx.z;
-    const float s_cls = up_cls / (cls_out[1] + 1e-10f), s_vtx = up_vtx / (vtx_out[1] + 1e-10f);
+    const float s_cls = up_cls / (cls_out[1] + 1e-10f), s_vtx = kVertex ? up_vtx / (vtx_out[1] + 1e-10f) : 0.f;
     const size_t img = (size_t)n * H * W;
     extern __shared__ float sm[];
     float* v_s = sm;                                 // [kSCols][C]       finished vertical sums of the score channels
     float* vacc = v_s + kSCols * C;                  // [2][kSCols][VC]   running vertical sums of the vertex channels
-    float* bs = vacc + 2 * kSCols * VC;              // [kSCols][C]       bias-gradient sums (score), per column
+    float* bs = vacc + (kVertex ? 2 * kSCols * VC : 0);   // [kSCols][C]  bias-gradient sums (score), per column
     float* bv = bs + kSCols * C;                     // [kSCols][VC]      bias-gradient sums (vertex), per column
     float* logz = bv + kSCols * VC;                  // [C]               log of the listed centre depth of each class of this image
                                                      //                   (kCoord: 1 if the class is listed, else 0)
     float* ab = logz + C;                            // [C][6]            kCoord: (a_0, b_0, a_1, b_1, a_2, b_2) of each class
     const int t = threadIdx.x, col = t / CP, j = t - col * CP;
-    for (int i = t; i < C; i += NT) {
-        const float z = centers[((size_t)n * C + i) * 3 + 2];
-        if constexpr (kCoord) {
-            logz[i] = z > 0.f ? 1.f : 0.f;
-            coord_scale(extents + 3 * i, ab + 6 * i);
-        } else {
-            logz[i] = z > 0.f ? (float)log((double)z) : 0.f;
+    if constexpr (kVertex) {
+        for (int i = t; i < C; i += NT) {
+            const float z = centers[((size_t)n * C + i) * 3 + 2];
+            if constexpr (kCoord) {
+                logz[i] = z > 0.f ? 1.f : 0.f;
+                coord_scale(extents + 3 * i, ab + 6 * i);
+            } else {
+                logz[i] = z > 0.f ? (float)log((double)z) : 0.f;
+            }
         }
+        for (int i = t; i < 2 * kSCols * VC; i += NT) vacc[i] = 0.f;
+        for (int i = t; i < kSCols * VC; i += NT) bv[i] = 0.f;
     }
-    for (int i = t; i < 2 * kSCols * VC; i += NT) vacc[i] = 0.f;
-    for (int i = t; i < kSCols * VC; i += NT) bv[i] = 0.f;
     __syncthreads();
     const int x = 8 * c_lo - 4 + col;
     const bool xin = x >= 0 && x < W && x < 8 * c_hi + 4;
@@ -240,13 +248,13 @@ k_up8_bwd_strip(const float* __restrict__ prob, const float* __restrict__ score,
     const int* gpB2 = gtB_c + r0 + 2 * (size_t)W;
     const size_t stepQ = (size_t)W * C, stepS = (size_t)W * CP;
     int gB0 = -1, gB1 = -1;
-    if (xinB) {
+    if (kVertex && xinB) {
         if (y_first <= y_last) gB0 = __ldg(gtB_c + r0);
         if (y_first + 1 <= y_last) gB1 = __ldg(gtB_c + r0 + W);
     }
     // kCoord: object coordinate of the vertex-role pixel of the current row, loaded one row ahead for weighted pixels only
     float vB[3] = {0.f, 0.f, 0.f};
-    if constexpr (kCoord) {
+    if constexpr (kCoord && kVertex) {
         if (gB0 > 0 && gB0 < C && logz[gB0] > 0.f) {
             const float* vp = vertmap + (img + r0 + xB) * 3;
             vB[0] = __ldg(vp); vB[1] = __ldg(vp + 1); vB[2] = __ldg(vp + 2);
@@ -287,7 +295,7 @@ k_up8_bwd_strip(const float* __restrict__ prob, const float* __restrict__ score,
         // The target direction needs a double sqrt and two double divisions per labelled pixel (the reference forms it in float64,
         // minibatch.py:582-594); keeping that on kSCols densely packed lanes instead of three lanes of every column costs 1/7 of the
         // double-precision issue slots at C = 22 (the (column, k) mapping made the whole kernel FP64-bound: 3.2 ms at batch 64).
-        if (t < kSCols) {
+        if (kVertex && t < kSCols) {
             const int gB = gB0;
             if (gB > 0 && gB < C) {
                 const float* cen = centers + ((size_t)n * C + gB) * 3;
@@ -340,8 +348,9 @@ k_up8_bwd_strip(const float* __restrict__ prob, const float* __restrict__ score,
             __syncthreads();                          // every thread's updates of vacc for this row are done (also when the row is discarded)
             if (m_old >= m_lo) {
                 const float* va = vacc + (size_t)slot_lo * kSCols * VC;
-                for (int item = t; item < (c_hi - c_lo) * (Cs + Cv); item += NT) {
-                    const int ml = item / (Cs + Cv), ch = item - ml * (Cs + Cv);
+                const int Ct = kVertex ? Cs + Cv : Cs;   // channels of a d_sc (+ d_vt) cell
+                for (int item = t; item < (c_hi - c_lo) * Ct; item += NT) {
+                    const int ml = item / Ct, ch = item - ml * Ct;
                     const size_t cell = ((size_t)n * h + m_old) * w + c_lo + ml;
                     float acc = 0.f;
                     if (ch < Cs) {
@@ -361,7 +370,8 @@ k_up8_bwd_strip(const float* __restrict__ prob, const float* __restrict__ score,
                 }
                 __syncthreads();
             }
-            for (int i = t; i < kSCols * VC; i += NT) vacc[(size_t)slot_lo * kSCols * VC + i] = 0.f;
+            if constexpr (kVertex)
+                for (int i = t; i < kSCols * VC; i += NT) vacc[(size_t)slot_lo * kSCols * VC + i] = 0.f;
             __syncthreads();
             lo0 = hi0; lo1 = hi1; hi0 = 0.f; hi1 = 0.f;
             slot_lo ^= 1;
@@ -371,11 +381,12 @@ k_up8_bwd_strip(const float* __restrict__ prob, const float* __restrict__ score,
     else { bs[col * C + 2 * j] = b0; bs[col * C + 2 * j + 1] = b1; }
     __syncthreads();
     const size_t cta = ((size_t)blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
-    for (int ch = t; ch < No; ch += NT) {
+    const int NB = kVertex ? No : C;                 // bias channels
+    for (int ch = t; ch < NB; ch += NT) {
         float acc = 0.f;
         if (ch < C) { for (int q = 0; q < kSCols; q++) acc += bs[q * C + ch]; }
         else { for (int q = 0; q < kSCols; q++) acc += bv[q * VC + ch - C]; }
-        dbias_partial[cta * No + ch] = acc;
+        dbias_partial[cta * NB + ch] = acc;
     }
 }
 
@@ -508,27 +519,100 @@ extern "C" int pcnn_up2_bwd_bf16(const void* dadd, const void* y5, int B, int h,
     return check_launch("up2_bwd");
 }
 
+extern "C" int pcnn_pack_lowres_nv(const void* sc, int Cs, const void* vt, int Cv, int B, int h, int w, int C, int num_vertex, float* lowres,
+                                   void* stream)
+{
+    PCNN_REQUIRE(num_vertex == 3 * C || num_vertex == 0, "pack_lowres: num_vertex must be 3C or 0 (got %d, C = %d)", num_vertex, C);
+    const bool vtx = num_vertex != 0;
+    PCNN_REQUIRE(sc && lowres && Cs >= C && (vtx ? vt && Cv >= 3 * C : !vt), "pack_lowres: bad arguments");
+    const size_t npix = (size_t)B * h * w;
+    const int blocks = ew_blocks(npix * (vtx ? 4 : 1) * C);
+    if (vtx)
+        k_pack_lowres<true><<<blocks, 256, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)sc, Cs, (const __nv_bfloat16*)vt, Cv, npix, C, lowres);
+    else
+        k_pack_lowres<false><<<blocks, 256, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)sc, Cs, nullptr, 0, npix, C, lowres);
+    return check_launch("pack_lowres");
+}
+
 extern "C" int pcnn_pack_lowres(const void* sc, int Cs, const void* vt, int Cv, int B, int h, int w, int C, float* lowres, void* stream)
 {
-    PCNN_REQUIRE(sc && vt && lowres && Cs >= C && Cv >= 3 * C, "pack_lowres: bad arguments");
-    const size_t npix = (size_t)B * h * w;
-    k_pack_lowres<<<ew_blocks(npix * 4 * C), 256, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)sc, Cs, (const __nv_bfloat16*)vt, Cv, npix, C, lowres);
-    return check_launch("pack_lowres");
+    PCNN_REQUIRE(vt, "pack_lowres: bad arguments");
+    return pcnn_pack_lowres_nv(sc, Cs, vt, Cv, B, h, w, C, 3 * C, lowres, stream);
+}
+
+// CTAs of k_up8_bwd_strip: (image, strip of cells, band of kBand rows); each writes one row of bias partial sums
+static size_t up8_bwd_ctas(int B, int h, int w, int C)
+{
+    const int sc = C == 2 ? kStrip2 : kStrip;
+    return (size_t)B * ((w + sc - 1) / sc) * ((h + kBand - 1) / kBand);
 }
 
 extern "C" int pcnn_up8_heads_bwd_workspace_bytes(int B, int h, int w, int C, size_t* bytes)
 {
     PCNN_REQUIRE(bytes && B >= 1 && h >= 1 && w >= 1 && C >= 1, "up8_heads_bwd_workspace_bytes: bad arguments");
-    // partial bias sums of k_up8_bwd_strip: one row of 4C floats per CTA = (image, strip of cells, band of kBand rows)
-    const int sc = C == 2 ? kStrip2 : kStrip;
-    *bytes = sizeof(float) * (size_t)B * ((w + sc - 1) / sc) * ((h + kBand - 1) / kBand) * 4 * C;
+    // partial bias sums of k_up8_bwd_strip: one row of 4C floats per CTA
+    *bytes = sizeof(float) * up8_bwd_ctas(B, h, w, C) * 4 * C;
     return PCNN_OK;
 }
 
-// every instantiation of the strip kernel has this signature; the entry point picks one by class count and target mode
-using UpBwdKernel = decltype(&k_up8_bwd_strip<2, kStrip2, false, 2>);
+extern "C" int pcnn_up8_scores_bwd_workspace_bytes(int B, int h, int w, int C, size_t* bytes)
+{
+    PCNN_REQUIRE(bytes && B >= 1 && h >= 1 && w >= 1 && C >= 1, "up8_scores_bwd_workspace_bytes: bad arguments");
+    // partial bias sums of k_up8_bwd_strip in target mode "none": one row of C floats per CTA
+    *bytes = sizeof(float) * up8_bwd_ctas(B, h, w, C) * C;
+    return PCNN_OK;
+}
+
+// every instantiation of the strip kernel has this signature; the launch picks one by class count and target mode
+using UpBwdKernel = decltype(&k_up8_bwd_strip<2, kStrip2, false, 2, true>);
+enum UpBwdTarget { kTarget2D, kTargetCoord, kTargetNone };
 template <int CT, int SC, int CPT>
-static UpBwdKernel up8_bwd_kernel(bool coord) { return coord ? k_up8_bwd_strip<CT, SC, true, CPT> : k_up8_bwd_strip<CT, SC, false, CPT>; }
+static UpBwdKernel up8_bwd_kernel(UpBwdTarget target)
+{
+    return target == kTargetNone ? k_up8_bwd_strip<CT, SC, false, CPT, false>
+                                 : (target == kTargetCoord ? k_up8_bwd_strip<CT, SC, true, CPT, true> : k_up8_bwd_strip<CT, SC, false, CPT, true>);
+}
+
+// the shared tail of pcnn_up8_heads_bwd and pcnn_up8_scores_bwd (arguments validated by the caller)
+static int up8_bwd_launch(UpBwdTarget target, const float* prob, const float* score, const int32_t* gt, const float* cls_loss_out,
+                          float upstream_cls, float threshold, const float* lowres, const float* bias_vertex, const float* centers,
+                          const float* vertmap, const float* extents, const float* vertex_loss_out, float upstream_vertex, float w_inside,
+                          float sigma, int B, int h, int w, int C, int Cs, int Cv, void* d_sc_bf16, void* d_vt_bf16, float* dbias,
+                          void* workspace, void* stream)
+{
+    // coalesced strip kernel (see k_up8_bwd_strip)
+    const int sc = C == 2 ? kStrip2 : kStrip, cols = 8 * sc + 8;
+    const int bands = (h + kBand - 1) / kBand, strips = (w + sc - 1) / sc;
+    PCNN_REQUIRE(bands <= 65535, "up8_heads_bwd: bad shape");
+    UpBwdKernel kernel;
+    int threads;
+    if (C == 22) {
+        kernel = up8_bwd_kernel<22, kStrip, 2>(target);
+        threads = cols * 11;
+    } else if (C == 2) {
+        kernel = up8_bwd_kernel<2, kStrip2, 2>(target);
+        threads = cols;
+    } else if (C % 2) {   // C = 9: one channel per thread (at 40 x 9 threads the strip's shared memory is 16 KB: no opt-in)
+        kernel = up8_bwd_kernel<0, kStrip, 1>(target);
+        threads = cols * C;
+    } else {
+        kernel = up8_bwd_kernel<0, kStrip, 2>(target);
+        threads = cols * (C / 2);
+        PCNN_SMEM_OPTIN(kernel, 100 * 1024,
+                        target == kTargetNone ? "up8_bwd_strip<0, none>" : (target == kTargetCoord ? "up8_bwd_strip<0, coord>" : "up8_bwd_strip<0>"));
+    }
+    cudaStream_t st = (cudaStream_t)stream;
+    // score-only: v_s + bs ([kSCols][C] each); vertex modes add vacc, bv, logz (and the 3-D mode's ab)
+    const size_t smem = sizeof(float) * (target == kTargetNone ? (size_t)cols * 2 * C
+                                                               : (size_t)cols * 11 * C + C + (target == kTargetCoord ? 6 * C : 0));
+    kernel<<<dim3(strips, bands, B), threads, smem, st>>>(prob, score, gt, cls_loss_out, upstream_cls, threshold, lowres, bias_vertex, centers,
+                                                          vertex_loss_out, upstream_vertex, w_inside, sigma * sigma, h, w, kBand, C, Cs, Cv,
+                                                          (__nv_bfloat16*)d_sc_bf16, (__nv_bfloat16*)d_vt_bf16, (float*)workspace, vertmap,
+                                                          extents);
+    const int nb = target == kTargetNone ? C : 4 * C;
+    k_sum_partials<<<(nb + 31) / 32, 256, 0, st>>>((const float*)workspace, B * strips * bands, nb, 1.f, nullptr, 0.f, dbias);
+    return check_launch("up8_heads_bwd");
+}
 
 // the target mode follows vertmap / extents: both NULL = 2-D centre direction, both given = 3-D object coordinate (VERTEX_REG_3D:
 // vertmap [B,8h,8w,3] f32 and extents [C,3] f32; centers stays the presence table, a class's pixels are weighted iff
@@ -549,35 +633,23 @@ extern "C" int pcnn_up8_heads_bwd(const float* prob, const float* score, const i
     size_t need = 0;
     PCNN_REQUIRE(pcnn_up8_heads_bwd_workspace_bytes(B, h, w, C, &need) == PCNN_OK, "up8_heads_bwd: bad shape");
     PCNN_REQUIRE(workspace_bytes >= need, "up8_heads_bwd: workspace too small (%zu < %zu)", workspace_bytes, need);
-    // coalesced strip kernel (see k_up8_bwd_strip)
-    const bool coord = vertmap != nullptr;
-    const int sc = C == 2 ? kStrip2 : kStrip, cols = 8 * sc + 8;
-    const int bands = (h + kBand - 1) / kBand, strips = (w + sc - 1) / sc;
-    PCNN_REQUIRE(bands <= 65535, "up8_heads_bwd: bad shape");
-    UpBwdKernel kernel;
-    int threads;
-    if (C == 22) {
-        kernel = up8_bwd_kernel<22, kStrip, 2>(coord);
-        threads = cols * 11;
-    } else if (C == 2) {
-        kernel = up8_bwd_kernel<2, kStrip2, 2>(coord);
-        threads = cols;
-    } else if (C % 2) {   // C = 9: one channel per thread (at 40 x 9 threads the strip's shared memory is 16 KB: no opt-in)
-        kernel = up8_bwd_kernel<0, kStrip, 1>(coord);
-        threads = cols * C;
-    } else {
-        kernel = up8_bwd_kernel<0, kStrip, 2>(coord);
-        threads = cols * (C / 2);
-        PCNN_SMEM_OPTIN(kernel, 100 * 1024, coord ? "up8_bwd_strip<0, coord>" : "up8_bwd_strip<0>");
-    }
-    cudaStream_t st = (cudaStream_t)stream;
-    const size_t smem = sizeof(float) * ((size_t)cols * 11 * C + C + (coord ? 6 * C : 0));
-    kernel<<<dim3(strips, bands, B), threads, smem, st>>>(prob, score, gt, cls_loss_out, upstream_cls, threshold, lowres, bias_vertex, centers,
-                                                          vertex_loss_out, upstream_vertex, w_inside, sigma * sigma, h, w, kBand, C, Cs, Cv,
-                                                          (__nv_bfloat16*)d_sc_bf16, (__nv_bfloat16*)d_vt_bf16, (float*)workspace, vertmap,
-                                                          extents);
-    k_sum_partials<<<(4 * C + 31) / 32, 256, 0, st>>>((const float*)workspace, B * strips * bands, 4 * C, 1.f, nullptr, 0.f, dbias);
-    return check_launch("up8_heads_bwd");
+    return up8_bwd_launch(vertmap ? kTargetCoord : kTarget2D, prob, score, gt, cls_loss_out, upstream_cls, threshold, lowres, bias_vertex,
+                          centers, vertmap, extents, vertex_loss_out, upstream_vertex, w_inside, sigma, B, h, w, C, Cs, Cv, d_sc_bf16,
+                          d_vt_bf16, dbias, workspace, stream);
+}
+
+extern "C" int pcnn_up8_scores_bwd(const float* prob, const float* score, const int32_t* gt, const float* cls_loss_out, float upstream_cls,
+                                   float threshold, int B, int h, int w, int C, int Cs, void* d_sc_bf16, float* dbias, void* workspace,
+                                   size_t workspace_bytes, void* stream)
+{
+    PCNN_REQUIRE(prob && score && gt && cls_loss_out && d_sc_bf16 && dbias && workspace, "up8_scores_bwd: NULL tensor pointer");
+    PCNN_REQUIRE(Cs >= C && h <= 65535 && B <= 65535, "up8_scores_bwd: bad shape");
+    PCNN_REQUIRE(C == 2 || C == 9 || (C % 2 == 0 && C >= 6 && C <= 50), "up8_scores_bwd: C must be even and 2 or in 6..50, or 9 (C = %d)", C);
+    size_t need = 0;
+    PCNN_REQUIRE(pcnn_up8_scores_bwd_workspace_bytes(B, h, w, C, &need) == PCNN_OK, "up8_scores_bwd: bad shape");
+    PCNN_REQUIRE(workspace_bytes >= need, "up8_scores_bwd: workspace too small (%zu < %zu)", workspace_bytes, need);
+    return up8_bwd_launch(kTargetNone, prob, score, gt, cls_loss_out, upstream_cls, threshold, nullptr, nullptr, nullptr, nullptr, nullptr,
+                          nullptr, 0.f, 0.f, 1.f, B, h, w, C, Cs, 0, d_sc_bf16, nullptr, dbias, workspace, stream);
 }
 
 extern "C" int pcnn_pose_chain_bwd(const float* bottom_diff, const float* poses_tanh, const float* poses_weight, int N, int D, float upstream,

@@ -33,6 +33,30 @@ def lowres_heads(s4, s5, v4, v5, w_score, w_vertex, num_classes):
     return lowres
 
 
+def lowres_scores(s4, s5, w_score, num_classes):
+    """pcnn_lowres_heads_nv at num_vertex = 0: the segmentation network's score-only head tensor [B,h,w,C] f32 of
+    add = s4 + up2(s5); s4 [B,h,w,Cs] bf16, s5 [B,h/2,w/2,Cs], w_score [Cs][C] f32."""
+    B, h, w, Cs = s4.shape
+    C = num_classes
+    lowres = torch.empty((B, h, w, C), dtype=torch.float32, device=s4.device)
+    check(lib().pcnn_lowres_heads_nv(ptr(s4), ptr(s5), None, None, ptr(w_score), None, B, h, w, Cs, 0, C, 0, ptr(lowres), stream()))
+    return lowres
+
+
+def up8_scores(lowres, bias_score, prob=False, score=False, out=None):
+    """pcnn_up8_heads_nv at num_vertex = 0 on the score-only head tensor lowres [B,h,w,C] f32: returns (label_2d [B,8h,8w] int32,
+    prob_normalized [B,8h,8w,C], score [B,8h,8w,C]) f32, None for each of the last two not asked for (neither: the label-only
+    call).  out: the three buffers to write instead (None where not wanted); prob / score are then ignored."""
+    B, h, w, C = lowres.shape
+    if out is None:
+        dev, H, W = lowres.device, 8 * h, 8 * w
+        f32 = lambda on: torch.empty((B, H, W, C), dtype=torch.float32, device=dev) if on else None
+        out = (torch.empty((B, H, W), dtype=torch.int32, device=dev), f32(prob), f32(score))
+    label, p, s = out
+    check(lib().pcnn_up8_heads_nv(ptr(lowres), ptr(bias_score), None, B, h, w, C, 0, ptr(label), None, ptr(p), ptr(s), stream()))
+    return out
+
+
 def up8_heads(lowres, bias_score, bias_vertex, vertex=False, prob=False, score=False, out=None):
     """pcnn_up8_heads on lowres [B,h,w,4C] f32: returns (label_2d [B,8h,8w] int32, vertex_pred [B,8h,8w,3C], prob_normalized
     [B,8h,8w,C], score [B,8h,8w,C]) f32, None for each of the last three not asked for.  Asking for none of them is the
@@ -73,6 +97,32 @@ def pack_lowres(sc, vt, num_classes):
     lowres = torch.empty((B, h, w, 4 * C), dtype=torch.float32, device=sc.device)
     check(lib().pcnn_pack_lowres(ptr(sc), Cs, ptr(vt), vt.shape[3], B, h, w, C, ptr(lowres), stream()))
     return lowres
+
+
+def pack_scores(sc, num_classes):
+    """pcnn_pack_lowres_nv at num_vertex = 0: the score-only head tensor [B,h,w,C] f32 from the first C channels of sc [B,h,w,Cs] bf16."""
+    B, h, w, Cs = sc.shape
+    C = num_classes
+    lowres = torch.empty((B, h, w, C), dtype=torch.float32, device=sc.device)
+    check(lib().pcnn_pack_lowres_nv(ptr(sc), Cs, None, 0, B, h, w, C, 0, ptr(lowres), stream()))
+    return lowres
+
+
+def up8_scores_bwd(prob, score, gt, cls_out, upstream_cls, threshold, out=None):
+    """pcnn_up8_scores_bwd: the gradient of upstream_cls * loss_cls w.r.t. the score-only head tensor.  prob / score [B,8h,8w,C] f32,
+    gt [B,8h,8w] int32, cls_out the loss's [value, normaliser].  Returns (d_sc [B,h,w,SCORE_ROWS] bf16, dbias [C] f32); channels past
+    C are written as 0.  out: the two buffers to write instead (any channel stride >= C)."""
+    B, H, W, C = prob.shape
+    h, w, dev = H // 8, W // 8, prob.device
+    if out is None:
+        out = (torch.empty((B, h, w, SCORE_ROWS), dtype=torch.bfloat16, device=dev), torch.empty((C,), dtype=torch.float32, device=dev))
+    d_sc, dbias = out
+    nbytes = ctypes.c_size_t(0)
+    check(lib().pcnn_up8_scores_bwd_workspace_bytes(B, h, w, C, ctypes.byref(nbytes)))
+    ws = workspace("up8_bwd", nbytes.value, dev)
+    check(lib().pcnn_up8_scores_bwd(ptr(prob), ptr(score), ptr(gt), ptr(cls_out), upstream_cls, threshold, B, h, w, C, d_sc.shape[3],
+                                    ptr(d_sc), ptr(dbias), ptr(ws), ws.numel(), stream()))
+    return out
 
 
 def up8_heads_bwd(prob, score, gt, cls_out, upstream_cls, threshold, lowres, bias_vertex, centers, vtx_out, upstream_vertex, w_inside,

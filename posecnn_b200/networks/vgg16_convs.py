@@ -7,6 +7,7 @@ vgg16_convs.setup() (vgg16_convs.py:79-212) is executed eagerly on one CUDA stre
 
     conv1_1 .. conv5_3 (+ _p trunk for RGBD)   wgmma implicit GEMM, bf16 x bf16 -> fp32   csrc/conv_tc.cu
     score / vertex heads                         1x1 on wgmma + fused bilinear/softmax     csrc/heads.cu
+                                                 (score heads only on the segmentation network: vertex_reg_2d=False, vertex_reg_3d=False)
     hough_voting_gpu                             csrc/hough_vote.cu
     roi_pool x2 + add, fc6-fc8, tanh             csrc/fc_tc.cu (fused pooling, split-K wgmma GEMMs, fused epilogues)
     adaptation: fc9, domain_score / prob / label  fc9 on csrc/fc_tc.cu, the 256 -> 2 tail in one launch (csrc/domain.cu)
@@ -29,16 +30,22 @@ from .trunk import PIXEL_MEANS, VGG_CFG, conv_weights_to_tc, run_trunk, trunk_sh
 
 class vgg16_convs:
     def __init__(self, input_format="COLOR", num_classes=22, num_units=64, scales=(1.0,), threshold_label=1.0,
-                 vote_threshold=-1.0, vertex_reg_2d=True, vertex_reg_3d=False, pose_reg=True, adaptation=False,
+                 vote_threshold=-1.0, vertex_reg_2d=True, vertex_reg_3d=None, pose_reg=True, adaptation=False,
                  trainable=True, is_train=False, device="cuda", fold_vertex_head=True):
         self.input_format = input_format
         # fold_vertex_head: multiply the vertex_pred matrix (128 -> 3C) into score_conv4_vertex / score_conv5_vertex
         # (512 -> 128) once at prepare() time; exact algebra (no non-linearity between them, vgg16_convs.py:151-163),
         # removes 86 % of the 1/8-resolution matrix work.  False keeps the reference's intermediate layers.
-        self.fold_vertex_head = bool(fold_vertex_head) and 3 * num_classes <= 128
+        # vertex_head: False only for the segmentation network, built by giving vertex_reg_2d=False AND vertex_reg_3d=False
+        # (vgg16_convs.py:79-149, the vertex block :151-212 skipped): score heads only, pose_reg and adaptation ignored, as the
+        # reference ignores them outside vertex_reg_2d.  vertex_reg_3d left at its default (None, read as False) keeps the vertex
+        # head, so a network built as vgg16_convs(vertex_reg_2d=False) has the parameter set and graph it always had.
+        self.vertex_head = bool(vertex_reg_2d) or vertex_reg_3d is not False
+        self.fold_vertex_head = bool(fold_vertex_head) and 3 * num_classes <= 128 and self.vertex_head
         self.num_classes = num_classes
         self.num_units = num_units
         self.threshold_label = threshold_label
+        vertex_reg_3d = bool(vertex_reg_3d)
         self.vertex_reg = vertex_reg_2d or vertex_reg_3d
         self.vertex_reg_2d = vertex_reg_2d
         self.vertex_reg_3d = vertex_reg_3d
@@ -66,10 +73,13 @@ class vgg16_convs:
         for sfx in trunks:
             shapes.update(trunk_shapes(sfx))
         cin_head = 1024 if self.input_format == "RGBD" else 512
-        for name, co in (("score_conv5", U), ("score_conv4", U), ("score_conv5_vertex", 128), ("score_conv4_vertex", 128)):
+        vertex_heads = (("score_conv5_vertex", 128), ("score_conv4_vertex", 128)) if self.vertex_head else ()
+        for name, co in (("score_conv5", U), ("score_conv4", U)) + vertex_heads:
             shapes[f"{name}/weights"] = (1, 1, cin_head if not name.endswith("vertex") else 512, co)
             shapes[f"{name}/biases"] = (co,)
         shapes["score/weights"] = (1, 1, U, C); shapes["score/biases"] = (C,)
+        if not self.vertex_head:
+            return shapes
         shapes["vertex_pred/weights"] = (1, 1, 128, 3 * C); shapes["vertex_pred/biases"] = (3 * C,)
         shapes["fc6/weights"] = (7 * 7 * 512, 4096); shapes["fc6/biases"] = (4096,)
         shapes["fc7/weights"] = (4096, 4096); shapes["fc7/biases"] = (4096,)
@@ -100,15 +110,19 @@ class vgg16_convs:
         self.forward(data, meta_data, extents, want_prob=False, sync_rois=False, **forward_kwargs)
         C = self.num_classes
         B, H, W, _ = data.shape
-        bufs = (torch.empty((B, H, W), dtype=torch.int32, device=data.device),
-                torch.empty((B, H, W, 3 * C), dtype=torch.float32, device=data.device), None, None)
+        label = torch.empty((B, H, W), dtype=torch.int32, device=data.device)
+        if self.vertex_head:
+            bufs = (label, torch.empty((B, H, W, 3 * C), dtype=torch.float32, device=data.device), None, None)
         lowres = self._last_lowres
         bias = self.params["score/biases"]
         base = float(bias[0])
 
         def fg_fraction(b0):
             bias[0] = b0
-            lab = heads.up8_heads(lowres, bias, self.params["vertex_pred/biases"], out=bufs)[0]
+            if self.vertex_head:
+                lab = heads.up8_heads(lowres, bias, self.params["vertex_pred/biases"], out=bufs)[0]
+            else:
+                lab = heads.up8_scores(lowres, bias, out=(label, None, None))[0]
             return float((lab > 0).float().mean())
 
         scale = float(lowres[..., :C].abs().max()) + 1.0
@@ -144,12 +158,14 @@ class vgg16_convs:
             if not name.endswith("weights") or name.startswith("fc") or name in ("score/weights", "vertex_pred/weights", "domain_score/weights"):
                 continue
             T[name] = conv_weights_to_tc(P[name])
+        T["score/w"] = P["score/weights"].reshape(self.num_units, self.num_classes).contiguous()
+        if not self.vertex_head:
+            return
         for name in ("fc6", "fc7", "fc8"):
             T[f"{name}/weights"] = pose_head.fc_weights_to_tc(P[f"{name}/weights"])   # [out (padded to x128), in] fp16
         if self.domain_branch:
             T["fc9/weights"] = pose_head.fc_weights_to_tc(P["fc9/weights"])                # [256][25088] fp16
             T["domain_score/w"] = P["domain_score/weights"].t().contiguous()               # [2][256] f32
-        T["score/w"] = P["score/weights"].reshape(self.num_units, self.num_classes).contiguous()
         T["vertex_pred/w"] = P["vertex_pred/weights"].reshape(128, 3 * self.num_classes).contiguous()
         if self.fold_vertex_head:
             Wp = T["vertex_pred/w"].double()
@@ -168,14 +184,16 @@ class vgg16_convs:
         return run_trunk(self.params, self._tc, data, sfx)
 
     def forward(self, data, meta_data, extents, poses=None, data_p=None, want_prob=False, sync_rois=True, want_score=False,
-                dense_vertex=True, batch_global=None, batch_offset=0, depth=None, refine_depth=None, refine_points=None,
+                dense_vertex=None, batch_global=None, batch_offset=0, depth=None, refine_depth=None, refine_points=None,
                 depth_factor=10000.0, estimate_depth=None, estimate_keys=None, estimate_rgb=False):
         """Inference / forward pass.  data [B,H,W,3] (u8 BGR or pre-processed f32), H, W multiples of 16
         (pad_im, lib/utils/blob.py:48-58).  Returns self.layers with the reference's layer names.
 
         dense_vertex=False: the pipeline mode — `vertex_pred` [B,H,W,3C] (81 MB / frame, only read back by the
         reference for visualisation, lib/fcn/test.py:587-599) is not materialised; Houghvotinggpu samples the vertex
-        head on demand from the 1/8-resolution head tensor (bit-identical ROIs, pcnn_hough_vote_fwd_ex).
+        head on demand from the 1/8-resolution head tensor (bit-identical ROIs, pcnn_hough_vote_fwd_ex).  The default (None) is
+        True where the network has a vertex head; a segmentation network (no vertex head) returns conv4_3, conv5_3,
+        score_conv4, score_conv5, label_2d and prob_normalized / score when asked for, and refuses every vertex output.
         batch_global / batch_offset: this call is the image shard [batch_offset, batch_offset + B) of a batch of
         batch_global images (SURVEY.md §8(e)): ROI budget 128 // batch_global per image, global batch indices.
         refine_depth [B,H,W] f32 raw depth (sensor units, z = depth / depth_factor) + refine_points [C,P,3] (the model point
@@ -193,6 +211,11 @@ class vgg16_convs:
         On a vertex_reg_3d network, refine_depth + refine_points refine the depth estimate's detections_* records (test.py:1403-1416;
         for C = 2 pass refine_points in the dataset's numbering and map the outputs with utils/results.py::to_dataset_classes)."""
         C = self.num_classes
+        if dense_vertex is None:
+            dense_vertex = self.vertex_head
+        if not self.vertex_head and (dense_vertex or estimate_depth is not None or estimate_rgb or refine_depth is not None):
+            raise ValueError("a segmentation network (vertex_reg_2d and vertex_reg_3d both False) has no vertex head: dense_vertex, "
+                             "estimate_depth, estimate_rgb and refine_depth need one")
         coord_net = not self.is_train and self.vertex_reg_3d and not self.vertex_reg_2d
         if estimate_depth is not None and not coord_net:
             raise ValueError("estimate_depth estimates poses from object coordinates: it needs is_train=False and vertex_reg_3d "
@@ -221,6 +244,17 @@ class vgg16_convs:
         s5 = conv.conv_bf16(h5, T["score_conv5/weights"], P["score_conv5/biases"], 1, True)
         s4 = conv.conv_bf16(h4, T["score_conv4/weights"], P["score_conv4/biases"], 1, True)
         L["score_conv4"], L["score_conv5"] = s4, s5
+        if not self.vertex_head:
+            # the segmentation network's graph ends here (test fetch: label_2d, prob_normalized, lib/fcn/test.py:233-234); its head
+            # tensor holds the C score channels only
+            lowres = heads.lowres_scores(s4, s5, T["score/w"], C)
+            self._last_lowres = lowres
+            L["label_2d"], prob, score = heads.up8_scores(lowres, P["score/biases"], prob=want_prob, score=want_score)
+            if want_prob:
+                L["prob_normalized"] = prob
+            if want_score:
+                L["score"] = score
+            return L
         if self.fold_vertex_head:
             v5 = conv.conv_bf16(c5, T["score_conv5_vertex/folded_weights"], T["score_conv5_vertex/folded_biases"], 1, False)
             v4 = conv.conv_bf16(c4, T["score_conv4_vertex/folded_weights"], T["score_conv4_vertex/folded_biases"], 1, False)

@@ -16,6 +16,10 @@ A network built with vertex_reg_2d=False, vertex_reg_3d=True (the object-coordin
 its vertex head on 3-D targets (minibatch.py:595-600, 605-616): a labelled pixel of a listed class regresses its object coordinate
 vertmap [B,H,W,3] scaled into [0, 1] by the class's extents.  Its graph has no pose head whatever pose_reg says (vgg16_convs.py:165-200
 builds Hough voting, RoiPool and fc6-fc8 only under vertex_reg_2d), so it trains loss_cls + VERTEX_W * loss_vertex (+ l2).
+A network built with vertex_reg_2d=False, vertex_reg_3d=False (the segmentation models rgbd_scene_single_*.yml, shapenet_*_single_*.yml,
+lov_single_color_*.yml) has no vertex head (vgg16_convs.py:79-149) and trains loss = loss_cls + l2 regularisation (train.py:518-521):
+its head tensor holds the C score channels only, its adjoint is the classification-only one (heads.up8_scores_bwd), and conv4_3 /
+conv5_3 receive gradient through score_conv4 / score_conv5 alone.  pose_reg and adaptation do not apply to it.
 input_format='RGBD' adds the depth trunk conv1_1_p .. conv5_3_p (vgg16_convs.py:99-126): score_conv4 / score_conv5 read the channel
 concat [colour | depth] of conv4_3 / conv5_3 (c_i = 1024), the vertex heads, Hough voting and RoiPool read the colour trunk only.
 A network built with adaptation=True adds the domain classifier (vgg16_convs.py:202-212) and
@@ -98,17 +102,31 @@ def trains_coords(net) -> bool:
     return bool(net.vertex_reg_3d) and not bool(net.vertex_reg_2d)
 
 
+def trains_segmentation(net) -> bool:
+    """True for the segmentation training graph: no vertex head (built with vertex_reg_2d=False, vertex_reg_3d=False), loss_cls alone."""
+    return not net.vertex_head
+
+
+def head_names(net) -> tuple:
+    """The 1x1 head layers of the training graph: score_conv4 / 5 and score, plus the vertex heads where the network has them."""
+    if trains_segmentation(net):
+        return ("score_conv4", "score_conv5", "score")
+    return SCORE_HEADS + ("score", "vertex_pred")
+
+
 def param_layout(net) -> dict:
     """{master name: (TF parameter name, kind, master rows)} for every parameter the training step updates.  score / vertex_pred
     keep C / 3C rows zero-padded to heads.SCORE_ROWS / heads.vertex_rows(C): the channel counts of their 1x1 GEMMs, which
     heads.pack_lowres and heads.up8_heads_bwd read.  A pose_reg=False network has no fc6-fc8: the reference creates those
     variables only under POSE_REG (vgg16_convs.py:175-200), so they are neither trained, decayed nor exported.  Neither has an object-coordinate network, whose
-    pose head sits under vertex_reg_2d in the reference graph."""
+    pose head sits under vertex_reg_2d in the reference graph.  A segmentation network has the trunk(s), score_conv4 / 5 and score
+    only."""
     trunks = ("", "_p") if net.input_format == "RGBD" else ("",)
     weights = [(layer + sfx, "conv1_1" if layer == "conv1_1" else "conv", None) for sfx in trunks for layer in CONV_NAMES]
-    weights += [(name, "conv", None) for name in SCORE_HEADS] + [("score", "conv", heads.SCORE_ROWS),
-                                                               ("vertex_pred", "conv", heads.vertex_rows(net.num_classes))]
-    fc = (("fc6", "fc7", "fc8") if net.pose_reg and not trains_coords(net) else ()) + (("fc9",) if net.domain_branch else ())
+    rows = {"score": heads.SCORE_ROWS, "vertex_pred": heads.vertex_rows(net.num_classes)}
+    weights += [(name, "conv", rows.get(name)) for name in head_names(net)]
+    pose = net.pose_reg and not trains_coords(net) and not trains_segmentation(net)
+    fc = (("fc6", "fc7", "fc8") if pose else ()) + (("fc9",) if net.domain_branch else ())
     weights += [(name, "fc", None) for name in fc]
     if net.domain_branch:
         weights.append(("domain_score", "domain_score", None))
@@ -141,7 +159,8 @@ class Trainer:
         # loss_cls + VERTEX_W * loss_vertex (+ l2 regularisation) alone, as lib/fcn/train.py:517 trains it.  The object-coordinate
         # graph (3-D vertex targets) never has the pose head
         self.coord = trains_coords(net)
-        self.pose_reg = bool(net.pose_reg) and not self.coord
+        self.seg = trains_segmentation(net)      # no vertex head: loss_cls alone
+        self.pose_reg = bool(net.pose_reg) and not self.coord and not self.seg
         self.pose_loss_scale = 1.0               # last dynamic loss scale of the fp16 pose-head backward (see backward())
         self.adapt = net.domain_branch           # the domain classifier and loss_domain (ADAPT_WEIGHT, lib/fcn/config.py:95)
         self.adapt_weight = float(adapt_weight)
@@ -170,7 +189,7 @@ class Trainer:
         for sfx in self.trunks:
             for name in CONV_NAMES[1:]:
                 self.dg[name + sfx] = _tc_dgrad(self.tc[name + sfx + "/w"], 3)
-        for name in SCORE_HEADS + ("score", "vertex_pred"):
+        for name in head_names(self.net):
             self.dg[name] = _tc_dgrad(self.tc[name + "/w"], 1)
         if self.rgbd:
             # score_conv4/5 read the concat [colour 512 | depth 512]: their input-gradient weights [1024][U] split into two
@@ -223,12 +242,12 @@ class Trainer:
             raise ValueError(f"vertmap must be a [{B},{H},{W},3] float32 tensor on {data.device}")
         return vertmap.contiguous()
 
-    def forward(self, data, gt_label_2d, centers, meta_data, extents, gt_poses, points, symmetry, batch_global=None, batch_offset=0,
-                depth=None, data_p=None, vertmap=None):
+    def forward(self, data, gt_label_2d, centers=None, meta_data=None, extents=None, gt_poses=None, points=None, symmetry=None,
+                batch_global=None, batch_offset=0, depth=None, data_p=None, vertmap=None):
         """RGBD: the depth trunk reads depth= (a raw [B,H,W] f32 depth image, sensor units; its blob is formed in conv1_1_p's loader)
         or data_p= (the pre-processed blob [B,H,W,3] f32), as vgg16_convs.forward does.  An object-coordinate network reads
         vertmap= [B,H,W,3] f32 (each pixel's object coordinate, metres in the model frame) and extents [C,3]; other networks ignore
-        vertmap."""
+        vertmap.  A segmentation network reads data, gt_label_2d and the depth input only."""
         net, C, M, T = self.net, self.C, self.master, self.tc
         B, H, W, _ = data.shape
         if self.coord:
@@ -252,6 +271,15 @@ class Trainer:
             A.update(concat_conv4=h4, concat_conv5=h5, depth_in=depth if depth is not None else data_p)
         s4 = conv.conv_bf16(h4, T["score_conv4/w"], M["score_conv4/b"], 1, True)
         s5 = conv.conv_bf16(h5, T["score_conv5/w"], M["score_conv5/b"], 1, True)
+        if self.seg:
+            # score heads only: add + up2, `score` at 1/8 resolution, the score-only head tensor, its x8 up-sampling and loss_cls
+            add_s = heads.add_up2(s4, s5)
+            lr_s = conv.conv_bf16(add_s, T["score/w"], self.zero_bias[heads.SCORE_ROWS], 1, False)
+            lowres = heads.pack_scores(lr_s, C)
+            label, prob, score = heads.up8_scores(lowres, M["score/b"], prob=True, score=True)
+            A.update(s4=s4, s5=s5, add_s=add_s, label_2d=label, lowres=lowres, prob_normalized=prob, score=score, data=data)
+            A["cls_out"] = train_ops.loss_cls(score, prob, gt_label_2d, net.threshold_label)
+            return A
         v4 = conv.conv_bf16(c4, T["score_conv4_vertex/w"], M["score_conv4_vertex/b"], 1, False)
         v5 = conv.conv_bf16(c5, T["score_conv5_vertex/w"], M["score_conv5_vertex/b"], 1, False)
         add_s, add_v = heads.add_up2(s4, s5), heads.add_up2(v4, v5)
@@ -317,54 +345,68 @@ class Trainer:
             with torch.cuda.stream(self.comm):
                 dist.all_reduce(g, op=dist.ReduceOp.SUM)
 
-    def backward(self, A, gt_label_2d, centers, vertmap=None):
+    def backward(self, A, gt_label_2d, centers=None, vertmap=None):
         """All parameter gradients of loss = loss_cls + vertex_w * loss_vertex + loss_pose (weight decay is applied in the update);
         without pose_reg, of loss_cls + vertex_w * loss_vertex.  Loss normalisers (selected-pixel count, vertex weight sum, ROI rows)
-        are GLOBAL over the ranks.  An object-coordinate network needs the forward's vertmap= again (its extents are kept in A)."""
+        are GLOBAL over the ranks.  An object-coordinate network needs the forward's vertmap= again (its extents are kept in A).  A
+        segmentation network's loss is loss_cls alone, and centers is not read."""
         net, C, M, T = self.net, self.C, self.master, self.tc
         data = A["data"]
         dev = data.device
         grads = {}
         # ---- global loss normalisers: one all-reduce of [count_cls, sum_w_vertex(, rows)]
         rows = [torch.tensor(float(A["rows"]), device=dev)] if self.pose_reg else []
-        norm = torch.stack([A["cls_out"][1], A["vtx_out"][1]] + rows)
+        norm = torch.stack([A["cls_out"][1]] + ([] if self.seg else [A["vtx_out"][1]]) + rows)
         if self.world > 1:
             local = norm.clone()
             dist.all_reduce(norm, op=dist.ReduceOp.SUM)
             A["cls_out"] = torch.stack([A["cls_out"][0] * local[0] / norm[0].clamp(min=1.0), norm[0]])     # this rank's share of the global mean
-            A["vtx_out"] = torch.stack([A["vtx_out"][0] * local[1] / norm[1].clamp(min=1e-10), norm[1]])
+            if not self.seg:
+                A["vtx_out"] = torch.stack([A["vtx_out"][0] * local[1] / norm[1].clamp(min=1e-10), norm[1]])
         g5_roi = g4_roi = None                    # the RoiPool gradients of the pose head (and the domain branch)
         if self.pose_reg:
             g5_roi, g4_roi = self._pose_bwd(grads, A, norm)
         # ---- FCN heads
-        vm, ext = (self._require_vertmap(vertmap, data), A["extents"]) if self.coord else (None, None)
-        d_sc, d_vt, dbias = heads.up8_heads_bwd(A["prob_normalized"], A["score"], gt_label_2d, A["cls_out"], 1.0, net.threshold_label,
-                                                A["lowres"], M["vertex_pred/b"], centers, A["vtx_out"], self.vertex_w, self.w_inside, 1.0,
-                                                vertmap=vm, extents=ext)
-        self._emit(grads, "score/b", dbias[:C].contiguous())
-        self._emit(grads, "vertex_pred/b", dbias[C:].contiguous())
+        if self.seg:
+            d_sc, dbias = heads.up8_scores_bwd(A["prob_normalized"], A["score"], gt_label_2d, A["cls_out"], 1.0, net.threshold_label)
+            self._emit(grads, "score/b", dbias)
+        else:
+            vm, ext = (self._require_vertmap(vertmap, data), A["extents"]) if self.coord else (None, None)
+            d_sc, d_vt, dbias = heads.up8_heads_bwd(A["prob_normalized"], A["score"], gt_label_2d, A["cls_out"], 1.0, net.threshold_label,
+                                                    A["lowres"], M["vertex_pred/b"], centers, A["vtx_out"], self.vertex_w, self.w_inside, 1.0,
+                                                    vertmap=vm, extents=ext)
+            self._emit(grads, "score/b", dbias[:C].contiguous())
+            self._emit(grads, "vertex_pred/b", dbias[C:].contiguous())
         self._emit(grads, "score/w", bw.conv_wgrad(A["add_s"], d_sc, 1))
-        self._emit(grads, "vertex_pred/w", bw.conv_wgrad(A["add_v"], d_vt, 1))
+        if not self.seg:
+            self._emit(grads, "vertex_pred/w", bw.conv_wgrad(A["add_v"], d_vt, 1))
         d_add_s = conv.conv_bf16(d_sc, self.dg["score"], self.zero_bias[64], 1, False)
-        d_add_v = conv.conv_bf16(d_vt, self.dg["vertex_pred"], self.zero_bias[128], 1, False)
+        if not self.seg:
+            d_add_v = conv.conv_bf16(d_vt, self.dg["vertex_pred"], self.zero_bias[128], 1, False)
         d_s4, db = bw.relu_bwd(d_add_s, A["s4"], True, want_bias=True)
         self._emit(grads, "score_conv4/b", db)
         d_s5 = heads.up2_bwd(d_add_s, A["s5"])
         self._emit(grads, "score_conv5/b", bw.relu_bwd(d_s5, None, False, want_bias=True, want_dz=False)[1])
-        self._emit(grads, "score_conv4_vertex/b", bw.relu_bwd(d_add_v, None, False, want_bias=True, want_dz=False)[1])
-        d_v5 = heads.up2_bwd(d_add_v)
-        self._emit(grads, "score_conv5_vertex/b", bw.relu_bwd(d_v5, None, False, want_bias=True, want_dz=False)[1])
+        if not self.seg:
+            self._emit(grads, "score_conv4_vertex/b", bw.relu_bwd(d_add_v, None, False, want_bias=True, want_dz=False)[1])
+            d_v5 = heads.up2_bwd(d_add_v)
+            self._emit(grads, "score_conv5_vertex/b", bw.relu_bwd(d_v5, None, False, want_bias=True, want_dz=False)[1])
         c4, c5 = A["conv4_3"], A["conv5_3"]
         # RGB-D: score_conv4/5 read the 1024-channel concat, so their weight gradient is one wgrad on it
         self._emit(grads, "score_conv4/w", bw.conv_wgrad(A["concat_conv4"] if self.rgbd else c4, d_s4, 1))
         self._emit(grads, "score_conv5/w", bw.conv_wgrad(A["concat_conv5"] if self.rgbd else c5, d_s5, 1))
-        self._emit(grads, "score_conv4_vertex/w", bw.conv_wgrad(c4, d_add_v, 1))
-        self._emit(grads, "score_conv5_vertex/w", bw.conv_wgrad(c5, d_v5, 1))
         z512 = self.zero_bias[512]
-        g4 = bw.add_to_bf16(conv.conv_bf16(d_s4, self.dg["score_conv4"], z512, 1, False),
-                            conv.conv_bf16(d_add_v, self.dg["score_conv4_vertex"], z512, 1, False), g4_roi)
-        g5 = bw.add_to_bf16(conv.conv_bf16(d_s5, self.dg["score_conv5"], z512, 1, False),
-                            conv.conv_bf16(d_v5, self.dg["score_conv5_vertex"], z512, 1, False), g5_roi)
+        if self.seg:
+            # conv4_3 / conv5_3 receive gradient through score_conv4 / score_conv5 alone
+            g4 = conv.conv_bf16(d_s4, self.dg["score_conv4"], z512, 1, False)
+            g5 = conv.conv_bf16(d_s5, self.dg["score_conv5"], z512, 1, False)
+        else:
+            self._emit(grads, "score_conv4_vertex/w", bw.conv_wgrad(c4, d_add_v, 1))
+            self._emit(grads, "score_conv5_vertex/w", bw.conv_wgrad(c5, d_v5, 1))
+            g4 = bw.add_to_bf16(conv.conv_bf16(d_s4, self.dg["score_conv4"], z512, 1, False),
+                                conv.conv_bf16(d_add_v, self.dg["score_conv4_vertex"], z512, 1, False), g4_roi)
+            g5 = bw.add_to_bf16(conv.conv_bf16(d_s5, self.dg["score_conv5"], z512, 1, False),
+                                conv.conv_bf16(d_v5, self.dg["score_conv5_vertex"], z512, 1, False), g5_roi)
         # ---- trunk, top down
         self._trunk_bwd(grads, A, g5, g4, "", lambda: conv.im2col_c3(data, self._mean(data)))
         if self.rgbd:
@@ -483,17 +525,20 @@ class Trainer:
                                           1.0, ptr(c16), int(c16 is not None and c16.dtype == torch.float16), stream()))
         self._refresh_derived()
 
-    def step(self, data, gt_label_2d, centers, meta_data, extents, gt_poses, points, symmetry, batch_global=None, batch_offset=0,
-             depth=None, data_p=None, vertmap=None):
+    def step(self, data, gt_label_2d, centers=None, meta_data=None, extents=None, gt_poses=None, points=None, symmetry=None,
+             batch_global=None, batch_offset=0, depth=None, data_p=None, vertmap=None):
         """One forward, backward and update.  Returns loss_cls, loss_vertex, loss_pose, their sum `loss`, num_rois and the gradients
         `grads` (master layouts), plus loss_domain, label_domain and domain_label with the domain branch.  A pose_reg=False network
         returns no pose entries (loss_pose, num_rois): its loss is loss_cls + loss_vertex, and extents, gt_poses, points, symmetry,
         meta_data, batch_global and batch_offset are not read.  An object-coordinate (vertex_reg_3d) network steps the same way
-        whatever its pose_reg, and reads vertmap= [B,H,W,3] f32 and extents [C,3]."""
+        whatever its pose_reg, and reads vertmap= [B,H,W,3] f32 and extents [C,3].  A segmentation network (no vertex head) returns
+        loss_cls, loss (= loss_cls) and grads, and reads neither centers nor any argument after it but the depth input."""
         A = self.forward(data, gt_label_2d, centers, meta_data, extents, gt_poses, points, symmetry, batch_global, batch_offset,
                          depth=depth, data_p=data_p, vertmap=vertmap)
         grads = self.backward(A, gt_label_2d, centers, vertmap=vertmap)
         self.update(grads)
+        if self.seg:
+            return dict(loss_cls=A["cls_out"][0:1], loss=A["cls_out"][0:1].clone(), grads=grads)
         if not self.pose_reg:
             loss_cls, loss_vertex = A["cls_out"][0:1], self.vertex_w * A["vtx_out"][0:1]
             return dict(loss_cls=loss_cls, loss_vertex=loss_vertex, loss=loss_cls + loss_vertex, grads=grads)
